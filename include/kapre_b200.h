@@ -113,7 +113,10 @@ int kapre_istft_inverse(const kapre_istft_plan* plan, const void* stft_dev, int 
 
 /* ---- filterbank (kapre.ApplyFilterbank, kapre/time_frequency.py:501-548) --------------------
  * `fb_host`: row-major (n_freq, n_bands) float32 matrix, e.g. backend.filterbank_mel(...)
- * (kapre/backend.py:197-231) or backend.filterbank_log(...) (kapre/backend.py:234-299). */
+ * (kapre/backend.py:197-231) or backend.filterbank_log(...) (kapre/backend.py:234-299).
+ * Gradient: the layer is linear, so its vector-Jacobian product is kapre_apply_filterbank with a
+ * second filterbank made from the TRANSPOSED (n_bands, n_freq) matrix, applied to the gradient of
+ * the output (n_bands bins in, n_freq bins out).  A mel or log bank is banded and so is its transpose. */
 int kapre_filterbank_create(const float* fb_host, int n_freq, int n_bands, kapre_filterbank** out);
 void kapre_filterbank_destroy(kapre_filterbank* fb);
 int kapre_apply_filterbank(const kapre_filterbank* fb, const float* x_dev, int batch, int channels,
@@ -144,6 +147,36 @@ int kapre_concat_frequency_map(const float* x_dev, float* out_dev, int64_t batch
 int kapre_spec_augment(const float* x_dev, float* out_dev, int64_t batch, int64_t frames, int64_t n_freq,
                        const int* time_masks_dev, int n_time_masks, const int* freq_masks_dev, int n_freq_masks,
                        float mask_value, void* stream);
+
+/* ---- backward passes (vector-Jacobian products) ----------------------------------------------
+ * Gradients follow PyTorch's convention for complex tensors: dL/dRe + i dL/dIm.  Same stream and
+ * ownership rules as the forward calls; the library allocates no data buffers.
+ *
+ * Gradient of kapre_stft_forward(KAPRE_OUT_COMPLEX): g (complex64, `frames` frames of n_fft/2+1 bins)
+ * -> gx (float32 waveform of gx_desc->length samples, the length the forward call saw).  Runs the
+ * inverse-STFT kernel of an adjoint plan (made on first use, freed with `plan`) and one small pass.
+ * `workspace_dev`: kapre_stft_backward_workspace_bytes() bytes of scratch for the overlap-add of the
+ * padded signal (contents ignored); that size is 0, and NULL may be passed, when the overlap-add can be
+ * written straight into gx (no pad_begin and no frame past the signal's end). */
+int64_t kapre_stft_backward_workspace_bytes(const kapre_stft_plan* plan, int batch, int channels, int length,
+                                            int pad_begin, int pad_end);
+int kapre_stft_backward(const kapre_stft_plan* plan, const void* g_dev, const kapre_spec_desc* g_desc, int batch,
+                        int channels, int frames, int pad_begin, int pad_end, float* gx_dev,
+                        const kapre_wave_desc* gx_desc, void* workspace_dev, void* stream);
+/* Gradient of kapre_istft_inverse: gy (float32, (frames-1)*hop + win_length samples) -> gX (complex64,
+ * `frames` frames of n_fft/2+1 bins).  Runs the forward STFT kernel of an adjoint plan (made on first
+ * use, freed with `plan`) and one small pass over the DC and Nyquist bins. */
+int kapre_istft_backward(const kapre_istft_plan* plan, const float* gy_dev, const kapre_wave_desc* gy_desc, int batch,
+                         int channels, int frames, void* gX_dev, const kapre_spec_desc* gX_desc, void* stream);
+/* Gradient of kapre_magnitude: gX = g X / |X|, 0 where |X| = 0; n complex elements. */
+int kapre_magnitude_backward(const void* x_complex_dev, const float* g_dev, void* gx_complex_dev, int64_t n,
+                             void* stream);
+/* Gradient of kapre_magnitude_to_decibel (and of the decibel tail of the fused modes) with respect to its
+ * input x, given the gradient g of its output; TensorFlow's rules: tf.maximum passes the gradient to its
+ * first argument on ties, the threshold's gradient goes to the item's maximum (split among tied maxima).
+ * workspace_dev: >= 12 * n_items bytes, zero on entry, left zero (self-cleaning).  gx may alias g, not x. */
+int kapre_magnitude_to_decibel_backward(const float* x_dev, const float* g_dev, float* gx_dev, int64_t n_items,
+                                        int64_t item_size, const kapre_db_cfg* db, void* workspace_dev, void* stream);
 
 /* ---- adjacent layers ------------------------------------------------------------------------ */
 /* kapre.Delta (kapre/time_frequency.py:563-644): y[t] = sum_{m=-n..n} m * x[t+m] / (2 sum m^2) along the

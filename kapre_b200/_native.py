@@ -52,6 +52,14 @@ SYMBOLS = [
     ('kapre_magnitude', c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     ('kapre_phase', c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     ('kapre_magnitude_to_decibel', c_int, [c_void_p, c_void_p, c_int64, c_int64, POINTER(DbCfg), c_void_p, c_void_p]),
+    ('kapre_stft_backward_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int, c_int, c_int]),
+    ('kapre_stft_backward', c_int, [c_void_p, c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                    POINTER(WaveDesc), c_void_p, c_void_p]),
+    ('kapre_istft_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_int, c_int, c_int, c_void_p,
+                                     POINTER(SpecDesc), c_void_p]),
+    ('kapre_magnitude_backward', c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    ('kapre_magnitude_to_decibel_backward', c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, POINTER(DbCfg),
+                                                    c_void_p, c_void_p]),
     ('kapre_delta', c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
     ('kapre_frame', c_int, [c_void_p, POINTER(WaveDesc), c_int, c_int, c_int, c_float, c_void_p, POINTER(SpecDesc), c_void_p]),
     ('kapre_energy', c_int, [c_void_p, POINTER(WaveDesc), c_int, c_int, c_int, c_float, c_float, c_void_p, POINTER(WaveDesc), c_void_p]),

@@ -22,6 +22,7 @@
 #include "mr_core.cuh"
 #include "tc_dft.cuh"
 #include "tc_mel.cuh"
+#include "grad_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -378,6 +379,10 @@ struct kapre_stft_plan {
     float* tc_cs = nullptr;   // stage-2 C / S matrices hi/lo
     float2* tc_tw = nullptr;  // a e^{-2 pi i n2 k1 / 1024}
     float2* tc_w32 = nullptr; // e^{-2 pi i j / 32}
+    // adjoint (kapre_stft_backward): the inverse plan with dual window w * n_fft / 2, made on first use
+    std::vector<float> window_host;
+    std::mutex adj_mu;
+    kapre_istft_plan* adj = nullptr;
 };
 
 // (K = 32 rows, N = 32 columns) matrix -> the K-major (8 kchunk, 32 col, 4) layout of the wgmma B operand, TF32 hi / lo
@@ -432,6 +437,10 @@ struct kapre_istft_plan {
     float2* twn = nullptr;
     float* dualn = nullptr;   // generic path: dual / n_fft
     float2* tw = nullptr;     // generic path: exp(+2 pi i r / n_fft)
+    // adjoint (kapre_istft_backward): the forward plan with window dual * 2 / n_fft, made on first use
+    std::vector<float> dual_host;
+    std::mutex adj_mu;
+    kapre_stft_plan* adj = nullptr;
 };
 
 struct kapre_filterbank {
@@ -846,6 +855,7 @@ int kapre_stft_plan_create(int n_fft, int win_length, int hop_length, const floa
     p->n_fft = n_fft; p->win_length = win_length; p->hop = hop_length;
     p->Q = kb_q_for_nfft(n_fft);
     p->win_eff = win_length < n_fft ? win_length : n_fft;
+    p->window_host.assign(window_host, window_host + win_length);
     int rc = kb_dev_info(&p->dev);
     if (rc) { delete p; return rc; }
     if (p->Q) {
@@ -888,6 +898,7 @@ void kapre_stft_plan_destroy(kapre_stft_plan* p) {
     if (!p) return;
     cudaFree(p->wh); cudaFree(p->cwq); cudaFree(p->twp); cudaFree(p->twn); cudaFree(p->twn2); cudaFree(p->w); cudaFree(p->tw);
     cudaFree(p->tc_f1); cudaFree(p->tc_cs); cudaFree(p->tc_tw); cudaFree(p->tc_w32);
+    kapre_istft_plan_destroy(p->adj);
     delete p;
 }
 
@@ -1213,6 +1224,7 @@ int kapre_istft_plan_create(int n_fft, int win_length, int hop_length, const flo
     p->n_fft = n_fft; p->win_length = win_length; p->hop = hop_length;
     p->Q = kb_q_for_nfft(n_fft);
     p->win = win_length < n_fft ? win_length : n_fft;
+    p->dual_host.assign(dual_window_host, dual_window_host + win_length);
     int rc = kb_dev_info(&p->dev);
     if (rc) { delete p; return rc; }
     if (p->Q) {
@@ -1241,6 +1253,7 @@ int kapre_istft_plan_create(int n_fft, int win_length, int hop_length, const flo
 void kapre_istft_plan_destroy(kapre_istft_plan* p) {
     if (!p) return;
     cudaFree(p->dual); cudaFree(p->twp); cudaFree(p->twn); cudaFree(p->dualn); cudaFree(p->tw);
+    kapre_stft_plan_destroy(p->adj);
     delete p;
 }
 
@@ -1639,6 +1652,211 @@ int kapre_tc_dft_stage1(const float* x_dev, int n_items, long long item_stride, 
     kb_tc_dft_stage1_kernel<<<grid, KB_TC_THREADS, KB_TC_SMEM, (cudaStream_t)stream>>>(p);
     KB_CUDA(cudaGetLastError());
     g_launches++;
+    return 0;
+}
+
+}  // extern "C"
+
+// ---- backward passes (grad_core.cuh) ---------------------------------------------------------------
+// Adjoint plans are constants of their owner: made on first use under the owner's lock, freed with it.
+static int kb_stft_adjoint_plan(const kapre_stft_plan* cp, kapre_istft_plan** out) {
+    kapre_stft_plan* p = const_cast<kapre_stft_plan*>(cp);
+    std::lock_guard<std::mutex> lk(p->adj_mu);
+    if (!p->adj) {
+        // dual window w * N/2: the inverse kernel's irfft carries 1/N and weighs interior bins 2
+        std::vector<float> d(p->win_length, 0.0f);
+        for (int m = 0; m < p->win_eff; ++m) d[m] = (float)((double)p->window_host[m] * (double)p->n_fft * 0.5);
+        int rc = kapre_istft_plan_create(p->n_fft, p->win_length, p->hop, d.data(), &p->adj);
+        if (rc) { p->adj = nullptr; return rc; }
+    }
+    *out = p->adj;
+    return 0;
+}
+
+static int kb_istft_adjoint_plan(const kapre_istft_plan* cp, kapre_stft_plan** out) {
+    kapre_istft_plan* p = const_cast<kapre_istft_plan*>(cp);
+    std::lock_guard<std::mutex> lk(p->adj_mu);
+    if (!p->adj) {
+        // window dual * 2/N over the first min(win_length, n_fft) samples (the only ones the inverse produces)
+        std::vector<float> w(p->win_length, 0.0f);
+        for (int m = 0; m < p->win; ++m) w[m] = (float)((double)p->dual_host[m] * 2.0 / (double)p->n_fft);
+        int rc = kapre_stft_plan_create(p->n_fft, p->win_length, p->hop, w.data(), &p->adj);
+        if (rc) { p->adj = nullptr; return rc; }
+    }
+    *out = p->adj;
+    return 0;
+}
+
+__global__ void kb_stft_adj_kernel(const __grid_constant__ KbStftAdjParams p, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_stft_adj_elem(p, i);
+}
+
+__global__ void kb_istft_adj_kernel(const __grid_constant__ KbIstftAdjParams p, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_istft_adj_elem(p, i);
+}
+
+__global__ void kb_mag_bwd_kernel(const float2* __restrict__ X, const float* __restrict__ g, float2* __restrict__ gX,
+                                  long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_mag_bwd_elem(X, g, gX, i);
+}
+
+// one decibel-backward pass: `chunks` CTAs per item, each walking a strided share of the item
+template <int PASS>
+__global__ void __launch_bounds__(256) kb_dbb_kernel(const __grid_constant__ KbDbBwdParams p, int chunks) {
+    const long long item = blockIdx.x / chunks;
+    const int chunk = (int)(blockIdx.x - item * chunks);
+    const long long i0 = (long long)chunk * blockDim.x + threadIdx.x, step = (long long)chunks * blockDim.x;
+    if (PASS == 0) kb_dbb_max(p, item, i0, step, threadIdx.x);
+    else if (PASS == 1) kb_dbb_pass(p, item, i0, step, threadIdx.x);
+    else kb_dbb_share(p, item, i0, step);
+}
+
+// padded-signal geometry of the STFT adjoint: frames, overlap-add length, and whether the overlap-add can be
+// written straight into gx (no pad in front and no sample past the signal's end)
+static void kb_stft_adj_geom(const kapre_stft_plan* p, int length, int pad_begin, int pad_end, int* T, long long* ola_len,
+                             bool* direct) {
+    *T = kapre_stft_num_frames(p, length, pad_begin, pad_end);
+    *ola_len = *T > 0 ? (long long)(*T - 1) * p->hop + p->win_length : 0;
+    *direct = !pad_begin && *ola_len <= length;
+}
+
+extern "C" {
+
+int64_t kapre_stft_backward_workspace_bytes(const kapre_stft_plan* plan, int batch, int channels, int length,
+                                            int pad_begin, int pad_end) {
+    if (!plan || batch < 0 || channels < 0 || length < 0) return kb_fail(KAPRE_E_INVALID, "bad argument");
+    int T;
+    long long ola_len;
+    bool direct;
+    kb_stft_adj_geom(plan, length, pad_begin, pad_end, &T, &ola_len, &direct);
+    if (direct || T <= 0) return 0;
+    return (int64_t)batch * channels * ola_len * (int64_t)sizeof(float);
+}
+
+int kapre_stft_backward(const kapre_stft_plan* plan, const void* g_dev, const kapre_spec_desc* gd, int batch,
+                        int channels, int frames, int pad_begin, int pad_end, float* gx_dev, const kapre_wave_desc* xd,
+                        void* workspace_dev, void* stream) {
+    if (!plan || !gd || !xd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
+    if (xd->batch != batch || xd->channels != channels || batch < 0 || channels < 0 || xd->length < 0)
+        return kb_fail(KAPRE_E_INVALID, "gx descriptor (%d, %d) does not match batch=%d channels=%d", xd->batch,
+                       xd->channels, batch, channels);
+    if (pad_begin && plan->hop > plan->n_fft)
+        return kb_fail(KAPRE_E_INVALID, "pad_begin needs hop_length <= n_fft");
+    const int L = xd->length;
+    int T;
+    long long ola_len;
+    bool direct;
+    kb_stft_adj_geom(plan, L, pad_begin, pad_end, &T, &ola_len, &direct);
+    if (frames != T) return kb_fail(KAPRE_E_INVALID, "%d samples give %d frames, got frames=%d", L, T, frames);
+    const long long n = (long long)batch * channels * L;
+    if (n == 0) return 0;
+    if (!gx_dev || (T > 0 && !g_dev)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if (T > 0 && !direct && !workspace_dev)
+        return kb_fail(KAPRE_E_INVALID, "workspace of kapre_stft_backward_workspace_bytes() bytes required");
+    cudaStream_t st = (cudaStream_t)stream;
+    KbStftAdjParams q{};
+    q.G = (const float2*)g_dev; q.g_sb = gd->stride_b; q.g_sc = gd->stride_c; q.g_st = gd->stride_t; q.g_sk = gd->stride_f;
+    q.gx = gx_dev; q.x_sb = xd->stride_b; q.x_sc = xd->stride_c; q.x_sl = xd->stride_l;
+    q.B = batch; q.C = channels; q.L = L; q.T = T;
+    q.n_fft = plan->n_fft; q.hop = plan->hop; q.win_eff = plan->win_eff; q.pad_left = pad_begin ? plan->n_fft - plan->hop : 0;
+    q.w = plan->w;
+    if (T > 0) {
+        kapre_istft_plan* adj;
+        if ((rc = kb_stft_adjoint_plan(plan, &adj))) return rc;
+        kapre_wave_desc od;
+        od.batch = batch; od.channels = channels; od.length = (int)ola_len;
+        if (direct) {   // in place: the pass below reads and writes the same sample
+            od.stride_b = xd->stride_b; od.stride_c = xd->stride_c; od.stride_l = xd->stride_l;
+            q.ola = gx_dev;
+        } else {
+            od.stride_b = (long long)channels * ola_len; od.stride_c = ola_len; od.stride_l = 1;
+            q.ola = (const float*)workspace_dev;
+        }
+        q.a_sb = od.stride_b; q.a_sc = od.stride_c; q.a_sl = od.stride_l;
+        if ((rc = kapre_istft_inverse(adj, g_dev, batch, channels, T, gd, (float*)q.ola, &od, stream))) return rc;
+    }
+    int grid;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_stft_adj_kernel<<<grid, 256, 0, st>>>(q, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+int kapre_istft_backward(const kapre_istft_plan* plan, const float* gy_dev, const kapre_wave_desc* yd, int batch,
+                         int channels, int frames, void* gX_dev, const kapre_spec_desc* sd, void* stream) {
+    if (!plan || !yd || !sd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
+    if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (yd->batch != batch || yd->channels != channels)
+        return kb_fail(KAPRE_E_INVALID, "gy descriptor (%d, %d) does not match batch=%d channels=%d", yd->batch,
+                       yd->channels, batch, channels);
+    if (batch == 0 || channels == 0 || frames == 0) return 0;
+    const long long out_len = (long long)(frames - 1) * plan->hop + plan->win_length;
+    if (yd->length != out_len)
+        return kb_fail(KAPRE_E_INVALID, "gy length must be (frames-1)*hop+win_length = %lld, got %d", out_len, yd->length);
+    if (!gy_dev || !gX_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    kapre_stft_plan* adj;
+    if ((rc = kb_istft_adjoint_plan(plan, &adj))) return rc;
+    if ((rc = kapre_stft_forward(adj, gy_dev, yd, 0, 0, KAPRE_OUT_COMPLEX, gX_dev, sd, nullptr, nullptr, nullptr, stream)))
+        return rc;
+    KbIstftAdjParams q{};
+    q.gX = (float2*)gX_dev; q.sb = sd->stride_b; q.sc = sd->stride_c; q.st = sd->stride_t; q.sk = sd->stride_f;
+    q.B = batch; q.C = channels; q.T = frames; q.n_fft = plan->n_fft;
+    const long long n = (long long)batch * channels * frames * ((plan->n_fft & 1) ? 1 : 2);
+    int grid;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_istft_adj_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(q, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+int kapre_magnitude_backward(const void* x_complex_dev, const float* g_dev, void* gx_complex_dev, int64_t n, void* stream) {
+    if (n < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (n == 0) return 0;
+    if (!x_complex_dev || !g_dev || !gx_complex_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    int grid, rc;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_mag_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float2*)x_complex_dev, g_dev, (float2*)gx_complex_dev, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+int kapre_magnitude_to_decibel_backward(const float* x_dev, const float* g_dev, float* gx_dev, int64_t n_items,
+                                        int64_t item_size, const kapre_db_cfg* db, void* workspace_dev, void* stream) {
+    int rc = kb_check_db(db);
+    if (rc) return rc;
+    if (n_items < 0 || item_size < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (n_items == 0 || item_size == 0) return 0;
+    if (!x_dev || !g_dev || !gx_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if (gx_dev == x_dev) return kb_fail(KAPRE_E_INVALID, "gx must not alias x (the last pass re-reads x)");
+    cudaStream_t st = (cudaStream_t)stream;
+    KbDbBwdParams p{};
+    p.x = x_dev; p.g = g_dev; p.gx = gx_dev; p.item_size = item_size; p.ws = (unsigned int*)workspace_dev;
+    p.n_items = n_items; p.amin = db->amin; p.dyn_range = db->dynamic_range;
+    p.dscale = (float)(10.0 / log(10.0));
+    kb_db_consts(db, &p.db_mul, &p.db_sub);
+    long long chunks = (item_size + 256 * 8 - 1) / (256 * 8);
+    if (chunks > 64) chunks = 64;
+    if (chunks < 1) chunks = 1;
+    const long long grid = n_items * chunks;
+    if (grid > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many items");
+    kb_dbb_kernel<0><<<(unsigned)grid, 256, 0, st>>>(p, (int)chunks);
+    KB_CUDA(cudaGetLastError());
+    kb_dbb_kernel<1><<<(unsigned)grid, 256, 0, st>>>(p, (int)chunks);
+    KB_CUDA(cudaGetLastError());
+    kb_dbb_kernel<2><<<(unsigned)grid, 256, 0, st>>>(p, (int)chunks);
+    KB_CUDA(cudaGetLastError());
+    g_launches += 3;
+    KB_CUDA(cudaMemsetAsync(workspace_dev, 0, (size_t)n_items * 3 * sizeof(unsigned int), st));   // self-cleaning
     return 0;
 }
 

@@ -84,6 +84,11 @@ def _workspace(n_items: int, device) -> torch.Tensor:
     return ws
 
 
+def _wants_grad(t) -> bool:
+    """True when a CUDA tensor input should be recorded for autograd (see ``autograd.py``)."""
+    return isinstance(t, torch.Tensor) and t.is_cuda and t.requires_grad and torch.is_grad_enabled()
+
+
 def _device_of_first_arg(fn):
     """Run an op with the device of its first (tensor) argument current; host inputs keep the current device."""
     import functools
@@ -185,6 +190,14 @@ class Filterbank:
             raise ValueError('filterbank must be (n_freq, n_bands)')
         self.n_freq, self.n_bands = self.matrix.shape
         self._per_device = {}
+        self._transposed = None
+
+    def transposed(self) -> 'Filterbank':
+        """The (n_bands, n_freq) filterbank: applying it to the gradient of ``apply_filterbank``'s output
+        gives the gradient of its input."""
+        if self._transposed is None:
+            self._transposed = Filterbank(self.matrix.T)
+        return self._transposed
 
     def handle(self):
         _require_cuda()
@@ -242,6 +255,10 @@ def stft_forward(x: torch.Tensor, plan: StftPlan, input_data_format, output_data
     ``db`` = (ref_value, amin, dynamic_range); ``workspace``: caller-owned decibel scratch (``new_workspace``)."""
     if not x.is_cuda:
         raise N.KapreNativeError('stft_forward needs a CUDA tensor')
+    if _wants_grad(x) and mode != N.OUT_MAG_PHASE:
+        from . import autograd
+        return autograd.stft_forward(x, plan, input_data_format, output_data_format, pad_begin, pad_end, mode, fb, db,
+                                     workspace)
     with _on_device_of(x):
         return _stft_forward(x, plan, input_data_format, output_data_format, pad_begin, pad_end, mode, fb, db, workspace)
 
@@ -284,6 +301,9 @@ def _stft_forward(x, plan, input_data_format, output_data_format, pad_begin, pad
 def istft(X: torch.Tensor, plan: IstftPlan, input_data_format, output_data_format):
     if not X.is_cuda:
         raise N.KapreNativeError('istft needs a CUDA tensor')
+    if _wants_grad(X):
+        from . import autograd
+        return autograd.istft(X, plan, input_data_format, output_data_format)
     if X.dtype != torch.complex64:
         X = X.to(torch.complex64)
     sd, (B, C, T, F) = _spec_desc(X, input_data_format)
@@ -308,6 +328,9 @@ def istft(X: torch.Tensor, plan: IstftPlan, input_data_format, output_data_forma
 def apply_filterbank(x: torch.Tensor, fb: Filterbank, data_format):
     if not x.is_cuda:
         raise N.KapreNativeError('apply_filterbank needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.apply_filterbank(x, fb, data_format)
     if x.dtype != torch.float32:
         x = x.float()
     xd, (B, C, T, F) = _spec_desc(x, data_format)
@@ -327,6 +350,9 @@ def magnitude(x: torch.Tensor):
         raise N.KapreNativeError('magnitude needs a CUDA tensor')
     if not x.is_complex():
         return x.abs()  # tf.abs of a real tensor: plain |x| (not on the hot path)
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.magnitude(x)
     x = x.to(torch.complex64).contiguous()
     out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
     if out.numel():
@@ -347,6 +373,9 @@ def phase(x: torch.Tensor):
 
 @_device_of_first_arg
 def magnitude_to_decibel(x, ref_value=1.0, amin=1e-5, dynamic_range=80.0):
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.magnitude_to_decibel(x, ref_value, amin, dynamic_range)
     t, was_host = to_device(x, torch.float32)
     t = t.contiguous()
     out = torch.empty_like(t)
@@ -360,6 +389,84 @@ def magnitude_to_decibel(x, ref_value=1.0, amin=1e-5, dynamic_range=80.0):
         N.check(N.lib().kapre_magnitude_to_decibel(_ptr(t), _ptr(out), n_items, item, ctypes.byref(dbc), _ptr(ws),
                                                    _stream_ptr()))
     return to_host(out) if was_host and isinstance(x, np.ndarray) else out
+
+
+# ------------------------------------------------------------------------------- backward passes
+def _raw(t: torch.Tensor) -> torch.Tensor:
+    """Materialise lazy conjugate / negative views: the kernels read the tensor's memory as it is."""
+    return t.resolve_conj().resolve_neg()
+
+
+@_device_of_first_arg
+def stft_backward(g: torch.Tensor, plan: StftPlan, input_data_format, output_data_format, pad_begin, pad_end, length):
+    """Gradient of ``stft_forward(..., OUT_COMPLEX)`` with respect to its waveform of ``length`` samples, given the
+    gradient ``g`` of the complex spectrum (any strides)."""
+    g = _raw(g.to(torch.complex64))
+    gd, (B, C, T, F) = _spec_desc(g, output_data_format)
+    L = int(length)
+    if input_data_format == _CH_LAST_STR:
+        gx = torch.empty((B, L, C), dtype=torch.float32, device=g.device)
+        sb, sl, sc = gx.stride()
+    else:
+        gx = torch.empty((B, C, L), dtype=torch.float32, device=g.device)
+        sb, sc, sl = gx.stride()
+    if gx.numel() == 0:
+        return gx
+    lib = N.lib()
+    nbytes = int(lib.kapre_stft_backward_workspace_bytes(plan.handle(), B, C, L, int(bool(pad_begin)), int(bool(pad_end))))
+    if nbytes < 0:
+        N.check(nbytes)
+    ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=g.device) if nbytes else None
+    xd = N.WaveDesc(B, C, L, sb, sc, sl)
+    N.check(lib.kapre_stft_backward(plan.handle(), _ptr(g), ctypes.byref(gd), B, C, T, int(bool(pad_begin)),
+                                    int(bool(pad_end)), _ptr(gx), ctypes.byref(xd), _ptr(ws) if ws is not None else None,
+                                    _stream_ptr()))
+    return gx
+
+
+@_device_of_first_arg
+def istft_backward(gy: torch.Tensor, plan: IstftPlan, input_data_format, output_data_format, frames):
+    """Gradient of ``istft`` with respect to its complex spectrum of ``frames`` frames, given the gradient ``gy`` of
+    the waveform (any strides)."""
+    gy = _raw(gy.to(torch.float32))
+    yd, (B, C, _) = _wave_desc(gy, output_data_format)
+    gX, sd = _spec_alloc(B, C, int(frames), plan.n_fft // 2 + 1, input_data_format, torch.complex64, gy.device)
+    if gX.numel() == 0:
+        return gX
+    N.check(N.lib().kapre_istft_backward(plan.handle(), _ptr(gy), ctypes.byref(yd), B, C, int(frames), _ptr(gX),
+                                         ctypes.byref(sd), _stream_ptr()))
+    return gX
+
+
+@_device_of_first_arg
+def magnitude_backward(X: torch.Tensor, g: torch.Tensor):
+    """Gradient of ``magnitude`` with respect to the complex64 tensor ``X``: ``g X / |X|``, 0 where ``|X| = 0``."""
+    X = _raw(X.to(torch.complex64)).contiguous()
+    g = _raw(g.to(torch.float32)).contiguous()
+    if g.shape != X.shape:
+        raise ValueError('gradient shape %s does not match %s' % (tuple(g.shape), tuple(X.shape)))
+    gX = torch.empty_like(X)
+    if X.numel():
+        N.check(N.lib().kapre_magnitude_backward(_ptr(X), _ptr(g), _ptr(gX), X.numel(), _stream_ptr()))
+    return gX
+
+
+@_device_of_first_arg
+def magnitude_to_decibel_backward(x: torch.Tensor, g: torch.Tensor, ref_value=1.0, amin=1e-5, dynamic_range=80.0):
+    """Gradient of ``magnitude_to_decibel`` with respect to its input ``x`` (items along axis 0, as the forward),
+    with TensorFlow's tie rules."""
+    x = x.to(torch.float32).contiguous()
+    g = _raw(g.to(torch.float32)).contiguous()
+    if g.shape != x.shape:
+        raise ValueError('gradient shape %s does not match %s' % (tuple(g.shape), tuple(x.shape)))
+    gx = torch.empty_like(x)
+    if x.numel():
+        n_items, item = (x.shape[0], x.numel() // x.shape[0]) if x.dim() > 1 else (1, x.numel())
+        ws = torch.zeros(3 * max(n_items, 1), dtype=torch.int32, device=x.device)
+        dbc = N.DbCfg(float(ref_value), float(amin), float(dynamic_range))
+        N.check(N.lib().kapre_magnitude_to_decibel_backward(_ptr(x), _ptr(g), _ptr(gx), n_items, item,
+                                                            ctypes.byref(dbc), _ptr(ws), _stream_ptr()))
+    return gx
 
 
 # ------------------------------------------------------------------------------- adjacent layers
