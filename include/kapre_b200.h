@@ -177,6 +177,41 @@ int kapre_magnitude_backward(const void* x_complex_dev, const float* g_dev, void
  * workspace_dev: >= 12 * n_items bytes, zero on entry, left zero (self-cleaning).  gx may alias g, not x. */
 int kapre_magnitude_to_decibel_backward(const float* x_dev, const float* g_dev, float* gx_dev, int64_t n_items,
                                         int64_t item_size, const kapre_db_cfg* db, void* workspace_dev, void* stream);
+/* Gradient of kapre_phase: gX = g i X / |X|^2 (torch.angle's rule), 0 where |X| = 0; n complex elements. */
+int kapre_phase_backward(const void* x_complex_dev, const float* g_dev, void* gx_complex_dev, int64_t n, void* stream);
+/* Gradient of kapre_stft_forward(KAPRE_OUT_MAG_PHASE) with respect to the complex spectrum X (recomputed by the
+ * caller with KAPRE_OUT_COMPLEX): gX = X / |X| (g_mag + i g_phase / |X|), 0 where |X| = 0.  g_mag is the magnitude
+ * half's gradient, taken through kapre_magnitude_to_decibel_backward first when the forward was decibel-scaled;
+ * g_phase the phase half's.  Every tensor is (batch, channels, frames, n_freq) with its own element strides, so
+ * both halves can be read where they lie in the 2C-channel gradient; a NULL g_mag or g_phase (and its descriptor)
+ * means zero.  gX must not alias X. */
+int kapre_mag_phase_backward(const void* x_complex_dev, const kapre_spec_desc* x_desc, const float* g_mag_dev,
+                             const kapre_spec_desc* g_mag_desc, const float* g_phase_dev,
+                             const kapre_spec_desc* g_phase_desc, void* gx_complex_dev, const kapre_spec_desc* gx_desc,
+                             int batch, int channels, int frames, int n_freq, void* stream);
+/* Gradient of kapre_delta on the same contiguous (outer, frames, inner) layout:
+ *   gx[s] = sum_t sum_{m=1..n} m ([P(t+m) = s] - [P(t-m) = s]) g[t] / (2 sum m^2),
+ * P the pad_mode extension of the time axis (a position P sends to zero contributes nothing); in the interior
+ * gx[s] = sum_m m (g[s-m] - g[s+m]) / (2 sum m^2).  One gather per element, no atomics; not in place. */
+int kapre_delta_backward(const float* g_dev, float* gx_dev, int64_t outer, int64_t frames, int64_t inner,
+                         int win_length, int pad_mode, void* stream);
+/* Gradient of kapre_frame: g (frames frames of frame_length samples, g_desc strides as kapre_frame's out_desc)
+ * -> gx[s] = sum over frames t with 0 <= s - t*hop < frame_length of g[t, s - t*hop], for the gx_desc->length
+ * samples of the signal (pad_value positions are constants and drop out); samples no frame covers get 0. */
+int kapre_frame_backward(const float* g_dev, const kapre_spec_desc* g_desc, int frames, int frame_length,
+                         int hop_length, float* gx_dev, const kapre_wave_desc* gx_desc, void* stream);
+/* Gradient of kapre_energy: g (g_desc->length = frames) and the forward's input x ->
+ * gx[s] = 2 * scale * x[s] * sum over frames t covering s of g[t]; 0 for samples no frame covers (the gaps when
+ * hop_length > frame_length). */
+int kapre_energy_backward(const float* x_dev, const kapre_wave_desc* x_desc, const float* g_dev,
+                          const kapre_wave_desc* g_desc, int frame_length, int hop_length, float scale, float* gx_dev,
+                          const kapre_wave_desc* gx_desc, void* stream);
+/* Gradient of kapre_concat_frequency_map: gx = the first `channels` channels of the contiguous (channels + 1)-channel
+ * gradient g, in either data format; gx contiguous with `channels` channels. */
+int kapre_concat_frequency_map_backward(const float* g_dev, float* gx_dev, int64_t batch, int64_t channels,
+                                        int64_t frames, int64_t n_freq, int channels_last, void* stream);
+/* SpecAugment has no entry of its own: its gradient is kapre_spec_augment over the gradient with mask_value = 0
+ * and the same device masks. */
 
 /* ---- adjacent layers ------------------------------------------------------------------------ */
 /* kapre.Delta (kapre/time_frequency.py:563-644): y[t] = sum_{m=-n..n} m * x[t+m] / (2 sum m^2) along the

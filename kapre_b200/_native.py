@@ -60,6 +60,17 @@ SYMBOLS = [
     ('kapre_magnitude_backward', c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     ('kapre_magnitude_to_decibel_backward', c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, POINTER(DbCfg),
                                                     c_void_p, c_void_p]),
+    ('kapre_phase_backward', c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    ('kapre_mag_phase_backward', c_int, [c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p,
+                                         POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int,
+                                         c_void_p]),
+    ('kapre_delta_backward', c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
+    ('kapre_frame_backward', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_void_p, POINTER(WaveDesc),
+                                     c_void_p]),
+    ('kapre_energy_backward', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_int, c_int, c_float,
+                                      c_void_p, POINTER(WaveDesc), c_void_p]),
+    ('kapre_concat_frequency_map_backward', c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int,
+                                                    c_void_p]),
     ('kapre_delta', c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
     ('kapre_frame', c_int, [c_void_p, POINTER(WaveDesc), c_int, c_int, c_int, c_float, c_void_p, POINTER(SpecDesc), c_void_p]),
     ('kapre_energy', c_int, [c_void_p, POINTER(WaveDesc), c_int, c_int, c_int, c_float, c_float, c_void_p, POINTER(WaveDesc), c_void_p]),

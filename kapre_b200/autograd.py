@@ -10,10 +10,16 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * Magnitude       -> ``kapre_magnitude_backward`` (g X / |X|)
 * ApplyFilterbank -> ``kapre_apply_filterbank`` with the transposed matrix
 * MagnitudeToDecibel -> ``kapre_magnitude_to_decibel_backward`` (TensorFlow's tie rules)
+* Phase           -> ``kapre_phase_backward``     (g i X / |X|^2)
+* Delta           -> ``kapre_delta_backward``     (gather over the padded taps)
+* Frame, Energy   -> ``kapre_frame_backward``, ``kapre_energy_backward`` (sum over the frames covering a sample)
+* ConcatenateFrequencyMap -> ``kapre_concat_frequency_map_backward`` (the first C channels)
+* SpecAugment     -> ``kapre_spec_augment`` over the gradient, mask value 0, the forward's device masks
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
-only the waveform and recomputes the complex spectrum and the pre-decibel values in its backward.  Backward
-passes are once-differentiable: a second derivative raises.
+only the waveform and recomputes the complex spectrum and the pre-decibel values in its backward; so does
+``get_stft_mag_phase``'s fused magnitude + phase launch, whose backward ends in ``kapre_mag_phase_backward``.
+Backward passes are once-differentiable: a second derivative raises.
 """
 from __future__ import annotations
 
@@ -64,6 +70,39 @@ class _FusedStack(torch.autograd.Function):
         gS = ops.magnitude_backward(S, g)
         gx = ops.stft_backward(gS, plan, idf, odf, pb, pe, x.shape[1] if idf == ops._CH_LAST_STR else x.shape[2])
         return (gx,) + (None,) * 9
+
+
+class _MagPhase(torch.autograd.Function):
+    """``get_stft_mag_phase``'s fused mode (|STFT| [-> dB] and angle(STFT) side by side) as one launch forward."""
+
+    @staticmethod
+    def forward(ctx, x, plan, input_data_format, output_data_format, pad_begin, pad_end, db, workspace):
+        ctx.save_for_backward(x)
+        ctx.cfg = (plan, input_data_format, output_data_format, pad_begin, pad_end, db)
+        return ops.stft_forward(x, plan, input_data_format, output_data_format, pad_begin, pad_end, N.OUT_MAG_PHASE,
+                                None, db, workspace)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        plan, idf, odf, pb, pe, db = ctx.cfg
+        S = ops.stft_forward(x, plan, idf, odf, pb, pe, N.OUT_COMPLEX)
+        cl = odf == ops._CH_LAST_STR
+        C = S.shape[3] if cl else S.shape[1]
+
+        def half(t, lo):        # channels [lo, lo + C) of the 2C-channel output, as a view
+            return t[..., lo:lo + C] if cl else t[:, lo:lo + C]
+        g_mag, g_phase = half(g, 0), half(g, C)
+        if db is not None:
+            # The same fused launch without its decibel tail gives the very magnitudes the forward clamped (the
+            # OUT_MAG launch pairs FFT outputs differently at some sizes, so its last bits may differ), and the
+            # clamp decision is recomputed from them.  Each batch item is one clamp item, as in the forward.
+            pre = ops.stft_forward(x, plan, idf, odf, pb, pe, N.OUT_MAG_PHASE)
+            g_mag = ops.magnitude_to_decibel_backward(half(pre, 0), g_mag, *db)
+        gS = ops.mag_phase_backward(S, g_mag, g_phase, odf)
+        gx = ops.stft_backward(gS, plan, idf, odf, pb, pe, x.shape[1] if idf == ops._CH_LAST_STR else x.shape[2])
+        return (gx,) + (None,) * 7
 
 
 class _Istft(torch.autograd.Function):
@@ -120,14 +159,120 @@ class _MagnitudeToDecibel(torch.autograd.Function):
         return ops.magnitude_to_decibel_backward(x, g, *ctx.db), None, None, None
 
 
+class _Phase(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, X):
+        ctx.save_for_backward(X)
+        return ops.phase(X)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (X,) = ctx.saved_tensors
+        return ops.phase_backward(X, g)
+
+
+class _Delta(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, win_length, mode, data_format):
+        ctx.cfg = (win_length, mode, data_format)
+        return ops.delta(x, win_length, mode, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return ops.delta_backward(g, *ctx.cfg), None, None, None
+
+
+class _Frame(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, frame_length, hop_length, pad_end, pad_value, data_format):
+        ctx.cfg = (frame_length, hop_length, data_format, x.shape[1] if data_format == ops._CH_LAST_STR else x.shape[2])
+        return ops.frame(x, frame_length, hop_length, pad_end, pad_value, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return (ops.frame_backward(g, *ctx.cfg),) + (None,) * 5
+
+
+class _Energy(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, frame_length, hop_length, pad_end, pad_value, scale, data_format):
+        ctx.save_for_backward(x)
+        ctx.cfg = (frame_length, hop_length, scale, data_format)
+        return ops.energy(x, frame_length, hop_length, pad_end, pad_value, scale, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        return (ops.energy_backward(x, g, *ctx.cfg),) + (None,) * 6
+
+
+class _ConcatFrequencyMap(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, data_format):
+        ctx.data_format = data_format
+        return ops.concat_frequency_map(x, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return ops.concat_frequency_map_backward(g, ctx.data_format), None
+
+
+class _SpecAugment(torch.autograd.Function):
+    """The backward pass is the forward launch over the gradient, with mask value 0 and the masks the forward drew
+    (saved on the device): it never draws new ones."""
+
+    @staticmethod
+    def forward(ctx, x, time_masks, freq_masks, mask_value, data_format):
+        ctx.save_for_backward(time_masks, freq_masks)
+        ctx.data_format = data_format
+        return ops.spec_augment_masked(x, time_masks, freq_masks, mask_value, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        tm, fm = ctx.saved_tensors
+        return ops.spec_augment_masked(g, tm, fm, 0.0, ctx.data_format), None, None, None, None
+
+
 # Entry points used by ``ops``.  Dtype conversions happen outside the Functions so that autograd casts the
 # gradient back to the caller's dtype.
 def stft_forward(x, plan, input_data_format, output_data_format, pad_begin, pad_end, mode, fb, db, workspace):
     x = x.float()
     if mode == N.OUT_COMPLEX:
         return _Stft.apply(x, plan, input_data_format, output_data_format, pad_begin, pad_end, workspace)
+    if mode == N.OUT_MAG_PHASE:
+        return _MagPhase.apply(x, plan, input_data_format, output_data_format, pad_begin, pad_end, db, workspace)
     return _FusedStack.apply(x, plan, input_data_format, output_data_format, pad_begin, pad_end, mode, fb, db,
                              workspace)
+
+
+def phase(X):
+    return _Phase.apply(X.to(torch.complex64))
+
+
+def delta(x, win_length, mode, data_format):
+    return _Delta.apply(x.float(), win_length, mode, data_format)
+
+
+def frame(x, frame_length, hop_length, pad_end, pad_value, data_format):
+    return _Frame.apply(x.float(), frame_length, hop_length, pad_end, pad_value, data_format)
+
+
+def energy(x, frame_length, hop_length, pad_end, pad_value, scale, data_format):
+    return _Energy.apply(x.float(), frame_length, hop_length, pad_end, pad_value, scale, data_format)
+
+
+def concat_frequency_map(x, data_format):
+    return _ConcatFrequencyMap.apply(x.float(), data_format)
+
+
+def spec_augment(x, time_masks, freq_masks, mask_value, data_format):
+    return _SpecAugment.apply(x.float(), time_masks, freq_masks, mask_value, data_format)
 
 
 def istft(X, plan, input_data_format, output_data_format):

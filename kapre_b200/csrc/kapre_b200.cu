@@ -23,6 +23,7 @@
 #include "tc_dft.cuh"
 #include "tc_mel.cuh"
 #include "grad_core.cuh"
+#include "grad_aux_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -269,15 +270,7 @@ __global__ void kb_spec_augment_kernel(const float* __restrict__ x, float* __res
 }
 
 // ---- adjacent layers: Delta / Frame / Energy (element-wise or small-window kernels, HBM-bound) ----
-__device__ __forceinline__ long long kb_pad_index(long long t, long long T, int mode) {
-    // index into [0, T) for an out-of-range t under tf.pad's SYMMETRIC (0) / REFLECT (1); -1 = zero (CONSTANT)
-    if (t >= 0 && t < T) return t;
-    if (mode == 2) return -1;
-    if (t < 0) t = (mode == 0) ? (-t - 1) : (-t);
-    else t = (mode == 0) ? (2 * T - 1 - t) : (2 * T - 2 - t);
-    return (t >= 0 && t < T) ? t : -1;
-}
-
+// kb_pad_index (tf.pad's extension of the time axis) lives in grad_aux_core.cuh: Delta's backward uses it too.
 __global__ void kb_delta_kernel(const float* __restrict__ x, float* __restrict__ y, long long outer, long long T,
                                 long long inner, int n, float inv_denom, int mode) {
     const long long total = outer * T * inner;
@@ -1714,6 +1707,40 @@ __global__ void __launch_bounds__(256) kb_dbb_kernel(const __grid_constant__ KbD
     else kb_dbb_share(p, item, i0, step);
 }
 
+// adjacent layers' backward passes (grad_aux_core.cuh): grid-stride loops over the gradient they write
+__global__ void kb_phase_bwd_kernel(const float2* __restrict__ X, const float* __restrict__ g, float2* __restrict__ gX,
+                                    long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_phase_bwd_elem(X, g, gX, i);
+}
+
+__global__ void kb_mag_phase_bwd_kernel(const __grid_constant__ KbMagPhaseBwdParams p, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_mag_phase_bwd_elem(p, i);
+}
+
+__global__ void kb_delta_bwd_kernel(const float* __restrict__ g, float* __restrict__ gx, long long T, long long inner,
+                                    int n, float inv_denom, int mode, long long total) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
+        kb_delta_bwd_elem(g, gx, T, inner, n, inv_denom, mode, i);
+}
+
+__global__ void kb_frame_bwd_kernel(const __grid_constant__ KbFrameBwdParams p, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_frame_bwd_elem(p, i);
+}
+
+__global__ void kb_energy_bwd_kernel(const __grid_constant__ KbFrameBwdParams p, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_energy_bwd_elem(p, i);
+}
+
+__global__ void kb_concat_fm_bwd_kernel(const float* __restrict__ g, float* __restrict__ gx, long long C, long long T,
+                                        long long F, int channels_last, long long n) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        kb_concat_fm_bwd_elem(g, gx, C, T, F, channels_last, i);
+}
+
 // padded-signal geometry of the STFT adjoint: frames, overlap-add length, and whether the overlap-add can be
 // written straight into gx (no pad in front and no sample past the signal's end)
 static void kb_stft_adj_geom(const kapre_stft_plan* p, int length, int pad_begin, int pad_end, int* T, long long* ola_len,
@@ -1857,6 +1884,144 @@ int kapre_magnitude_to_decibel_backward(const float* x_dev, const float* g_dev, 
     KB_CUDA(cudaGetLastError());
     g_launches += 3;
     KB_CUDA(cudaMemsetAsync(workspace_dev, 0, (size_t)n_items * 3 * sizeof(unsigned int), st));   // self-cleaning
+    return 0;
+}
+
+int kapre_phase_backward(const void* x_complex_dev, const float* g_dev, void* gx_complex_dev, int64_t n, void* stream) {
+    if (n < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (n == 0) return 0;
+    if (!x_complex_dev || !g_dev || !gx_complex_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    int grid, rc;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_phase_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float2*)x_complex_dev, g_dev, (float2*)gx_complex_dev, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+int kapre_mag_phase_backward(const void* x_complex_dev, const kapre_spec_desc* x_desc, const float* g_mag_dev,
+                             const kapre_spec_desc* gm_desc, const float* g_phase_dev, const kapre_spec_desc* gp_desc,
+                             void* gx_complex_dev, const kapre_spec_desc* gx_desc, int batch, int channels, int frames,
+                             int n_freq, void* stream) {
+    if (!x_desc || !gx_desc || (g_mag_dev && !gm_desc) || (g_phase_dev && !gp_desc))
+        return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (batch < 0 || channels < 0 || frames < 0 || n_freq < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    const long long n = (long long)batch * channels * frames * n_freq;
+    if (n == 0) return 0;
+    if (!x_complex_dev || !gx_complex_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if (gx_complex_dev == x_complex_dev) return kb_fail(KAPRE_E_INVALID, "gX must not alias X");
+    KbMagPhaseBwdParams p{};
+    p.X = (const float2*)x_complex_dev;
+    p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_st = x_desc->stride_t; p.x_sf = x_desc->stride_f;
+    p.gm = g_mag_dev;
+    if (gm_desc) { p.m_sb = gm_desc->stride_b; p.m_sc = gm_desc->stride_c; p.m_st = gm_desc->stride_t; p.m_sf = gm_desc->stride_f; }
+    p.gp = g_phase_dev;
+    if (gp_desc) { p.p_sb = gp_desc->stride_b; p.p_sc = gp_desc->stride_c; p.p_st = gp_desc->stride_t; p.p_sf = gp_desc->stride_f; }
+    p.gX = (float2*)gx_complex_dev;
+    p.o_sb = gx_desc->stride_b; p.o_sc = gx_desc->stride_c; p.o_st = gx_desc->stride_t; p.o_sf = gx_desc->stride_f;
+    p.C = channels; p.T = frames; p.F = n_freq;
+    p.c_inner = (channels > 1 && gx_desc->stride_c < gx_desc->stride_f) ? 1 : 0;   // channels_last: walk c fastest
+    int grid, rc;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_mag_phase_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+int kapre_delta_backward(const float* g_dev, float* gx_dev, int64_t outer, int64_t frames, int64_t inner, int win_length,
+                         int pad_mode, void* stream) {
+    if (win_length < 3 || (win_length & 1) == 0) return kb_fail(KAPRE_E_INVALID, "win_length must be odd and >= 3, got %d", win_length);
+    if (pad_mode < 0 || pad_mode > 2) return kb_fail(KAPRE_E_INVALID, "bad pad_mode %d", pad_mode);
+    if (outer < 0 || frames < 0 || inner < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    const long long total = (long long)outer * frames * inner;
+    if (total == 0) return 0;
+    if (!g_dev || !gx_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if (g_dev == gx_dev) return kb_fail(KAPRE_E_INVALID, "delta backward cannot run in place");
+    const int n = (win_length - 1) / 2;
+    double denom = 0;
+    for (int m = 1; m <= n; ++m) denom += 2.0 * m * m;
+    int grid, rc;
+    if ((rc = kb_ew_grid(total, &grid))) return rc;
+    kb_delta_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(g_dev, gx_dev, frames, inner, n, (float)(1.0 / denom),
+                                                              pad_mode, total);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+// the frame counts kapre_frame / kapre_energy give `length` samples (pad_end off, on): the gradient must have one of them
+static bool kb_frames_match(int length, int fl, int hop, int frames) {
+    return frames == kb_frames_for(length, fl, hop, 0) || frames == kb_frames_for(length, fl, hop, 1);
+}
+
+int kapre_frame_backward(const float* g_dev, const kapre_spec_desc* g_desc, int frames, int frame_length, int hop_length,
+                         float* gx_dev, const kapre_wave_desc* gx_desc, void* stream) {
+    if (!g_desc || !gx_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (frame_length <= 0 || hop_length <= 0) return kb_fail(KAPRE_E_INVALID, "frame_length and hop_length must be positive");
+    if (gx_desc->batch < 0 || gx_desc->channels < 0 || gx_desc->length < 0 || frames < 0)
+        return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (!kb_frames_match(gx_desc->length, frame_length, hop_length, frames))
+        return kb_fail(KAPRE_E_INVALID, "%d samples do not give %d frames of %d every %d", gx_desc->length, frames,
+                       frame_length, hop_length);
+    const long long n = (long long)gx_desc->batch * gx_desc->channels * gx_desc->length;
+    if (n == 0) return 0;
+    if (!gx_dev || (frames > 0 && !g_dev)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    KbFrameBwdParams p{};
+    p.g = g_dev; p.g_sb = g_desc->stride_b; p.g_sc = g_desc->stride_c; p.g_st = g_desc->stride_t; p.g_sn = g_desc->stride_f;
+    p.gx = gx_dev; p.o_sb = gx_desc->stride_b; p.o_sc = gx_desc->stride_c; p.o_sl = gx_desc->stride_l;
+    p.C = gx_desc->channels; p.L = gx_desc->length; p.T = frames; p.fl = frame_length; p.hop = hop_length;
+    int grid, rc;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_frame_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+int kapre_energy_backward(const float* x_dev, const kapre_wave_desc* x_desc, const float* g_dev,
+                          const kapre_wave_desc* g_desc, int frame_length, int hop_length, float scale, float* gx_dev,
+                          const kapre_wave_desc* gx_desc, void* stream) {
+    if (!x_desc || !g_desc || !gx_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (frame_length <= 0 || hop_length <= 0) return kb_fail(KAPRE_E_INVALID, "frame_length and hop_length must be positive");
+    if (x_desc->batch < 0 || x_desc->channels < 0 || x_desc->length < 0 || g_desc->length < 0)
+        return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (gx_desc->batch != x_desc->batch || gx_desc->channels != x_desc->channels || gx_desc->length != x_desc->length ||
+        g_desc->batch != x_desc->batch || g_desc->channels != x_desc->channels)
+        return kb_fail(KAPRE_E_INVALID, "x, g and gx descriptors disagree on batch / channels / length");
+    const int T = g_desc->length;
+    if (!kb_frames_match(x_desc->length, frame_length, hop_length, T))
+        return kb_fail(KAPRE_E_INVALID, "%d samples do not give %d frames of %d every %d", x_desc->length, T,
+                       frame_length, hop_length);
+    const long long n = (long long)x_desc->batch * x_desc->channels * x_desc->length;
+    if (n == 0) return 0;
+    if (!x_dev || !gx_dev || (T > 0 && !g_dev)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    KbFrameBwdParams p{};
+    p.g = g_dev; p.g_sb = g_desc->stride_b; p.g_sc = g_desc->stride_c; p.g_st = g_desc->stride_l;
+    p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_sl = x_desc->stride_l;
+    p.gx = gx_dev; p.o_sb = gx_desc->stride_b; p.o_sc = gx_desc->stride_c; p.o_sl = gx_desc->stride_l;
+    p.C = x_desc->channels; p.L = x_desc->length; p.T = T; p.fl = frame_length; p.hop = hop_length;
+    p.scale2 = 2.0f * scale;
+    int grid, rc;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_energy_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+int kapre_concat_frequency_map_backward(const float* g_dev, float* gx_dev, int64_t batch, int64_t channels,
+                                        int64_t frames, int64_t n_freq, int channels_last, void* stream) {
+    if (batch < 0 || channels < 0 || frames < 0 || n_freq < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    const long long n = (long long)batch * channels * frames * n_freq;
+    if (n == 0) return 0;
+    if (!g_dev || !gx_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    int grid, rc;
+    if ((rc = kb_ew_grid(n, &grid))) return rc;
+    kb_concat_fm_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(g_dev, gx_dev, channels, frames, n_freq,
+                                                                  channels_last ? 1 : 0, n);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
     return 0;
 }
 

@@ -255,7 +255,7 @@ def stft_forward(x: torch.Tensor, plan: StftPlan, input_data_format, output_data
     ``db`` = (ref_value, amin, dynamic_range); ``workspace``: caller-owned decibel scratch (``new_workspace``)."""
     if not x.is_cuda:
         raise N.KapreNativeError('stft_forward needs a CUDA tensor')
-    if _wants_grad(x) and mode != N.OUT_MAG_PHASE:
+    if _wants_grad(x):
         from . import autograd
         return autograd.stft_forward(x, plan, input_data_format, output_data_format, pad_begin, pad_end, mode, fb, db,
                                      workspace)
@@ -364,6 +364,9 @@ def magnitude(x: torch.Tensor):
 def phase(x: torch.Tensor):
     if not x.is_cuda:
         raise N.KapreNativeError('phase needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.phase(x)
     x = x.to(torch.complex64).contiguous()
     out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
     if out.numel():
@@ -469,6 +472,46 @@ def magnitude_to_decibel_backward(x: torch.Tensor, g: torch.Tensor, ref_value=1.
     return gx
 
 
+@_device_of_first_arg
+def phase_backward(X: torch.Tensor, g: torch.Tensor):
+    """Gradient of ``phase`` with respect to the complex64 tensor ``X``: ``g i X / |X|^2``, 0 where ``|X| = 0``."""
+    X = _raw(X.to(torch.complex64)).contiguous()
+    g = _raw(g.to(torch.float32)).contiguous()
+    if g.shape != X.shape:
+        raise ValueError('gradient shape %s does not match %s' % (tuple(g.shape), tuple(X.shape)))
+    gX = torch.empty_like(X)
+    if X.numel():
+        N.check(N.lib().kapre_phase_backward(_ptr(X), _ptr(g), _ptr(gX), X.numel(), _stream_ptr()))
+    return gX
+
+
+@_device_of_first_arg
+def mag_phase_backward(X: torch.Tensor, g_mag, g_phase, data_format):
+    """Gradient of the magnitude + phase pair of the complex spectrum ``X`` (``data_format`` layout, any strides)
+    with respect to ``X``: ``X / |X| (g_mag + i g_phase / |X|)``.  ``g_mag`` / ``g_phase``: float tensors of X's
+    shape (any strides, e.g. the two halves of the 2C-channel gradient), or None for zero."""
+    X = _raw(X.to(torch.complex64))
+    xd, (B, C, T, F) = _spec_desc(X, data_format)
+    gX, od = _spec_alloc(B, C, T, F, data_format, torch.complex64, X.device)
+    descs = []
+    for g in (g_mag, g_phase):
+        if g is None:
+            descs.append((None, None))
+            continue
+        g = _raw(g.to(torch.float32))
+        if g.shape != X.shape:
+            raise ValueError('gradient shape %s does not match %s' % (tuple(g.shape), tuple(X.shape)))
+        descs.append((g, _spec_desc(g, data_format)[0]))
+    if gX.numel() == 0:
+        return gX
+    (gm, gmd), (gp, gpd) = descs
+    N.check(N.lib().kapre_mag_phase_backward(
+        _ptr(X), ctypes.byref(xd), _ptr(gm) if gm is not None else None, ctypes.byref(gmd) if gmd is not None else None,
+        _ptr(gp) if gp is not None else None, ctypes.byref(gpd) if gpd is not None else None, _ptr(gX),
+        ctypes.byref(od), B, C, T, F, _stream_ptr()))
+    return gX
+
+
 # ------------------------------------------------------------------------------- adjacent layers
 _PAD_MODES = {'symmetric': 0, 'reflect': 1, 'constant': 2}
 
@@ -478,13 +521,11 @@ def delta(x: torch.Tensor, win_length: int, mode: str, data_format: str):
     """kapre.Delta along the time axis of (b, t, f, ch) / (b, ch, t, f)."""
     if not x.is_cuda:
         raise N.KapreNativeError('delta needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.delta(x, win_length, mode, data_format)
     x = x.float().contiguous()
-    if x.dim() != 4:
-        raise ValueError('Delta expects a 4-D batch, got shape %s' % (tuple(x.shape),))
-    if data_format == _CH_LAST_STR:
-        outer, frames, inner = x.shape[0], x.shape[1], x.shape[2] * x.shape[3]
-    else:
-        outer, frames, inner = x.shape[0] * x.shape[1], x.shape[2], x.shape[3]
+    outer, frames, inner = _delta_view(x, data_format)
     out = torch.empty_like(x)
     if x.numel():
         N.check(N.lib().kapre_delta(_ptr(x), _ptr(out), outer, frames, inner, int(win_length),
@@ -492,11 +533,35 @@ def delta(x: torch.Tensor, win_length: int, mode: str, data_format: str):
     return out
 
 
+def _delta_view(x, data_format):
+    """(outer, frames, inner) of a contiguous 4-D batch whose time axis is 1 (channels_last) or 2."""
+    if x.dim() != 4:
+        raise ValueError('Delta expects a 4-D batch, got shape %s' % (tuple(x.shape),))
+    if data_format == _CH_LAST_STR:
+        return x.shape[0], x.shape[1], x.shape[2] * x.shape[3]
+    return x.shape[0] * x.shape[1], x.shape[2], x.shape[3]
+
+
+@_device_of_first_arg
+def delta_backward(g: torch.Tensor, win_length: int, mode: str, data_format: str):
+    """Gradient of ``delta`` with respect to its input, given the gradient ``g`` of its output."""
+    g = _raw(g.to(torch.float32)).contiguous()
+    outer, frames, inner = _delta_view(g, data_format)
+    gx = torch.empty_like(g)
+    if g.numel():
+        N.check(N.lib().kapre_delta_backward(_ptr(g), _ptr(gx), outer, frames, inner, int(win_length),
+                                             _PAD_MODES[mode.lower()], _stream_ptr()))
+    return gx
+
+
 @_device_of_first_arg
 def concat_frequency_map(x: torch.Tensor, data_format: str):
     """kapre.ConcatenateFrequencyMap: (b, t, f, ch) -> (b, t, f, ch + 1) or (b, ch, t, f) -> (b, ch + 1, t, f)."""
     if not x.is_cuda:
         raise N.KapreNativeError('concat_frequency_map needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.concat_frequency_map(x, data_format)
     x = x.float().contiguous()
     if x.dim() != 4:
         raise ValueError('ConcatenateFrequencyMap expects a 4-D batch, got shape %s' % (tuple(x.shape),))
@@ -517,18 +582,36 @@ def spec_augment(x: torch.Tensor, time_masks: np.ndarray, freq_masks: np.ndarray
     """kapre.SpecAugment with given masks: x (b, t, f, 1) or (b, 1, t, f); masks (b, n, 2) int32 (start, width)."""
     if not x.is_cuda:
         raise N.KapreNativeError('spec_augment needs a CUDA tensor')
-    x = x.float().contiguous()
+    B, _, _ = _spec_augment_dims(x, data_format)
+    if x.numel() == 0:
+        return torch.empty_like(x, dtype=torch.float32)
+    tm = torch.as_tensor(np.ascontiguousarray(time_masks, dtype=np.int32).reshape(B, -1, 2)).to(x.device)
+    fm = torch.as_tensor(np.ascontiguousarray(freq_masks, dtype=np.int32).reshape(B, -1, 2)).to(x.device)
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.spec_augment(x, tm, fm, mask_value, data_format)
+    return spec_augment_masked(x, tm, fm, mask_value, data_format)
+
+
+def _spec_augment_dims(x, data_format):
     if data_format == _CH_LAST_STR:
         B, T, F, C = x.shape
     else:
         B, C, T, F = x.shape
     if C != 1:
         raise RuntimeError('SpecAugment does not support spectrograms with depth greater than 1')
+    return B, T, F
+
+
+@_device_of_first_arg
+def spec_augment_masked(x: torch.Tensor, tm: torch.Tensor, fm: torch.Tensor, mask_value: float, data_format: str):
+    """The masking launch of ``spec_augment`` with device masks ``tm`` / ``fm`` ((b, n, 2) int32).  Run on a gradient
+    with ``mask_value`` 0 and the forward's masks, it is the layer's backward pass."""
+    x = _raw(x.float()).contiguous()
+    B, T, F = _spec_augment_dims(x, data_format)
     out = torch.empty_like(x)
     if x.numel() == 0:
         return out
-    tm = torch.as_tensor(np.ascontiguousarray(time_masks, dtype=np.int32).reshape(B, -1, 2)).to(x.device)
-    fm = torch.as_tensor(np.ascontiguousarray(freq_masks, dtype=np.int32).reshape(B, -1, 2)).to(x.device)
     N.check(N.lib().kapre_spec_augment(_ptr(x), _ptr(out), B, T, F, _ptr(tm) if tm.numel() else None, tm.shape[1],
                                        _ptr(fm) if fm.numel() else None, fm.shape[1], ctypes.c_float(mask_value), _stream_ptr()))
     return out
@@ -543,6 +626,9 @@ def frame(x: torch.Tensor, frame_length, hop_length, pad_end, pad_value, data_fo
     """kapre.Frame: (b, t, ch) -> (b, frames, frame_length, ch) or (b, ch, t) -> (b, ch, frames, frame_length)."""
     if not x.is_cuda:
         raise N.KapreNativeError('frame needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.frame(x, frame_length, hop_length, pad_end, pad_value, data_format)
     x = x.float()
     xd, (B, C, L) = _wave_desc(x, data_format)
     T = _frames_for(L, frame_length, hop_length, pad_end)
@@ -558,6 +644,9 @@ def energy(x: torch.Tensor, frame_length, hop_length, pad_end, pad_value, scale,
     """kapre.Energy: scale * sum of squares per frame; (b, t, ch) -> (b, frames, ch), (b, ch, t) -> (b, ch, frames)."""
     if not x.is_cuda:
         raise N.KapreNativeError('energy needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.energy(x, frame_length, hop_length, pad_end, pad_value, scale, data_format)
     x = x.float()
     xd, (B, C, L) = _wave_desc(x, data_format)
     T = _frames_for(L, frame_length, hop_length, pad_end)
@@ -573,3 +662,68 @@ def energy(x: torch.Tensor, frame_length, hop_length, pad_end, pad_value, scale,
                                      ctypes.c_float(pad_value), ctypes.c_float(scale), _ptr(out), ctypes.byref(od),
                                      _stream_ptr()))
     return out
+
+
+def _wave_grad_alloc(B, C, L, data_format, device):
+    """Contiguous (B, L, C) / (B, C, L) float32 waveform gradient and its descriptor."""
+    if data_format == _CH_LAST_STR:
+        gx = torch.empty((B, L, C), dtype=torch.float32, device=device)
+        sb, sl, sc = gx.stride()
+    else:
+        gx = torch.empty((B, C, L), dtype=torch.float32, device=device)
+        sb, sc, sl = gx.stride()
+    return gx, N.WaveDesc(B, C, L, sb, sc, sl)
+
+
+@_device_of_first_arg
+def frame_backward(g: torch.Tensor, frame_length, hop_length, data_format, length):
+    """Gradient of ``frame`` with respect to its waveform of ``length`` samples, given the gradient ``g`` of the
+    frames (any strides)."""
+    g = _raw(g.to(torch.float32))
+    gd, (B, C, T, _) = _spec_desc(g, data_format)
+    gx, xd = _wave_grad_alloc(B, C, int(length), data_format, g.device)
+    if gx.numel():
+        N.check(N.lib().kapre_frame_backward(_ptr(g), ctypes.byref(gd), T, int(frame_length), int(hop_length), _ptr(gx),
+                                             ctypes.byref(xd), _stream_ptr()))
+    return gx
+
+
+@_device_of_first_arg
+def energy_backward(x: torch.Tensor, g: torch.Tensor, frame_length, hop_length, scale, data_format):
+    """Gradient of ``energy`` with respect to its float32 input ``x``, given the gradient ``g`` of the per-frame
+    energies (any strides)."""
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    g = _raw(g.to(torch.float32))
+    if g.dim() != 3:
+        raise ValueError('energy gradient must be 3-D, got shape %s' % (tuple(g.shape),))
+    if data_format == _CH_LAST_STR:
+        sb, st, sc = g.stride()
+        T = g.shape[1]
+    else:
+        sb, sc, st = g.stride()
+        T = g.shape[2]
+    gd = N.WaveDesc(B, C, T, sb, sc, st)
+    gx, od = _wave_grad_alloc(B, C, L, data_format, x.device)
+    if gx.numel():
+        N.check(N.lib().kapre_energy_backward(_ptr(x), ctypes.byref(xd), _ptr(g), ctypes.byref(gd), int(frame_length),
+                                              int(hop_length), ctypes.c_float(scale), _ptr(gx), ctypes.byref(od),
+                                              _stream_ptr()))
+    return gx
+
+
+@_device_of_first_arg
+def concat_frequency_map_backward(g: torch.Tensor, data_format):
+    """Gradient of ``concat_frequency_map`` with respect to its input: the first C of the C + 1 channels of ``g``."""
+    g = _raw(g.to(torch.float32)).contiguous()
+    if g.dim() != 4:
+        raise ValueError('ConcatenateFrequencyMap gradient must be 4-D, got shape %s' % (tuple(g.shape),))
+    cl = data_format == _CH_LAST_STR
+    if cl:
+        B, T, F, C1 = g.shape
+        gx = torch.empty((B, T, F, C1 - 1), dtype=torch.float32, device=g.device)
+    else:
+        B, C1, T, F = g.shape
+        gx = torch.empty((B, C1 - 1, T, F), dtype=torch.float32, device=g.device)
+    if gx.numel():
+        N.check(N.lib().kapre_concat_frequency_map_backward(_ptr(g), _ptr(gx), B, C1 - 1, T, F, int(cl), _stream_ptr()))
+    return gx
