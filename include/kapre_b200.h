@@ -227,6 +227,28 @@ int kapre_frame(const float* x_dev, const kapre_wave_desc* x_desc, int frame_len
 int kapre_energy(const float* x_dev, const kapre_wave_desc* x_desc, int frame_length, int hop_length, int pad_end,
                  float pad_value, float scale, float* out_dev, const kapre_wave_desc* out_desc, void* stream);
 
+/* ---- resampling ------------------------------------------------------------------------------
+ * Polyphase resampler, scipy.signal.resample_poly(x, up, down) with zeros outside the signal:
+ *   y[n] = up * sum_i x[i] h[hl + n*down - i*up]   (h: n_taps = 2*hl + 1 taps, terms outside h are zero).
+ * `taps_host`: the n_taps float32 filter taps (host memory), e.g. kapre_b200.signal.resample_filter(up, down), the
+ * windowed sinc firwin(20 max(up, down) + 1, 1 / max(up, down), window=('kaiser', 5.0)).  up and down must be
+ * coprime and max(up, down) <= 1280 (every pair of 8, 11.025, 16, 22.05, 24, 32, 44.1, 48, 88.2 and 96 kHz);
+ * larger ratios return KAPRE_E_UNSUPPORTED, because the polyphase table (up to 143 KB) must fit in shared memory. */
+typedef struct kapre_resample_plan kapre_resample_plan;
+int kapre_resample_plan_create(int up, int down, const float* taps_host, int n_taps, kapre_resample_plan** out);
+void kapre_resample_plan_destroy(kapre_resample_plan* plan);
+/* ceil(length * up / down): the output length of scipy.signal.resample_poly. */
+int64_t kapre_resample_output_length(const kapre_resample_plan* plan, int64_t length);
+/* Resample along the sample axis.  y_desc has x_desc's batch and channels; y_desc->length outputs are written
+ * (normally kapre_resample_output_length(x_desc->length)).  Any strides; y must not overlap x. */
+int kapre_resample(const kapre_resample_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* y_dev,
+                   const kapre_wave_desc* y_desc, void* stream);
+/* Gradient of kapre_resample: gx = (up / down) * resample(g; down, up), cropped to gx_desc->length samples (the
+ * length the forward call saw).  This is the adjoint because the filter is symmetric (KAPRE_E_UNSUPPORTED
+ * otherwise).  Runs the forward kernel of an adjoint plan (made on first use, freed with `plan`). */
+int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
+                            float* gx_dev, const kapre_wave_desc* gx_desc, void* stream);
+
 /* ---- misc ---------------------------------------------------------------------------------- */
 const char* kapre_last_error(void);
 int kapre_version(void);

@@ -76,6 +76,11 @@ SYMBOLS = [
     ('kapre_energy', c_int, [c_void_p, POINTER(WaveDesc), c_int, c_int, c_int, c_float, c_float, c_void_p, POINTER(WaveDesc), c_void_p]),
     ('kapre_concat_frequency_map', c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p]),
     ('kapre_spec_augment', c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p]),
+    ('kapre_resample_plan_create', c_int, [c_int, c_int, c_void_p, c_int, POINTER(c_void_p)]),
+    ('kapre_resample_plan_destroy', None, [c_void_p]),
+    ('kapre_resample_output_length', c_int64, [c_void_p, c_int64]),
+    ('kapre_resample', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p]),
+    ('kapre_resample_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p]),
     ('kapre_last_error', c_char_p, []),
     ('kapre_version', c_int, []),
     ('kapre_launch_count', c_uint64, []),

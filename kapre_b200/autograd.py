@@ -15,6 +15,7 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * Frame, Energy   -> ``kapre_frame_backward``, ``kapre_energy_backward`` (sum over the frames covering a sample)
 * ConcatenateFrequencyMap -> ``kapre_concat_frequency_map_backward`` (the first C channels)
 * SpecAugment     -> ``kapre_spec_augment`` over the gradient, mask value 0, the forward's device masks
+* Resample        -> ``kapre_resample_backward`` (the resampling kernel with up and down exchanged)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
 only the waveform and recomputes the complex spectrum and the pre-decibel values in its backward; so does
@@ -222,6 +223,18 @@ class _ConcatFrequencyMap(torch.autograd.Function):
         return ops.concat_frequency_map_backward(g, ctx.data_format), None
 
 
+class _Resample(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, plan, data_format):
+        ctx.cfg = (plan, data_format, x.shape[1] if data_format == ops._CH_LAST_STR else x.shape[2])
+        return ops.resample(x, plan, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return ops.resample_backward(g, *ctx.cfg), None, None
+
+
 class _SpecAugment(torch.autograd.Function):
     """The backward pass is the forward launch over the gradient, with mask value 0 and the masks the forward drew
     (saved on the device): it never draws new ones."""
@@ -273,6 +286,10 @@ def concat_frequency_map(x, data_format):
 
 def spec_augment(x, time_masks, freq_masks, mask_value, data_format):
     return _SpecAugment.apply(x.float(), time_masks, freq_masks, mask_value, data_format)
+
+
+def resample(x, plan, data_format):
+    return _Resample.apply(x.float(), plan, data_format)
 
 
 def istft(X, plan, input_data_format, output_data_format):

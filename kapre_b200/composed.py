@@ -18,6 +18,7 @@ import torch
 from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
+from .signal import Resample
 from .time_frequency import (STFT, ApplyFilterbank, InverseSTFT, Layer, Magnitude, MagnitudeToDecibel, Phase,
                              get_registered_object)
 
@@ -82,10 +83,10 @@ class Sequential(Layer):
         self.layers.append(layer)
 
     # -- fusion -----------------------------------------------------------------------------
-    def _fused_prefix(self):
-        """(n_layers_consumed, mode, stft, filterbank_layer, db_layer) for the longest leading
-        run that one fused launch covers, or None."""
-        ls = self.layers
+    def _fused_prefix(self, start=0):
+        """(n_layers_consumed, mode, stft, filterbank_layer, db_layer) for the longest run from
+        ``layers[start]`` on that one fused launch covers, or None."""
+        ls = self.layers[start:]
         if not self.fuse or len(ls) < 2 or type(ls[0]) is not STFT or type(ls[1]) is not Magnitude:
             return None
         stft = ls[0]
@@ -103,7 +104,11 @@ class Sequential(Layer):
 
     def call(self, x):
         start = 0
-        fused = self._fused_prefix() if (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3) else None
+        # Leading Resample layers run first, so that the STFT stack behind them still takes the fused launch.
+        while start < len(self.layers) and type(self.layers[start]) is Resample:
+            x = self.layers[start].call(x)
+            start += 1
+        fused = self._fused_prefix(start) if (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3) else None
         if fused is not None:
             n, mode, stft, fbl, dbl = fused
             db = None
@@ -118,7 +123,7 @@ class Sequential(Layer):
                 db = (dbl.ref_value, dbl.amin, dbl.dynamic_range)
             x = ops.stft_forward(x, stft.plan, stft.input_data_format, stft.output_data_format, stft.pad_begin,
                                  stft.pad_end, mode, fbl.fb if fbl is not None else None, db)
-            start = n
+            start += n
         for layer in self.layers[start:]:
             x = layer.call(x)
         return x

@@ -24,6 +24,7 @@
 #include "tc_mel.cuh"
 #include "grad_core.cuh"
 #include "grad_aux_core.cuh"
+#include "resample_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -2023,6 +2024,164 @@ int kapre_concat_frequency_map_backward(const float* g_dev, float* gx_dev, int64
     KB_CUDA(cudaGetLastError());
     g_launches++;
     return 0;
+}
+
+}  // extern "C"
+
+// ---- polyphase resampler (resample_core.cuh) ------------------------------------------------------
+__global__ void __launch_bounds__(KB_RESAMPLE_THREADS) kb_resample_kernel(const __grid_constant__ KbResampleParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_resample_cta(p, kb_smem, (int)blockIdx.x, (int)gridDim.x);
+}
+
+struct kapre_resample_plan {
+    int up, down, n_taps, hl, f, Kp;
+    int symmetric;
+    DevInfo dev;
+    float* tab = nullptr;       // up rows of Kp taps, gain folded in (resample_core.cuh)
+    std::vector<float> taps_host;
+    // adjoint (kapre_resample_backward): up and down exchanged, gain up; made on first use
+    std::mutex adj_mu;
+    kapre_resample_plan* adj = nullptr;
+};
+
+static long long kb_gcd(long long a, long long b) {
+    while (b) { const long long t = a % b; a = b; b = t; }
+    return a;
+}
+
+static int kb_resample_plan_build(int up, int down, const float* taps, int n_taps, double gain, kapre_resample_plan** out) {
+    kapre_resample_plan* p = new kapre_resample_plan();
+    p->up = up; p->down = down; p->n_taps = n_taps;
+    p->hl = (n_taps - 1) / 2;
+    p->f = p->hl / up;
+    p->Kp = kb_resample_kp(up, n_taps);
+    p->taps_host.assign(taps, taps + n_taps);
+    p->symmetric = 1;
+    for (int k = 0; k < n_taps; ++k)
+        if (taps[k] != taps[n_taps - 1 - k]) p->symmetric = 0;
+    int rc = kb_dev_info(&p->dev);
+    if (rc) { delete p; return rc; }
+    if (kb_resample_smem(up, p->Kp, 1, down, 1) > p->dev.smem_optin) {
+        const int need = up * p->Kp * 4;
+        kapre_resample_plan_destroy(p);
+        return kb_fail(KAPRE_E_UNSUPPORTED, "resampling table of %d x %d taps (%d B) does not fit in shared memory", up,
+                       need / 4 / up, need);
+    }
+    std::vector<float> tab;
+    kb_resample_table(up, down, taps, n_taps, gain, tab);
+    if ((rc = kb_upload(tab, &p->tab))) { kapre_resample_plan_destroy(p); return rc; }
+    *out = p;
+    return 0;
+}
+
+// Largest tile (outputs, a power of two <= 2048) whose staged span fits beside the table: in half of the opt-in
+// shared memory when possible, so that two CTAs share an SM, else in all of it.
+static int kb_resample_pick_nt(const kapre_resample_plan* p, int G) {
+    for (int budget : {p->dev.smem_optin / 2 - 1024, p->dev.smem_optin})
+        for (int nt = 2048; nt >= 1; nt /= 2)
+            if (kb_resample_smem(p->up, p->Kp, nt, p->down, G) <= budget) return nt;
+    return 0;
+}
+
+static int kb_resample_launch(const kapre_resample_plan* plan, const float* x_dev, const kapre_wave_desc* xd, float* y_dev,
+                              const kapre_wave_desc* yd, void* stream) {
+    if (!plan || !xd || !yd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (xd->batch < 0 || xd->channels < 0 || xd->length < 0 || yd->length < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (yd->batch != xd->batch || yd->channels != xd->channels)
+        return kb_fail(KAPRE_E_INVALID, "input and output descriptors disagree on batch / channels");
+    if ((long long)yd->batch * yd->channels * yd->length == 0) return 0;
+    if (!x_dev || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)x_dev == (const void*)y_dev) return kb_fail(KAPRE_E_INVALID, "resampling cannot run in place");
+    int cur = -1;
+    KB_CUDA(cudaGetDevice(&cur));
+    if (cur != plan->dev.device)
+        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    KbResampleParams p{};
+    const int B = xd->batch, C = xd->channels;
+    p.x = x_dev; p.x_sb = xd->stride_b; p.x_sc = xd->stride_c; p.x_sl = xd->stride_l;
+    p.B = B; p.C = C; p.L = xd->length;
+    p.y = y_dev; p.y_sb = yd->stride_b; p.y_sc = yd->stride_c; p.y_sl = yd->stride_l;
+    p.L_out = yd->length;
+    p.tab = plan->tab; p.up = plan->up; p.down = plan->down; p.f = plan->f; p.Kp = plan->Kp;
+    // channel-interleaved input: all channels in one tile
+    const bool interleaved = C > 1 && C <= KB_RESAMPLE_THREADS && llabs(xd->stride_c) < llabs(xd->stride_l);
+    p.G = interleaved ? C : 1;
+    const bool nonneg = xd->stride_b >= 0 && xd->stride_c >= 0 && xd->stride_l >= 0;
+    p.x_numel = (B > 0 && C > 0 && p.L > 0)
+        ? (long long)(B - 1) * xd->stride_b + (long long)(C - 1) * xd->stride_c + (long long)(p.L - 1) * xd->stride_l + 1 : 0;
+    p.x_align = (unsigned)(((uintptr_t)x_dev >> 2) & 3u);
+    p.bulk_ok = nonneg && (((uintptr_t)x_dev & 3u) == 0) &&
+                (p.G == 1 ? xd->stride_l == 1 : (xd->stride_c == 1 && xd->stride_l == C)) ? 1 : 0;
+    p.NT = kb_resample_pick_nt(plan, p.G);
+    if (p.NT == 0)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "%d channels of a %d:%d resampler do not fit in shared memory", p.G, plan->up, plan->down);
+    if (!kb_resample_setup(p, KB_RESAMPLE_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
+    const long long tiles = p.n_tiles;
+    const int smem = kb_resample_smem(p.up, p.Kp, p.NT, p.down, p.G);
+    KB_CUDA(cudaFuncSetAttribute(kb_resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    int per_sm = 0;
+    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kb_resample_kernel, KB_RESAMPLE_THREADS, smem));
+    if (per_sm < 1) per_sm = 1;
+    const long long cap = (long long)plan->dev.sm_count * per_sm;
+    const int grid = (int)(tiles < cap ? tiles : cap);
+    {
+        KbProfScope prof((cudaStream_t)stream);
+        kb_resample_kernel<<<grid, KB_RESAMPLE_THREADS, smem, (cudaStream_t)stream>>>(p);
+    }
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+extern "C" {
+
+int kapre_resample_plan_create(int up, int down, const float* taps_host, int n_taps, kapre_resample_plan** out) {
+    if (!out || !taps_host) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (up < 1 || down < 1) return kb_fail(KAPRE_E_INVALID, "up=%d and down=%d must be positive", up, down);
+    if (kb_gcd(up, down) != 1) return kb_fail(KAPRE_E_INVALID, "up=%d and down=%d must be coprime (divide both by their gcd)", up, down);
+    if (n_taps < 1 || (n_taps & 1) == 0) return kb_fail(KAPRE_E_INVALID, "n_taps=%d must be odd", n_taps);
+    const int M = up > down ? up : down;
+    if (M > KB_RESAMPLE_MAX_M)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "resampling by %d/%d is not supported: max(up, down) = %d exceeds %d (the "
+                       "anti-aliasing filter of %d taps would not fit in shared memory)", up, down, M, KB_RESAMPLE_MAX_M,
+                       20 * M + 1);
+    return kb_resample_plan_build(up, down, taps_host, n_taps, (double)up, out);
+}
+
+void kapre_resample_plan_destroy(kapre_resample_plan* p) {
+    if (!p) return;
+    cudaFree(p->tab);
+    kapre_resample_plan_destroy(p->adj);
+    delete p;
+}
+
+int64_t kapre_resample_output_length(const kapre_resample_plan* plan, int64_t length) {
+    if (!plan || length < 0) return kb_fail(KAPRE_E_INVALID, "bad argument");
+    return (length * plan->up + plan->down - 1) / plan->down;
+}
+
+int kapre_resample(const kapre_resample_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* y_dev,
+                   const kapre_wave_desc* y_desc, void* stream) {
+    return kb_resample_launch(plan, x_dev, x_desc, y_dev, y_desc, stream);
+}
+
+int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
+                            float* gx_dev, const kapre_wave_desc* gx_desc, void* stream) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (!plan->symmetric) return kb_fail(KAPRE_E_UNSUPPORTED, "the resampling backward pass needs a symmetric filter");
+    kapre_resample_plan* p = const_cast<kapre_resample_plan*>(plan);
+    kapre_resample_plan* adj;
+    {
+        std::lock_guard<std::mutex> lk(p->adj_mu);
+        if (!p->adj) {
+            // A^T g = (up / down) resample(g; down, up): gain down of the exchanged plan times up / down
+            int rc = kb_resample_plan_build(p->down, p->up, p->taps_host.data(), p->n_taps, (double)p->up, &p->adj);
+            if (rc) { p->adj = nullptr; return rc; }
+        }
+        adj = p->adj;
+    }
+    return kb_resample_launch(adj, g_dev, g_desc, gx_dev, gx_desc, stream);
 }
 
 }  // extern "C"

@@ -214,6 +214,35 @@ class Filterbank:
         return h.ptr
 
 
+class ResamplePlan:
+    """kapre_resample_plan per CUDA device for one (up, down, filter)."""
+
+    def __init__(self, up, down, taps: np.ndarray):
+        self.up, self.down = int(up), int(down)
+        self.taps = np.ascontiguousarray(taps, dtype=np.float32)
+        if self.taps.ndim != 1:
+            raise ValueError('resampling filter must be 1-D, got shape %s' % (self.taps.shape,))
+        self._per_device = {}
+
+    def handle(self):
+        _require_cuda()
+        dev = torch.cuda.current_device()
+        with _lock:
+            h = self._per_device.get(dev)
+            if h is None:
+                lib = N.lib()
+                out = ctypes.c_void_p()
+                N.check(lib.kapre_resample_plan_create(self.up, self.down, self.taps.ctypes.data_as(ctypes.c_void_p),
+                                                       self.taps.size, ctypes.byref(out)))
+                h = _Handle(out, lib.kapre_resample_plan_destroy)
+                self._per_device[dev] = h
+        return h.ptr
+
+    def output_length(self, length):
+        """ceil(length * up / down), the output length of ``scipy.signal.resample_poly``."""
+        return -(-int(length) * self.up // self.down)
+
+
 def _wave_desc(t: torch.Tensor, data_format: str):
     """(B, L, C) channels_last or (B, C, L) channels_first -> kapre_wave_desc."""
     if t.dim() != 3:
@@ -708,6 +737,36 @@ def energy_backward(x: torch.Tensor, g: torch.Tensor, frame_length, hop_length, 
         N.check(N.lib().kapre_energy_backward(_ptr(x), ctypes.byref(xd), _ptr(g), ctypes.byref(gd), int(frame_length),
                                               int(hop_length), ctypes.c_float(scale), _ptr(gx), ctypes.byref(od),
                                               _stream_ptr()))
+    return gx
+
+
+@_device_of_first_arg
+def resample(x: torch.Tensor, plan: ResamplePlan, data_format):
+    """Polyphase resampling along the time axis of (b, t, ch) / (b, ch, t): ``scipy.signal.resample_poly(x, up, down)``."""
+    if not x.is_cuda:
+        raise N.KapreNativeError('resample needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.resample(x, plan, data_format)
+    if x.dtype != torch.float32:
+        x = x.float()
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    y, yd = _wave_grad_alloc(B, C, plan.output_length(L), data_format, x.device)
+    if y.numel():
+        N.check(N.lib().kapre_resample(plan.handle(), _ptr(x), ctypes.byref(xd), _ptr(y), ctypes.byref(yd), _stream_ptr()))
+    return y
+
+
+@_device_of_first_arg
+def resample_backward(g: torch.Tensor, plan: ResamplePlan, data_format, length):
+    """Gradient of ``resample`` with respect to its input of ``length`` samples, given the gradient ``g`` of its
+    output (any strides)."""
+    g = _raw(g.to(torch.float32))
+    gd, (B, C, _) = _wave_desc(g, data_format)
+    gx, xd = _wave_grad_alloc(B, C, int(length), data_format, g.device)
+    if gx.numel():
+        N.check(N.lib().kapre_resample_backward(plan.handle(), _ptr(g), ctypes.byref(gd), _ptr(gx), ctypes.byref(xd),
+                                                _stream_ptr()))
     return gx
 
 

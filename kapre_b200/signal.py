@@ -1,8 +1,11 @@
 """Mirrors of the waveform-side layers of ``kapre/signal.py`` that sit next to the hot path
 ``Frame`` (reference :22-119), ``Energy`` (:123-233) and ``LogmelToMFCC``
 (:365-447).  Same constructor arguments, validation and ``get_config`` keys; ``call`` runs CUDA
-kernels through the C ABI."""
+kernels through the C ABI.  ``Resample`` (polyphase sample-rate conversion) has no counterpart in the
+reference, which expects audio to be resampled before it reaches the model."""
 from __future__ import annotations
+
+import math
 
 import numpy as np
 
@@ -10,7 +13,7 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
-__all__ = ['Frame', 'Energy', 'LogmelToMFCC']
+__all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample']
 
 
 def _resolve(fmt):
@@ -79,6 +82,59 @@ class Energy(Layer):
         ('hop_length', 'hop_length'),
         ('pad_end', 'pad_end'),
         ('pad_value', 'pad_value'),
+        ('data_format', 'data_format_str'),
+    )
+
+
+def resample_filter(up: int, down: int) -> np.ndarray:
+    """The anti-aliasing filter of ``scipy.signal.resample_poly`` with its default window:
+    ``firwin(2 hl + 1, 1 / M, window=('kaiser', 5.0))`` with ``M = max(up, down)``, ``hl = 10 M``, i.e. the
+    Kaiser-windowed ``sinc((k - hl) / M) / M`` normalised to unit sum.  Computed in float64, returned as float32."""
+    M = max(int(up), int(down))
+    hl = 10 * M
+    n = 2 * hl + 1
+    k = np.arange(n, dtype=np.float64)
+    h = np.sinc((k - hl) / M) / M * np.kaiser(n, 5.0)
+    h = 0.5 * (h + h[::-1])         # exactly symmetric: the backward pass relies on it
+    return (h / h.sum()).astype(np.float32)
+
+
+def _positive_int(name, v):
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v <= 0:
+        raise ValueError('%s must be a positive integer, got: %r' % (name, v))
+    return int(v)
+
+
+@register_keras_serializable(package='Kapre')
+class Resample(Layer):
+    """Sample-rate conversion along the time axis: ``scipy.signal.resample_poly(x, up, down)`` with its default
+    Kaiser (beta 5) filter and zeros outside the signal, ``up / down = target_sample_rate / orig_sample_rate``
+    reduced.  ``(batch, time, ch)`` -> ``(batch, ceil(time * up / down), ch)`` or the same with ``(batch, ch, time)``.
+    Equal rates return the input unchanged.  Supports every ratio with ``max(up, down) <= 1280``, which includes
+    every pair of 8, 11.025, 16, 22.05, 24, 32, 44.1, 48, 88.2 and 96 kHz."""
+
+    def __init__(self, orig_sample_rate, target_sample_rate, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        self.orig_sample_rate = _positive_int('orig_sample_rate', orig_sample_rate)
+        self.target_sample_rate = _positive_int('target_sample_rate', target_sample_rate)
+        g = math.gcd(self.orig_sample_rate, self.target_sample_rate)
+        self.up, self.down = self.target_sample_rate // g, self.orig_sample_rate // g
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+        self.plan = None if self.up == self.down else ops.ResamplePlan(self.up, self.down,
+                                                                      resample_filter(self.up, self.down))
+
+    def call(self, x):
+        if x.dim() != 3:
+            raise ValueError('Resample expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        if self.plan is None:
+            return x
+        return ops.resample(x, self.plan, self.data_format)
+
+    _config_fields = (
+        ('orig_sample_rate', 'orig_sample_rate'),
+        ('target_sample_rate', 'target_sample_rate'),
         ('data_format', 'data_format_str'),
     )
 
