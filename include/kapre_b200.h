@@ -249,6 +249,35 @@ int kapre_resample(const kapre_resample_plan* plan, const float* x_dev, const ka
 int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
                             float* gx_dev, const kapre_wave_desc* gx_desc, void* stream);
 
+/* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
+ * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
+ * processed along time:
+ *   M[-1] = E[0],  M[t] = (1 - s) M[t-1] + s E[t],  y[t] = d^r expm1(r log1p(E[t] (eps + M[t])^-a / d))
+ * with a = gain, d = bias, r = power, s = smooth_coef.  Each parameter is a device pointer with an element
+ * stride of 0 (one value for every band) or 1 (one value per band); values are used as given (no clamping). */
+typedef struct {
+    const float *gain, *bias, *power, *smooth;
+    int gain_stride, bias_stride, power_stride, smooth_stride;
+    float eps;
+} kapre_pcen_params;
+/* The time chunking a call on the current device uses for this shape (`*chunks`, >= 1) and the device scratch it
+ * needs (`*workspace_bytes`: chunks x batch x channels x bands floats when chunks > 1, else 0).  The same shape
+ * gives the same chunking on the same device, so the numbers hold for both kapre_pcen and kapre_pcen_backward. */
+int kapre_pcen_workspace(int batch, int channels, int frames, int bands, int* chunks, int64_t* workspace_bytes);
+/* y = PCEN(E).  `M_dev` (nullable): also write the smoother state M, which kapre_pcen_backward reads.  y and M must
+ * not overlap E.  `workspace_dev`: kapre_pcen_workspace's bytes (NULL when 0). */
+int kapre_pcen(const float* E_dev, const kapre_spec_desc* E_desc, int batch, int channels, int frames, int bands,
+               const kapre_pcen_params* params, float* y_dev, const kapre_spec_desc* y_desc, float* M_dev,
+               const kapre_spec_desc* M_desc, void* workspace_dev, void* stream);
+/* Gradient of kapre_pcen given E, the M it wrote and the output gradient gy: writes gE (every element once) and
+ * the parameter partial sums `param_partials_dev`, a contiguous (4, chunks, batch, channels, bands) float array
+ * (gain, bias, power, smooth_coef; chunks from kapre_pcen_workspace).  Summed over chunks, batch and channels they
+ * give the per-band gradients, summed over bands as well the gradient of a shared parameter. */
+int kapre_pcen_backward(const float* E_dev, const kapre_spec_desc* E_desc, const float* M_dev,
+                        const kapre_spec_desc* M_desc, const float* gy_dev, const kapre_spec_desc* gy_desc, int batch,
+                        int channels, int frames, int bands, const kapre_pcen_params* params, float* gE_dev,
+                        const kapre_spec_desc* gE_desc, float* param_partials_dev, void* workspace_dev, void* stream);
+
 /* ---- misc ---------------------------------------------------------------------------------- */
 const char* kapre_last_error(void);
 int kapre_version(void);

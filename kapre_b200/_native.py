@@ -29,6 +29,12 @@ class SpecDesc(Structure):
                 ('stride_f', c_int64)]
 
 
+class PcenParams(Structure):
+    _fields_ = [('gain', c_void_p), ('bias', c_void_p), ('power', c_void_p), ('smooth', c_void_p),
+                ('gain_stride', c_int), ('bias_stride', c_int), ('power_stride', c_int), ('smooth_stride', c_int),
+                ('eps', c_float)]
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -81,6 +87,12 @@ SYMBOLS = [
     ('kapre_resample_output_length', c_int64, [c_void_p, c_int64]),
     ('kapre_resample', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p]),
     ('kapre_resample_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p]),
+    ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
+    ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
+                           POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_pcen_backward', c_int, [c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc),
+                                    c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p, POINTER(SpecDesc),
+                                    c_void_p, c_void_p, c_void_p]),
     ('kapre_last_error', c_char_p, []),
     ('kapre_version', c_int, []),
     ('kapre_launch_count', c_uint64, []),

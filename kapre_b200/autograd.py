@@ -16,6 +16,7 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * ConcatenateFrequencyMap -> ``kapre_concat_frequency_map_backward`` (the first C channels)
 * SpecAugment     -> ``kapre_spec_augment`` over the gradient, mask value 0, the forward's device masks
 * Resample        -> ``kapre_resample_backward`` (the resampling kernel with up and down exchanged)
+* PCEN            -> ``kapre_pcen_backward`` (reverse-time scan; input and parameter gradients)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
 only the waveform and recomputes the complex spectrum and the pre-decibel values in its backward; so does
@@ -235,6 +236,25 @@ class _Resample(torch.autograd.Function):
         return ops.resample_backward(g, *ctx.cfg), None, None
 
 
+class _Pcen(torch.autograd.Function):
+    """The forward is the plain PCEN launch that also writes the smoother state M; the backward reads E and M and
+    returns the gradients of the input and of the four parameters (gain, bias, power, smooth_coef)."""
+
+    @staticmethod
+    def forward(ctx, E, gain, bias, power, smooth, eps, data_format):
+        y, M = ops.pcen_forward(E, (gain, bias, power, smooth), eps, data_format, save_M=True)
+        ctx.save_for_backward(E, M, gain, bias, power, smooth)
+        ctx.cfg = (eps, data_format)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        E, M, *params = ctx.saved_tensors
+        gE, gp = ops.pcen_backward(E, M, gy, params, *ctx.cfg)
+        return (gE, *gp, None, None)
+
+
 class _SpecAugment(torch.autograd.Function):
     """The backward pass is the forward launch over the gradient, with mask value 0 and the masks the forward drew
     (saved on the device): it never draws new ones."""
@@ -290,6 +310,10 @@ def spec_augment(x, time_masks, freq_masks, mask_value, data_format):
 
 def resample(x, plan, data_format):
     return _Resample.apply(x.float(), plan, data_format)
+
+
+def pcen(E, params, eps, data_format):
+    return _Pcen.apply(E.float(), *params, eps, data_format)
 
 
 def istft(X, plan, input_data_format, output_data_format):

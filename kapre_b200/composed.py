@@ -161,7 +161,12 @@ class Sequential(Layer):
         an eighth of the batch) and chunk i+1's host->device copy, chunk i's kernels and chunk
         i-1's device->host copy run on three CUDA streams, so PCIe runs in both directions while
         the SMs compute.  Results do not depend on the chunking: every op on the path, including
-        the decibel clamp, is per batch item (kapre/backend.py:178-179)."""
+        the decibel clamp, is per batch item (kapre/backend.py:178-179).  NumPy comes out, so nothing is recorded
+        for autograd, even for layers with trainable weights."""
+        with torch.no_grad():
+            return self._predict(x, batch_size)
+
+    def _predict(self, x, batch_size):
         if isinstance(x, torch.Tensor) and x.is_cuda:
             return ops.to_host(self.call(x))
         xh = torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else torch.as_tensor(x)
@@ -275,13 +280,15 @@ class CapturedSequential:
         cur = torch.cuda.current_stream()
         self._stream = torch.cuda.Stream(device=x.device)
         self._stream.wait_stream(cur)
-        with torch.cuda.stream(self._stream):      # warm-up on the capture stream: plans, workspace, smem attrs
-            for _ in range(2):
-                model.call(self.static_in)
-        self._stream.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph, stream=self._stream):
-            self.static_out = model.call(self.static_in)
+        # the graph replays forward launches only: nothing is recorded for autograd, even for trainable weights
+        with torch.no_grad():
+            with torch.cuda.stream(self._stream):      # warm-up on the capture stream: plans, workspace, smem attrs
+                for _ in range(2):
+                    model.call(self.static_in)
+            self._stream.synchronize()
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph, stream=self._stream):
+                self.static_out = model.call(self.static_in)
         cur.wait_stream(self._stream)
 
     def __call__(self, x):

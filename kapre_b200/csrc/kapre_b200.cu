@@ -25,6 +25,7 @@
 #include "grad_core.cuh"
 #include "grad_aux_core.cuh"
 #include "resample_core.cuh"
+#include "pcen_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -2182,6 +2183,141 @@ int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev,
         adj = p->adj;
     }
     return kb_resample_launch(adj, g_dev, g_desc, gx_dev, gx_desc, stream);
+}
+
+}  // extern "C"
+
+// ---- per-channel energy normalisation (pcen_core.cuh) ------------------------------------------------
+__global__ void __launch_bounds__(KB_PCEN_THREADS) kb_pcen_state_kernel(const __grid_constant__ KbPcenParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_pcen_fwd_state(p, i);
+}
+__global__ void __launch_bounds__(KB_PCEN_THREADS) kb_pcen_kernel(const __grid_constant__ KbPcenParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_pcen_fwd_out(p, i);
+}
+__global__ void __launch_bounds__(KB_PCEN_THREADS) kb_pcen_bwd_state_kernel(const __grid_constant__ KbPcenParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_pcen_bwd_state(p, i);
+}
+__global__ void __launch_bounds__(KB_PCEN_THREADS) kb_pcen_bwd_kernel(const __grid_constant__ KbPcenParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_pcen_bwd_out(p, i);
+}
+
+// Chunking of n_cols columns of `frames` frames against the current device's resident-thread capacity.
+static int kb_pcen_pick_chunks(long long n_cols, int frames, int* chunks) {
+    int dev = 0, sms = 0, per_sm = 0;
+    KB_CUDA(cudaGetDevice(&dev));
+    KB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    KB_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxThreadsPerMultiProcessor, dev));
+    *chunks = kb_pcen_chunks(n_cols, frames, (long long)sms * per_sm);
+    return 0;
+}
+
+static int kb_pcen_setup(KbPcenParams& p, const kapre_spec_desc* E_desc, int batch, int channels, int frames, int bands,
+                         const kapre_pcen_params* prm) {
+    if (!E_desc || !prm) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (batch < 0 || channels < 0 || frames < 0 || bands < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (!prm->gain || !prm->bias || !prm->power || !prm->smooth) return kb_fail(KAPRE_E_INVALID, "null parameter pointer");
+    for (int st : {prm->gain_stride, prm->bias_stride, prm->power_stride, prm->smooth_stride})
+        if (st != 0 && st != 1) return kb_fail(KAPRE_E_INVALID, "parameter strides must be 0 (shared) or 1 (per band), got %d", st);
+    if (!(prm->eps > 0.0f)) return kb_fail(KAPRE_E_INVALID, "eps must be positive, got %g", prm->eps);
+    p.B = batch; p.C = channels; p.T = frames; p.F = bands;
+    p.n_cols = (long long)batch * channels * bands;
+    p.E = nullptr;
+    p.e_sb = E_desc->stride_b; p.e_sc = E_desc->stride_c; p.e_st = E_desc->stride_t; p.e_sf = E_desc->stride_f;
+    p.c_inner = channels > 1 && llabs(E_desc->stride_c) < llabs(E_desc->stride_f) ? 1 : 0;
+    p.gain = prm->gain; p.bias = prm->bias; p.power = prm->power; p.smooth = prm->smooth;
+    p.gain_st = prm->gain_stride; p.bias_st = prm->bias_stride; p.power_st = prm->power_stride;
+    p.smooth_st = prm->smooth_stride;
+    p.eps = prm->eps;
+    int K = 1, rc;
+    if (p.n_cols * frames > 0 && (rc = kb_pcen_pick_chunks(p.n_cols, frames, &K))) return rc;
+    kb_pcen_set_chunks(p, K);
+    return 0;
+}
+
+template <typename Kern>
+static int kb_pcen_launch(Kern kernel, const KbPcenParams& p, long long n, cudaStream_t st) {
+    const long long grid = (n + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS;
+    if (grid > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many PCEN columns");
+    {
+        KbProfScope prof(st);
+        kernel<<<(int)grid, KB_PCEN_THREADS, 0, st>>>(p, n);
+    }
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+extern "C" {
+
+int kapre_pcen_workspace(int batch, int channels, int frames, int bands, int* chunks, int64_t* workspace_bytes) {
+    if (!chunks || !workspace_bytes) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (batch < 0 || channels < 0 || frames < 0 || bands < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    KbPcenParams p{};
+    p.T = frames;
+    const long long n_cols = (long long)batch * channels * bands;
+    int K = 1, rc;
+    if (n_cols * frames > 0 && (rc = kb_pcen_pick_chunks(n_cols, frames, &K))) return rc;
+    kb_pcen_set_chunks(p, K);
+    *chunks = p.K;
+    *workspace_bytes = p.K > 1 ? (int64_t)p.K * n_cols * 4 : 0;
+    return 0;
+}
+
+int kapre_pcen(const float* E_dev, const kapre_spec_desc* E_desc, int batch, int channels, int frames, int bands,
+               const kapre_pcen_params* params, float* y_dev, const kapre_spec_desc* y_desc, float* M_dev,
+               const kapre_spec_desc* M_desc, void* workspace_dev, void* stream) {
+    KbPcenParams p{};
+    int rc = kb_pcen_setup(p, E_desc, batch, channels, frames, bands, params);
+    if (rc) return rc;
+    if (!y_desc || (M_dev && !M_desc)) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (p.n_cols * frames == 0) return 0;
+    if (!E_dev || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)E_dev == (const void*)y_dev || (const void*)E_dev == (const void*)M_dev)
+        return kb_fail(KAPRE_E_INVALID, "PCEN cannot run in place");
+    if (p.K > 1 && !workspace_dev) return kb_fail(KAPRE_E_INVALID, "PCEN over %d time chunks needs a workspace", p.K);
+    p.E = E_dev;
+    p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_st = y_desc->stride_t; p.y_sf = y_desc->stride_f;
+    p.M = M_dev;
+    if (M_dev) { p.m_sb = M_desc->stride_b; p.m_sc = M_desc->stride_c; p.m_st = M_desc->stride_t; p.m_sf = M_desc->stride_f; }
+    p.state = (float*)workspace_dev;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (p.K > 1 && (rc = kb_pcen_launch(kb_pcen_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
+    return kb_pcen_launch(kb_pcen_kernel, p, (long long)p.K * p.n_cols, st);
+}
+
+int kapre_pcen_backward(const float* E_dev, const kapre_spec_desc* E_desc, const float* M_dev,
+                        const kapre_spec_desc* M_desc, const float* gy_dev, const kapre_spec_desc* gy_desc, int batch,
+                        int channels, int frames, int bands, const kapre_pcen_params* params, float* gE_dev,
+                        const kapre_spec_desc* gE_desc, float* param_partials_dev, void* workspace_dev, void* stream) {
+    KbPcenParams p{};
+    int rc = kb_pcen_setup(p, E_desc, batch, channels, frames, bands, params);
+    if (rc) return rc;
+    if (!M_desc || !gy_desc || !gE_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (p.n_cols == 0) return 0;
+    if (!param_partials_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if (frames == 0) {
+        KB_CUDA(cudaMemsetAsync(param_partials_dev, 0, (size_t)4 * p.n_cols * sizeof(float), (cudaStream_t)stream));
+        return 0;
+    }
+    if (!E_dev || !M_dev || !gy_dev || !gE_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)gE_dev == (const void*)E_dev || (const void*)gE_dev == (const void*)M_dev ||
+        (const void*)gE_dev == (const void*)gy_dev)
+        return kb_fail(KAPRE_E_INVALID, "PCEN backward cannot run in place");
+    if (p.K > 1 && !workspace_dev) return kb_fail(KAPRE_E_INVALID, "PCEN over %d time chunks needs a workspace", p.K);
+    p.E = E_dev;
+    p.M = const_cast<float*>(M_dev);
+    p.m_sb = M_desc->stride_b; p.m_sc = M_desc->stride_c; p.m_st = M_desc->stride_t; p.m_sf = M_desc->stride_f;
+    p.gy = gy_dev; p.g_sb = gy_desc->stride_b; p.g_sc = gy_desc->stride_c; p.g_st = gy_desc->stride_t; p.g_sf = gy_desc->stride_f;
+    p.gE = gE_dev; p.o_sb = gE_desc->stride_b; p.o_sc = gE_desc->stride_c; p.o_st = gE_desc->stride_t; p.o_sf = gE_desc->stride_f;
+    p.state = (float*)workspace_dev;
+    p.part = param_partials_dev;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (p.K > 1 && (rc = kb_pcen_launch(kb_pcen_bwd_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
+    return kb_pcen_launch(kb_pcen_bwd_kernel, p, (long long)p.K * p.n_cols, st);
 }
 
 }  // extern "C"

@@ -770,6 +770,79 @@ def resample_backward(g: torch.Tensor, plan: ResamplePlan, data_format, length):
     return gx
 
 
+def _pcen_params(params, eps, device):
+    """kapre_pcen_params over the four parameter tensors (gain, bias, power, smooth_coef): float32, 0-d (one value
+    for every band) or 1-d (one per band), on ``device``."""
+    ts = []
+    for t in params:
+        if t.device != device:
+            raise ValueError('PCEN parameters live on %s, the input on %s' % (t.device, device))
+        ts.append(t.detach().to(torch.float32).contiguous())
+    prm = N.PcenParams(*[t.data_ptr() for t in ts], *[int(t.dim() == 1) for t in ts], float(eps))
+    return prm, ts
+
+
+def _pcen_workspace(B, C, T, F, device):
+    """(chunks, scratch tensor or None) the library uses for this shape on the current device."""
+    k, nbytes = ctypes.c_int(1), ctypes.c_int64(0)
+    N.check(N.lib().kapre_pcen_workspace(B, C, T, F, ctypes.byref(k), ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value // 4, dtype=torch.float32, device=device) if nbytes.value else None
+    return k.value, ws
+
+
+@_device_of_first_arg
+def pcen(E: torch.Tensor, params, eps, data_format):
+    """Per-channel energy normalisation along the time axis of (b, t, band, ch) / (b, ch, t, band).  ``params``:
+    gain, bias, power and smooth_coef tensors, each 0-d or with one value per band."""
+    if not E.is_cuda:
+        raise N.KapreNativeError('pcen needs a CUDA tensor')
+    if torch.is_grad_enabled() and (E.requires_grad or any(p.requires_grad for p in params)):
+        from . import autograd
+        return autograd.pcen(E, params, eps, data_format)
+    return pcen_forward(E, params, eps, data_format, save_M=False)[0]
+
+
+def pcen_forward(E, params, eps, data_format, save_M):
+    """(y, M): one launch (two when the time axis is chunked); M is written only with ``save_M``, else None."""
+    E = _raw(E.to(torch.float32))
+    ed, (B, C, T, F) = _spec_desc(E, data_format)
+    prm, keep = _pcen_params(params, eps, E.device)
+    y, yd = _spec_alloc(B, C, T, F, data_format, torch.float32, E.device)
+    M, md = _spec_alloc(B, C, T, F, data_format, torch.float32, E.device) if save_M else (None, None)
+    if y.numel():
+        _, ws = _pcen_workspace(B, C, T, F, E.device)
+        N.check(N.lib().kapre_pcen(_ptr(E), ctypes.byref(ed), B, C, T, F, ctypes.byref(prm), _ptr(y), ctypes.byref(yd),
+                                   _ptr(M) if save_M else None, ctypes.byref(md) if save_M else None,
+                                   _ptr(ws) if ws is not None else None, _stream_ptr()))
+    return y, M
+
+
+@_device_of_first_arg
+def pcen_backward(E: torch.Tensor, M: torch.Tensor, gy: torch.Tensor, params, eps, data_format):
+    """Gradients of ``pcen`` given its input ``E``, the smoother state ``M`` its forward wrote and the output
+    gradient ``gy``: (gE, [g_gain, g_bias, g_power, g_smooth]), each parameter gradient shaped like the parameter.
+    The kernel writes per-(chunk, item, channel, band) partial sums; summing them here keeps the result
+    deterministic."""
+    E = _raw(E.to(torch.float32))
+    gy = _raw(gy.to(torch.float32))
+    ed, (B, C, T, F) = _spec_desc(E, data_format)
+    md, _ = _spec_desc(M, data_format)
+    gd, _ = _spec_desc(gy, data_format)
+    if gy.shape != E.shape or M.shape != E.shape:
+        raise ValueError('PCEN gradient shapes %s / %s do not match %s' % (tuple(gy.shape), tuple(M.shape), tuple(E.shape)))
+    prm, keep = _pcen_params(params, eps, E.device)
+    gE, od = _spec_alloc(B, C, T, F, data_format, torch.float32, E.device)
+    K, ws = _pcen_workspace(B, C, T, F, E.device)
+    part = torch.empty((4, K, B, C, F), dtype=torch.float32, device=E.device)
+    if part.numel():
+        N.check(N.lib().kapre_pcen_backward(_ptr(E), ctypes.byref(ed), _ptr(M), ctypes.byref(md), _ptr(gy),
+                                            ctypes.byref(gd), B, C, T, F, ctypes.byref(prm), _ptr(gE), ctypes.byref(od),
+                                            _ptr(part), _ptr(ws) if ws is not None else None, _stream_ptr()))
+    per_band = part.sum(dim=(1, 2, 3))
+    grads = [per_band[j] if p.dim() == 1 else per_band[j].sum() for j, p in enumerate(params)]
+    return gE, grads
+
+
 @_device_of_first_arg
 def concat_frequency_map_backward(g: torch.Tensor, data_format):
     """Gradient of ``concat_frequency_map`` with respect to its input: the first C of the C + 1 channels of ``g``."""

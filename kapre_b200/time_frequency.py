@@ -13,6 +13,7 @@ as NumPy, like ``model.predict``) or CUDA tensors (result stays on the device).
 from __future__ import annotations
 
 import itertools
+import math
 
 import numpy as np
 import torch
@@ -21,7 +22,8 @@ from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
-__all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta']
+__all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
+           'PCEN']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -69,7 +71,11 @@ class Layer:
     def __call__(self, x, *args, **kwargs):
         kwargs.pop('training', None)
         t, was_host = ops.to_device(x)
-        y = self.call(t, *args, **kwargs)
+        if was_host:        # host in, NumPy out (like predict): nothing to record for autograd
+            with torch.no_grad():
+                y = self.call(t, *args, **kwargs)
+        else:
+            y = self.call(t, *args, **kwargs)
         if was_host and isinstance(y, torch.Tensor):
             return ops.to_host(y)
         return y
@@ -346,3 +352,115 @@ class ConcatenateFrequencyMap(Layer):
 
     _config_fields = (('data_format', 'data_format_original'),)
 
+
+
+def _pcen_value(name, v, low, low_inclusive, high=None):
+    """A PCEN parameter as a float, or a list of floats (one per band); finite and in range, else ValueError."""
+    def one(e):
+        if isinstance(e, (bool, np.bool_)) or not isinstance(e, (int, float, np.integer, np.floating)):
+            raise ValueError('%s must be a number or a sequence of numbers, got: %r' % (name, v))
+        e = float(e)
+        if not math.isfinite(e) or e < low or (e == low and not low_inclusive) or (high is not None and e > high):
+            raise ValueError('%s must be finite and %s %s%s, got: %r' % (
+                name, '>=' if low_inclusive else '>', low, '' if high is None else ' and <= %s' % high, v))
+        return e
+    if isinstance(v, (list, tuple, np.ndarray, torch.Tensor)):
+        seq = np.asarray(v.detach().cpu() if isinstance(v, torch.Tensor) else v, dtype=object)
+        if seq.ndim != 1 or seq.size == 0:
+            raise ValueError('%s must be a number or a non-empty 1-D sequence (one value per band), got: %r' % (name, v))
+        return [one(e) for e in seq]
+    return one(v)
+
+
+@register_keras_serializable(package='Kapre')
+class PCEN(Layer):
+    """Per-channel energy normalisation of a non-negative spectrogram (normally mel magnitudes), along time:
+
+    ``M[t] = (1 - s) M[t-1] + s E[t]`` from ``M[-1] = E[0]``, then ``y = (E / (eps + M)^gain + bias)^power -
+    bias^power``, computed as ``bias^power expm1(power log1p(E (eps + M)^-gain / bias))`` so that small inputs do not
+    cancel.  ``s`` is ``smooth_coef``, or when that is None the coefficient librosa derives from
+    ``time_constant`` seconds at ``sample_rate / hop_length`` frames per second.  ``(batch, time, band, ch)`` or
+    ``(batch, ch, time, band)`` in, the same shape out.
+
+    ``gain`` (>= 0), ``bias`` (> 0), ``power`` (> 0) and ``smooth_coef`` (in [0, 1]) are each one number shared by
+    all bands or a sequence with one value per band.  They are the layer's weights: float32 tensors made on the
+    first call, on the input's device, shape ``()`` or ``(bands,)``, with ``requires_grad = trainable``.  Trained
+    values are used as they are: nothing clamps them back into the ranges above.  ``eps`` (> 0) is a constant.
+
+    When a batch has too few (item, channel, band) columns to fill the GPU, the time axis is processed in chunks.  The
+    result then agrees with the unchunked one to float32 rounding, not bit for bit, so outputs can differ in the last
+    bits between batch sizes (for example between a call and ``predict`` with a smaller ``batch_size``)."""
+
+    def __init__(self, sample_rate=22050, hop_length=512, time_constant=0.4, smooth_coef=None, gain=0.98, bias=2.0,
+                 power=0.5, eps=1e-6, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.sample_rate = _pcen_value('sample_rate', sample_rate, 0.0, False)
+        self.hop_length = _pcen_value('hop_length', hop_length, 0.0, False)
+        self.time_constant = _pcen_value('time_constant', time_constant, 0.0, False)
+        for name in ('sample_rate', 'hop_length', 'time_constant'):
+            if isinstance(getattr(self, name), list):
+                raise ValueError('%s must be a number' % name)
+        self.smooth_coef = None if smooth_coef is None else _pcen_value('smooth_coef', smooth_coef, 0.0, True, 1.0)
+        self.gain = _pcen_value('gain', gain, 0.0, True)
+        self.bias = _pcen_value('bias', bias, 0.0, False)
+        self.power = _pcen_value('power', power, 0.0, False)
+        self.eps = _pcen_value('eps', eps, 0.0, False)
+        if isinstance(self.eps, list):
+            raise ValueError('eps must be a number')
+        if self.smooth_coef is None:
+            t = self.time_constant * self.sample_rate / self.hop_length
+            self.smooth_coef_value = (math.sqrt(1.0 + 4.0 * t * t) - 1.0) / (2.0 * t * t)
+        else:
+            self.smooth_coef_value = self.smooth_coef
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self.built = False
+        self._weights = []
+
+    def build(self, bands, device):
+        """Make the four weights for ``bands`` bands on ``device``; a per-band value must have ``bands`` entries."""
+        ws = []
+        for name, v in (('gain', self.gain), ('bias', self.bias), ('power', self.power),
+                        ('smooth_coef', self.smooth_coef_value)):
+            if isinstance(v, list) and len(v) != bands:
+                raise ValueError('%s has %d values but the input has %d bands' % (name, len(v), bands))
+            ws.append(torch.tensor(v, dtype=torch.float32, device=device).requires_grad_(bool(self.trainable)))
+        self._weights = ws
+        self.built = True
+
+    @property
+    def weights(self):
+        """[gain, bias, power, smooth_coef] once built (the first call), else []."""
+        return list(self._weights)
+
+    def count_params(self):
+        if not self.built:
+            raise ValueError('You tried to call `count_params` on layer %s, but the layer isn\'t built.' % self.name)
+        return sum(int(w.numel()) for w in self._weights)
+
+    def call(self, x):
+        if x.dim() != 4:
+            raise ValueError('PCEN expects a 4-D batch, got shape %s' % (tuple(x.shape),))
+        bands = x.shape[3] if self.data_format == _CH_FIRST_STR else x.shape[2]
+        if not self.built:
+            self.build(bands, x.device)
+        elif self._weights[0].device != x.device:
+            raise ValueError('PCEN %s was built on %s and cannot run on %s' % (self.name, self._weights[0].device, x.device))
+        elif any(w.dim() == 1 and w.shape[0] != bands for w in self._weights):
+            raise ValueError('PCEN %s was built for %d bands, the input has %d'
+                             % (self.name, max(w.numel() for w in self._weights), bands))
+        return ops.pcen(x, self._weights, self.eps, self.data_format)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'),
+        ('hop_length', 'hop_length'),
+        ('time_constant', 'time_constant'),
+        ('smooth_coef', 'smooth_coef'),
+        ('gain', 'gain'),
+        ('bias', 'bias'),
+        ('power', 'power'),
+        ('eps', 'eps'),
+        ('data_format', 'data_format_original'),
+    )
