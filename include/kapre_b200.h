@@ -278,6 +278,38 @@ int kapre_pcen_backward(const float* E_dev, const kapre_spec_desc* E_desc, const
                         int channels, int frames, int bands, const kapre_pcen_params* params, float* gE_dev,
                         const kapre_spec_desc* gE_desc, float* param_partials_dev, void* workspace_dev, void* stream);
 
+/* ---- Griffin-Lim phase reconstruction ------------------------------------------------------------
+ * Fast Griffin-Lim (the momentum form librosa and torchaudio use) over this library's transform pair: given a
+ * magnitude spectrogram S (batch x channels x frames x (n_fft/2 + 1) bins, any strides),
+ *   X = S A_0;  repeat n_iter times: y = ISTFT(X); Y = STFT(y) (no padding: `frames` frames again);
+ *               A = Y - beta Yprev (A = Y the first time); X = S A / (|A| + 1e-16); Yprev = Y
+ *   then y = ISTFT(X): (frames - 1) * hop + win_length samples, untrimmed, as kapre_istft_inverse writes them,
+ * with beta = momentum / (1 + momentum).  A_0 = 1 (KAPRE_GL_INIT_ONES) or exp(2 pi i u) (KAPRE_GL_INIT_RANDOM) with
+ *   u = (mix(seed ^ mix(i)) >> 40) * 2^-24,  i = ((b * channels + c) * frames + t) * (n_fft/2 + 1) + f,
+ *   mix(z): z += 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9; z = (z ^ (z >> 27)) * 0x94D049BB133111EB;
+ *           return z ^ (z >> 31)          (splitmix64, uint64 arithmetic)
+ * so the phases depend on the seed and the canonical index only, not on S's strides.
+ * `stft` and `istft` must agree on n_fft, win_length and hop and live on the same device; pair the STFT window with
+ * its dual in the inverse plan, as InverseSTFT does (tf.signal.inverse_stft_window_fn), or the loop does not
+ * reconstruct.  One call enqueues the whole loop: 2 + 3 n_iter launches where the STFT and the inverse are one
+ * launch each (n_fft 256 / 512 / 1024 / 2048).  Not differentiable. */
+enum { KAPRE_GL_INIT_ONES = 0, KAPRE_GL_INIT_RANDOM = 1 };
+typedef struct {
+    int n_iter;        /* >= 0 */
+    float momentum;    /* in [0, 1) */
+    int init;          /* KAPRE_GL_INIT_* */
+    uint64_t seed;     /* KAPRE_GL_INIT_RANDOM only */
+} kapre_griffin_lim_cfg;
+/* Device scratch of kapre_griffin_lim: two (batch, channels, frames, n_fft/2 + 1) complex64 spectra and one
+ * (batch, channels, (frames - 1) * hop + win_length) float32 waveform.  0 for an empty batch; < 0 on error. */
+int64_t kapre_griffin_lim_workspace_bytes(const kapre_stft_plan* plan, int batch, int channels, int frames);
+/* y = GriffinLim(S).  `y_desc`: batch, channels and (frames - 1) * hop + win_length samples, any strides.
+ * `workspace_dev`: kapre_griffin_lim_workspace_bytes bytes (contents ignored); S and y must not overlap it. */
+int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft, const float* S_dev,
+                      const kapre_spec_desc* S_desc, int batch, int channels, int frames,
+                      const kapre_griffin_lim_cfg* cfg, float* y_dev, const kapre_wave_desc* y_desc,
+                      void* workspace_dev, void* stream);
+
 /* ---- misc ---------------------------------------------------------------------------------- */
 const char* kapre_last_error(void);
 int kapre_version(void);

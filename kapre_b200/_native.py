@@ -35,6 +35,13 @@ class PcenParams(Structure):
                 ('eps', c_float)]
 
 
+class GlCfg(Structure):
+    _fields_ = [('n_iter', c_int), ('momentum', c_float), ('init', c_int), ('seed', c_uint64)]
+
+
+GL_INIT_ONES, GL_INIT_RANDOM = 0, 1
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -93,6 +100,9 @@ SYMBOLS = [
     ('kapre_pcen_backward', c_int, [c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc),
                                     c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p, POINTER(SpecDesc),
                                     c_void_p, c_void_p, c_void_p]),
+    ('kapre_griffin_lim_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int]),
+    ('kapre_griffin_lim', c_int, [c_void_p, c_void_p, c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, POINTER(GlCfg),
+                                  c_void_p, POINTER(WaveDesc), c_void_p, c_void_p]),
     ('kapre_last_error', c_char_p, []),
     ('kapre_version', c_int, []),
     ('kapre_launch_count', c_uint64, []),

@@ -26,6 +26,7 @@
 #include "grad_aux_core.cuh"
 #include "resample_core.cuh"
 #include "pcen_core.cuh"
+#include "gl_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -2318,6 +2319,101 @@ int kapre_pcen_backward(const float* E_dev, const kapre_spec_desc* E_desc, const
     const cudaStream_t st = (cudaStream_t)stream;
     if (p.K > 1 && (rc = kb_pcen_launch(kb_pcen_bwd_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
     return kb_pcen_launch(kb_pcen_bwd_kernel, p, (long long)p.K * p.n_cols, st);
+}
+
+}  // extern "C"
+
+// ---- Griffin-Lim (gl_core.cuh) -------------------------------------------------------------------------
+__global__ void __launch_bounds__(KB_GL_THREADS) kb_gl_init_kernel(const __grid_constant__ KbGlParams p) {
+    const long long step = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += step) kb_gl_init_elem(p, i);
+}
+__global__ void __launch_bounds__(KB_GL_THREADS) kb_gl_project_kernel(const __grid_constant__ KbGlParams p) {
+    const long long step = (long long)gridDim.x * blockDim.x;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += step) kb_gl_project_elem(p, i);
+}
+
+// Workspace layout: spectrum buffers 0 and 1 (each n complex64, rounded up to 256 B), then the (B, C, L) waveform.
+static long long kb_gl_spec_bytes(long long n) { return (n * 8 + 255) / 256 * 256; }
+
+template <typename Kern>
+static int kb_gl_launch(Kern kernel, const KbGlParams& p, cudaStream_t st) {
+    int grid, rc;
+    if ((rc = kb_ew_grid(p.n, &grid))) return rc;
+    kernel<<<grid, KB_GL_THREADS, 0, st>>>(p);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+extern "C" {
+
+int64_t kapre_griffin_lim_workspace_bytes(const kapre_stft_plan* plan, int batch, int channels, int frames) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (batch == 0 || channels == 0 || frames == 0) return 0;
+    const long long n = (long long)batch * channels * frames * (plan->n_fft / 2 + 1);
+    const long long L = (long long)(frames - 1) * plan->hop + plan->win_length;
+    return 2 * kb_gl_spec_bytes(n) + (long long)batch * channels * L * 4;
+}
+
+int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft, const float* S_dev,
+                      const kapre_spec_desc* S_desc, int batch, int channels, int frames,
+                      const kapre_griffin_lim_cfg* cfg, float* y_dev, const kapre_wave_desc* y_desc,
+                      void* workspace_dev, void* stream) {
+    if (!stft || !istft || !S_desc || !cfg || !y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (stft->n_fft != istft->n_fft || stft->win_length != istft->win_length || stft->hop != istft->hop)
+        return kb_fail(KAPRE_E_INVALID, "STFT plan (n_fft=%d win_length=%d hop=%d) and inverse plan (n_fft=%d win_length=%d "
+                       "hop=%d) disagree", stft->n_fft, stft->win_length, stft->hop, istft->n_fft, istft->win_length, istft->hop);
+    if (stft->dev.device != istft->dev.device)
+        return kb_fail(KAPRE_E_INVALID, "STFT plan lives on device %d, inverse plan on device %d", stft->dev.device,
+                       istft->dev.device);
+    int rc = kb_check_device(stft->dev);
+    if (rc) return rc;
+    if (cfg->n_iter < 0) return kb_fail(KAPRE_E_INVALID, "n_iter must be >= 0, got %d", cfg->n_iter);
+    if (!(cfg->momentum >= 0.0f && cfg->momentum < 1.0f))
+        return kb_fail(KAPRE_E_INVALID, "momentum must be in [0, 1), got %g", cfg->momentum);
+    if (cfg->init != KAPRE_GL_INIT_ONES && cfg->init != KAPRE_GL_INIT_RANDOM)
+        return kb_fail(KAPRE_E_INVALID, "init must be KAPRE_GL_INIT_ONES or KAPRE_GL_INIT_RANDOM, got %d", cfg->init);
+    if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    const long long L = frames > 0 ? (long long)(frames - 1) * stft->hop + stft->win_length : 0;
+    if (L > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "signal too long");
+    if (y_desc->batch != batch || y_desc->channels != channels || y_desc->length != (int)L)
+        return kb_fail(KAPRE_E_INVALID, "output must be %d x %d x %lld samples, got %d x %d x %d", batch, channels, L,
+                       y_desc->batch, y_desc->channels, y_desc->length);
+    if (batch == 0 || channels == 0 || frames == 0) return 0;
+    if (!S_dev || !y_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+
+    const int F = stft->n_fft / 2 + 1;
+    KbGlParams p{};
+    p.S = S_dev; p.s_sb = S_desc->stride_b; p.s_sc = S_desc->stride_c; p.s_st = S_desc->stride_t; p.s_sf = S_desc->stride_f;
+    p.C = channels; p.T = frames; p.F = F;
+    p.n = (long long)batch * channels * frames * F;
+    p.beta = cfg->momentum / (1.0f + cfg->momentum);
+    p.init = cfg->init;
+    p.seed = (unsigned long long)cfg->seed;
+    float2* X[2] = {(float2*)workspace_dev, (float2*)((char*)workspace_dev + kb_gl_spec_bytes(p.n))};
+    float* wave = (float*)((char*)workspace_dev + 2 * kb_gl_spec_bytes(p.n));
+    const kapre_spec_desc sd = {(int64_t)channels * frames * F, (int64_t)frames * F, F, 1};
+    const kapre_wave_desc wd = {batch, channels, (int32_t)L, (int64_t)channels * L, L, 1};
+    const cudaStream_t st = (cudaStream_t)stream;
+
+    p.X = X[0];
+    if ((rc = kb_gl_launch(kb_gl_init_kernel, p, st))) return rc;
+    int cur = 0;
+    for (int it = 0; it < cfg->n_iter; ++it) {
+        // X (buffer cur) -> waveform -> Y over X in buffer cur; the new X goes over Yprev in the other buffer
+        if ((rc = kapre_istft_inverse(istft, X[cur], batch, channels, frames, &sd, wave, &wd, stream))) return rc;
+        if ((rc = kapre_stft_forward(stft, wave, &wd, 0, 0, KAPRE_OUT_COMPLEX, X[cur], &sd, nullptr, nullptr, nullptr,
+                                     stream)))
+            return rc;
+        p.Y = X[cur];
+        p.Yprev = (it > 0 && p.beta != 0.0f) ? X[1 - cur] : nullptr;
+        p.X = X[1 - cur];
+        if ((rc = kb_gl_launch(kb_gl_project_kernel, p, st))) return rc;
+        cur = 1 - cur;
+    }
+    return kapre_istft_inverse(istft, X[cur], batch, channels, frames, &sd, y_dev, y_desc, stream);
 }
 
 }  // extern "C"

@@ -844,6 +844,43 @@ def pcen_backward(E: torch.Tensor, M: torch.Tensor, gy: torch.Tensor, params, ep
 
 
 @_device_of_first_arg
+def griffin_lim(S: torch.Tensor, stft_plan: StftPlan, istft_plan: IstftPlan, n_iter, momentum, init, seed,
+                input_data_format, output_data_format):
+    """Griffin-Lim reconstruction of a (b, t, f, ch) / (b, ch, t, f) magnitude spectrogram by one library call that
+    enqueues the whole loop.  Returns the untrimmed (b, L, ch) / (b, ch, L) waveform, L = (T - 1) hop + win_length,
+    as ``istft`` does.  ``init``: ``N.GL_INIT_ONES`` or ``N.GL_INIT_RANDOM``; ``seed``: an int in [0, 2^64).
+    The loop has no gradient: an input that requires grad under grad mode raises rather than being detached."""
+    if not S.is_cuda:
+        raise N.KapreNativeError('griffin_lim needs a CUDA tensor')
+    if _wants_grad(S):
+        raise RuntimeError('Griffin-Lim is not differentiable: call it under torch.no_grad() or on a detached input')
+    if S.dtype != torch.float32:
+        S = S.float()
+    sd, (B, C, T, F) = _spec_desc(S, input_data_format)
+    if F != stft_plan.n_fft // 2 + 1:
+        raise ValueError('expected %d frequency bins for n_fft=%d, got %d' % (stft_plan.n_fft // 2 + 1, stft_plan.n_fft, F))
+    L = (T - 1) * stft_plan.hop_length + stft_plan.win_length if T > 0 else 0
+    if output_data_format == _CH_LAST_STR:
+        y = torch.empty((B, L, C), dtype=torch.float32, device=S.device)
+        sb, sl, sc = y.stride()
+    else:
+        y = torch.empty((B, C, L), dtype=torch.float32, device=S.device)
+        sb, sc, sl = y.stride()
+    if y.numel() == 0:
+        return y
+    yd = N.WaveDesc(B, C, L, sb, sc, sl)
+    lib = N.lib()
+    nbytes = lib.kapre_griffin_lim_workspace_bytes(stft_plan.handle(), B, C, T)
+    if nbytes < 0:
+        N.check(nbytes)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=S.device)
+    cfg = N.GlCfg(int(n_iter), float(momentum), int(init), int(seed))
+    N.check(lib.kapre_griffin_lim(stft_plan.handle(), istft_plan.handle(), _ptr(S), ctypes.byref(sd), B, C, T,
+                                  ctypes.byref(cfg), _ptr(y), ctypes.byref(yd), _ptr(ws), _stream_ptr()))
+    return y
+
+
+@_device_of_first_arg
 def concat_frequency_map_backward(g: torch.Tensor, data_format):
     """Gradient of ``concat_frequency_map`` with respect to its input: the first C of the C + 1 channels of ``g``."""
     g = _raw(g.to(torch.float32)).contiguous()

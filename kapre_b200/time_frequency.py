@@ -23,7 +23,7 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
 __all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
-           'PCEN']
+           'PCEN', 'GriffinLim']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -463,4 +463,99 @@ class PCEN(Layer):
         ('power', 'power'),
         ('eps', 'eps'),
         ('data_format', 'data_format_original'),
+    )
+
+
+def _gl_int(name, v, low, high=None):
+    """An int in [low, high) (bool and non-integral values rejected), else ValueError."""
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < low or \
+            (high is not None and v >= high):
+        raise ValueError('%s must be an int >= %d%s, got: %r' % (name, low, '' if high is None else ' and < %d' % high, v))
+    return int(v)
+
+
+@register_keras_serializable(package='Kapre')
+class GriffinLim(Layer):
+    """Waveform from a magnitude spectrogram by fast Griffin-Lim (the momentum form of librosa and torchaudio), run
+    over this library's own transform pair: ``STFT`` without padding and ``InverseSTFT`` with the dual window, so it
+    inverts ``get_stft_magnitude_layer`` / ``STFT -> Magnitude`` as they are computed here.
+
+    ``(batch, time, freq, ch)`` / ``(batch, ch, time, freq)`` float32 magnitudes with ``n_fft // 2 + 1`` bins ->
+    ``(batch, L, ch)`` / ``(batch, ch, L)`` waveform, ``L = (time - 1) * hop_length + win_length``, untrimmed exactly
+    as ``InverseSTFT`` returns it (for a spectrogram from ``get_perfectly_reconstructing_stft_istft``, drop the first
+    ``n_fft - hop_length`` samples).  ``win_length``, ``hop_length`` and ``window_name`` default as in ``STFT``.
+
+    Starting from ``X = S A_0``, each of ``n_iter`` iterations runs ``y = ISTFT(X)``, ``Y = STFT(y)``,
+    ``A = Y - beta Yprev`` (``beta = momentum / (1 + momentum)``; ``A = Y`` the first time) and
+    ``X = S A / (|A| + 1e-16)``; the result is ``ISTFT(X)``.  ``momentum`` is in [0, 1) (torchaudio's rule; 0 is
+    the original Griffin-Lim).  ``init='ones'`` starts from zero phase; ``init='random'`` from uniform random phases
+    drawn by a counter-based hash of ``seed`` and each element's (item, channel, frame, bin) index, so the result does
+    not depend on the data format or strides.  The index counts items within one call: ``predict`` with a
+    ``batch_size`` smaller than the batch draws other phases than one call on the whole batch.  ``seed=None`` draws a
+    fresh seed from torch's CPU generator on every call; a captured graph (``Sequential.capture``) keeps the seed of
+    the call it recorded.
+
+    The whole loop is one library call.  It has no gradient: calling the layer under grad mode on an input that
+    requires grad raises ``RuntimeError``; run it under ``torch.no_grad()`` or on a detached tensor."""
+
+    def __init__(self, n_fft=2048, win_length=None, hop_length=None, window_name=None, n_iter=32, momentum=0.99,
+                 init='random', seed=0, input_data_format='default', output_data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        for data_format in (input_data_format, output_data_format):
+            backend.validate_data_format_str(data_format)
+        input_data_format = _unwrap_format(input_data_format)
+        output_data_format = _unwrap_format(output_data_format)
+        if win_length is None:
+            win_length = n_fft
+        if hop_length is None:
+            hop_length = win_length // 4
+        self.n_iter = _gl_int('n_iter', n_iter, 0)
+        if isinstance(momentum, (bool, np.bool_)) or not isinstance(momentum, (int, float, np.integer, np.floating)) \
+                or not 0.0 <= float(momentum) < 1.0:
+            raise ValueError('momentum must be a number in [0, 1), got: %r' % (momentum,))
+        if init not in ('random', 'ones'):
+            raise ValueError("init must be 'random' or 'ones', got: %r" % (init,))
+        self.seed = None if seed is None else _gl_int('seed', seed, 0, 2 ** 64)
+        self.n_fft = n_fft
+        self.win_length = win_length
+        self.hop_length = hop_length
+        self.window_name = window_name
+        self.momentum = momentum
+        self.init = init
+        self.input_data_format_original = input_data_format
+        self.output_data_format_original = output_data_format
+        self.input_data_format = _resolve(input_data_format)
+        self.output_data_format = _resolve(output_data_format)
+        self._plans = None
+
+    @property
+    def plans(self):
+        """(StftPlan, IstftPlan): the forward window and its dual (``tf.signal.inverse_stft_window_fn``)."""
+        if self._plans is None:
+            window_fn = backend.get_window_fn(self.window_name)
+            dual_fn = backend.inverse_stft_window_fn(frame_step=self.hop_length, forward_window_fn=window_fn)
+            self._plans = (ops.StftPlan(self.n_fft, self.win_length, self.hop_length, window_fn(self.win_length)),
+                           ops.IstftPlan(self.n_fft, self.win_length, self.hop_length, dual_fn(self.win_length)))
+        return self._plans
+
+    def call(self, x):
+        seed = self.seed
+        if seed is None:
+            seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64)) % 2 ** 64
+        stft_plan, istft_plan = self.plans
+        return ops.griffin_lim(x, stft_plan, istft_plan, self.n_iter, self.momentum,
+                               N.GL_INIT_RANDOM if self.init == 'random' else N.GL_INIT_ONES, seed,
+                               self.input_data_format, self.output_data_format)
+
+    _config_fields = (
+        ('n_fft', 'n_fft'),
+        ('win_length', 'win_length'),
+        ('hop_length', 'hop_length'),
+        ('window_name', 'window_name'),
+        ('n_iter', 'n_iter'),
+        ('momentum', 'momentum'),
+        ('init', 'init'),
+        ('seed', 'seed'),
+        ('input_data_format', 'input_data_format_original'),
+        ('output_data_format', 'output_data_format_original'),
     )
