@@ -310,6 +310,36 @@ int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft
                       const kapre_griffin_lim_cfg* cfg, float* y_dev, const kapre_wave_desc* y_desc,
                       void* workspace_dev, void* stream);
 
+/* ---- phase-vocoder time stretch ----------------------------------------------------------------
+ * torchaudio.functional.phase_vocoder on a complex64 spectrogram X (batch x channels x frames x bins, any strides):
+ * frames' = ceil(frames / rate) output frames; for output u, ts = (double)u * rate, k = floor(ts), alpha = ts - k and
+ * (X[frames] = X[frames + 1] = 0)
+ *   m[u] = alpha |X[k + 1]| + (1 - alpha) |X[k]|
+ *   phi[u] = q(X[0]) + sum_{v < u} (q(X[k_v + 1]) - q(X[k_v]))    in uint32 arithmetic (mod 2^32)
+ *   Y[u] = m[u] (cospi(s), sinpi(s)),  s = (int32)phi[u] * 2^-31
+ * with q(z) = rint(atan2(z) * 2^31 / pi) mod 2^32, each angle a count of 2^-32 turns.  Modulo 2 pi, torchaudio's
+ * wrapped phase advance cancels, so the result does not depend on hop length or phase advance and none is taken.  The
+ * integer phase sum does not drift, and the output does not depend on the time chunking below.  rate must be finite
+ * and positive and frames' must fit in int32 (KAPRE_E_INVALID otherwise, before anything is launched). */
+/* The time chunking a call on the current device uses for this shape (`*chunks`, >= 1) and the device scratch it needs
+ * (`*workspace_bytes`: 4 x chunks x batch x channels x bins when chunks > 1, else 0); the same for the backward. */
+int kapre_time_stretch_workspace(int batch, int channels, int frames, int bins, double rate, int* chunks,
+                                 int64_t* workspace_bytes);
+/* Y = stretch(X): frames' output frames with Y_desc's strides.  Y must not overlap X.  `workspace_dev`:
+ * kapre_time_stretch_workspace's bytes (NULL when 0). */
+int kapre_time_stretch(const void* X_dev, const kapre_spec_desc* X_desc, int batch, int channels, int frames, int bins,
+                       double rate, void* Y_dev, const kapre_spec_desc* Y_desc, void* workspace_dev, void* stream);
+/* Gradient of kapre_time_stretch given X, the Y it wrote and the output gradient G (torch's convention dL/dRe +
+ * i dL/dIm): with gm = Re(conj(Y) G) / |Y|, gphi = Im(conj(Y) G) (0 where Y = 0) and lam_u = sum_{v > u} gphi[v],
+ * input frame j collects g|X| (the (1 - alpha) and alpha shares of gm of the outputs that read it) and gth (+lam_u
+ * where it is frame k_u + 1, -lam_u where it is frame k_u, and the sum of all gphi at frame 0), and
+ * gX = X / |X| (g|X| + i gth / |X|), 0 where |X| = 0.  Every gX element is written once (frames no output reads get
+ * 0); gX must not overlap X, Y or G. */
+int kapre_time_stretch_backward(const void* X_dev, const kapre_spec_desc* X_desc, const void* Y_dev,
+                                const kapre_spec_desc* Y_desc, const void* G_dev, const kapre_spec_desc* G_desc,
+                                int batch, int channels, int frames, int bins, double rate, void* gX_dev,
+                                const kapre_spec_desc* gX_desc, void* workspace_dev, void* stream);
+
 /* ---- misc ---------------------------------------------------------------------------------- */
 const char* kapre_last_error(void);
 int kapre_version(void);

@@ -103,6 +103,13 @@ SYMBOLS = [
     ('kapre_griffin_lim_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int]),
     ('kapre_griffin_lim', c_int, [c_void_p, c_void_p, c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, POINTER(GlCfg),
                                   c_void_p, POINTER(WaveDesc), c_void_p, c_void_p]),
+    ('kapre_time_stretch_workspace', c_int, [c_int, c_int, c_int, c_int, ctypes.c_double, POINTER(c_int),
+                                             POINTER(c_int64)]),
+    ('kapre_time_stretch', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p,
+                                   POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_time_stretch_backward', c_int, [c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p,
+                                            POINTER(SpecDesc), c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p,
+                                            POINTER(SpecDesc), c_void_p, c_void_p]),
     ('kapre_last_error', c_char_p, []),
     ('kapre_version', c_int, []),
     ('kapre_launch_count', c_uint64, []),

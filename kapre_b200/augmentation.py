@@ -1,5 +1,6 @@
-"""Augmentation layers (reference: kapre/augmentation.py).  ``SpecAugment`` only: the masks are drawn on the host, the
-masking is one CUDA pass (``kapre_spec_augment``)."""
+"""Augmentation layers (reference: kapre/augmentation.py).  ``SpecAugment``: the masks are drawn on the host, the
+masking is one CUDA pass (``kapre_spec_augment``).  ``TimeStretch``: a phase vocoder, one CUDA scan over time
+(``kapre_time_stretch``)."""
 from __future__ import annotations
 
 import numpy as np
@@ -75,3 +76,39 @@ class SpecAugment(Layer):
                        'mask_value': self.mask_value,
                        'data_format': self.data_format if self.data_format in (_CH_FIRST_STR, _CH_LAST_STR) else _CH_DEFAULT_STR})
         return config
+
+
+@register_keras_serializable(package='Kapre')
+class TimeStretch(Layer):
+    """Stretches a complex spectrogram in time without changing its pitch: ``torchaudio.transforms.TimeStretch`` /
+    ``torchaudio.functional.phase_vocoder``.  ``(batch, time, freq, ch)`` / ``(batch, ch, time, freq)`` complex in,
+    ``ceil(time / rate)`` frames out in the same data format (complex64; complex128 input is cast).  ``rate > 1``
+    speeds up, ``rate < 1`` slows down; ``rate == 1`` returns the input itself.  ``call(x, rate=...)`` overrides the
+    rate for one call, like torchaudio's ``overriding_rate``.
+
+    Output frame ``u`` reads frames ``k = floor(u * rate)`` and ``k + 1`` (zeros past the end), with
+    ``alpha = u * rate - k`` in float64: its magnitude is ``alpha |X[k + 1]| + (1 - alpha) |X[k]|`` and its phase is
+    ``angle(X[0])`` plus the sum of ``angle(X[k_v + 1]) - angle(X[k_v])`` over the outputs ``v < u``.  torchaudio adds
+    and removes a ``phase_advance`` inside a wrap to 2 pi; modulo 2 pi that cancels exactly, so the result does not
+    depend on the hop length and the layer takes none.  The phase sum is kept as a 32-bit fixed-point count of
+    turns, so it does not drift over long inputs (torchaudio's float32 ``cumsum`` does) and the output does not depend
+    on the batch size or data format.  The gradient with respect to the input is available when the CUDA input
+    requires grad."""
+
+    def __init__(self, rate, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.rate = ops._check_rate(rate)
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+
+    def call(self, x, rate=None):
+        if x.dim() != 4:
+            raise ValueError('TimeStretch expects a 4-D complex batch, got shape %s' % (tuple(x.shape),))
+        return ops.time_stretch(x, self.rate if rate is None else ops._check_rate(rate), self.data_format)
+
+    _config_fields = (
+        ('rate', 'rate'),
+        ('data_format', 'data_format_original'),
+    )

@@ -17,6 +17,7 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * SpecAugment     -> ``kapre_spec_augment`` over the gradient, mask value 0, the forward's device masks
 * Resample        -> ``kapre_resample_backward`` (the resampling kernel with up and down exchanged)
 * PCEN            -> ``kapre_pcen_backward`` (reverse-time scan; input and parameter gradients)
+* TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
 only the waveform and recomputes the complex spectrum and the pre-decibel values in its backward; so does
@@ -255,6 +256,24 @@ class _Pcen(torch.autograd.Function):
         return (gE, *gp, None, None)
 
 
+class _TimeStretch(torch.autograd.Function):
+    """The forward is the plain time-stretch launch; autograd saves its output, from which the backward takes the
+    magnitude and phase gradients, so the forward writes nothing extra."""
+
+    @staticmethod
+    def forward(ctx, X, rate, data_format):
+        Y = ops.time_stretch_forward(X, rate, data_format)
+        ctx.save_for_backward(X, Y)
+        ctx.cfg = (rate, data_format)
+        return Y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, G):
+        X, Y = ctx.saved_tensors
+        return ops.time_stretch_backward(X, Y, G, *ctx.cfg), None, None
+
+
 class _SpecAugment(torch.autograd.Function):
     """The backward pass is the forward launch over the gradient, with mask value 0 and the masks the forward drew
     (saved on the device): it never draws new ones."""
@@ -314,6 +333,10 @@ def resample(x, plan, data_format):
 
 def pcen(E, params, eps, data_format):
     return _Pcen.apply(E.float(), *params, eps, data_format)
+
+
+def time_stretch(X, rate, data_format):
+    return _TimeStretch.apply(X.to(torch.complex64), rate, data_format)
 
 
 def istft(X, plan, input_data_format, output_data_format):

@@ -18,12 +18,14 @@ import torch
 from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
+from .augmentation import TimeStretch
 from .signal import Resample
 from .time_frequency import (STFT, ApplyFilterbank, InverseSTFT, Layer, Magnitude, MagnitudeToDecibel, Phase,
                              get_registered_object)
 
 __all__ = ['CapturedSequential', 'Sequential', 'StftMagPhase', 'get_stft_magnitude_layer', 'get_melspectrogram_layer',
-           'get_log_frequency_spectrogram_layer', 'get_perfectly_reconstructing_stft_istft', 'get_stft_mag_phase']
+           'get_log_frequency_spectrogram_layer', 'get_perfectly_reconstructing_stft_istft', 'get_stft_mag_phase',
+           'get_time_stretch_layer']
 
 
 _streams = {}
@@ -435,3 +437,18 @@ def get_stft_mag_phase(input_shape, n_fft=2048, win_length=None, hop_length=None
         if return_decibel else None
     ch_axis = 1 if output_data_format == _CH_FIRST_STR else 3     # sic: the unresolved string, composed.py:504
     return StftMagPhase(waveform_to_stft, Magnitude(), Phase(), mag_to_decibel, ch_axis, name=name)
+
+
+def get_time_stretch_layer(rate, n_fft=2048, win_length=None, hop_length=None, window_name=None,
+                           waveform_data_format='default', name='time_stretch'):
+    """Waveform time stretch by a phase vocoder: ``Sequential([STFT, TimeStretch(rate), InverseSTFT])`` with the
+    inverse taking the dual of the STFT window.  ``(batch, time, ch)`` / ``(batch, ch, time)`` in; out the untrimmed
+    ``(T' - 1) * hop_length + win_length`` samples ``InverseSTFT`` returns, ``T' = ceil(T / rate)`` for the ``T``
+    frames of the STFT (no padding).  ``win_length`` and ``hop_length`` default as in ``STFT``."""
+    backend.validate_data_format_str(waveform_data_format)
+    stft = STFT(n_fft=n_fft, win_length=win_length, hop_length=hop_length, window_name=window_name,
+                input_data_format=waveform_data_format, output_data_format=_CH_LAST_STR)
+    stretch = TimeStretch(rate, data_format=_CH_LAST_STR)
+    istft = InverseSTFT(n_fft=n_fft, win_length=win_length, hop_length=hop_length, forward_window_name=window_name,
+                        input_data_format=_CH_LAST_STR, output_data_format=waveform_data_format)
+    return Sequential([stft, stretch, istft], name=name)

@@ -27,6 +27,7 @@
 #include "resample_core.cuh"
 #include "pcen_core.cuh"
 #include "gl_core.cuh"
+#include "ts_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -2414,6 +2415,156 @@ int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft
         cur = 1 - cur;
     }
     return kapre_istft_inverse(istft, X[cur], batch, channels, frames, &sd, y_dev, y_desc, stream);
+}
+
+}  // extern "C"
+
+// ---- phase-vocoder time stretch (ts_core.cuh) ----------------------------------------------------------
+__global__ void __launch_bounds__(KB_TS_THREADS) kb_ts_state_kernel(const __grid_constant__ KbTsParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_ts_fwd<false>(p, i);
+}
+__global__ void __launch_bounds__(KB_TS_THREADS) kb_ts_kernel(const __grid_constant__ KbTsParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_ts_fwd<true>(p, i);
+}
+__global__ void __launch_bounds__(KB_TS_THREADS) kb_ts_bwd_state_kernel(const __grid_constant__ KbTsParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_ts_bwd_state(p, i);
+}
+__global__ void __launch_bounds__(KB_TS_THREADS) kb_ts_bwd_kernel(const __grid_constant__ KbTsParams p, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) kb_ts_bwd_out(p, i);
+}
+
+// Output frames of a time stretch, ceil(frames / rate) as torch.arange counts them; negative on a bad argument.
+static long long kb_ts_out_frames(int frames, double rate) {
+    if (!std::isfinite(rate) || !(rate > 0.0)) return kb_fail(KAPRE_E_INVALID, "rate must be finite and positive, got %g", rate);
+    if (frames < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    const double n = std::ceil((double)frames / rate);
+    if (!(n <= 2147483647.0))
+        return kb_fail(KAPRE_E_INVALID, "%d frames at rate %g give %.0f output frames, more than 2^31 - 1", frames, rate, n);
+    return (long long)n;
+}
+
+static int kb_ts_setup(KbTsParams& p, const kapre_spec_desc* X_desc, int batch, int channels, int frames, int bins,
+                       double rate) {
+    if (!X_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (batch < 0 || channels < 0 || frames < 0 || bins < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    const long long n_out = kb_ts_out_frames(frames, rate);
+    if (n_out < 0) return (int)n_out;
+    p.B = batch; p.C = channels; p.T = frames; p.F = bins; p.T_out = (int)n_out;
+    p.rate = rate;
+    p.inv_rate = 1.0 / rate;
+    p.n_cols = (long long)batch * channels * bins;
+    p.x_sb = X_desc->stride_b; p.x_sc = X_desc->stride_c; p.x_st = X_desc->stride_t; p.x_sf = X_desc->stride_f;
+    p.c_inner = channels > 1 && llabs(X_desc->stride_c) < llabs(X_desc->stride_f) ? 1 : 0;
+    int K = 1;
+    if (p.n_cols * frames > 0) {
+        int dev = 0, sms = 0, per_sm = 0;
+        KB_CUDA(cudaGetDevice(&dev));
+        KB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        KB_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxThreadsPerMultiProcessor, dev));
+        K = kb_ts_chunks(p.n_cols, frames, (long long)sms * per_sm);
+    }
+    kb_ts_set_chunks(p, K);
+    return 0;
+}
+
+// Byte range [lo, hi) of a (batch, channels, frames, bins) complex64 tensor with these element strides.
+static void kb_ts_span(const void* base, const kapre_spec_desc* d, int B, int C, int T, int F, uintptr_t* lo, uintptr_t* hi) {
+    long long a = 0, b = 0;
+    const long long n[4] = {B, C, T, F}, s[4] = {d->stride_b, d->stride_c, d->stride_t, d->stride_f};
+    for (int j = 0; j < 4; ++j) {
+        const long long e = (n[j] - 1) * s[j];
+        if (e < 0) a += e; else b += e;
+    }
+    *lo = (uintptr_t)base + (uintptr_t)(a * 8);
+    *hi = (uintptr_t)base + (uintptr_t)(b * 8 + 8);
+}
+
+static bool kb_ts_overlap(const void* p, const kapre_spec_desc* pd, int pt, const void* q, const kapre_spec_desc* qd, int qt,
+                          int B, int C, int F) {
+    uintptr_t a0, a1, b0, b1;
+    kb_ts_span(p, pd, B, C, pt, F, &a0, &a1);
+    kb_ts_span(q, qd, B, C, qt, F, &b0, &b1);
+    return a0 < b1 && b0 < a1;
+}
+
+template <typename Kern>
+static int kb_ts_launch(Kern kernel, const KbTsParams& p, long long n, cudaStream_t st) {
+    const long long grid = (n + KB_TS_THREADS - 1) / KB_TS_THREADS;
+    if ((long long)p.K * p.n_cols > 0xffffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many time-stretch columns");
+    {
+        KbProfScope prof(st);
+        kernel<<<(int)grid, KB_TS_THREADS, 0, st>>>(p, n);
+    }
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
+}
+
+extern "C" {
+
+int kapre_time_stretch_workspace(int batch, int channels, int frames, int bins, double rate, int* chunks,
+                                 int64_t* workspace_bytes) {
+    if (!chunks || !workspace_bytes) return kb_fail(KAPRE_E_INVALID, "null argument");
+    const kapre_spec_desc d = {0, 0, 0, 0};
+    KbTsParams p{};
+    int rc = kb_ts_setup(p, &d, batch, channels, frames, bins, rate);
+    if (rc) return rc;
+    *chunks = p.K;
+    *workspace_bytes = p.K > 1 ? (int64_t)p.K * p.n_cols * 4 : 0;
+    return 0;
+}
+
+int kapre_time_stretch(const void* X_dev, const kapre_spec_desc* X_desc, int batch, int channels, int frames, int bins,
+                       double rate, void* Y_dev, const kapre_spec_desc* Y_desc, void* workspace_dev, void* stream) {
+    KbTsParams p{};
+    int rc = kb_ts_setup(p, X_desc, batch, channels, frames, bins, rate);
+    if (rc) return rc;
+    if (!Y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (p.n_cols * p.T_out == 0) return 0;
+    if (!X_dev || !Y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if (kb_ts_overlap(X_dev, X_desc, frames, Y_dev, Y_desc, p.T_out, batch, channels, bins))
+        return kb_fail(KAPRE_E_INVALID, "the time-stretch output overlaps its input");
+    if (p.K > 1 && !workspace_dev)
+        return kb_fail(KAPRE_E_INVALID, "a time stretch over %d time chunks needs a workspace", p.K);
+    p.X = (const float2*)X_dev;
+    p.Y = (float2*)Y_dev; p.y_sb = Y_desc->stride_b; p.y_sc = Y_desc->stride_c; p.y_st = Y_desc->stride_t; p.y_sf = Y_desc->stride_f;
+    p.state = workspace_dev;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (p.K > 1 && (rc = kb_ts_launch(kb_ts_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
+    return kb_ts_launch(kb_ts_kernel, p, (long long)p.K * p.n_cols, st);
+}
+
+int kapre_time_stretch_backward(const void* X_dev, const kapre_spec_desc* X_desc, const void* Y_dev,
+                                const kapre_spec_desc* Y_desc, const void* G_dev, const kapre_spec_desc* G_desc,
+                                int batch, int channels, int frames, int bins, double rate, void* gX_dev,
+                                const kapre_spec_desc* gX_desc, void* workspace_dev, void* stream) {
+    KbTsParams p{};
+    int rc = kb_ts_setup(p, X_desc, batch, channels, frames, bins, rate);
+    if (rc) return rc;
+    if (!Y_desc || !G_desc || !gX_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (p.n_cols * frames == 0) return 0;
+    if (!X_dev || !Y_dev || !G_dev || !gX_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if (kb_ts_overlap(gX_dev, gX_desc, frames, X_dev, X_desc, frames, batch, channels, bins) ||
+        kb_ts_overlap(gX_dev, gX_desc, frames, Y_dev, Y_desc, p.T_out, batch, channels, bins) ||
+        kb_ts_overlap(gX_dev, gX_desc, frames, G_dev, G_desc, p.T_out, batch, channels, bins))
+        return kb_fail(KAPRE_E_INVALID, "the time-stretch input gradient overlaps X, Y or the output gradient");
+    if (p.K > 1 && !workspace_dev)
+        return kb_fail(KAPRE_E_INVALID, "a time stretch over %d time chunks needs a workspace", p.K);
+    p.X = (const float2*)X_dev;
+    p.Y = (float2*)const_cast<void*>(Y_dev);
+    p.y_sb = Y_desc->stride_b; p.y_sc = Y_desc->stride_c; p.y_st = Y_desc->stride_t; p.y_sf = Y_desc->stride_f;
+    p.G = (const float2*)G_dev;
+    p.g_sb = G_desc->stride_b; p.g_sc = G_desc->stride_c; p.g_st = G_desc->stride_t; p.g_sf = G_desc->stride_f;
+    p.gX = (float2*)gX_dev;
+    p.o_sb = gX_desc->stride_b; p.o_sc = gX_desc->stride_c; p.o_st = gX_desc->stride_t; p.o_sf = gX_desc->stride_f;
+    p.state = workspace_dev;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (p.K > 1 && (rc = kb_ts_launch(kb_ts_bwd_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
+    return kb_ts_launch(kb_ts_bwd_kernel, p, (long long)p.K * p.n_cols, st);
 }
 
 }  // extern "C"

@@ -7,6 +7,7 @@ a missing library, a CPU-only process or a non-CUDA tensor raises.
 from __future__ import annotations
 
 import ctypes
+import math
 import threading
 
 import numpy as np
@@ -878,6 +879,78 @@ def griffin_lim(S: torch.Tensor, stft_plan: StftPlan, istft_plan: IstftPlan, n_i
     N.check(lib.kapre_griffin_lim(stft_plan.handle(), istft_plan.handle(), _ptr(S), ctypes.byref(sd), B, C, T,
                                   ctypes.byref(cfg), _ptr(y), ctypes.byref(yd), _ptr(ws), _stream_ptr()))
     return y
+
+
+def time_stretch_frames(frames, rate):
+    """ceil(frames / rate): the output frames of ``time_stretch`` (the length of torch.arange(0, frames, rate))."""
+    return math.ceil(int(frames) / float(rate))
+
+
+def _check_rate(rate):
+    if isinstance(rate, (bool, np.bool_)) or not isinstance(rate, (int, float, np.integer, np.floating)) \
+            or not math.isfinite(float(rate)) or not float(rate) > 0.0:
+        raise ValueError('rate must be a finite number > 0, got: %r' % (rate,))
+    return float(rate)
+
+
+def _time_stretch_workspace(B, C, T, F, rate, device):
+    """(chunks, scratch tensor or None) the library uses for this shape on the current device."""
+    k, nbytes = ctypes.c_int(1), ctypes.c_int64(0)
+    N.check(N.lib().kapre_time_stretch_workspace(B, C, T, F, rate, ctypes.byref(k), ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value // 4, dtype=torch.int32, device=device) if nbytes.value else None
+    return k.value, ws
+
+
+@_device_of_first_arg
+def time_stretch(X: torch.Tensor, rate, data_format):
+    """Phase-vocoder time stretch of a complex (b, t, f, ch) / (b, ch, t, f) spectrogram along time:
+    ``torchaudio.functional.phase_vocoder`` with ``ceil(t / rate)`` output frames (see ``include/kapre_b200.h``).
+    ``rate == 1`` returns ``X`` itself."""
+    if not X.is_cuda:
+        raise N.KapreNativeError('time_stretch needs a CUDA tensor')
+    if not X.is_complex():
+        raise TypeError('time_stretch needs a complex spectrogram, got %s' % (X.dtype,))
+    rate = _check_rate(rate)
+    if rate == 1.0:
+        return X
+    if _wants_grad(X):
+        from . import autograd
+        return autograd.time_stretch(X, rate, data_format)
+    return time_stretch_forward(X, rate, data_format)
+
+
+def time_stretch_forward(X, rate, data_format):
+    X = _raw(X.to(torch.complex64))
+    xd, (B, C, T, F) = _spec_desc(X, data_format)
+    Y, yd = _spec_alloc(B, C, time_stretch_frames(T, rate), F, data_format, torch.complex64, X.device)
+    if Y.numel():
+        _, ws = _time_stretch_workspace(B, C, T, F, rate, X.device)
+        N.check(N.lib().kapre_time_stretch(_ptr(X), ctypes.byref(xd), B, C, T, F, rate, _ptr(Y), ctypes.byref(yd),
+                                           _ptr(ws) if ws is not None else None, _stream_ptr()))
+    return Y
+
+
+@_device_of_first_arg
+def time_stretch_backward(X: torch.Tensor, Y: torch.Tensor, G: torch.Tensor, rate, data_format):
+    """Gradient of ``time_stretch`` with respect to ``X`` given the output ``Y`` it wrote and the output gradient
+    ``G`` (any strides)."""
+    X = _raw(X.to(torch.complex64))
+    Y = _raw(Y.to(torch.complex64))
+    G = _raw(G.to(torch.complex64))
+    rate = _check_rate(rate)
+    xd, (B, C, T, F) = _spec_desc(X, data_format)
+    yd, _ = _spec_desc(Y, data_format)
+    gd, _ = _spec_desc(G, data_format)
+    if G.shape != Y.shape or _spec_desc(Y, data_format)[1] != (B, C, time_stretch_frames(T, rate), F):
+        raise ValueError('time-stretch gradient shapes %s / %s do not match input %s at rate %g'
+                         % (tuple(G.shape), tuple(Y.shape), tuple(X.shape), rate))
+    gX, od = _spec_alloc(B, C, T, F, data_format, torch.complex64, X.device)
+    if gX.numel():
+        _, ws = _time_stretch_workspace(B, C, T, F, rate, X.device)
+        N.check(N.lib().kapre_time_stretch_backward(_ptr(X), ctypes.byref(xd), _ptr(Y), ctypes.byref(yd), _ptr(G),
+                                                    ctypes.byref(gd), B, C, T, F, rate, _ptr(gX), ctypes.byref(od),
+                                                    _ptr(ws) if ws is not None else None, _stream_ptr()))
+    return gX
 
 
 @_device_of_first_arg
