@@ -163,7 +163,10 @@ class Sequential(Layer):
         an eighth of the batch) and chunk i+1's host->device copy, chunk i's kernels and chunk
         i-1's device->host copy run on three CUDA streams, so PCIe runs in both directions while
         the SMs compute.  Results do not depend on the chunking: every op on the path, including
-        the decibel clamp, is per batch item (kapre/backend.py:178-179).  NumPy comes out, so nothing is recorded
+        the decibel clamp, is per batch item (kapre/backend.py:178-179), and the forward transforms give an item the
+        same bits wherever it sits in the batch.  Two exceptions agree with the unchunked result to float32 rounding,
+        not bit for bit: ``InverseSTFT``, whose tile length (and with it the order in which overlapping frames are
+        summed) follows the batch size, and ``PCEN`` (see its docstring).  NumPy comes out, so nothing is recorded
         for autograd, even for layers with trainable weights."""
         with torch.no_grad():
             return self._predict(x, batch_size)

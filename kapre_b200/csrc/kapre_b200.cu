@@ -857,14 +857,6 @@ int kapre_stft_plan_create(int n_fft, int win_length, int hop_length, const floa
     if (rc) { delete p; return rc; }
     if (p->Q) {
         std::vector<float> wh; std::vector<float2> twp, twn, twn2;
-        kb_make_wh(window_host, win_length, n_fft, wh);
-        kb_make_twp(p->Q, twp);
-        kb_make_twn(n_fft, twn);
-        kb_make_twn2(n_fft, twn2);
-        if ((rc = kb_upload(wh, &p->wh)) || (rc = kb_upload(twp, &p->twp)) || (rc = kb_upload(twn, &p->twn)) ||
-            (rc = kb_upload(twn2, &p->twn2))) {
-            kapre_stft_plan_destroy(p); return rc;
-        }
         double ca = 0.0, cb = 0.0;
         if (kb_fit_cosine_window(window_host, win_length, n_fft, &ca, &cb) && kb_env_int("KAPRE_B200_NOCOSW", 0) == 0) {
             std::vector<kb_f4> cwq;
@@ -872,6 +864,16 @@ int kapre_stft_plan_create(int n_fft, int win_length, int hop_length, const floa
             if ((rc = kb_upload(cwq, &p->cwq))) { kapre_stft_plan_destroy(p); return rc; }
             p->cosw = 1;
             p->cw_a0 = (float)(0.5 * ca);
+            kb_make_wh_cosw(p->Q, p->cw_a0, cwq, wh);   // the table frames read when not windowed in registers
+        } else {
+            kb_make_wh(window_host, win_length, n_fft, wh);
+        }
+        kb_make_twp(p->Q, twp);
+        kb_make_twn(n_fft, twn);
+        kb_make_twn2(n_fft, twn2);
+        if ((rc = kb_upload(wh, &p->wh)) || (rc = kb_upload(twp, &p->twp)) || (rc = kb_upload(twn, &p->twn)) ||
+            (rc = kb_upload(twn2, &p->twn2))) {
+            kapre_stft_plan_destroy(p); return rc;
         }
         if (n_fft == 1024 && win_length == 1024 && kb_fit_cosine_window(window_host, win_length, n_fft, &ca, &cb) && ca > 0.0) {
             p->win_a = ca; p->win_b = cb;

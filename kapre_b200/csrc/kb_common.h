@@ -196,7 +196,7 @@ KB_HD cpx cfma_s(cpx a, float s, cpx c) {
 #if defined(__CUDA_ARCH__)
     return cmake(__fmaf_rn(a.re, s, c.re), __fmaf_rn(a.im, s, c.im));
 #else
-    return cmake(a.re * s + c.re, a.im * s + c.im);
+    return cmake(std::fmaf(a.re, s, c.re), std::fmaf(a.im, s, c.im));   // one rounding, as on the device
 #endif
 }
 // d * (c - i sn): twiddle with separately given cosine / sine (compile-time constants at the call sites)

@@ -7,6 +7,7 @@
 #include <cstring>
 #include <vector>
 #include "kb_common.h"
+#include "fft_regs.cuh"
 
 static inline int kb_q_for_nfft(int n_fft) {
     // supported fast-path sizes: n_fft = 64 * Q, Q in {4, 8, 16, 32}
@@ -90,6 +91,27 @@ static inline void kb_make_cwq(int Q, int n_fft, double b, std::vector<kb_f4>& o
         v.x = (float)(0.5 * b * cos(ae)); v.y = (float)(0.5 * b * cos(ao));
         v.z = (float)(0.5 * b * sin(ae)); v.w = (float)(0.5 * b * sin(ao));
         out[q] = v;
+    }
+}
+
+// Window table of a cosine-sum window holding exactly what the in-register form of kb_col_window_dft32 computes
+// (a0, then fma(cc, -cos(2 pi j / 32), .), then fma(ss, sin(2 pi j / 32), .), each rounded once like __fmaf_rn):
+// frames read through the table (odd sample offset, cooperative staging, odd hop) then get the same bits as frames
+// windowed in registers, so an item's output does not depend on its alignment, its place in the batch or the tile shape.
+static inline void kb_make_wh_cosw(int Q, float a0, const std::vector<kb_f4>& cwq, std::vector<float>& out) {
+    out.assign((size_t)64 * Q, 0.0f);
+    for (int q = 0; q < Q; ++q) {
+        const float cc[2] = {cwq[q].x, cwq[q].y}, ss[2] = {cwq[q].z, cwq[q].w};
+        for (int j = 0; j < 32; ++j) {
+            const float cj = j <= 16 ? kb_cos32(j) : kb_cos32(32 - j);
+            const float sj = j <= 16 ? kb_sin32(j) : -kb_sin32(32 - j);
+            for (int e = 0; e < 2; ++e) {
+                float wv = a0;
+                if (cj != 0.0f) wv = std::fmaf(cc[e], -cj, wv);
+                if (sj != 0.0f) wv = std::fmaf(ss[e], sj, wv);
+                out[(size_t)2 * (q + Q * j) + e] = wv;
+            }
+        }
     }
 }
 

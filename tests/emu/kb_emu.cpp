@@ -98,6 +98,14 @@ static void run_istft2(const KbIstftParams& p, int n_cta) {
     }
 }
 
+// The plan's window table (kapre_stft_plan_create): the register form's values for a cosine-sum window, else 0.5 * window.
+static void kb_emu_make_wh(const float* window, int win_length, int n_fft, int Q, KbStftParams& p,
+                           const std::vector<kb_f4>& cwq, std::vector<float>& wh) {
+    if (p.cosw) kb_make_wh_cosw(Q, p.cw_a0, cwq, wh);
+    else kb_make_wh(window, win_length, n_fft, wh);
+    p.wh = wh.data();
+}
+
 extern "C" {
 
 int kb_emu_stft(const float* x, long long x_sb, long long x_sc, long long x_sl, int B, int C, int L,
@@ -115,7 +123,6 @@ int kb_emu_stft(const float* x, long long x_sb, long long x_sc, long long x_sl, 
     std::vector<KbBand> bands;
     std::vector<float> fbw;
     std::vector<kb_f4> cw; std::vector<kb_i2> cm; std::vector<int> cg;
-    kb_make_wh(window, win_length, n_fft, wh);
     kb_make_twp(Q, twp);
     kb_make_twn(n_fft, twn);
     kb_make_twn2(n_fft, twn2);
@@ -126,7 +133,7 @@ int kb_emu_stft(const float* x, long long x_sb, long long x_sc, long long x_sl, 
     KbStftParams p{};
     p.x = x; p.x_sb = x_sb; p.x_sc = x_sc; p.x_sl = x_sl; p.B = B; p.C = C; p.L = L;
     p.n_fft = n_fft; p.hop = hop; p.T = T; p.pad_left = pad_left;
-    p.wh = wh.data(); p.twp = twp.data(); p.twn = twn.data(); p.twn2 = twn2.data();
+    p.twp = twp.data(); p.twn = twn.data(); p.twn2 = twn2.data();
     std::vector<kb_f4> cwq;
     {
         double ca = 0.0, cb = 0.0;
@@ -135,6 +142,7 @@ int kb_emu_stft(const float* x, long long x_sb, long long x_sc, long long x_sl, 
             p.cosw = 1; p.cw_a0 = (float)(0.5 * ca); p.cwq = cwq.data();
         }
     }
+    kb_emu_make_wh(window, win_length, n_fft, Q, p, cwq, wh);
     p.out = out; p.o_sb = o_sb; p.o_sc = o_sc; p.o_st = o_st; p.o_sk = o_sk; p.mode = mode;
     p.bands = fb ? bands.data() : nullptr; p.fbw = fb ? fbw.data() : nullptr; p.n_bands = fb ? n_bands : 0;
     p.n_fbw = fb ? (int)fbw.size() : 0;
@@ -179,14 +187,13 @@ int kb_emu_stft_mc(const float* x, long long x_sb, long long x_sc, long long x_s
     std::vector<float> wh; std::vector<float2> twp, twn, twn2;
     std::vector<kb_f4> cw; std::vector<kb_i2> cm; std::vector<int> cg;
     if (fbm) kb_make_fb_chunks(fb, n_freq, n_bands, 32, cw, cm, cg);
-    kb_make_wh(window, win_length, n_fft, wh);
     kb_make_twp(Q, twp);
     kb_make_twn(n_fft, twn);
     kb_make_twn2(n_fft, twn2);
     KbStftParams p{};
     p.x = x; p.x_sb = x_sb; p.x_sc = x_sc; p.x_sl = x_sl; p.B = B; p.C = C; p.L = L;
     p.n_fft = n_fft; p.hop = hop; p.T = T; p.pad_left = pad_left;
-    p.wh = wh.data(); p.twp = twp.data(); p.twn = twn.data(); p.twn2 = twn2.data();
+    p.twp = twp.data(); p.twn = twn.data(); p.twn2 = twn2.data();
     std::vector<kb_f4> cwq;
     {
         double ca = 0.0, cb = 0.0;
@@ -195,6 +202,7 @@ int kb_emu_stft_mc(const float* x, long long x_sb, long long x_sc, long long x_s
             p.cosw = 1; p.cw_a0 = (float)(0.5 * ca); p.cwq = cwq.data();
         }
     }
+    kb_emu_make_wh(window, win_length, n_fft, Q, p, cwq, wh);
     p.out = out; p.o_sb = o_sb; p.o_sc = o_sc; p.o_st = o_st; p.o_sk = o_sk; p.mode = mode;
     p.amin = amin; p.db_mul = db_mul; p.db_sub = db_sub; p.item_max = item_max; p.db_on = db_on; p.ph_off = ph_off;
     p.db_ftz = (amin >= 1.17549435e-38f) ? 1 : 0;
@@ -387,6 +395,39 @@ int kb_emu_fb(const float* x, long long x_sb, long long x_sc, long long x_st, lo
         kb_fb_cta(p, smem.data(), cta, n_cta);
     }
     return 0;
+}
+
+// The plan's window tables: wh (n_fft floats), and for a cosine-sum window cwq (4 * Q floats) and a0.  Returns cosw.
+int kb_emu_window_tables(const float* window, int win_length, int n_fft, float* wh_out, float* cwq_out, float* a0_out) {
+    const int Q = kb_q_for_nfft(n_fft);
+    if (!Q) return -1;
+    KbStftParams p{};
+    std::vector<kb_f4> cwq;
+    std::vector<float> wh;
+    double ca = 0.0, cb = 0.0;
+    if (kb_fit_cosine_window(window, win_length, n_fft, &ca, &cb)) {
+        kb_make_cwq(Q, n_fft, cb, cwq);
+        p.cosw = 1; p.cw_a0 = (float)(0.5 * ca);
+        for (int q = 0; q < Q; ++q) std::memcpy(cwq_out + 4 * q, &cwq[q], 16);
+        *a0_out = p.cw_a0;
+    }
+    kb_emu_make_wh(window, win_length, n_fft, Q, p, cwq, wh);
+    std::memcpy(wh_out, wh.data(), (size_t)n_fft * 4);
+    return p.cosw;
+}
+
+// Shared memory of the single-channel kernel at a tile shape (kb_stft_smem_layout), for enumerating the shapes the
+// launcher may pick; n_chunks is the filterbank's chunk count (kb_make_fb_chunks over 32 lane groups).
+int kb_emu_stft_smem(int n_fft, int hop, int TF, int n_warps, int mode, int n_bands, int n_chunks) {
+    const int Q = kb_q_for_nfft(n_fft);
+    if (!Q) return -1;
+    return kb_stft_smem_layout(Q, n_fft, hop, TF, n_warps, mode, n_bands, n_chunks, 0).total;
+}
+
+int kb_emu_fb_chunks(const float* fb, int n_freq, int n_bands) {
+    std::vector<kb_f4> cw; std::vector<kb_i2> cm; std::vector<int> cg;
+    kb_make_fb_chunks(fb, n_freq, n_bands, 32, cw, cm, cg);
+    return (int)cm.size();
 }
 
 // kb_atan2 (the Phase outputs' polynomial atan2) on arrays, for the accuracy test
