@@ -340,6 +340,35 @@ int kapre_time_stretch_backward(const void* X_dev, const kapre_spec_desc* X_desc
                                 int batch, int channels, int frames, int bins, double rate, void* gX_dev,
                                 const kapre_spec_desc* gX_desc, void* workspace_dev, void* stream);
 
+/* ---- filterbank inversion (mel / log spectrogram -> linear magnitudes) ----------------------------------------
+ * With A the (n_bands x n_freq) transpose of a row-major (n_freq x n_bands) filterbank `fb_host` (as given to
+ * kapre_filterbank_create), each frame's n_bands values m are mapped to the n_freq values s that a fixed number of
+ * projected accelerated gradient (FISTA) steps take towards  min ||A s - m||^2  subject to s >= 0:
+ *   s_0 = max(A^T (m / d), 0) with d = A A^T 1 (m / d = 0 where d = 0);  y_0 = s_0;  t_0 = 1;
+ *   s_{k+1} = max(y_k - step A^T (A y_k - m), 0);  t_{k+1} = (1 + sqrt(1 + 4 t_k^2)) / 2;
+ *   y_{k+1} = s_{k+1} + ((t_k - 1) / t_{k+1}) (s_{k+1} - s_k);   output s_{n_iter}.
+ * step = 1 / ||A||_2^2 (float64 power iteration when the plan is made).  Bins no band touches come out 0.  The
+ * minimiser is not unique (n_freq > n_bands); the output is this iteration's result.  With from_decibel the input is
+ * dB and is converted on load: m = 10^(x / 10) max(amin, ref_value), the inverse of kapre_magnitude_to_decibel where
+ * its dynamic-range clamp did not bind.  One launch; each input element is read once and each output element written
+ * once, and a frame's output does not depend on its place in the batch, the strides or the data format.  Not
+ * differentiable. */
+typedef struct kapre_fb_inverse_plan kapre_fb_inverse_plan;
+int kapre_fb_inverse_plan_create(const float* fb_host, int n_freq, int n_bands, kapre_fb_inverse_plan** out);
+void kapre_fb_inverse_plan_destroy(kapre_fb_inverse_plan* plan);
+typedef struct {
+    int n_iter;          /* >= 0 */
+    int from_decibel;    /* 0 or 1 */
+    float ref_value;     /* from_decibel only: > 0 */
+    float amin;          /* from_decibel only: > 0 */
+} kapre_fb_inverse_cfg;
+/* out = invert(x).  x: (batch, channels, frames) x n_bands, out: ... x n_freq, any strides; out must not overlap x.
+ * KAPRE_E_UNSUPPORTED when one frame's state (2 n_freq + 2 n_bands floats, doubled for the padded tile) does not fit
+ * the device's shared memory. */
+int kapre_filterbank_invert(const kapre_fb_inverse_plan* plan, const kapre_fb_inverse_cfg* cfg, const float* x_dev,
+                            int batch, int channels, int frames, const kapre_spec_desc* x_desc, float* out_dev,
+                            const kapre_spec_desc* out_desc, void* stream);
+
 /* ---- misc ---------------------------------------------------------------------------------- */
 const char* kapre_last_error(void);
 int kapre_version(void);

@@ -42,6 +42,10 @@ class GlCfg(Structure):
 GL_INIT_ONES, GL_INIT_RANDOM = 0, 1
 
 
+class FbInvCfg(Structure):
+    _fields_ = [('n_iter', c_int), ('from_decibel', c_int), ('ref_value', c_float), ('amin', c_float)]
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -110,6 +114,10 @@ SYMBOLS = [
     ('kapre_time_stretch_backward', c_int, [c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p,
                                             POINTER(SpecDesc), c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p,
                                             POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_fb_inverse_plan_create', c_int, [c_void_p, c_int, c_int, POINTER(c_void_p)]),
+    ('kapre_fb_inverse_plan_destroy', None, [c_void_p]),
+    ('kapre_filterbank_invert', c_int, [c_void_p, POINTER(FbInvCfg), c_void_p, c_int, c_int, c_int, POINTER(SpecDesc),
+                                        c_void_p, POINTER(SpecDesc), c_void_p]),
     ('kapre_last_error', c_char_p, []),
     ('kapre_version', c_int, []),
     ('kapre_launch_count', c_uint64, []),

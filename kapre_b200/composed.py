@@ -20,12 +20,12 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .augmentation import TimeStretch
 from .signal import Resample
-from .time_frequency import (STFT, ApplyFilterbank, InverseSTFT, Layer, Magnitude, MagnitudeToDecibel, Phase,
-                             get_registered_object)
+from .time_frequency import (STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
+                             MagnitudeToDecibel, Phase, get_registered_object)
 
 __all__ = ['CapturedSequential', 'Sequential', 'StftMagPhase', 'get_stft_magnitude_layer', 'get_melspectrogram_layer',
            'get_log_frequency_spectrogram_layer', 'get_perfectly_reconstructing_stft_istft', 'get_stft_mag_phase',
-           'get_time_stretch_layer']
+           'get_time_stretch_layer', 'get_inverse_melspectrogram_layer']
 
 
 _streams = {}
@@ -455,3 +455,31 @@ def get_time_stretch_layer(rate, n_fft=2048, win_length=None, hop_length=None, w
     istft = InverseSTFT(n_fft=n_fft, win_length=win_length, hop_length=hop_length, forward_window_name=window_name,
                         input_data_format=_CH_LAST_STR, output_data_format=waveform_data_format)
     return Sequential([stft, stretch, istft], name=name)
+
+
+def get_inverse_melspectrogram_layer(n_fft=2048, win_length=None, hop_length=None, window_name=None, sample_rate=22050,
+                                     n_mels=128, mel_f_min=0.0, mel_f_max=None, mel_htk=False, mel_norm='slaney',
+                                     return_decibel=False, db_amin=1e-5, db_ref_value=1.0, nnls_iter=100,
+                                     griffin_lim_iter=32, momentum=0.99, init='random', seed=0,
+                                     input_data_format='default', output_data_format='default',
+                                     name='inverse_melspectrogram'):
+    """Waveform from a mel spectrogram: ``Sequential([InverseFilterbank('mel', ...), GriffinLim(...)])``.
+
+    The spectrogram-describing arguments have the names and defaults of ``get_melspectrogram_layer``, so one kwargs
+    dict describes both directions; ``return_decibel`` says the input is in decibels (``db_amin`` and
+    ``db_ref_value`` as there; elements the dynamic-range clamp raised come back as the clamp floor).
+    ``nnls_iter`` is ``InverseFilterbank``'s ``n_iter``; ``griffin_lim_iter``, ``momentum``, ``init`` and ``seed``
+    go to ``GriffinLim``.  ``(batch, time, n_mels, ch)`` / ``(batch, ch, time, n_mels)`` in
+    (``input_data_format``); out the untrimmed ``(batch, L, ch)`` / ``(batch, ch, L)`` waveform
+    (``output_data_format``), ``L = (time - 1) * hop_length + win_length``, as ``GriffinLim`` returns it.  At
+    n_fft 256-2048 a call is ``1 + (2 + 3 * griffin_lim_iter)`` kernel launches.  Not differentiable."""
+    backend.validate_data_format_str(input_data_format)
+    backend.validate_data_format_str(output_data_format)
+    kwargs = {'sample_rate': sample_rate, 'n_freq': n_fft // 2 + 1, 'n_mels': n_mels, 'f_min': mel_f_min,
+              'f_max': mel_f_max, 'htk': mel_htk, 'norm': mel_norm}
+    inverse_fb = InverseFilterbank('mel', kwargs, n_iter=nnls_iter, from_decibel=return_decibel,
+                                   db_ref_value=db_ref_value, db_amin=db_amin, data_format=input_data_format)
+    gl = GriffinLim(n_fft=n_fft, win_length=win_length, hop_length=hop_length, window_name=window_name,
+                    n_iter=griffin_lim_iter, momentum=momentum, init=init, seed=seed,
+                    input_data_format=input_data_format, output_data_format=output_data_format)
+    return Sequential([inverse_fb, gl], name=name)

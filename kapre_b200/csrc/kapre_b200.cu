@@ -28,6 +28,7 @@
 #include "pcen_core.cuh"
 #include "gl_core.cuh"
 #include "ts_core.cuh"
+#include "fbinv_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -2567,6 +2568,101 @@ int kapre_time_stretch_backward(const void* X_dev, const kapre_spec_desc* X_desc
     const cudaStream_t st = (cudaStream_t)stream;
     if (p.K > 1 && (rc = kb_ts_launch(kb_ts_bwd_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
     return kb_ts_launch(kb_ts_bwd_kernel, p, (long long)p.K * p.n_cols, st);
+}
+
+}  // extern "C"
+
+// ---- filterbank inversion (fbinv_core.cuh) ----------------------------------------------------------------------
+__global__ void __launch_bounds__(KB_FBI_WARPS * 32, 1) kb_fbi_kernel(const __grid_constant__ KbFbiParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_fbi_cta(p, kb_smem, (int)blockIdx.x, (int)gridDim.x);
+}
+
+struct kapre_fb_inverse_plan {
+    int n_freq, n_bands;
+    DevInfo dev;
+    float step = 0.0f;
+    KbBand* bands = nullptr;
+    float* w = nullptr;
+    int* cptr = nullptr;
+    KbFbiCol* cols = nullptr;
+    float* inv_d = nullptr;
+};
+
+extern "C" {
+
+int kapre_fb_inverse_plan_create(const float* fb_host, int n_freq, int n_bands, kapre_fb_inverse_plan** out) {
+    if (!out || !fb_host) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (n_freq < 1 || n_bands < 1) return kb_fail(KAPRE_E_INVALID, "empty filterbank");
+    kapre_fb_inverse_plan* f = new kapre_fb_inverse_plan();
+    f->n_freq = n_freq; f->n_bands = n_bands;
+    int rc = kb_dev_info(&f->dev);
+    if (rc) { delete f; return rc; }
+    KbFbiTables t;
+    kb_fbi_make_tables(fb_host, n_freq, n_bands, t);
+    f->step = t.step;
+    if ((rc = kb_upload(t.bands, &f->bands)) || (rc = kb_upload(t.w, &f->w)) || (rc = kb_upload(t.cptr, &f->cptr)) ||
+        (rc = kb_upload(t.cols, &f->cols)) || (rc = kb_upload(t.inv_d, &f->inv_d))) {
+        kapre_fb_inverse_plan_destroy(f);
+        return rc;
+    }
+    *out = f;
+    return 0;
+}
+
+void kapre_fb_inverse_plan_destroy(kapre_fb_inverse_plan* f) {
+    if (!f) return;
+    cudaFree(f->bands); cudaFree(f->w); cudaFree(f->cptr); cudaFree(f->cols); cudaFree(f->inv_d);
+    delete f;
+}
+
+int kapre_filterbank_invert(const kapre_fb_inverse_plan* plan, const kapre_fb_inverse_cfg* cfg, const float* x_dev,
+                            int batch, int channels, int frames, const kapre_spec_desc* x_desc, float* out_dev,
+                            const kapre_spec_desc* out_desc, void* stream) {
+    if (!plan || !cfg || !x_desc || !out_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
+    if (cfg->n_iter < 0) return kb_fail(KAPRE_E_INVALID, "n_iter must be >= 0, got %d", cfg->n_iter);
+    if (cfg->from_decibel != 0 && cfg->from_decibel != 1)
+        return kb_fail(KAPRE_E_INVALID, "from_decibel must be 0 or 1, got %d", cfg->from_decibel);
+    if (cfg->from_decibel && !(cfg->ref_value > 0.0f && cfg->ref_value <= 3.402823466e38f))
+        return kb_fail(KAPRE_E_INVALID, "ref_value must be positive and finite, got %g", cfg->ref_value);
+    if (cfg->from_decibel && !(cfg->amin > 0.0f && cfg->amin <= 3.402823466e38f))
+        return kb_fail(KAPRE_E_INVALID, "amin must be positive and finite, got %g", cfg->amin);
+    if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (batch == 0 || channels == 0 || frames == 0) return 0;
+    if (!x_dev || !out_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    KbFbiParams p{};
+    p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_st = x_desc->stride_t; p.x_sk = x_desc->stride_f;
+    p.B = batch; p.C = channels; p.T = frames; p.F = plan->n_freq; p.M = plan->n_bands;
+    p.bands = plan->bands; p.fbw = plan->w; p.cptr = plan->cptr; p.cols = plan->cols; p.inv_d = plan->inv_d;
+    p.step = plan->step;
+    p.n_iter = cfg->n_iter;
+    p.from_db = cfg->from_decibel;
+    p.db_scale = cfg->amin > cfg->ref_value ? (double)cfg->amin : (double)cfg->ref_value;
+    p.out = out_dev; p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t;
+    p.o_sk = out_desc->stride_f;
+    p.R = kb_fbi_pick_r(plan->n_freq, plan->n_bands, plan->dev.smem_optin);
+    if (p.R == 0)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "filterbank inversion: one frame of a %dx%d filterbank does not fit shared memory",
+                       plan->n_freq, plan->n_bands);
+    p.n_tiles_t = (frames + p.R - 1) / p.R;
+    p.n_warps = KB_FBI_WARPS;
+    const long long tiles = (long long)batch * channels * p.n_tiles_t;
+    if (tiles > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many frames");
+    const int smem = kb_fbi_smem_layout(plan->n_freq, plan->n_bands, p.R).total;
+    if ((rc = kb_set_smem(kb_fbi_kernel, smem))) return rc;
+    // the CTAs loop over tiles, so the grid is what fits on the device at once (a CTA that waited for a slot would
+    // start its share of the tiles late)
+    int bps = 0;
+    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kb_fbi_kernel, KB_FBI_WARPS * 32, smem));
+    if (bps < 1) bps = 1;
+    const long long gmax = (long long)plan->dev.sm_count * bps;
+    const int grid = (int)(tiles < gmax ? tiles : gmax);
+    kb_fbi_kernel<<<grid, KB_FBI_WARPS * 32, smem, (cudaStream_t)stream>>>(p);
+    KB_CUDA(cudaGetLastError());
+    g_launches++;
+    return 0;
 }
 
 }  // extern "C"

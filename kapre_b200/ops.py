@@ -215,6 +215,32 @@ class Filterbank:
         return h.ptr
 
 
+class FilterbankInversePlan:
+    """kapre_fb_inverse_plan per CUDA device for one (n_freq, n_bands) filterbank matrix: the row and column band
+    lists of its transpose and the gradient step 1 / ||A||_2^2 of the NNLS iteration."""
+
+    def __init__(self, matrix: np.ndarray):
+        self.matrix = np.ascontiguousarray(matrix, dtype=np.float32)
+        if self.matrix.ndim != 2:
+            raise ValueError('filterbank must be (n_freq, n_bands)')
+        self.n_freq, self.n_bands = self.matrix.shape
+        self._per_device = {}
+
+    def handle(self):
+        _require_cuda()
+        dev = torch.cuda.current_device()
+        with _lock:
+            h = self._per_device.get(dev)
+            if h is None:
+                lib = N.lib()
+                out = ctypes.c_void_p()
+                N.check(lib.kapre_fb_inverse_plan_create(self.matrix.ctypes.data_as(ctypes.c_void_p), self.n_freq,
+                                                         self.n_bands, ctypes.byref(out)))
+                h = _Handle(out, lib.kapre_fb_inverse_plan_destroy)
+                self._per_device[dev] = h
+        return h.ptr
+
+
 class ResamplePlan:
     """kapre_resample_plan per CUDA device for one (up, down, filter)."""
 
@@ -951,6 +977,32 @@ def time_stretch_backward(X: torch.Tensor, Y: torch.Tensor, G: torch.Tensor, rat
                                                     ctypes.byref(gd), B, C, T, F, rate, _ptr(gX), ctypes.byref(od),
                                                     _ptr(ws) if ws is not None else None, _stream_ptr()))
     return gX
+
+
+@_device_of_first_arg
+def invert_filterbank(x: torch.Tensor, plan: FilterbankInversePlan, n_iter, from_decibel, ref_value, amin,
+                      data_format):
+    """Non-negative least-squares inversion of a filterbank output, one launch: (b, t, n_bands, ch) /
+    (b, ch, t, n_bands) -> float32 (b, t, n_freq, ch) / (b, ch, t, n_freq) in the same data format (see
+    ``kapre_filterbank_invert``).  ``from_decibel``: the input is ``magnitude_to_decibel(., ref_value, amin)``.
+    No gradient: an input that requires grad under grad mode raises rather than being detached."""
+    if not x.is_cuda:
+        raise N.KapreNativeError('invert_filterbank needs a CUDA tensor')
+    if _wants_grad(x):
+        raise RuntimeError('InverseFilterbank is not differentiable: call it under torch.no_grad() or on a detached '
+                           'input')
+    if x.dtype != torch.float32:
+        x = x.float()
+    xd, (B, C, T, M) = _spec_desc(x, data_format)
+    if M != plan.n_bands:
+        raise ValueError('the filterbank has %d bands, the input has %d' % (plan.n_bands, M))
+    out, od = _spec_alloc(B, C, T, plan.n_freq, data_format, torch.float32, x.device)
+    if out.numel() == 0:
+        return out
+    cfg = N.FbInvCfg(int(n_iter), int(bool(from_decibel)), float(ref_value), float(amin))
+    N.check(N.lib().kapre_filterbank_invert(plan.handle(), ctypes.byref(cfg), _ptr(x), B, C, T, ctypes.byref(xd),
+                                            _ptr(out), ctypes.byref(od), _stream_ptr()))
+    return out
 
 
 @_device_of_first_arg

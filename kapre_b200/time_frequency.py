@@ -23,7 +23,7 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
 __all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
-           'PCEN', 'GriffinLim']
+           'PCEN', 'GriffinLim', 'InverseFilterbank']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -558,4 +558,79 @@ class GriffinLim(Layer):
         ('seed', 'seed'),
         ('input_data_format', 'input_data_format_original'),
         ('output_data_format', 'output_data_format_original'),
+    )
+
+
+def _positive(name, v):
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or \
+            not 0.0 < float(v) < math.inf:
+        raise ValueError('%s must be a positive finite number, got: %r' % (name, v))
+    return v
+
+
+@register_keras_serializable(package='Kapre')
+class InverseFilterbank(Layer):
+    """Linear magnitudes from a filterbank output: the inverse of ``ApplyFilterbank(type, filterbank_kwargs)``, by
+    non-negative least squares.  Use it with ``GriffinLim`` to hear a mel spectrogram
+    (``composed.get_inverse_melspectrogram_layer``).
+
+    ``(batch, time, n_bands, ch)`` / ``(batch, ch, time, n_bands)`` -> float32 ``(batch, time, n_freq, ch)`` /
+    ``(batch, ch, time, n_freq)`` in the same data format.  With ``A`` the ``(n_bands, n_freq)`` transpose of the
+    filterbank and ``m`` one frame, the layer runs ``n_iter`` steps of projected accelerated gradient (FISTA) on
+    ``min ||A s - m||^2`` subject to ``s >= 0``: ``s_0 = max(A^T (m / d), 0)`` with ``d = A A^T 1``, step
+    ``1 / ||A||_2^2``, and returns ``s_n``.  There are more bins than bands, so the minimiser is not unique: the result
+    is this iteration's, not the spectrum the mel came from.  Bins that no band touches (for a mel bank, DC, Nyquist
+    and bins above ``f_max``) come out exactly 0.  On consistent mel input the residual ``||A s - m||`` falls below
+    1e-3 of ``||m||`` within the default 100 iterations; torchaudio's ``InverseMelScale`` (least squares, then
+    ``relu``) leaves 1e-2 to 1e-1.
+
+    ``from_decibel=True`` takes the output of ``MagnitudeToDecibel(ref_value=db_ref_value, amin=db_amin)`` (e.g.
+    ``get_melspectrogram_layer(return_decibel=True)``) and converts each element on load with
+    ``m = 10^(v / 10) * max(db_amin, db_ref_value)``: the exact inverse where the input was at least ``db_amin`` and
+    the dynamic-range clamp did not bind; clamped elements come back as the clamp floor.
+
+    One kernel launch.  A frame's output does not depend on its place in the batch or on the data format.  No
+    gradient: calling the layer under grad mode on an input that requires grad raises ``RuntimeError``."""
+
+    def __init__(self, type, filterbank_kwargs, n_iter=100, from_decibel=False, db_ref_value=1.0, db_amin=1e-5,
+                 data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        if type == 'log':
+            self.filterbank = backend.filterbank_log(**filterbank_kwargs)
+        elif type == 'mel':
+            self.filterbank = backend.filterbank_mel(**filterbank_kwargs)
+        else:
+            raise ValueError("type must be 'mel' or 'log', got: %r" % (type,))
+        self.type = type
+        self.filterbank_kwargs = filterbank_kwargs
+        self.n_iter = _gl_int('n_iter', n_iter, 0)
+        if not isinstance(from_decibel, (bool, np.bool_)):
+            raise ValueError('from_decibel must be a bool, got: %r' % (from_decibel,))
+        self.from_decibel = bool(from_decibel)
+        self.db_ref_value = _positive('db_ref_value', db_ref_value)
+        self.db_amin = _positive('db_amin', db_amin)
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self._plan = None
+
+    @property
+    def plan(self) -> ops.FilterbankInversePlan:
+        if self._plan is None:
+            self._plan = ops.FilterbankInversePlan(np.asarray(self.filterbank))
+        return self._plan
+
+    def call(self, x):
+        return ops.invert_filterbank(x, self.plan, self.n_iter, self.from_decibel, self.db_ref_value, self.db_amin,
+                                     self.data_format)
+
+    _config_fields = (
+        ('type', 'type'),
+        ('filterbank_kwargs', 'filterbank_kwargs'),
+        ('n_iter', 'n_iter'),
+        ('from_decibel', 'from_decibel'),
+        ('db_ref_value', 'db_ref_value'),
+        ('db_amin', 'db_amin'),
+        ('data_format', 'data_format_original'),
     )
