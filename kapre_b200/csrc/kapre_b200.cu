@@ -11,6 +11,7 @@
 #include <string.h>
 #include <atomic>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/kapre_b200.h"
@@ -47,9 +48,9 @@ static std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_prof_events;
 struct KbProfScope {
     cudaStream_t st;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
-    explicit KbProfScope(cudaStream_t s) : st(s) {
+    KbProfScope(cudaStream_t s, bool timed) : st(s) {
         const int every = g_prof_on;
-        if (!every) return;
+        if (!timed || !every) return;
         // sampling: an event record between two kernels serialises them (no programmatic dependent
         // launch across it), so a stride > 1 leaves most launches of a timed loop undisturbed
         if ((g_prof_seq++ % (uint64_t)every) != 0) return;
@@ -80,6 +81,72 @@ static int kb_fail(int code, const char* fmt, ...) {
             return kb_fail(KAPRE_E_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e_), \
                            __FILE__, __LINE__);                                               \
     } while (0)
+
+template <typename K>
+static int kb_set_smem(K kernel, int smem) {
+    if (smem > 48 * 1024)
+        KB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    return 0;
+}
+
+// One kernel launch.  Every launch of the library goes through kb_launch, which fixes two policies:
+// - kapre_launch_count() counts each successful launch once;
+// - `timed` launches are the ones kapre_profile_read() (bench.py's kernel time) brackets with events.
+// `pdl`: programmatic dependent launch, so that the kernel is scheduled while the previous one in the stream drains.
+// Only kernels whose body waits for the grid dependency (griddepcontrol.wait) may be launched that way.
+// Call sites name the fields ({.grid = ..., .timed = true}; nvcc and its host compilers accept designated
+// initializers in C++17 mode), so which launches are timed reads off each call.
+struct KbLaunch {
+    int grid, block, smem = 0;
+    cudaStream_t st;
+    bool pdl = false, timed = false;
+};
+
+template <typename... P, typename... A>
+static int kb_launch(void (*kernel)(P...), const KbLaunch& l, A&&... args) {
+    int rc = kb_set_smem(kernel, l.smem);
+    if (rc) return rc;
+    KbProfScope prof(l.st, l.timed);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)l.grid);
+    cfg.blockDim = dim3((unsigned)l.block);
+    cfg.dynamicSmemBytes = (size_t)l.smem;
+    cfg.stream = l.st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = l.pdl ? 1 : 0;
+    KB_CUDA(cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...));
+    g_launches++;
+    return 0;
+}
+
+// SMs x resident threads per SM of the current device: the thread count the time-scan kernels (PCEN, time stretch)
+// size their time chunks against.
+static int kb_resident_threads(long long* threads) {
+    int dev = 0, sms = 0, per_sm = 0;
+    KB_CUDA(cudaGetDevice(&dev));
+    KB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    KB_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxThreadsPerMultiProcessor, dev));
+    *threads = (long long)sms * per_sm;
+    return 0;
+}
+
+// Grid of a persistent kernel whose CTAs loop over `tiles`: what fits on the device at once (a CTA that waited for a
+// slot would start its share of the tiles late), and no more CTAs than tiles.  The shared-memory attribute is set
+// first because the occupancy query needs it above 48 KiB.
+template <typename K>
+static int kb_resident_grid(K kernel, int block, int smem, long long tiles, int sm_count, int* grid) {
+    int rc = kb_set_smem(kernel, smem);
+    if (rc) return rc;
+    int per_sm = 0;
+    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem));
+    if (per_sm < 1) per_sm = 1;
+    const long long cap = (long long)sm_count * per_sm;
+    *grid = (int)(tiles < cap ? tiles : cap);
+    return 0;
+}
 
 // ------------------------------------------------------------------------------------------
 // __global__ wrappers
@@ -538,72 +605,24 @@ static bool kb_pick_fwd_cfg(const DevInfo& dev, int Q, int n_fft, int hop, int m
     return found;
 }
 
-template <typename K>
-static int kb_set_smem(K kernel, int smem) {
-    if (smem > 48 * 1024)
-        KB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    return 0;
-}
-
-// Launch of a kernel whose body starts with griddepcontrol.wait (kb_stft_cta): programmatic dependent
-// launch lets its table prologue overlap the tail of the previous kernel in the stream (the clamp of the
-// previous call).  Only kernels that contain the wait may be launched this way.
-template <typename Kern>
-static int kb_launch_pdl(Kern kernel, int grid, int block, int smem, cudaStream_t st, const KbStftParams& p) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3((unsigned)block);
-    cfg.dynamicSmemBytes = (size_t)smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = kb_env_int("KAPRE_B200_PDL_FWD", 1) ? 1 : 0;
-    KB_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
-    return 0;
-}
-
+// The fused forward kernels start with griddepcontrol.wait (kb_stft_cta), so they are launched with programmatic
+// dependent launch: their table prologue overlaps the tail of the previous kernel in the stream (the clamp of the
+// previous call).
 template <int Q, int MODE>
 static int kb_launch_stft_qm(const KbStftParams& p, int grid, int smem, cudaStream_t st) {
+    constexpr bool FB = MODE == KB_OUT_FB || MODE == KB_OUT_FB_DB;
+    void (*kernel)(KbStftParams) = kb_stft_kernel<Q, MODE>;
     if (p.n_warps > KB_MAX_WARPS) {
-        if constexpr (Q == 32 && (MODE == KB_OUT_FB || MODE == KB_OUT_FB_DB)) {
-            int rc = kb_set_smem(kb_stft_kernel_w16<Q, MODE>, smem);
-            if (rc) return rc;
-            KbProfScope prof(st);
-            if ((rc = kb_launch_pdl(kb_stft_kernel_w16<Q, MODE>, grid, p.n_warps * 32, smem, st, p))) return rc;
-            g_launches++;
-            return 0;
-        } else {
-            return kb_fail(KAPRE_E_UNSUPPORTED, "no 16-warp instantiation for Q=%d mode=%d", Q, MODE);
-        }
+        if constexpr (Q == 32 && FB) kernel = kb_stft_kernel_w16<Q, MODE>;
+        else return kb_fail(KAPRE_E_UNSUPPORTED, "no 16-warp instantiation for Q=%d mode=%d", Q, MODE);
+    } else if (Q == 16 && (p.variant & 2)) {
+        // the other form of the pair step (KAPRE_B200_PAIRED=0): the A/B alternative, n_fft 1024 only
+        kernel = kb_stft_kernel_v<16, MODE, 2>;
+    } else if constexpr (FB) {
+        if (p.fb_mma) kernel = kb_stft_kernel_mma<Q, MODE>;
     }
-    if constexpr (Q == 16) {
-        if (p.variant & 2) {   // the other form of the pair step (KAPRE_B200_PAIRED=0): the A/B alternative, n_fft 1024 only
-            int rc = kb_set_smem(kb_stft_kernel_v<Q, MODE, 2>, smem);
-            if (rc) return rc;
-            KbProfScope prof(st);
-            if ((rc = kb_launch_pdl(kb_stft_kernel_v<Q, MODE, 2>, grid, p.n_warps * 32, smem, st, p))) return rc;
-            g_launches++;
-            return 0;
-        }
-    }
-    if constexpr (MODE == KB_OUT_FB || MODE == KB_OUT_FB_DB) {
-        if (p.fb_mma) {
-            int rc = kb_set_smem(kb_stft_kernel_mma<Q, MODE>, smem);
-            if (rc) return rc;
-            KbProfScope prof(st);
-            if ((rc = kb_launch_pdl(kb_stft_kernel_mma<Q, MODE>, grid, p.n_warps * 32, smem, st, p))) return rc;
-            g_launches++;
-            return 0;
-        }
-    }
-    int rc = kb_set_smem(kb_stft_kernel<Q, MODE>, smem);
-    if (rc) return rc;
-    KbProfScope prof(st);
-    if ((rc = kb_launch_pdl(kb_stft_kernel<Q, MODE>, grid, p.n_warps * 32, smem, st, p))) return rc;
-    g_launches++;
-    return 0;
+    return kb_launch(kernel, {.grid = grid, .block = p.n_warps * 32, .smem = smem, .st = st,
+                              .pdl = kb_env_int("KAPRE_B200_PDL_FWD", 1) != 0, .timed = true}, p);
 }
 
 template <int Q>
@@ -623,28 +642,6 @@ template <int Q>
 __global__ void __launch_bounds__(KB_ISTFT_MAX_WARPS * 32, 4) kb_istft2_kernel(const __grid_constant__ KbIstftParams p) {
     extern __shared__ __align__(128) char kb_smem[];
     kb_istft2_cta<Q>(p, kb_smem, (int)blockIdx.x, (int)gridDim.x);
-}
-
-template <int Q>
-static int kb_launch_istft2(const KbIstftParams& p, int grid, int smem, cudaStream_t st) {
-    int rc = kb_set_smem(kb_istft2_kernel<Q>, smem);
-    if (rc) return rc;
-    KbProfScope prof(st);
-    kb_istft2_kernel<Q><<<grid, p.n_warps * 32, smem, st>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
-}
-
-template <int Q>
-static int kb_launch_istft(const KbIstftParams& p, int grid, int smem, cudaStream_t st) {
-    int rc = kb_set_smem(kb_istft_kernel<Q>, smem);
-    if (rc) return rc;
-    KbProfScope prof(st);
-    kb_istft_kernel<Q><<<grid, p.n_warps * 32, smem, st>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
 }
 
 
@@ -715,44 +712,26 @@ static bool kb_pick_mcfb_cfg(const DevInfo& dev, int Q, int n_fft, int hop, int 
     return found;
 }
 
-template <int Q, int MODE>
-static int kb_launch_stft_mcfb_qm(const KbStftParams& p, int grid, int smem, cudaStream_t st) {
-    int rc = kb_set_smem(kb_stft_mcfb_kernel<Q, MODE>, smem);
-    if (rc) return rc;
-    KbProfScope prof(st);
-    kb_stft_mcfb_kernel<Q, MODE><<<grid, p.n_warps * 32, smem, st>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
-}
-
 template <int Q>
 static int kb_launch_stft_mcfb(const KbStftParams& p, int grid, int smem, cudaStream_t st) {
-    if (p.mode == KB_OUT_FB) return kb_launch_stft_mcfb_qm<Q, KB_OUT_FB>(p, grid, smem, st);
-    if (p.mode == KB_OUT_FB_DB) return kb_launch_stft_mcfb_qm<Q, KB_OUT_FB_DB>(p, grid, smem, st);
-    return kb_fail(KAPRE_E_INVALID, "bad mode for the multi-channel filterbank kernel");
-}
-
-template <int Q, int MODE>
-static int kb_launch_stft_mc_qm(const KbStftParams& p, int grid, int smem, cudaStream_t st) {
-    int rc = kb_set_smem(kb_stft_mc_kernel<Q, MODE>, smem);
-    if (rc) return rc;
-    KbProfScope prof(st);
-    kb_stft_mc_kernel<Q, MODE><<<grid, p.n_warps * 32, smem, st>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    void (*kernel)(KbStftParams);
+    if (p.mode == KB_OUT_FB) kernel = kb_stft_mcfb_kernel<Q, KB_OUT_FB>;
+    else if (p.mode == KB_OUT_FB_DB) kernel = kb_stft_mcfb_kernel<Q, KB_OUT_FB_DB>;
+    else return kb_fail(KAPRE_E_INVALID, "bad mode for the multi-channel filterbank kernel");
+    return kb_launch(kernel, {.grid = grid, .block = p.n_warps * 32, .smem = smem, .st = st, .timed = true}, p);
 }
 
 template <int Q>
 static int kb_launch_stft_mc(const KbStftParams& p, int grid, int smem, cudaStream_t st) {
+    void (*kernel)(KbStftParams);
     switch (p.mode) {
-        case KB_OUT_COMPLEX: return kb_launch_stft_mc_qm<Q, KB_OUT_COMPLEX>(p, grid, smem, st);
-        case KB_OUT_MAG: return kb_launch_stft_mc_qm<Q, KB_OUT_MAG>(p, grid, smem, st);
-        case KB_OUT_MAG_DB: return kb_launch_stft_mc_qm<Q, KB_OUT_MAG_DB>(p, grid, smem, st);
-        case KB_OUT_MAG_PHASE: return kb_launch_stft_mc_qm<Q, KB_OUT_MAG_PHASE>(p, grid, smem, st);
+        case KB_OUT_COMPLEX: kernel = kb_stft_mc_kernel<Q, KB_OUT_COMPLEX>; break;
+        case KB_OUT_MAG: kernel = kb_stft_mc_kernel<Q, KB_OUT_MAG>; break;
+        case KB_OUT_MAG_DB: kernel = kb_stft_mc_kernel<Q, KB_OUT_MAG_DB>; break;
+        case KB_OUT_MAG_PHASE: kernel = kb_stft_mc_kernel<Q, KB_OUT_MAG_PHASE>; break;
+        default: return kb_fail(KAPRE_E_INVALID, "bad mode for the multi-channel kernel");
     }
-    return kb_fail(KAPRE_E_INVALID, "bad mode for the multi-channel kernel");
+    return kb_launch(kernel, {.grid = grid, .block = p.n_warps * 32, .smem = smem, .st = st, .timed = true}, p);
 }
 
 static int kb_check_device(const DevInfo& d) {
@@ -772,20 +751,9 @@ static int kb_launch_clamp(float* y, long long n_items, long long item_size, uns
     if (chunks > 64) chunks = 64;
     if (chunks < 1) chunks = 1;
     if (n_items * chunks > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many items for the clamp kernel");
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(n_items * chunks));
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = kb_env_int("KAPRE_B200_PDL", 1) ? 1 : 0;
-    KB_CUDA(cudaLaunchKernelEx(&cfg, kb_db_clamp_kernel, y, item_size, run, period, item_max, (unsigned int)n_items,
-                               (int)chunks, amin, db_mul, db_sub, dr));
-    g_launches++;
-    return 0;
+    return kb_launch(kb_db_clamp_kernel, {.grid = (int)(n_items * chunks), .block = 256, .st = st,
+                                          .pdl = kb_env_int("KAPRE_B200_PDL", 1) != 0},
+                     y, item_size, run, period, item_max, (unsigned int)n_items, (int)chunks, amin, db_mul, db_sub, dr);
 }
 
 static void kb_db_consts(const kapre_db_cfg* db, float* db_mul, float* db_sub) {
@@ -1022,16 +990,11 @@ int kapre_stft_forward(const kapre_stft_plan* plan, const float* x_dev, const ka
                     q.amin = db->amin; q.db_mul = db_mul; q.db_sub = db_sub; q.item_max = (unsigned int*)workspace_dev;
                     q.db_ftz = (db->amin >= 1.17549435e-38f) ? 1 : 0;
                 }
-                if ((rc = kb_set_smem(kb_mr_kernel, smem))) return rc;
                 const long long tiles = (long long)B * C * ((T + q.TF - 1) / q.TF);
                 const long long gmax = (long long)plan->dev.sm_count * bps;
                 const int grid = (int)(tiles < gmax ? tiles : gmax);
-                {
-                    KbProfScope prof(st);
-                    kb_mr_kernel<<<grid, NW * 32, smem, st>>>(q);
-                    KB_CUDA(cudaGetLastError());
-                    g_launches++;
-                }
+                if ((rc = kb_launch(kb_mr_kernel, {.grid = grid, .block = NW * 32, .smem = smem, .st = st, .timed = true}, q)))
+                    return rc;
                 char buf[160];
                 snprintf(buf, sizeof(buf), "MR P%d passes%d NW%d G%d grid%d smem%d bps%d frt%d", q.P, q.n_pass, NW, G, grid, smem, bps, FRT);
                 g_launch_info = buf;
@@ -1045,12 +1008,9 @@ int kapre_stft_forward(const kapre_stft_plan* plan, const float* x_dev, const ka
             return kb_fail(KAPRE_E_UNSUPPORTED, "n_fft=%d (prime factor above 5) has no fused filterbank/decibel path; chain the stand-alone ops", plan->n_fft);
         const KbDftSmem L = kb_dft_smem_layout(plan->n_fft, plan->win_eff);
         if (L.total > plan->dev.smem_optin) return kb_fail(KAPRE_E_UNSUPPORTED, "n_fft=%d has a prime factor above 5 and is too large for the direct-DFT kernel (%d B of shared memory needed)", plan->n_fft, L.total);
-        if ((rc = kb_set_smem(kb_dft_kernel, L.total))) return rc;
         long long tiles = (long long)B * C * p.n_tiles_t;
         int grid = (int)(tiles < plan->dev.sm_count * 4LL ? tiles : plan->dev.sm_count * 4LL);
-        kb_dft_kernel<<<grid, 256, L.total, st>>>(p);
-        KB_CUDA(cudaGetLastError());
-        g_launches++;
+        if ((rc = kb_launch(kb_dft_kernel, {.grid = grid, .block = 256, .smem = L.total, .st = st}, p))) return rc;
         {
             char buf[96];
             snprintf(buf, sizeof(buf), "DFT n_fft%d grid%d smem%d (direct O(N^2): prime factor > 5)", plan->n_fft, grid, L.total);
@@ -1083,18 +1043,9 @@ int kapre_stft_forward(const kapre_stft_plan* plan, const float* x_dev, const ka
             const long long tiles = (long long)B * C * q.n_tiles_t;
             if (tiles > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
             const int grid = (int)(tiles < plan->dev.sm_count ? tiles : plan->dev.sm_count);
-            if ((rc = kb_set_smem(kb_tc_mel_kernel, TL.total))) return rc;
-            {
-                KbProfScope prof(st);
-                cudaLaunchConfig_t lc{};
-                lc.gridDim = dim3((unsigned)grid); lc.blockDim = dim3(TCM_THREADS); lc.dynamicSmemBytes = (size_t)TL.total; lc.stream = st;
-                cudaLaunchAttribute attr[1];
-                attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-                attr[0].val.programmaticStreamSerializationAllowed = 1;
-                lc.attrs = attr; lc.numAttrs = kb_env_int("KAPRE_B200_PDL_FWD", 1) ? 1 : 0;
-                KB_CUDA(cudaLaunchKernelEx(&lc, kb_tc_mel_kernel, q));
-                g_launches++;
-            }
+            if ((rc = kb_launch(kb_tc_mel_kernel, {.grid = grid, .block = TCM_THREADS, .smem = TL.total, .st = st,
+                                                   .pdl = kb_env_int("KAPRE_B200_PDL_FWD", 1) != 0, .timed = true}, q)))
+                return rc;
             char buf[160];
             snprintf(buf, sizeof(buf), "TC wgmma n_fft1024 hop%d grid%d smem%d tiles%lld", plan->hop, grid, TL.total, tiles);
             g_launch_info = buf;
@@ -1280,13 +1231,9 @@ int kapre_istft_inverse(const kapre_istft_plan* plan, const void* stft_dev, int 
         p.n_warps = 8; p.n_tiles_s = (int)((out_len + 255) / 256);
         const int smem = plan->n_fft * 8;
         if (smem > plan->dev.smem_optin) return kb_fail(KAPRE_E_UNSUPPORTED, "n_fft too large");
-        if ((rc = kb_set_smem(kb_idft_kernel, smem))) return rc;
         long long tiles = (long long)batch * channels * p.n_tiles_s;
         int grid = (int)(tiles < plan->dev.sm_count * 8LL ? tiles : plan->dev.sm_count * 8LL);
-        kb_idft_kernel<<<grid, 256, smem, st>>>(p);
-        KB_CUDA(cudaGetLastError());
-        g_launches++;
-        return 0;
+        return kb_launch(kb_idft_kernel, {.grid = grid, .block = 256, .smem = smem, .st = st}, p);
     }
 
     const int Q = plan->Q, FPW = 32 / Q;
@@ -1333,13 +1280,15 @@ int kapre_istft_inverse(const kapre_istft_plan* plan, const void* stft_dev, int 
                 snprintf(buf, sizeof(buf), "ISTFT2 Q%d NW%d seg%d rounds%d tiles%lld grid%d smem%d bps%d", Q, NW, best_seg, best_m, tiles, grid, L2.total, bps);
                 g_launch_info = buf;
             }
+            void (*kernel)(KbIstftParams);
             switch (Q) {
-                case 4: return kb_launch_istft2<4>(p, grid, L2.total, st);
-                case 8: return kb_launch_istft2<8>(p, grid, L2.total, st);
-                case 16: return kb_launch_istft2<16>(p, grid, L2.total, st);
-                case 32: return kb_launch_istft2<32>(p, grid, L2.total, st);
+                case 4: kernel = kb_istft2_kernel<4>; break;
+                case 8: kernel = kb_istft2_kernel<8>; break;
+                case 16: kernel = kb_istft2_kernel<16>; break;
+                case 32: kernel = kb_istft2_kernel<32>; break;
                 default: return kb_fail(KAPRE_E_UNSUPPORTED, "bad Q");
             }
+            return kb_launch(kernel, {.grid = grid, .block = NW * 32, .smem = L2.total, .st = st, .timed = true}, p);
         }
     }
     // one FFT round per overlap class: TFc = R * NW * FPW frames per tile
@@ -1368,14 +1317,15 @@ int kapre_istft_inverse(const kapre_istft_plan* plan, const void* stft_dev, int 
     if (tiles > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
     const long long gmax = (long long)plan->dev.sm_count * bps;
     const int grid = (int)(tiles < gmax ? tiles : gmax);
+    void (*kernel)(KbIstftParams);
     switch (Q) {
-        case 4: rc = kb_launch_istft<4>(p, grid, smem, st); break;
-        case 8: rc = kb_launch_istft<8>(p, grid, smem, st); break;
-        case 16: rc = kb_launch_istft<16>(p, grid, smem, st); break;
-        case 32: rc = kb_launch_istft<32>(p, grid, smem, st); break;
-        default: rc = kb_fail(KAPRE_E_UNSUPPORTED, "bad Q");
+        case 4: kernel = kb_istft_kernel<4>; break;
+        case 8: kernel = kb_istft_kernel<8>; break;
+        case 16: kernel = kb_istft_kernel<16>; break;
+        case 32: kernel = kb_istft_kernel<32>; break;
+        default: return kb_fail(KAPRE_E_UNSUPPORTED, "bad Q");
     }
-    return rc;
+    return kb_launch(kernel, {.grid = grid, .block = NW * 32, .smem = smem, .st = st, .timed = true}, p);
 }
 
 int kapre_filterbank_create(const float* fb_host, int n_freq, int n_bands, kapre_filterbank** out) {
@@ -1437,17 +1387,13 @@ int kapre_apply_filterbank(const kapre_filterbank* fb, const float* x_dev, int b
         return kb_fail(KAPRE_E_UNSUPPORTED, "filterbank %dx%d does not fit shared memory", fb->n_freq, fb->n_bands);
     p.n_tiles_t = (frames + p.R - 1) / p.R; p.n_warps = 8;
     const KbFbSmem L = kb_fb_smem_layout(fb->n_freq, fb->n_bands, p.R);
-    if ((rc = kb_set_smem(kb_fb_kernel, L.total))) return rc;
     int bps = (228 * 1024) / (L.total + 1024);
     if (bps > 8) bps = 8;
     if (bps < 1) bps = 1;
     const long long tiles = (long long)batch * channels * p.n_tiles_t;
     const long long gmax = (long long)fb->dev.sm_count * bps;
     const int grid = (int)(tiles < gmax ? tiles : gmax);
-    kb_fb_kernel<<<grid, 256, L.total, (cudaStream_t)stream>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_fb_kernel, {.grid = grid, .block = 256, .smem = L.total, .st = (cudaStream_t)stream}, p);
 }
 
 static int kb_ew_grid(int64_t n, int* grid) {
@@ -1467,10 +1413,8 @@ int kapre_magnitude(const void* x_complex_dev, float* out_dev, int64_t n, void* 
     if (!x_complex_dev || !out_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_magnitude_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float2*)x_complex_dev, out_dev, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_magnitude_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream},
+                     (const float2*)x_complex_dev, out_dev, n);
 }
 
 int kapre_phase(const void* x_complex_dev, float* out_dev, int64_t n, void* stream) {
@@ -1479,10 +1423,8 @@ int kapre_phase(const void* x_complex_dev, float* out_dev, int64_t n, void* stre
     if (!x_complex_dev || !out_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_phase_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float2*)x_complex_dev, out_dev, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_phase_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream},
+                     (const float2*)x_complex_dev, out_dev, n);
 }
 
 int kapre_concat_frequency_map(const float* x_dev, float* out_dev, int64_t batch, int64_t channels, int64_t frames,
@@ -1493,10 +1435,8 @@ int kapre_concat_frequency_map(const float* x_dev, float* out_dev, int64_t batch
     if (!out_dev || (!x_dev && channels > 0)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(total, &grid))) return rc;
-    kb_concat_freq_map_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x_dev, out_dev, batch, channels, frames, n_freq, channels_last ? 1 : 0);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_concat_freq_map_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, x_dev, out_dev,
+                     batch, channels, frames, n_freq, channels_last ? 1 : 0);
 }
 
 int kapre_spec_augment(const float* x_dev, float* out_dev, int64_t batch, int64_t frames, int64_t n_freq,
@@ -1509,11 +1449,8 @@ int kapre_spec_augment(const float* x_dev, float* out_dev, int64_t batch, int64_
         return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(total, &grid))) return rc;
-    kb_spec_augment_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x_dev, out_dev, batch, frames, n_freq, time_masks_dev,
-                                                                 n_time_masks, freq_masks_dev, n_freq_masks, mask_value);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_spec_augment_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, x_dev, out_dev,
+                     batch, frames, n_freq, time_masks_dev, n_time_masks, freq_masks_dev, n_freq_masks, mask_value);
 }
 
 static int kb_frames_for(int L, int fl, int hop, int pad_end) {
@@ -1535,10 +1472,8 @@ int kapre_delta(const float* x_dev, float* out_dev, int64_t outer, int64_t frame
     for (int m = 1; m <= n; ++m) denom += 2.0 * m * m;
     int grid, rc;
     if ((rc = kb_ew_grid(total, &grid))) return rc;
-    kb_delta_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x_dev, out_dev, outer, frames, inner, n, (float)(1.0 / denom), pad_mode);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_delta_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, x_dev, out_dev, outer,
+                     frames, inner, n, (float)(1.0 / denom), pad_mode);
 }
 
 int kapre_frame(const float* x_dev, const kapre_wave_desc* xd, int frame_length, int hop_length, int pad_end, float pad_value,
@@ -1551,12 +1486,9 @@ int kapre_frame(const float* x_dev, const kapre_wave_desc* xd, int frame_length,
     if (!x_dev || !out_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(total, &grid))) return rc;
-    kb_frame_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x_dev, xd->stride_b, xd->stride_c, xd->stride_l, xd->batch,
-                                                          xd->channels, xd->length, frame_length, hop_length, T, pad_value,
-                                                          out_dev, od->stride_b, od->stride_c, od->stride_t, od->stride_f);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_frame_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, x_dev, xd->stride_b,
+                     xd->stride_c, xd->stride_l, xd->batch, xd->channels, xd->length, frame_length, hop_length, T,
+                     pad_value, out_dev, od->stride_b, od->stride_c, od->stride_t, od->stride_f);
 }
 
 int kapre_energy(const float* x_dev, const kapre_wave_desc* xd, int frame_length, int hop_length, int pad_end, float pad_value,
@@ -1570,12 +1502,9 @@ int kapre_energy(const float* x_dev, const kapre_wave_desc* xd, int frame_length
     if (od->length != T) return kb_fail(KAPRE_E_INVALID, "output must have %d frames, got %d", T, od->length);
     int grid, rc;
     if ((rc = kb_ew_grid(n_frames * 32, &grid))) return rc;
-    kb_energy_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x_dev, xd->stride_b, xd->stride_c, xd->stride_l, xd->batch,
-                                                           xd->channels, xd->length, frame_length, hop_length, T, pad_value,
-                                                           scale, out_dev, od->stride_b, od->stride_c, od->stride_l);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_energy_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, x_dev, xd->stride_b,
+                     xd->stride_c, xd->stride_l, xd->batch, xd->channels, xd->length, frame_length, hop_length, T,
+                     pad_value, scale, out_dev, od->stride_b, od->stride_c, od->stride_l);
 }
 
 int kapre_magnitude_to_decibel(const float* x_dev, float* out_dev, int64_t n_items, int64_t item_size,
@@ -1593,10 +1522,9 @@ int kapre_magnitude_to_decibel(const float* x_dev, float* out_dev, int64_t n_ite
     if (chunks < 1) chunks = 1;
     const long long grid = n_items * chunks;
     if (grid > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many items");
-    kb_db_kernel<<<(unsigned)grid, 256, 0, st>>>(x_dev, out_dev, item_size, (int)chunks, (unsigned int*)workspace_dev,
-                                                 db->amin, db_mul, db_sub);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
+    if ((rc = kb_launch(kb_db_kernel, {.grid = (int)grid, .block = 256, .st = st}, x_dev, out_dev, item_size, (int)chunks,
+                        (unsigned int*)workspace_dev, db->amin, db_mul, db_sub)))
+        return rc;
     return kb_launch_clamp(out_dev, n_items, item_size, (unsigned int*)workspace_dev, db->amin, db_mul, db_sub,
                            db->dynamic_range, st);
 }
@@ -1647,12 +1575,8 @@ int kapre_tc_dft_stage1(const float* x_dev, int n_items, long long item_stride, 
     const long long gmax = (long long)dev.sm_count * 2;
     const int grid = (int)(tiles < gmax ? tiles : gmax);
     if (grid_out) *grid_out = grid;
-    if ((rc = kb_set_smem(kb_tc_dft_stage1_kernel, KB_TC_SMEM))) return rc;
-    KbProfScope prof((cudaStream_t)stream);
-    kb_tc_dft_stage1_kernel<<<grid, KB_TC_THREADS, KB_TC_SMEM, (cudaStream_t)stream>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_tc_dft_stage1_kernel, {.grid = grid, .block = KB_TC_THREADS, .smem = KB_TC_SMEM,
+                                               .st = (cudaStream_t)stream, .timed = true}, p);
 }
 
 }  // extern "C"
@@ -1816,10 +1740,7 @@ int kapre_stft_backward(const kapre_stft_plan* plan, const void* g_dev, const ka
     }
     int grid;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_stft_adj_kernel<<<grid, 256, 0, st>>>(q, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_stft_adj_kernel, {.grid = grid, .block = 256, .st = st}, q, n);
 }
 
 int kapre_istft_backward(const kapre_istft_plan* plan, const float* gy_dev, const kapre_wave_desc* yd, int batch,
@@ -1846,10 +1767,7 @@ int kapre_istft_backward(const kapre_istft_plan* plan, const float* gy_dev, cons
     const long long n = (long long)batch * channels * frames * ((plan->n_fft & 1) ? 1 : 2);
     int grid;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_istft_adj_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(q, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_istft_adj_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, q, n);
 }
 
 int kapre_magnitude_backward(const void* x_complex_dev, const float* g_dev, void* gx_complex_dev, int64_t n, void* stream) {
@@ -1858,10 +1776,8 @@ int kapre_magnitude_backward(const void* x_complex_dev, const float* g_dev, void
     if (!x_complex_dev || !g_dev || !gx_complex_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_mag_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float2*)x_complex_dev, g_dev, (float2*)gx_complex_dev, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_mag_bwd_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream},
+                     (const float2*)x_complex_dev, g_dev, (float2*)gx_complex_dev, n);
 }
 
 int kapre_magnitude_to_decibel_backward(const float* x_dev, const float* g_dev, float* gx_dev, int64_t n_items,
@@ -1883,13 +1799,10 @@ int kapre_magnitude_to_decibel_backward(const float* x_dev, const float* g_dev, 
     if (chunks < 1) chunks = 1;
     const long long grid = n_items * chunks;
     if (grid > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many items");
-    kb_dbb_kernel<0><<<(unsigned)grid, 256, 0, st>>>(p, (int)chunks);
-    KB_CUDA(cudaGetLastError());
-    kb_dbb_kernel<1><<<(unsigned)grid, 256, 0, st>>>(p, (int)chunks);
-    KB_CUDA(cudaGetLastError());
-    kb_dbb_kernel<2><<<(unsigned)grid, 256, 0, st>>>(p, (int)chunks);
-    KB_CUDA(cudaGetLastError());
-    g_launches += 3;
+    const KbLaunch l{.grid = (int)grid, .block = 256, .st = st};
+    if ((rc = kb_launch(kb_dbb_kernel<0>, l, p, (int)chunks)) || (rc = kb_launch(kb_dbb_kernel<1>, l, p, (int)chunks)) ||
+        (rc = kb_launch(kb_dbb_kernel<2>, l, p, (int)chunks)))
+        return rc;
     KB_CUDA(cudaMemsetAsync(workspace_dev, 0, (size_t)n_items * 3 * sizeof(unsigned int), st));   // self-cleaning
     return 0;
 }
@@ -1900,10 +1813,8 @@ int kapre_phase_backward(const void* x_complex_dev, const float* g_dev, void* gx
     if (!x_complex_dev || !g_dev || !gx_complex_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_phase_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float2*)x_complex_dev, g_dev, (float2*)gx_complex_dev, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_phase_bwd_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream},
+                     (const float2*)x_complex_dev, g_dev, (float2*)gx_complex_dev, n);
 }
 
 int kapre_mag_phase_backward(const void* x_complex_dev, const kapre_spec_desc* x_desc, const float* g_mag_dev,
@@ -1930,10 +1841,7 @@ int kapre_mag_phase_backward(const void* x_complex_dev, const kapre_spec_desc* x
     p.c_inner = (channels > 1 && gx_desc->stride_c < gx_desc->stride_f) ? 1 : 0;   // channels_last: walk c fastest
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_mag_phase_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_mag_phase_bwd_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, p, n);
 }
 
 int kapre_delta_backward(const float* g_dev, float* gx_dev, int64_t outer, int64_t frames, int64_t inner, int win_length,
@@ -1950,11 +1858,8 @@ int kapre_delta_backward(const float* g_dev, float* gx_dev, int64_t outer, int64
     for (int m = 1; m <= n; ++m) denom += 2.0 * m * m;
     int grid, rc;
     if ((rc = kb_ew_grid(total, &grid))) return rc;
-    kb_delta_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(g_dev, gx_dev, frames, inner, n, (float)(1.0 / denom),
-                                                              pad_mode, total);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_delta_bwd_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, g_dev, gx_dev, frames,
+                     inner, n, (float)(1.0 / denom), pad_mode, total);
 }
 
 // the frame counts kapre_frame / kapre_energy give `length` samples (pad_end off, on): the gradient must have one of them
@@ -1980,10 +1885,7 @@ int kapre_frame_backward(const float* g_dev, const kapre_spec_desc* g_desc, int 
     p.C = gx_desc->channels; p.L = gx_desc->length; p.T = frames; p.fl = frame_length; p.hop = hop_length;
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_frame_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_frame_bwd_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, p, n);
 }
 
 int kapre_energy_backward(const float* x_dev, const kapre_wave_desc* x_desc, const float* g_dev,
@@ -2011,10 +1913,7 @@ int kapre_energy_backward(const float* x_dev, const kapre_wave_desc* x_desc, con
     p.scale2 = 2.0f * scale;
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_energy_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_energy_bwd_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, p, n);
 }
 
 int kapre_concat_frequency_map_backward(const float* g_dev, float* gx_dev, int64_t batch, int64_t channels,
@@ -2025,11 +1924,8 @@ int kapre_concat_frequency_map_backward(const float* g_dev, float* gx_dev, int64
     if (!g_dev || !gx_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     int grid, rc;
     if ((rc = kb_ew_grid(n, &grid))) return rc;
-    kb_concat_fm_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(g_dev, gx_dev, channels, frames, n_freq,
-                                                                  channels_last ? 1 : 0, n);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    return kb_launch(kb_concat_fm_bwd_kernel, {.grid = grid, .block = 256, .st = (cudaStream_t)stream}, g_dev, gx_dev,
+                     channels, frames, n_freq, channels_last ? 1 : 0, n);
 }
 
 }  // extern "C"
@@ -2123,21 +2019,12 @@ static int kb_resample_launch(const kapre_resample_plan* plan, const float* x_de
     if (p.NT == 0)
         return kb_fail(KAPRE_E_UNSUPPORTED, "%d channels of a %d:%d resampler do not fit in shared memory", p.G, plan->up, plan->down);
     if (!kb_resample_setup(p, KB_RESAMPLE_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
-    const long long tiles = p.n_tiles;
     const int smem = kb_resample_smem(p.up, p.Kp, p.NT, p.down, p.G);
-    KB_CUDA(cudaFuncSetAttribute(kb_resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int per_sm = 0;
-    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kb_resample_kernel, KB_RESAMPLE_THREADS, smem));
-    if (per_sm < 1) per_sm = 1;
-    const long long cap = (long long)plan->dev.sm_count * per_sm;
-    const int grid = (int)(tiles < cap ? tiles : cap);
-    {
-        KbProfScope prof((cudaStream_t)stream);
-        kb_resample_kernel<<<grid, KB_RESAMPLE_THREADS, smem, (cudaStream_t)stream>>>(p);
-    }
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    int grid, rc;
+    if ((rc = kb_resident_grid(kb_resample_kernel, KB_RESAMPLE_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_resample_kernel, {.grid = grid, .block = KB_RESAMPLE_THREADS, .smem = smem,
+                                          .st = (cudaStream_t)stream, .timed = true}, p);
 }
 
 extern "C" {
@@ -2212,11 +2099,10 @@ __global__ void __launch_bounds__(KB_PCEN_THREADS) kb_pcen_bwd_kernel(const __gr
 
 // Chunking of n_cols columns of `frames` frames against the current device's resident-thread capacity.
 static int kb_pcen_pick_chunks(long long n_cols, int frames, int* chunks) {
-    int dev = 0, sms = 0, per_sm = 0;
-    KB_CUDA(cudaGetDevice(&dev));
-    KB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    KB_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxThreadsPerMultiProcessor, dev));
-    *chunks = kb_pcen_chunks(n_cols, frames, (long long)sms * per_sm);
+    long long threads = 0;
+    int rc = kb_resident_threads(&threads);
+    if (rc) return rc;
+    *chunks = kb_pcen_chunks(n_cols, frames, threads);
     return 0;
 }
 
@@ -2240,19 +2126,6 @@ static int kb_pcen_setup(KbPcenParams& p, const kapre_spec_desc* E_desc, int bat
     int K = 1, rc;
     if (p.n_cols * frames > 0 && (rc = kb_pcen_pick_chunks(p.n_cols, frames, &K))) return rc;
     kb_pcen_set_chunks(p, K);
-    return 0;
-}
-
-template <typename Kern>
-static int kb_pcen_launch(Kern kernel, const KbPcenParams& p, long long n, cudaStream_t st) {
-    const long long grid = (n + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS;
-    if (grid > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many PCEN columns");
-    {
-        KbProfScope prof(st);
-        kernel<<<(int)grid, KB_PCEN_THREADS, 0, st>>>(p, n);
-    }
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
     return 0;
 }
 
@@ -2289,9 +2162,15 @@ int kapre_pcen(const float* E_dev, const kapre_spec_desc* E_desc, int batch, int
     p.M = M_dev;
     if (M_dev) { p.m_sb = M_desc->stride_b; p.m_sc = M_desc->stride_c; p.m_st = M_desc->stride_t; p.m_sf = M_desc->stride_f; }
     p.state = (float*)workspace_dev;
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (p.K > 1 && (rc = kb_pcen_launch(kb_pcen_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
-    return kb_pcen_launch(kb_pcen_kernel, p, (long long)p.K * p.n_cols, st);
+    // one thread per (chunk, column): the state pass covers chunks 0 .. K - 2, the output pass all K
+    const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
+    const long long grid = (n + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS;
+    if (grid > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many PCEN columns");
+    const KbLaunch l{.grid = (int)grid, .block = KB_PCEN_THREADS, .st = (cudaStream_t)stream, .timed = true};
+    if (p.K > 1 && (rc = kb_launch(kb_pcen_state_kernel, {.grid = (int)((ns + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS),
+                                                          .block = KB_PCEN_THREADS, .st = l.st, .timed = true}, p, ns)))
+        return rc;
+    return kb_launch(kb_pcen_kernel, l, p, n);
 }
 
 int kapre_pcen_backward(const float* E_dev, const kapre_spec_desc* E_desc, const float* M_dev,
@@ -2320,9 +2199,14 @@ int kapre_pcen_backward(const float* E_dev, const kapre_spec_desc* E_desc, const
     p.gE = gE_dev; p.o_sb = gE_desc->stride_b; p.o_sc = gE_desc->stride_c; p.o_st = gE_desc->stride_t; p.o_sf = gE_desc->stride_f;
     p.state = (float*)workspace_dev;
     p.part = param_partials_dev;
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (p.K > 1 && (rc = kb_pcen_launch(kb_pcen_bwd_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
-    return kb_pcen_launch(kb_pcen_bwd_kernel, p, (long long)p.K * p.n_cols, st);
+    const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
+    const long long grid = (n + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS;
+    if (grid > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many PCEN columns");
+    const KbLaunch l{.grid = (int)grid, .block = KB_PCEN_THREADS, .st = (cudaStream_t)stream, .timed = true};
+    if (p.K > 1 && (rc = kb_launch(kb_pcen_bwd_state_kernel, {.grid = (int)((ns + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS),
+                                                              .block = KB_PCEN_THREADS, .st = l.st, .timed = true}, p, ns)))
+        return rc;
+    return kb_launch(kb_pcen_bwd_kernel, l, p, n);
 }
 
 }  // extern "C"
@@ -2339,16 +2223,6 @@ __global__ void __launch_bounds__(KB_GL_THREADS) kb_gl_project_kernel(const __gr
 
 // Workspace layout: spectrum buffers 0 and 1 (each n complex64, rounded up to 256 B), then the (B, C, L) waveform.
 static long long kb_gl_spec_bytes(long long n) { return (n * 8 + 255) / 256 * 256; }
-
-template <typename Kern>
-static int kb_gl_launch(Kern kernel, const KbGlParams& p, cudaStream_t st) {
-    int grid, rc;
-    if ((rc = kb_ew_grid(p.n, &grid))) return rc;
-    kernel<<<grid, KB_GL_THREADS, 0, st>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
-}
 
 extern "C" {
 
@@ -2400,10 +2274,12 @@ int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft
     float* wave = (float*)((char*)workspace_dev + 2 * kb_gl_spec_bytes(p.n));
     const kapre_spec_desc sd = {(int64_t)channels * frames * F, (int64_t)frames * F, F, 1};
     const kapre_wave_desc wd = {batch, channels, (int32_t)L, (int64_t)channels * L, L, 1};
-    const cudaStream_t st = (cudaStream_t)stream;
+    int grid;
+    if ((rc = kb_ew_grid(p.n, &grid))) return rc;
+    const KbLaunch l{.grid = grid, .block = KB_GL_THREADS, .st = (cudaStream_t)stream};
 
     p.X = X[0];
-    if ((rc = kb_gl_launch(kb_gl_init_kernel, p, st))) return rc;
+    if ((rc = kb_launch(kb_gl_init_kernel, l, p))) return rc;
     int cur = 0;
     for (int it = 0; it < cfg->n_iter; ++it) {
         // X (buffer cur) -> waveform -> Y over X in buffer cur; the new X goes over Yprev in the other buffer
@@ -2414,7 +2290,7 @@ int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft
         p.Y = X[cur];
         p.Yprev = (it > 0 && p.beta != 0.0f) ? X[1 - cur] : nullptr;
         p.X = X[1 - cur];
-        if ((rc = kb_gl_launch(kb_gl_project_kernel, p, st))) return rc;
+        if ((rc = kb_launch(kb_gl_project_kernel, l, p))) return rc;
         cur = 1 - cur;
     }
     return kapre_istft_inverse(istft, X[cur], batch, channels, frames, &sd, y_dev, y_desc, stream);
@@ -2464,11 +2340,10 @@ static int kb_ts_setup(KbTsParams& p, const kapre_spec_desc* X_desc, int batch, 
     p.c_inner = channels > 1 && llabs(X_desc->stride_c) < llabs(X_desc->stride_f) ? 1 : 0;
     int K = 1;
     if (p.n_cols * frames > 0) {
-        int dev = 0, sms = 0, per_sm = 0;
-        KB_CUDA(cudaGetDevice(&dev));
-        KB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        KB_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxThreadsPerMultiProcessor, dev));
-        K = kb_ts_chunks(p.n_cols, frames, (long long)sms * per_sm);
+        long long threads = 0;
+        int rc = kb_resident_threads(&threads);
+        if (rc) return rc;
+        K = kb_ts_chunks(p.n_cols, frames, threads);
     }
     kb_ts_set_chunks(p, K);
     return 0;
@@ -2492,19 +2367,6 @@ static bool kb_ts_overlap(const void* p, const kapre_spec_desc* pd, int pt, cons
     kb_ts_span(p, pd, B, C, pt, F, &a0, &a1);
     kb_ts_span(q, qd, B, C, qt, F, &b0, &b1);
     return a0 < b1 && b0 < a1;
-}
-
-template <typename Kern>
-static int kb_ts_launch(Kern kernel, const KbTsParams& p, long long n, cudaStream_t st) {
-    const long long grid = (n + KB_TS_THREADS - 1) / KB_TS_THREADS;
-    if ((long long)p.K * p.n_cols > 0xffffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many time-stretch columns");
-    {
-        KbProfScope prof(st);
-        kernel<<<(int)grid, KB_TS_THREADS, 0, st>>>(p, n);
-    }
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
 }
 
 extern "C" {
@@ -2536,9 +2398,15 @@ int kapre_time_stretch(const void* X_dev, const kapre_spec_desc* X_desc, int bat
     p.X = (const float2*)X_dev;
     p.Y = (float2*)Y_dev; p.y_sb = Y_desc->stride_b; p.y_sc = Y_desc->stride_c; p.y_st = Y_desc->stride_t; p.y_sf = Y_desc->stride_f;
     p.state = workspace_dev;
+    // one thread per (chunk, column): the state pass covers chunks 0 .. K - 2, the output pass all K
+    const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
+    if (n > 0xffffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many time-stretch columns");
     const cudaStream_t st = (cudaStream_t)stream;
-    if (p.K > 1 && (rc = kb_ts_launch(kb_ts_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
-    return kb_ts_launch(kb_ts_kernel, p, (long long)p.K * p.n_cols, st);
+    if (p.K > 1 && (rc = kb_launch(kb_ts_state_kernel, {.grid = (int)((ns + KB_TS_THREADS - 1) / KB_TS_THREADS),
+                                                        .block = KB_TS_THREADS, .st = st, .timed = true}, p, ns)))
+        return rc;
+    return kb_launch(kb_ts_kernel, {.grid = (int)((n + KB_TS_THREADS - 1) / KB_TS_THREADS), .block = KB_TS_THREADS,
+                                    .st = st, .timed = true}, p, n);
 }
 
 int kapre_time_stretch_backward(const void* X_dev, const kapre_spec_desc* X_desc, const void* Y_dev,
@@ -2565,9 +2433,14 @@ int kapre_time_stretch_backward(const void* X_dev, const kapre_spec_desc* X_desc
     p.gX = (float2*)gX_dev;
     p.o_sb = gX_desc->stride_b; p.o_sc = gX_desc->stride_c; p.o_st = gX_desc->stride_t; p.o_sf = gX_desc->stride_f;
     p.state = workspace_dev;
+    const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
+    if (n > 0xffffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many time-stretch columns");
     const cudaStream_t st = (cudaStream_t)stream;
-    if (p.K > 1 && (rc = kb_ts_launch(kb_ts_bwd_state_kernel, p, (long long)(p.K - 1) * p.n_cols, st))) return rc;
-    return kb_ts_launch(kb_ts_bwd_kernel, p, (long long)p.K * p.n_cols, st);
+    if (p.K > 1 && (rc = kb_launch(kb_ts_bwd_state_kernel, {.grid = (int)((ns + KB_TS_THREADS - 1) / KB_TS_THREADS),
+                                                            .block = KB_TS_THREADS, .st = st, .timed = true}, p, ns)))
+        return rc;
+    return kb_launch(kb_ts_bwd_kernel, {.grid = (int)((n + KB_TS_THREADS - 1) / KB_TS_THREADS), .block = KB_TS_THREADS,
+                                        .st = st, .timed = true}, p, n);
 }
 
 }  // extern "C"
@@ -2651,18 +2524,9 @@ int kapre_filterbank_invert(const kapre_fb_inverse_plan* plan, const kapre_fb_in
     const long long tiles = (long long)batch * channels * p.n_tiles_t;
     if (tiles > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many frames");
     const int smem = kb_fbi_smem_layout(plan->n_freq, plan->n_bands, p.R).total;
-    if ((rc = kb_set_smem(kb_fbi_kernel, smem))) return rc;
-    // the CTAs loop over tiles, so the grid is what fits on the device at once (a CTA that waited for a slot would
-    // start its share of the tiles late)
-    int bps = 0;
-    KB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kb_fbi_kernel, KB_FBI_WARPS * 32, smem));
-    if (bps < 1) bps = 1;
-    const long long gmax = (long long)plan->dev.sm_count * bps;
-    const int grid = (int)(tiles < gmax ? tiles : gmax);
-    kb_fbi_kernel<<<grid, KB_FBI_WARPS * 32, smem, (cudaStream_t)stream>>>(p);
-    KB_CUDA(cudaGetLastError());
-    g_launches++;
-    return 0;
+    int grid;
+    if ((rc = kb_resident_grid(kb_fbi_kernel, KB_FBI_WARPS * 32, smem, tiles, plan->dev.sm_count, &grid))) return rc;
+    return kb_launch(kb_fbi_kernel, {.grid = grid, .block = KB_FBI_WARPS * 32, .smem = smem, .st = (cudaStream_t)stream}, p);
 }
 
 }  // extern "C"

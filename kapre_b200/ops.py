@@ -127,15 +127,12 @@ class _Handle:
             pass
 
 
-class StftPlan:
-    """kapre_stft_plan per CUDA device for one (n_fft, win_length, hop, window)."""
+class _PerDevice:
+    """One C-ABI object per CUDA device, made on first use on that device.  Subclasses set ``_per_device = {}`` in
+    their constructor, name the destroy function in ``_destroy`` and make the object in ``_create(lib, out)``, which
+    returns the library's status and writes the new pointer through ``out``."""
 
-    def __init__(self, n_fft, win_length, hop_length, window: np.ndarray):
-        self.n_fft, self.win_length, self.hop_length = int(n_fft), int(win_length), int(hop_length)
-        self.window = np.ascontiguousarray(window, dtype=np.float32)
-        if self.window.shape != (self.win_length,):
-            raise ValueError('window must have win_length=%d samples, got %s' % (self.win_length, self.window.shape))
-        self._per_device = {}
+    _destroy = None
 
     def handle(self):
         _require_cuda()
@@ -145,11 +142,27 @@ class StftPlan:
             if h is None:
                 lib = N.lib()
                 out = ctypes.c_void_p()
-                N.check(lib.kapre_stft_plan_create(self.n_fft, self.win_length, self.hop_length,
-                                                   self.window.ctypes.data_as(ctypes.c_void_p), ctypes.byref(out)))
-                h = _Handle(out, lib.kapre_stft_plan_destroy)
+                N.check(self._create(lib, ctypes.byref(out)))
+                h = _Handle(out, getattr(lib, self._destroy))
                 self._per_device[dev] = h
         return h.ptr
+
+
+class StftPlan(_PerDevice):
+    """kapre_stft_plan per CUDA device for one (n_fft, win_length, hop, window)."""
+
+    def __init__(self, n_fft, win_length, hop_length, window: np.ndarray):
+        self.n_fft, self.win_length, self.hop_length = int(n_fft), int(win_length), int(hop_length)
+        self.window = np.ascontiguousarray(window, dtype=np.float32)
+        if self.window.shape != (self.win_length,):
+            raise ValueError('window must have win_length=%d samples, got %s' % (self.win_length, self.window.shape))
+        self._per_device = {}
+
+    _destroy = 'kapre_stft_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_stft_plan_create(self.n_fft, self.win_length, self.hop_length,
+                                          self.window.ctypes.data_as(ctypes.c_void_p), out)
 
     def num_frames(self, length, pad_begin, pad_end):
         lp = int(length) + ((self.n_fft - self.hop_length) if pad_begin else 0)
@@ -161,28 +174,20 @@ class StftPlan:
         return bool(N.lib().kapre_stft_supports_mode(self.handle(), int(mode)))
 
 
-class IstftPlan:
+class IstftPlan(_PerDevice):
     def __init__(self, n_fft, win_length, hop_length, dual_window: np.ndarray):
         self.n_fft, self.win_length, self.hop_length = int(n_fft), int(win_length), int(hop_length)
         self.dual = np.ascontiguousarray(dual_window, dtype=np.float32)
         self._per_device = {}
 
-    def handle(self):
-        _require_cuda()
-        dev = torch.cuda.current_device()
-        with _lock:
-            h = self._per_device.get(dev)
-            if h is None:
-                lib = N.lib()
-                out = ctypes.c_void_p()
-                N.check(lib.kapre_istft_plan_create(self.n_fft, self.win_length, self.hop_length,
-                                                    self.dual.ctypes.data_as(ctypes.c_void_p), ctypes.byref(out)))
-                h = _Handle(out, lib.kapre_istft_plan_destroy)
-                self._per_device[dev] = h
-        return h.ptr
+    _destroy = 'kapre_istft_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_istft_plan_create(self.n_fft, self.win_length, self.hop_length,
+                                           self.dual.ctypes.data_as(ctypes.c_void_p), out)
 
 
-class Filterbank:
+class Filterbank(_PerDevice):
     """kapre_filterbank per CUDA device for one (n_freq, n_bands) matrix."""
 
     def __init__(self, matrix: np.ndarray):
@@ -200,22 +205,13 @@ class Filterbank:
             self._transposed = Filterbank(self.matrix.T)
         return self._transposed
 
-    def handle(self):
-        _require_cuda()
-        dev = torch.cuda.current_device()
-        with _lock:
-            h = self._per_device.get(dev)
-            if h is None:
-                lib = N.lib()
-                out = ctypes.c_void_p()
-                N.check(lib.kapre_filterbank_create(self.matrix.ctypes.data_as(ctypes.c_void_p), self.n_freq,
-                                                    self.n_bands, ctypes.byref(out)))
-                h = _Handle(out, lib.kapre_filterbank_destroy)
-                self._per_device[dev] = h
-        return h.ptr
+    _destroy = 'kapre_filterbank_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_filterbank_create(self.matrix.ctypes.data_as(ctypes.c_void_p), self.n_freq, self.n_bands, out)
 
 
-class FilterbankInversePlan:
+class FilterbankInversePlan(_PerDevice):
     """kapre_fb_inverse_plan per CUDA device for one (n_freq, n_bands) filterbank matrix: the row and column band
     lists of its transpose and the gradient step 1 / ||A||_2^2 of the NNLS iteration."""
 
@@ -226,22 +222,14 @@ class FilterbankInversePlan:
         self.n_freq, self.n_bands = self.matrix.shape
         self._per_device = {}
 
-    def handle(self):
-        _require_cuda()
-        dev = torch.cuda.current_device()
-        with _lock:
-            h = self._per_device.get(dev)
-            if h is None:
-                lib = N.lib()
-                out = ctypes.c_void_p()
-                N.check(lib.kapre_fb_inverse_plan_create(self.matrix.ctypes.data_as(ctypes.c_void_p), self.n_freq,
-                                                         self.n_bands, ctypes.byref(out)))
-                h = _Handle(out, lib.kapre_fb_inverse_plan_destroy)
-                self._per_device[dev] = h
-        return h.ptr
+    _destroy = 'kapre_fb_inverse_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_fb_inverse_plan_create(self.matrix.ctypes.data_as(ctypes.c_void_p), self.n_freq, self.n_bands,
+                                                out)
 
 
-class ResamplePlan:
+class ResamplePlan(_PerDevice):
     """kapre_resample_plan per CUDA device for one (up, down, filter)."""
 
     def __init__(self, up, down, taps: np.ndarray):
@@ -251,19 +239,11 @@ class ResamplePlan:
             raise ValueError('resampling filter must be 1-D, got shape %s' % (self.taps.shape,))
         self._per_device = {}
 
-    def handle(self):
-        _require_cuda()
-        dev = torch.cuda.current_device()
-        with _lock:
-            h = self._per_device.get(dev)
-            if h is None:
-                lib = N.lib()
-                out = ctypes.c_void_p()
-                N.check(lib.kapre_resample_plan_create(self.up, self.down, self.taps.ctypes.data_as(ctypes.c_void_p),
-                                                       self.taps.size, ctypes.byref(out)))
-                h = _Handle(out, lib.kapre_resample_plan_destroy)
-                self._per_device[dev] = h
-        return h.ptr
+    _destroy = 'kapre_resample_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_resample_plan_create(self.up, self.down, self.taps.ctypes.data_as(ctypes.c_void_p),
+                                              self.taps.size, out)
 
     def output_length(self, length):
         """ceil(length * up / down), the output length of ``scipy.signal.resample_poly``."""
@@ -281,6 +261,17 @@ def _wave_desc(t: torch.Tensor, data_format: str):
         B, C, L = t.shape
         sb, sc, sl = t.stride()
     return N.WaveDesc(B, C, L, sb, sc, sl), (B, C, L)
+
+
+def _wave_alloc(B, C, L, data_format, device):
+    """Contiguous (B, L, C) / (B, C, L) float32 waveform and its descriptor."""
+    if data_format == _CH_LAST_STR:
+        y = torch.empty((B, L, C), dtype=torch.float32, device=device)
+        sb, sl, sc = y.stride()
+    else:
+        y = torch.empty((B, C, L), dtype=torch.float32, device=device)
+        sb, sc, sl = y.stride()
+    return y, N.WaveDesc(B, C, L, sb, sc, sl)
 
 
 def _spec_alloc(B, C, T, K, data_format, dtype, device):
@@ -366,15 +357,9 @@ def istft(X: torch.Tensor, plan: IstftPlan, input_data_format, output_data_forma
     if F != plan.n_fft // 2 + 1:
         raise ValueError('expected %d frequency bins for n_fft=%d, got %d' % (plan.n_fft // 2 + 1, plan.n_fft, F))
     out_len = (T - 1) * plan.hop_length + plan.win_length if T > 0 else 0
-    if output_data_format == _CH_LAST_STR:
-        y = torch.empty((B, out_len, C), dtype=torch.float32, device=X.device)
-        sb, sl, sc = y.stride()
-    else:
-        y = torch.empty((B, C, out_len), dtype=torch.float32, device=X.device)
-        sb, sc, sl = y.stride()
+    y, yd = _wave_alloc(B, C, out_len, output_data_format, X.device)
     if y.numel() == 0:
         return y
-    yd = N.WaveDesc(B, C, out_len, sb, sc, sl)
     N.check(N.lib().kapre_istft_inverse(plan.handle(), _ptr(X), B, C, T, ctypes.byref(sd), _ptr(y),
                                         ctypes.byref(yd), _stream_ptr()))
     return y
@@ -463,12 +448,7 @@ def stft_backward(g: torch.Tensor, plan: StftPlan, input_data_format, output_dat
     g = _raw(g.to(torch.complex64))
     gd, (B, C, T, F) = _spec_desc(g, output_data_format)
     L = int(length)
-    if input_data_format == _CH_LAST_STR:
-        gx = torch.empty((B, L, C), dtype=torch.float32, device=g.device)
-        sb, sl, sc = gx.stride()
-    else:
-        gx = torch.empty((B, C, L), dtype=torch.float32, device=g.device)
-        sb, sc, sl = gx.stride()
+    gx, xd = _wave_alloc(B, C, L, input_data_format, g.device)
     if gx.numel() == 0:
         return gx
     lib = N.lib()
@@ -476,7 +456,6 @@ def stft_backward(g: torch.Tensor, plan: StftPlan, input_data_format, output_dat
     if nbytes < 0:
         N.check(nbytes)
     ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=g.device) if nbytes else None
-    xd = N.WaveDesc(B, C, L, sb, sc, sl)
     N.check(lib.kapre_stft_backward(plan.handle(), _ptr(g), ctypes.byref(gd), B, C, T, int(bool(pad_begin)),
                                     int(bool(pad_end)), _ptr(gx), ctypes.byref(xd), _ptr(ws) if ws is not None else None,
                                     _stream_ptr()))
@@ -706,29 +685,12 @@ def energy(x: torch.Tensor, frame_length, hop_length, pad_end, pad_value, scale,
     x = x.float()
     xd, (B, C, L) = _wave_desc(x, data_format)
     T = _frames_for(L, frame_length, hop_length, pad_end)
-    if data_format == _CH_LAST_STR:
-        out = torch.empty((B, T, C), dtype=torch.float32, device=x.device)
-        sb, st, sc = out.stride()
-    else:
-        out = torch.empty((B, C, T), dtype=torch.float32, device=x.device)
-        sb, sc, st = out.stride()
+    out, od = _wave_alloc(B, C, T, data_format, x.device)     # one value per frame: a waveform of T samples
     if out.numel():
-        od = N.WaveDesc(B, C, T, sb, sc, st)
         N.check(N.lib().kapre_energy(_ptr(x), ctypes.byref(xd), int(frame_length), int(hop_length), int(bool(pad_end)),
                                      ctypes.c_float(pad_value), ctypes.c_float(scale), _ptr(out), ctypes.byref(od),
                                      _stream_ptr()))
     return out
-
-
-def _wave_grad_alloc(B, C, L, data_format, device):
-    """Contiguous (B, L, C) / (B, C, L) float32 waveform gradient and its descriptor."""
-    if data_format == _CH_LAST_STR:
-        gx = torch.empty((B, L, C), dtype=torch.float32, device=device)
-        sb, sl, sc = gx.stride()
-    else:
-        gx = torch.empty((B, C, L), dtype=torch.float32, device=device)
-        sb, sc, sl = gx.stride()
-    return gx, N.WaveDesc(B, C, L, sb, sc, sl)
 
 
 @_device_of_first_arg
@@ -737,7 +699,7 @@ def frame_backward(g: torch.Tensor, frame_length, hop_length, data_format, lengt
     frames (any strides)."""
     g = _raw(g.to(torch.float32))
     gd, (B, C, T, _) = _spec_desc(g, data_format)
-    gx, xd = _wave_grad_alloc(B, C, int(length), data_format, g.device)
+    gx, xd = _wave_alloc(B, C, int(length), data_format, g.device)
     if gx.numel():
         N.check(N.lib().kapre_frame_backward(_ptr(g), ctypes.byref(gd), T, int(frame_length), int(hop_length), _ptr(gx),
                                              ctypes.byref(xd), _stream_ptr()))
@@ -759,7 +721,7 @@ def energy_backward(x: torch.Tensor, g: torch.Tensor, frame_length, hop_length, 
         sb, sc, st = g.stride()
         T = g.shape[2]
     gd = N.WaveDesc(B, C, T, sb, sc, st)
-    gx, od = _wave_grad_alloc(B, C, L, data_format, x.device)
+    gx, od = _wave_alloc(B, C, L, data_format, x.device)
     if gx.numel():
         N.check(N.lib().kapre_energy_backward(_ptr(x), ctypes.byref(xd), _ptr(g), ctypes.byref(gd), int(frame_length),
                                               int(hop_length), ctypes.c_float(scale), _ptr(gx), ctypes.byref(od),
@@ -778,7 +740,7 @@ def resample(x: torch.Tensor, plan: ResamplePlan, data_format):
     if x.dtype != torch.float32:
         x = x.float()
     xd, (B, C, L) = _wave_desc(x, data_format)
-    y, yd = _wave_grad_alloc(B, C, plan.output_length(L), data_format, x.device)
+    y, yd = _wave_alloc(B, C, plan.output_length(L), data_format, x.device)
     if y.numel():
         N.check(N.lib().kapre_resample(plan.handle(), _ptr(x), ctypes.byref(xd), _ptr(y), ctypes.byref(yd), _stream_ptr()))
     return y
@@ -790,7 +752,7 @@ def resample_backward(g: torch.Tensor, plan: ResamplePlan, data_format, length):
     output (any strides)."""
     g = _raw(g.to(torch.float32))
     gd, (B, C, _) = _wave_desc(g, data_format)
-    gx, xd = _wave_grad_alloc(B, C, int(length), data_format, g.device)
+    gx, xd = _wave_alloc(B, C, int(length), data_format, g.device)
     if gx.numel():
         N.check(N.lib().kapre_resample_backward(plan.handle(), _ptr(g), ctypes.byref(gd), _ptr(gx), ctypes.byref(xd),
                                                 _stream_ptr()))
@@ -887,15 +849,9 @@ def griffin_lim(S: torch.Tensor, stft_plan: StftPlan, istft_plan: IstftPlan, n_i
     if F != stft_plan.n_fft // 2 + 1:
         raise ValueError('expected %d frequency bins for n_fft=%d, got %d' % (stft_plan.n_fft // 2 + 1, stft_plan.n_fft, F))
     L = (T - 1) * stft_plan.hop_length + stft_plan.win_length if T > 0 else 0
-    if output_data_format == _CH_LAST_STR:
-        y = torch.empty((B, L, C), dtype=torch.float32, device=S.device)
-        sb, sl, sc = y.stride()
-    else:
-        y = torch.empty((B, C, L), dtype=torch.float32, device=S.device)
-        sb, sc, sl = y.stride()
+    y, yd = _wave_alloc(B, C, L, output_data_format, S.device)
     if y.numel() == 0:
         return y
-    yd = N.WaveDesc(B, C, L, sb, sc, sl)
     lib = N.lib()
     nbytes = lib.kapre_griffin_lim_workspace_bytes(stft_plan.handle(), B, C, T)
     if nbytes < 0:
