@@ -430,6 +430,12 @@ int kb_emu_fb_chunks(const float* fb, int n_freq, int n_bands) {
     return (int)cm.size();
 }
 
+// The fused kernels' decibel tail on an array: db_mul * log2(max(x, amin)) - db_sub, with the same host stand-in for
+// the device log2 as the kernel bodies, so MODE_*_DB can be compared bit for bit with the tail applied to MODE_MAG / MODE_FB.
+void kb_emu_db_tail(const float* x, float* out, long long n, float amin, float db_mul, float db_sub) {
+    for (long long i = 0; i < n; ++i) out[i] = db_mul * kb_log2(kb_floor_keepnan(x[i], amin)) - db_sub;
+}
+
 // kb_atan2 (the Phase outputs' polynomial atan2) on arrays, for the accuracy test
 void kb_emu_atan2(const float* y, const float* x, float* out, long long n) {
     for (long long i = 0; i < n; ++i) out[i] = kb_atan2(y[i], x[i]);

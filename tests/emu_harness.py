@@ -263,6 +263,17 @@ def emu_fb(x, fb, fmt, n_cta=3, R=32):
     return out
 
 
+def emu_db_tail(x, amin=1e-5, ref=1.0):
+    """The fused kernels' decibel tail (db_mul * log2(max(x, amin)) - db_sub, host build of the same source) on a
+    float32 array, with the constants emu_stft passes."""
+    lib = load()
+    x = np.ascontiguousarray(x, np.float32)
+    out = np.empty_like(x)
+    lib.kb_emu_db_tail(_fp(x), _fp(out), ctypes.c_longlong(x.size), ctypes.c_float(amin),
+                       ctypes.c_float(10.0 * np.log10(2.0)), ctypes.c_float(10.0 * np.log10(max(amin, ref))))
+    return out
+
+
 def emu_atan2(y, x):
     """kb_atan2 of kapre_b200/csrc/stft_core.cuh (host build of the same source) on float32 arrays."""
     lib = load()
