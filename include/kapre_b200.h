@@ -249,6 +249,34 @@ int kapre_resample(const kapre_resample_plan* plan, const float* x_dev, const ka
 int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
                             float* gx_dev, const kapre_wave_desc* gx_desc, void* stream);
 
+/* ---- band-limited interpolation: resampling by any real ratio ------------------------------------
+ * J. O. Smith's algorithm (what resampy / librosa's kaiser_best do) with a table that does not depend on the
+ * ratio.  With Z = 10 zero crossings and Kaiser beta 5 (the family of the polyphase filter above):
+ *   h(u) = sinc(u) I0(5 sqrt(1 - (u/Z)^2)) / I0(5) for |u| < Z, else 0;      I = integral of h over [-Z, Z]
+ *   y[m] = (g / I) sum_j x[j] h(s (offset + m / ratio - j)),   s = g = min(1, ratio),   x[j] = 0 outside the signal.
+ * `ratio` = output rate / input rate; the cutoff is the lower of the two Nyquist rates.  `offset` is the position of
+ * output sample 0 in input samples (0: the two signals start together).  A ratio outside [0.25, 4] (two octaves
+ * either way, at most 80 taps per output), a non-finite ratio or offset, or |offset| > 2^40 returns KAPRE_E_INVALID
+ * before anything is launched.  The filter is tabulated at 1024 points per zero crossing and read by linear
+ * interpolation: an output is within 1.7e-5 max|x| of the sum above (1e-6 typical).  At rational ratios this is
+ * scipy.signal.resample_poly up to its normalisation (scipy divides by the tap sum): 1e-4 .. 6e-4 of unit-variance
+ * input at 1:3, 3:2 and 2:1.
+ * The plan is the device table of h for the current device; it takes no arguments, and one plan serves every ratio. */
+typedef struct kapre_sinc_plan kapre_sinc_plan;
+int kapre_sinc_plan_create(kapre_sinc_plan** out);
+void kapre_sinc_plan_destroy(kapre_sinc_plan* plan);
+/* Interpolate along the sample axis in one launch.  y_desc has x_desc's batch and channels; y_desc->length outputs are
+ * written whatever the ratio (ceil(x_desc->length * ratio) covers the input): outputs whose support lies past the
+ * signal are exactly 0, so cropping or zero-padding to a given length costs nothing.  Any strides; y must not overlap
+ * x.  An output sample does not depend on the batch size, the data layout or the strides. */
+int kapre_sinc_resample(const kapre_sinc_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* y_dev,
+                        const kapre_wave_desc* y_desc, double ratio, double offset, void* stream);
+/* Gradient of kapre_sinc_resample called with the same (ratio, offset): gx = A^T g, written for gx_desc->length
+ * samples (the length the forward call saw).  Because h is even this is the same sum with step ratio instead of
+ * 1 / ratio, offset -offset * ratio and s / ratio instead of s: the same kernel, one launch. */
+int kapre_sinc_resample_backward(const kapre_sinc_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
+                                 float* gx_dev, const kapre_wave_desc* gx_desc, double ratio, double offset, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

@@ -98,6 +98,12 @@ SYMBOLS = [
     ('kapre_resample_output_length', c_int64, [c_void_p, c_int64]),
     ('kapre_resample', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p]),
     ('kapre_resample_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p]),
+    ('kapre_sinc_plan_create', c_int, [POINTER(c_void_p)]),
+    ('kapre_sinc_plan_destroy', None, [c_void_p]),
+    ('kapre_sinc_resample', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), ctypes.c_double,
+                                    ctypes.c_double, c_void_p]),
+    ('kapre_sinc_resample_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc),
+                                             ctypes.c_double, ctypes.c_double, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

@@ -1,13 +1,14 @@
 """Augmentation layers (reference: kapre/augmentation.py).  ``SpecAugment``: the masks are drawn on the host, the
 masking is one CUDA pass (``kapre_spec_augment``).  ``TimeStretch``: a phase vocoder, one CUDA scan over time
-(``kapre_time_stretch``)."""
+(``kapre_time_stretch``).  ``PitchShift``: STFT, that phase vocoder, the inverse STFT and one band-limited
+interpolation (``kapre_sinc_resample``) back to the input length."""
 from __future__ import annotations
 
 import numpy as np
 
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
-from .time_frequency import Layer, _resolve, _unwrap_format, register_keras_serializable
+from .time_frequency import STFT, InverseSTFT, Layer, _resolve, _unwrap_format, register_keras_serializable
 
 
 def draw_masks(rng: np.random.Generator, batch: int, n_masks: int, mask_param: int, axis_limit: int) -> np.ndarray:
@@ -110,5 +111,87 @@ class TimeStretch(Layer):
 
     _config_fields = (
         ('rate', 'rate'),
+        ('data_format', 'data_format_original'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class PitchShift(Layer):
+    """Shifts the pitch of a waveform by ``n_steps`` steps of an octave divided into ``bins_per_octave`` without
+    changing its length (``torchaudio.transforms.PitchShift``): ``(batch, time, ch)`` / ``(batch, ch, time)`` in, the
+    same shape out.  ``n_steps`` is any number with ``|n_steps| <= 2 * bins_per_octave``; ``call(x, n_steps=...)``
+    overrides it for one call, and 0 returns the input itself.
+
+    With ``rate = 2 ** (-n_steps / bins_per_octave)`` the layer runs four steps: ``STFT``
+    (``pad_begin`` and ``pad_end``, so that frames cover every input sample), ``TimeStretch(rate)``, ``InverseSTFT``
+    with the dual window, and the band-limited interpolation ``ops.sinc_resample`` by the ratio ``rate`` to the input
+    length.  Two differences from torchaudio: the ratio is ``rate`` itself, not ``int(sample_rate / rate) /
+    sample_rate``, so the layer takes no sample rate; and the output is time-aligned with the input.
+
+    Alignment.  ``pad_begin`` prepends ``pad = n_fft - hop_length`` zeros, so input sample ``t`` is the centre of the
+    (fractional) frame ``k = (t + pad - win_length / 2) / hop_length``.  The stretch moves frame ``k`` to frame
+    ``k / rate``, and the inverse puts the centre of that frame at ``k / rate * hop_length + win_length / 2`` of its
+    untrimmed output.  Output sample ``m`` of the interpolation reads position ``offset + m / rate``, so it reads input
+    time ``m`` when ``offset = win_length / 2 + (pad - win_length / 2) / rate``.  That aligns the frames exactly; what
+    a phase vocoder does to the position of an event inside a frame (it keeps each bin's phase advance, not the
+    relation between bins) stays, so a tone burst comes out within ``hop_length`` of where it was and a click within
+    half a window.
+
+    Differentiable with respect to the input, because each of the four steps is."""
+
+    def __init__(self, n_steps, bins_per_octave=12, n_fft=2048, win_length=None, hop_length=None, window_name=None,
+                 data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        if isinstance(bins_per_octave, bool) or not isinstance(bins_per_octave, (int, np.integer)) or bins_per_octave <= 0:
+            raise ValueError('bins_per_octave must be a positive integer, got: %r' % (bins_per_octave,))
+        self.bins_per_octave = int(bins_per_octave)
+        self.n_steps = self._check(n_steps)
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self.stft = STFT(n_fft=n_fft, win_length=win_length, hop_length=hop_length, window_name=window_name,
+                         pad_begin=True, pad_end=True, input_data_format=self.data_format,
+                         output_data_format=_CH_LAST_STR)
+        self.n_fft, self.win_length, self.hop_length = self.stft.n_fft, self.stft.win_length, self.stft.hop_length
+        self.window_name = window_name
+        self.stretch = TimeStretch(self.rate(self.n_steps), data_format=_CH_LAST_STR)
+        self.istft = InverseSTFT(n_fft=n_fft, win_length=win_length, hop_length=hop_length,
+                                 forward_window_name=window_name, input_data_format=_CH_LAST_STR,
+                                 output_data_format=self.data_format)
+
+    def _check(self, n_steps):
+        if isinstance(n_steps, (bool, np.bool_)) or not isinstance(n_steps, (int, float, np.integer, np.floating)) \
+                or not abs(float(n_steps)) <= 2 * self.bins_per_octave:
+            raise ValueError('n_steps must be a number with |n_steps| <= 2 * bins_per_octave = %d, got: %r'
+                             % (2 * self.bins_per_octave, n_steps))
+        return float(n_steps)
+
+    def rate(self, n_steps):
+        """The time-stretch rate and the interpolation ratio of a shift by ``n_steps``."""
+        return 2.0 ** (-float(n_steps) / self.bins_per_octave)
+
+    def offset(self, rate):
+        """Where input sample 0 lands in the untrimmed inverse STFT of the stretched frames (see the class docstring)."""
+        return self.win_length / 2.0 + ((self.n_fft - self.hop_length) - self.win_length / 2.0) / rate
+
+    def call(self, x, n_steps=None):
+        if x.dim() != 3:
+            raise ValueError('PitchShift expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        n_steps = self.n_steps if n_steps is None else self._check(n_steps)
+        if n_steps == 0.0:
+            return x
+        rate = self.rate(n_steps)
+        length = x.shape[2] if self.data_format == _CH_FIRST_STR else x.shape[1]
+        y = self.istft.call(self.stretch.call(self.stft.call(x), rate=rate))
+        return ops.sinc_resample(y, rate, length, self.offset(rate), self.data_format)
+
+    _config_fields = (
+        ('n_steps', 'n_steps'),
+        ('bins_per_octave', 'bins_per_octave'),
+        ('n_fft', 'n_fft'),
+        ('win_length', 'win_length'),
+        ('hop_length', 'hop_length'),
+        ('window_name', 'window_name'),
         ('data_format', 'data_format_original'),
     )

@@ -16,6 +16,8 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * ConcatenateFrequencyMap -> ``kapre_concat_frequency_map_backward`` (the first C channels)
 * SpecAugment     -> ``kapre_spec_augment`` over the gradient, mask value 0, the forward's device masks
 * Resample        -> ``kapre_resample_backward`` (the resampling kernel with up and down exchanged)
+* Speed, PitchShift's last step -> ``kapre_sinc_resample_backward`` (the interpolation kernel with step, offset and
+  cutoff exchanged)
 * PCEN            -> ``kapre_pcen_backward`` (reverse-time scan; input and parameter gradients)
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
@@ -237,6 +239,18 @@ class _Resample(torch.autograd.Function):
         return ops.resample_backward(g, *ctx.cfg), None, None
 
 
+class _SincResample(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, ratio, length, offset, data_format):
+        ctx.cfg = (ratio, offset, data_format, x.shape[1] if data_format == ops._CH_LAST_STR else x.shape[2])
+        return ops.sinc_resample(x, ratio, length, offset, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return ops.sinc_resample_backward(g, *ctx.cfg), None, None, None, None
+
+
 class _Pcen(torch.autograd.Function):
     """The forward is the plain PCEN launch that also writes the smoother state M; the backward reads E and M and
     returns the gradients of the input and of the four parameters (gain, bias, power, smooth_coef)."""
@@ -329,6 +343,10 @@ def spec_augment(x, time_masks, freq_masks, mask_value, data_format):
 
 def resample(x, plan, data_format):
     return _Resample.apply(x.float(), plan, data_format)
+
+
+def sinc_resample(x, ratio, length, offset, data_format):
+    return _SincResample.apply(x.float(), ratio, length, offset, data_format)
 
 
 def pcen(E, params, eps, data_format):

@@ -19,7 +19,7 @@ from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .augmentation import TimeStretch
-from .signal import Resample
+from .signal import Resample, Speed
 from .time_frequency import (STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
                              MagnitudeToDecibel, Phase, get_registered_object)
 
@@ -106,8 +106,8 @@ class Sequential(Layer):
 
     def call(self, x):
         start = 0
-        # Leading Resample layers run first, so that the STFT stack behind them still takes the fused launch.
-        while start < len(self.layers) and type(self.layers[start]) is Resample:
+        # Leading Resample and Speed layers run first, so that the STFT stack behind them still takes the fused launch.
+        while start < len(self.layers) and type(self.layers[start]) in (Resample, Speed):
             x = self.layers[start].call(x)
             start += 1
         fused = self._fused_prefix(start) if (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3) else None

@@ -26,6 +26,7 @@
 #include "grad_core.cuh"
 #include "grad_aux_core.cuh"
 #include "resample_core.cuh"
+#include "sinc_core.cuh"
 #include "pcen_core.cuh"
 #include "gl_core.cuh"
 #include "ts_core.cuh"
@@ -2075,6 +2076,114 @@ int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev,
         adj = p->adj;
     }
     return kb_resample_launch(adj, g_dev, g_desc, gx_dev, gx_desc, stream);
+}
+
+}  // extern "C"
+
+// ---- band-limited interpolation (sinc_core.cuh) ---------------------------------------------------
+__global__ void __launch_bounds__(KB_SINC_THREADS, 2) kb_sinc_resample_kernel(const __grid_constant__ KbSincParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_sinc_cta(p, kb_smem, (int)blockIdx.x, (int)gridDim.x);
+}
+
+struct kapre_sinc_plan {
+    DevInfo dev;
+    float2* tab = nullptr;      // KB_SINC_NTAB pairs (h, forward difference)
+    double integral = 1.0;      // I
+};
+
+// Largest tile (outputs, a power of two <= 2048) whose staged span fits beside the table: in half of the opt-in
+// shared memory when possible (less the 1 KB the system reserves per CTA and 1 KB of static shared memory), so that
+// two CTAs share an SM, else in all of it.
+static int kb_sinc_pick_nt(const kapre_sinc_plan* p, double step, int nw, int G) {
+    for (int budget : {p->dev.smem_optin / 2 - 2048, p->dev.smem_optin - 1024})
+        for (int nt = 2048; nt >= 1; nt /= 2)
+            if (kb_sinc_smem(nt, step, nw, G) <= budget) return nt;
+    return 0;
+}
+
+// One launch of y[m] = (gain / I) sum_j x[j] h(s (offset + m step - j)): the forward and the adjoint differ only in
+// the four numbers kb_sinc_args makes.
+static int kb_sinc_launch(const kapre_sinc_plan* plan, const float* x_dev, const kapre_wave_desc* xd, float* y_dev,
+                          const kapre_wave_desc* yd, double ratio, double offset, int adjoint, void* stream) {
+    if (!plan || !xd || !yd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (!(ratio >= KB_SINC_RATIO_MIN && ratio <= KB_SINC_RATIO_MAX))
+        return kb_fail(KAPRE_E_INVALID, "ratio must lie in [%g, %g], got: %g", KB_SINC_RATIO_MIN, KB_SINC_RATIO_MAX, ratio);
+    if (!(fabs(offset) <= 1099511627776.0)) return kb_fail(KAPRE_E_INVALID, "offset must be finite and at most 2^40 in size, got: %g", offset);
+    if (xd->batch < 0 || xd->channels < 0 || xd->length < 0 || yd->length < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (yd->batch != xd->batch || yd->channels != xd->channels)
+        return kb_fail(KAPRE_E_INVALID, "input and output descriptors disagree on batch / channels");
+    if ((long long)yd->batch * yd->channels * yd->length == 0) return 0;
+    if ((!x_dev && xd->length > 0) || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)x_dev == (const void*)y_dev) return kb_fail(KAPRE_E_INVALID, "interpolation cannot run in place");
+    int cur = -1;
+    KB_CUDA(cudaGetDevice(&cur));
+    if (cur != plan->dev.device)
+        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    double step, off, s, gain;
+    kb_sinc_args(ratio, offset, adjoint, &step, &off, &s, &gain);
+    KbSincParams p{};
+    const int B = xd->batch, C = xd->channels;
+    p.x = x_dev; p.x_sb = xd->stride_b; p.x_sc = xd->stride_c; p.x_sl = xd->stride_l;
+    p.B = B; p.C = C; p.L = xd->length;
+    p.y = y_dev; p.y_sb = yd->stride_b; p.y_sc = yd->stride_c; p.y_sl = yd->stride_l;
+    p.L_out = yd->length;
+    p.tab = plan->tab;
+    // channel-interleaved input: all channels in one tile
+    const bool interleaved = C > 1 && C <= KB_SINC_THREADS && llabs(xd->stride_c) < llabs(xd->stride_l);
+    p.G = interleaved ? C : 1;
+    const bool nonneg = xd->stride_b >= 0 && xd->stride_c >= 0 && xd->stride_l >= 0;
+    p.x_numel = (B > 0 && C > 0 && p.L > 0)
+        ? (long long)(B - 1) * xd->stride_b + (long long)(C - 1) * xd->stride_c + (long long)(p.L - 1) * xd->stride_l + 1 : 0;
+    p.x_align = (unsigned)(((uintptr_t)x_dev >> 2) & 3u);
+    p.bulk_ok = nonneg && (((uintptr_t)x_dev & 3u) == 0) &&
+                (p.G == 1 ? xd->stride_l == 1 : (xd->stride_c == 1 && xd->stride_l == C)) ? 1 : 0;
+    const int nw = (int)ceil((double)KB_SINC_Z / s);
+    p.NT = kb_sinc_pick_nt(plan, step, nw, p.G);
+    if (p.NT == 0)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "%d interleaved channels at ratio %g do not fit in shared memory", p.G, ratio);
+    if (!kb_sinc_setup(p, step, off, s, gain, plan->integral, KB_SINC_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
+    const int smem = kb_sinc_smem(p.NT, step, p.nw, p.G);
+    int grid, rc;
+    if ((rc = kb_resident_grid(kb_sinc_resample_kernel, KB_SINC_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_sinc_resample_kernel, {.grid = grid, .block = KB_SINC_THREADS, .smem = smem,
+                                               .st = (cudaStream_t)stream, .timed = true}, p);
+}
+
+extern "C" {
+
+int kapre_sinc_plan_create(kapre_sinc_plan** out) {
+    if (!out) return kb_fail(KAPRE_E_INVALID, "null argument");
+    kapre_sinc_plan* p = new kapre_sinc_plan();
+    int rc = kb_dev_info(&p->dev);
+    if (rc) { delete p; return rc; }
+    if (kb_sinc_smem(1, 1.0 / KB_SINC_RATIO_MIN, (int)(KB_SINC_Z / KB_SINC_RATIO_MIN), 1) > p->dev.smem_optin) {
+        delete p;
+        return kb_fail(KAPRE_E_UNSUPPORTED, "the interpolation table (%d B) does not fit in shared memory", KB_SINC_NTAB * 8);
+    }
+    std::vector<float2> tab;
+    kb_sinc_table(tab);
+    p->integral = kb_sinc_integral();
+    if ((rc = kb_upload(tab, &p->tab))) { kapre_sinc_plan_destroy(p); return rc; }
+    *out = p;
+    return 0;
+}
+
+void kapre_sinc_plan_destroy(kapre_sinc_plan* p) {
+    if (!p) return;
+    cudaFree(p->tab);
+    delete p;
+}
+
+int kapre_sinc_resample(const kapre_sinc_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* y_dev,
+                        const kapre_wave_desc* y_desc, double ratio, double offset, void* stream) {
+    return kb_sinc_launch(plan, x_dev, x_desc, y_dev, y_desc, ratio, offset, 0, stream);
+}
+
+int kapre_sinc_resample_backward(const kapre_sinc_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
+                                 float* gx_dev, const kapre_wave_desc* gx_desc, double ratio, double offset, void* stream) {
+    return kb_sinc_launch(plan, g_dev, g_desc, gx_dev, gx_desc, ratio, offset, 1, stream);
 }
 
 }  // extern "C"

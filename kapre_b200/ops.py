@@ -759,6 +759,72 @@ def resample_backward(g: torch.Tensor, plan: ResamplePlan, data_format, length):
     return gx
 
 
+class SincPlan(_PerDevice):
+    """kapre_sinc_plan per CUDA device: the table of the band-limited interpolation filter.  Nothing in it depends on
+    a ratio, so the module holds one instance (``_sinc_plan``) that every ``Speed`` and ``PitchShift`` layer shares."""
+
+    def __init__(self):
+        self._per_device = {}
+
+    _destroy = 'kapre_sinc_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_sinc_plan_create(out)
+
+
+_sinc_plan = SincPlan()
+SINC_RATIO_MIN, SINC_RATIO_MAX = 0.25, 4.0
+
+
+def _check_ratio(ratio, name='ratio'):
+    if isinstance(ratio, (bool, np.bool_)) or not isinstance(ratio, (int, float, np.integer, np.floating)) \
+            or not SINC_RATIO_MIN <= float(ratio) <= SINC_RATIO_MAX:
+        raise ValueError('%s must be a number in [%g, %g], got: %r' % (name, SINC_RATIO_MIN, SINC_RATIO_MAX, ratio))
+    return float(ratio)
+
+
+def _check_offset(offset):
+    if isinstance(offset, (bool, np.bool_)) or not isinstance(offset, (int, float, np.integer, np.floating)) \
+            or not math.isfinite(float(offset)):
+        raise ValueError('offset must be a finite number, got: %r' % (offset,))
+    return float(offset)
+
+
+@_device_of_first_arg
+def sinc_resample(x: torch.Tensor, ratio, length, offset=0.0, data_format=_CH_LAST_STR):
+    """Band-limited interpolation along the time axis of (b, t, ch) / (b, ch, t) by any ``ratio`` (output rate /
+    input rate) in [0.25, 4]: output sample ``m`` of ``length`` is the input at position ``offset + m / ratio``,
+    low-passed to the lower of the two Nyquist rates (see ``include/kapre_b200.h``).  One launch, no per-ratio state."""
+    if not x.is_cuda:
+        raise N.KapreNativeError('sinc_resample needs a CUDA tensor')
+    ratio, offset = _check_ratio(ratio), _check_offset(offset)
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.sinc_resample(x, ratio, length, offset, data_format)
+    if x.dtype != torch.float32:
+        x = x.float()
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    y, yd = _wave_alloc(B, C, int(length), data_format, x.device)
+    if y.numel():
+        N.check(N.lib().kapre_sinc_resample(_sinc_plan.handle(), _ptr(x), ctypes.byref(xd), _ptr(y), ctypes.byref(yd),
+                                            ratio, offset, _stream_ptr()))
+    return y
+
+
+@_device_of_first_arg
+def sinc_resample_backward(g: torch.Tensor, ratio, offset, data_format, length):
+    """Gradient of ``sinc_resample`` with respect to its input of ``length`` samples, given the gradient ``g`` of its
+    output (any strides)."""
+    g = _raw(g.to(torch.float32))
+    gd, (B, C, _) = _wave_desc(g, data_format)
+    gx, xd = _wave_alloc(B, C, int(length), data_format, g.device)
+    if gx.numel():
+        N.check(N.lib().kapre_sinc_resample_backward(_sinc_plan.handle(), _ptr(g), ctypes.byref(gd), _ptr(gx),
+                                                     ctypes.byref(xd), _check_ratio(ratio), _check_offset(offset),
+                                                     _stream_ptr()))
+    return gx
+
+
 def _pcen_params(params, eps, device):
     """kapre_pcen_params over the four parameter tensors (gain, bias, power, smooth_coef): float32, 0-d (one value
     for every band) or 1-d (one per band), on ``device``."""

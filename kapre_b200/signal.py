@@ -2,7 +2,8 @@
 ``Frame`` (reference :22-119), ``Energy`` (:123-233) and ``LogmelToMFCC``
 (:365-447).  Same constructor arguments, validation and ``get_config`` keys; ``call`` runs CUDA
 kernels through the C ABI.  ``Resample`` (polyphase sample-rate conversion) has no counterpart in the
-reference, which expects audio to be resampled before it reaches the model."""
+reference, which expects audio to be resampled before it reaches the model; neither has ``Speed`` (speed perturbation by any
+real factor, band-limited interpolation)."""
 from __future__ import annotations
 
 import math
@@ -13,7 +14,7 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
-__all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample']
+__all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed']
 
 
 def _resolve(fmt):
@@ -135,6 +136,47 @@ class Resample(Layer):
     _config_fields = (
         ('orig_sample_rate', 'orig_sample_rate'),
         ('target_sample_rate', 'target_sample_rate'),
+        ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class Speed(Layer):
+    """Speed perturbation (``torchaudio.transforms.Speed``, Kaldi's 0.9 / 1.0 / 1.1 and the continuous variants):
+    the waveform played ``factor`` times faster, hence ``factor`` times higher.  ``(batch, time, ch)`` ->
+    ``(batch, ceil(time / factor), ch)`` or the same with ``(batch, ch, time)``.  ``factor`` is any number in
+    [0.25, 4]; ``call(x, factor=...)`` overrides it for one call, and ``factor == 1`` returns the input itself.
+
+    One launch of the band-limited interpolation kernel (``kapre_sinc_resample`` with ratio ``1 / factor``) whose
+    filter table does not depend on the factor, so a new factor per step costs nothing: no plan, no table, no cache
+    entry.  The gradient with respect to the input is available when the CUDA input requires grad."""
+
+    def __init__(self, factor, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        self.factor = self._check(factor)
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+
+    @staticmethod
+    def _check(factor):
+        # the interpolation ratio is 1 / factor, and [0.25, 4] is its own reciprocal
+        return ops._check_ratio(factor, 'factor')
+
+    def output_length(self, length, factor=None):
+        return math.ceil(int(length) / (self.factor if factor is None else factor))
+
+    def call(self, x, factor=None):
+        if x.dim() != 3:
+            raise ValueError('Speed expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        factor = self.factor if factor is None else self._check(factor)
+        if factor == 1.0:
+            return x
+        length = x.shape[2] if self.data_format == _CH_FIRST_STR else x.shape[1]
+        return ops.sinc_resample(x, 1.0 / factor, self.output_length(length, factor), 0.0, self.data_format)
+
+    _config_fields = (
+        ('factor', 'factor'),
         ('data_format', 'data_format_str'),
     )
 
