@@ -277,6 +277,65 @@ int kapre_sinc_resample(const kapre_sinc_plan* plan, const float* x_dev, const k
 int kapre_sinc_resample_backward(const kapre_sinc_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
                                  float* gx_dev, const kapre_wave_desc* gx_desc, double ratio, double offset, void* stream);
 
+/* ---- convolution with long filters (uniformly partitioned overlap-add) ---------------------------
+ * y = x * h (full linear convolution along the sample axis) through this library's transform pair: with a block size
+ * B in {128, 256, 512, 1024},
+ *   X = STFT(x; n_fft 2B, window ones(B), hop B, pad_end): J = ceil(L / B) blocks, block j = x[jB, jB + B) zero-padded
+ *   H = the same transform of h: P = ceil(K / B) blocks
+ *   Y_i = sum_{p < P} H_p X_{i - p}   (X_j = 0 outside [0, J)),  i < T = J + P - 1
+ *   y = InverseSTFT(Y; n_fft 2B, hop B, dual window ones(2B)): (T + 1) B samples, of which the first L + K - 1 are
+ *       the convolution and the rest are zero up to rounding.
+ * The per-bin sum runs in a fixed order (p ascending), so an output sample does not depend on the batch size, the
+ * item's position, the strides or broadcasting.  Across data layouts it agrees to float32 rounding: an interleaved
+ * multi-channel waveform is transformed by kapre_stft_forward's all-channel kernel.  An output is within a few 1e-6 of rms(x) ||h||_2
+ * (DESIGN.md §4 gives the bound).  Spectra (H, X, their gradients) are (batch, channels, blocks, B + 1 bins)
+ * complex64 with kapre_spec_desc strides; a batch or channel stride of 0 in H_desc broadcasts one filter over the
+ * batch or the channels, without a copy. */
+typedef struct kapre_convolve_plan kapre_convolve_plan;
+/* The block size B for a filter of ir_length taps: a function of the length alone (so an output's bits depend on the
+ * inputs alone), the one kapre_b200's layers use.  KAPRE_E_INVALID for ir_length < 1. */
+int64_t kapre_convolve_block_size(int64_t ir_length);
+/* The transform pair of one block size (128, 256, 512 or 1024, else KAPRE_E_INVALID) on the current device. */
+int kapre_convolve_plan_create(int block, kapre_convolve_plan** out);
+void kapre_convolve_plan_destroy(kapre_convolve_plan* plan);
+/* H = the block spectra of h (h_desc->length = K >= 1 taps, any batch and channels, any strides): P = ceil(K / B)
+ * blocks written through H_desc.  One launch; callers keep H, so a filter bank is transformed once. */
+int kapre_convolve_ir_spectrum(const kapre_convolve_plan* plan, const float* h_dev, const kapre_wave_desc* h_desc,
+                               void* H_dev, const kapre_spec_desc* H_desc, void* stream);
+/* Scratch of kapre_convolve: X (J blocks) and Y (T blocks) for batch x channels signals of `length` samples, each
+ * rounded up to 256 B.  < 0 on error (length < 1, P < 1, or (T + 1) B beyond int32). */
+int64_t kapre_convolve_workspace_bytes(const kapre_convolve_plan* plan, int batch, int channels, int length, int P);
+/* y = x * h given H (P blocks, batch and channels as x's or broadcast through zero strides).  y_desc: x's batch and
+ * channels and exactly (T + 1) B samples, any strides; crop it for torchaudio's 'full' / 'same' / 'valid'.  Three
+ * launches: STFT, the per-bin multiply-accumulate, the inverse.  `workspace_dev`: kapre_convolve_workspace_bytes
+ * bytes; on return it begins with X, (batch, channels, J, B + 1) complex64 contiguous, which
+ * kapre_convolve_backward reads for the filter's gradient.  Sizes that are invalid for kapre_convolve_workspace_bytes
+ * return KAPRE_E_INVALID here before anything is launched. */
+int kapre_convolve(const kapre_convolve_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, const void* H_dev,
+                   const kapre_spec_desc* H_desc, int P, float* y_dev, const kapre_wave_desc* y_desc, void* workspace_dev,
+                   void* stream);
+/* Scratch of kapre_convolve_backward: G (T blocks), the signal spectra's gradient (J blocks) and, when length is not a
+ * multiple of B, batch x channels x J B floats of overlap-add scratch. */
+int64_t kapre_convolve_backward_workspace_bytes(const kapre_convolve_plan* plan, int batch, int channels, int length,
+                                                int P);
+/* Gradients of kapre_convolve given the gradient gy of its untrimmed (T + 1) B-sample output (zero where the caller
+ * cropped it away).  G = InverseSTFT^T(gy); then
+ *   gx = STFT^T(gX),  gX_j = sum_{p < P} conj(H_p) G_{j + p}    (j < J; written when gx_dev is not NULL)
+ *   gH_p = sum_{j < J} conj(X_j) G_{j + p}                      (p < P; per (item, channel), written when gH_dev is
+ *                                                               not NULL, from the X kapre_convolve left in its workspace)
+ * gx_desc is required in both cases: its batch, channels and length (the forward's L) fix the geometry.  Sum gH
+ * over a broadcast filter's batch or channels before kapre_convolve_ir_spectrum_backward. */
+int kapre_convolve_backward(const kapre_convolve_plan* plan, const float* gy_dev, const kapre_wave_desc* gy_desc,
+                            const void* H_dev, const kapre_spec_desc* H_desc, const void* X_dev,
+                            const kapre_spec_desc* X_desc, int P, float* gx_dev, const kapre_wave_desc* gx_desc,
+                            void* gH_dev, const kapre_spec_desc* gH_desc, void* workspace_dev, void* stream);
+/* gh = the gradient of kapre_convolve_ir_spectrum given gH (P blocks), for gh_desc->length = K taps with
+ * ceil(K / B) = P.  `workspace_dev`: batch x channels x P B floats of scratch when K is not a multiple of B, else it
+ * may be NULL. */
+int kapre_convolve_ir_spectrum_backward(const kapre_convolve_plan* plan, const void* gH_dev, const kapre_spec_desc* gH_desc,
+                                        int P, float* gh_dev, const kapre_wave_desc* gh_desc, void* workspace_dev,
+                                        void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

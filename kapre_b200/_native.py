@@ -104,6 +104,19 @@ SYMBOLS = [
                                     ctypes.c_double, c_void_p]),
     ('kapre_sinc_resample_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc),
                                              ctypes.c_double, ctypes.c_double, c_void_p]),
+    ('kapre_convolve_block_size', c_int64, [c_int64]),
+    ('kapre_convolve_plan_create', c_int, [c_int, POINTER(c_void_p)]),
+    ('kapre_convolve_plan_destroy', None, [c_void_p]),
+    ('kapre_convolve_ir_spectrum', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(SpecDesc), c_void_p]),
+    ('kapre_convolve_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
+    ('kapre_convolve', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(SpecDesc), c_int, c_void_p,
+                               POINTER(WaveDesc), c_void_p, c_void_p]),
+    ('kapre_convolve_backward_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
+    ('kapre_convolve_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(SpecDesc), c_void_p,
+                                        POINTER(SpecDesc), c_int, c_void_p, POINTER(WaveDesc), c_void_p,
+                                        POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_convolve_ir_spectrum_backward', c_int, [c_void_p, c_void_p, POINTER(SpecDesc), c_int, c_void_p,
+                                                    POINTER(WaveDesc), c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

@@ -1,11 +1,14 @@
 """Augmentation layers (reference: kapre/augmentation.py).  ``SpecAugment``: the masks are drawn on the host, the
 masking is one CUDA pass (``kapre_spec_augment``).  ``TimeStretch``: a phase vocoder, one CUDA scan over time
 (``kapre_time_stretch``).  ``PitchShift``: STFT, that phase vocoder, the inverse STFT and one band-limited
-interpolation (``kapre_sinc_resample``) back to the input length."""
+interpolation (``kapre_sinc_resample``) back to the input length.  ``Reverb``: convolution with a room impulse response
+drawn from a bank (``kapre_convolve``)."""
 from __future__ import annotations
 
 import numpy as np
+import torch
 
+from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import STFT, InverseSTFT, Layer, _resolve, _unwrap_format, register_keras_serializable
@@ -195,3 +198,113 @@ class PitchShift(Layer):
         ('window_name', 'window_name'),
         ('data_format', 'data_format_original'),
     )
+
+
+def prepare_rirs(rirs) -> np.ndarray:
+    """The room impulse responses of a ``Reverb`` bank, prepared in float64 as the torchaudio augmentation tutorial
+    does by hand: each one trimmed to start at its largest-magnitude sample (the direct path), scaled to unit L2
+    norm, and zero-padded to the longest.  ``rirs``: a 2-D array or a sequence of 1-D arrays of any lengths.
+    Returns an (n_rirs, K) float32 array; an empty bank, or an all-zero or non-finite response, raises."""
+    if isinstance(rirs, np.ndarray) and rirs.ndim == 2:
+        rows = list(rirs)
+    elif isinstance(rirs, np.ndarray) and rirs.ndim != 2:
+        raise ValueError('rirs must be a 2-D array or a list of 1-D arrays, got an array of shape %s' % (rirs.shape,))
+    else:
+        try:
+            rows = list(rirs)
+        except TypeError:
+            raise ValueError('rirs must be a 2-D array or a list of 1-D arrays, got: %r' % (type(rirs),)) from None
+    if not rows:
+        raise ValueError('rirs is empty')
+    out = []
+    for i, r in enumerate(rows):
+        r = np.asarray(r.detach().cpu() if hasattr(r, 'detach') else r, dtype=np.float64)
+        if r.ndim != 1 or r.size == 0:
+            raise ValueError('rir %d must be a non-empty 1-D array, got shape %s' % (i, r.shape))
+        if not np.all(np.isfinite(r)):
+            raise ValueError('rir %d has non-finite samples' % i)
+        r = r[int(np.argmax(np.abs(r))):]
+        norm = np.sqrt(np.sum(r * r))
+        if not norm > 0:
+            raise ValueError('rir %d is all zeros' % i)
+        out.append(r / norm)
+    bank = np.zeros((len(out), max(r.size for r in out)), np.float64)
+    for i, r in enumerate(out):
+        bank[i, :r.size] = r
+    return bank.astype(np.float32)
+
+
+@register_keras_serializable(package='Kapre')
+class Reverb(Layer):
+    """Reverberation by a bank of room impulse responses (the RIR step of speed perturbation -> reverberation ->
+    noise recipes): ``(batch, time, ch)`` / ``(batch, ch, time)`` in, the same shape out,
+    ``y[t] = sum_k h'[k] x[t - k]`` for ``t < time`` with ``h'`` the drawn response after ``prepare_rirs`` (trimmed
+    to its direct path, unit L2 norm), so the output is time-aligned with the direct path.  Every channel of an item
+    gets the same response.
+
+    ``call(x, rir_index=None)`` draws one response per item, uniformly with ``np.random.default_rng(seed)``, and
+    records the draw in ``last_choice``; an int or an array of ``batch`` indices overrides the draw.  The layer
+    applies on every call, like ``Speed`` and ``PitchShift`` (``Sequential`` passes no ``training`` flag); a
+    captured graph (``Sequential.capture``) replays the draw made when it was captured.
+
+    The bank's block spectra are computed on first use on a device and kept; a call gathers the drawn items' spectra
+    and runs ``kapre_convolve`` (three launches).  The gradient reaches ``x`` only: the bank is a constant, like a
+    window or a filterbank."""
+
+    def __init__(self, rirs, seed=None, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.bank = prepare_rirs(rirs)
+        self.seed = seed
+        self.rng = np.random.default_rng(seed)
+        self.last_choice = None
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self.plan = ops.convolve_plan(ops.convolve_block_size(self.bank.shape[1]))
+        self._spectra = {}
+
+    def spectra(self, device):
+        """(n_rirs, 1, P, B + 1) complex64 block spectra of the bank on ``device``, made on first use."""
+        key = device.index if device.index is not None else torch.cuda.current_device()
+        H = self._spectra.get(key)
+        if H is None:
+            with torch.cuda.device(device):
+                h = torch.from_numpy(self.bank).to(device).unsqueeze(1)
+                H = self._spectra[key] = ops.convolve_ir_spectrum(h, self.plan, _CH_FIRST_STR)
+        return H
+
+    def _choice(self, batch, rir_index):
+        n = self.bank.shape[0]
+        if rir_index is None:
+            return self.rng.integers(0, n, size=batch)
+        idx = np.asarray(rir_index)
+        if idx.dtype.kind not in 'iu' or idx.ndim > 1 or (idx.ndim == 1 and idx.shape[0] != batch):
+            raise ValueError('rir_index must be an int or %d ints, got: %r' % (batch, rir_index))
+        if np.any(idx < 0) or np.any(idx >= n):
+            raise ValueError('rir_index must lie in [0, %d), got: %r' % (n, rir_index))
+        return np.broadcast_to(idx, (batch,)).astype(np.int64)
+
+    def call(self, x, rir_index=None):
+        if x.dim() != 3:
+            raise ValueError('Reverb expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise N.KapreNativeError('Reverb needs a CUDA tensor')
+        choice = self._choice(x.shape[0], rir_index)
+        self.last_choice = choice
+        length = x.shape[2] if self.data_format == _CH_FIRST_STR else x.shape[1]
+        if x.shape[0] == 0 or length == 0:
+            return x.float().clone()
+        H = self.spectra(x.device)
+        if np.all(choice == choice[0]):
+            H = H[int(choice[0]):int(choice[0]) + 1]          # one response: broadcast it, no gather
+        elif torch.cuda.is_current_stream_capturing():
+            H = torch.stack([H[int(i)] for i in choice])       # device-to-device only, so it can be captured
+        else:
+            H = H.index_select(0, torch.from_numpy(choice).to(x.device))
+        return ops.convolve_spectrum(x, H, self.plan, 0, length, self.data_format)
+
+    def get_config(self):
+        config = super().get_config()
+        config.update({'rirs': self.bank.tolist(), 'seed': self.seed, 'data_format': self.data_format_original})
+        return config

@@ -18,6 +18,8 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * Resample        -> ``kapre_resample_backward`` (the resampling kernel with up and down exchanged)
 * Speed, PitchShift's last step -> ``kapre_sinc_resample_backward`` (the interpolation kernel with step, offset and
   cutoff exchanged)
+* Convolve, Reverb -> ``kapre_convolve_backward`` (correlations of the output spectra's gradient with the filter's and
+  the signal's block spectra between the two transforms' adjoints) and ``kapre_convolve_ir_spectrum_backward``
 * PCEN            -> ``kapre_pcen_backward`` (reverse-time scan; input and parameter gradients)
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
@@ -251,6 +253,75 @@ class _SincResample(torch.autograd.Function):
         return ops.sinc_resample_backward(g, *ctx.cfg), None, None, None, None
 
 
+class _Convolve(torch.autograd.Function):
+    """x * h through ``kapre_convolve``.  The forward keeps H, and the signal spectra X only when h needs its
+    gradient (they are the start of the forward's workspace, so keeping them costs no launch)."""
+
+    @staticmethod
+    def forward(ctx, x, h, h3, plan, mode, data_format):
+        L = x.shape[ops._time_axis(data_format)]
+        K = h3.shape[ops._time_axis(data_format)]
+        H = ops.convolve_ir_spectrum(h3, plan, data_format)
+        y, ws = ops.convolve_full(x, H, plan, data_format)
+        start, n = ops.convolve_span(L, K, mode)
+        want_h = ctx.needs_input_grad[1]
+        if want_h:
+            Bn, C, P, F = x.shape[0], y.shape[1] if data_format == ops._CH_FIRST_STR else y.shape[2], H.shape[2], H.shape[3]
+            J = -(-L // plan.block)
+            ctx.save_for_backward(H, ws[:Bn * C * J * F * 8].view(torch.complex64).view(Bn, C, J, F))
+        else:
+            ctx.save_for_backward(H)
+        ctx.cfg = (plan, data_format, L, K, start, tuple(y.shape), tuple(h.shape), h3.shape)
+        return ops._crop(y, start, n, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        plan, fmt, L, K, start, full_shape, h_shape, h3_shape = ctx.cfg
+        H = ctx.saved_tensors[0]
+        X = ctx.saved_tensors[1] if len(ctx.saved_tensors) > 1 else None
+        g_full = _zero_padded(g, full_shape, start, fmt)
+        gx, gH = ops.convolve_backward(g_full, H, X, plan, fmt, L, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        gh = None
+        if gH is not None:
+            # a broadcast filter collects the gradient of every item / channel it served
+            if H.shape[0] == 1 and gH.shape[0] > 1:
+                gH = gH.sum(0, keepdim=True)
+            if H.shape[1] == 1 and gH.shape[1] > 1:
+                gH = gH.sum(1, keepdim=True)
+            gh = ops.convolve_ir_spectrum_backward(gH, plan, K)              # (Bh, Ch, K)
+            gh = gh.reshape(h_shape) if len(h_shape) == 1 else (gh if fmt == ops._CH_FIRST_STR else gh.transpose(1, 2))
+        return gx, gh, None, None, None, None
+
+
+class _ConvolveSpectrum(torch.autograd.Function):
+    """x * h with constant filter spectra H: the gradient reaches x only."""
+
+    @staticmethod
+    def forward(ctx, x, H, plan, start, length, data_format):
+        y, _ = ops.convolve_full(x, H, plan, data_format)
+        ctx.save_for_backward(H)
+        ctx.cfg = (plan, data_format, x.shape[ops._time_axis(data_format)], start, tuple(y.shape))
+        return ops._crop(y, start, length, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        plan, fmt, L, start, full_shape = ctx.cfg
+        (H,) = ctx.saved_tensors
+        gx, _ = ops.convolve_backward(_zero_padded(g, full_shape, start, fmt), H, None, plan, fmt, L, True, False)
+        return gx, None, None, None, None, None
+
+
+def _zero_padded(g, full_shape, start, data_format):
+    """The gradient of a cropped output, placed in zeros of the untrimmed output's shape."""
+    if tuple(g.shape) == tuple(full_shape):
+        return g
+    g_full = torch.zeros(full_shape, dtype=torch.float32, device=g.device)
+    ops._crop(g_full, start, g.shape[ops._time_axis(data_format)], data_format).copy_(g)
+    return g_full
+
+
 class _Pcen(torch.autograd.Function):
     """The forward is the plain PCEN launch that also writes the smoother state M; the backward reads E and M and
     returns the gradients of the input and of the four parameters (gain, bias, power, smooth_coef)."""
@@ -347,6 +418,14 @@ def resample(x, plan, data_format):
 
 def sinc_resample(x, ratio, length, offset, data_format):
     return _SincResample.apply(x.float(), ratio, length, offset, data_format)
+
+
+def convolve(x, h, h3, plan, mode, data_format):
+    return _Convolve.apply(x.float(), h, h3.float(), plan, mode, data_format)
+
+
+def convolve_spectrum(x, H, plan, start, length, data_format):
+    return _ConvolveSpectrum.apply(x.float(), H, plan, start, length, data_format)
 
 
 def pcen(E, params, eps, data_format):

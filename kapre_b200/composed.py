@@ -18,7 +18,7 @@ import torch
 from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
-from .augmentation import TimeStretch
+from .augmentation import Reverb, TimeStretch
 from .signal import Resample, Speed
 from .time_frequency import (STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
                              MagnitudeToDecibel, Phase, get_registered_object)
@@ -106,8 +106,9 @@ class Sequential(Layer):
 
     def call(self, x):
         start = 0
-        # Leading Resample and Speed layers run first, so that the STFT stack behind them still takes the fused launch.
-        while start < len(self.layers) and type(self.layers[start]) in (Resample, Speed):
+        # Leading Resample, Speed and Reverb layers run first, so that the STFT stack behind them still takes the fused
+        # launch.
+        while start < len(self.layers) and type(self.layers[start]) in (Resample, Speed, Reverb):
             x = self.layers[start].call(x)
             start += 1
         fused = self._fused_prefix(start) if (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3) else None
@@ -249,7 +250,9 @@ class Sequential(Layer):
     def capture(self, example):
         """Freeze this model for one input shape into a CUDA graph (``CapturedSequential``): replaying it
         costs one graph launch instead of one kernel launch + Python / ctypes dispatch per layer, which is
-        what bounds small batches (cfg1: 13 us of kernel under ~40 us of submission)."""
+        what bounds small batches (cfg1: 13 us of kernel under ~40 us of submission).  Random draws made on the
+        host (``Reverb``'s choice of responses) are part of what is captured: every replay reuses the draw made
+        at capture time."""
         return CapturedSequential(self, example)
 
     # -- serialisation ------------------------------------------------------------------------

@@ -27,6 +27,7 @@
 #include "grad_aux_core.cuh"
 #include "resample_core.cuh"
 #include "sinc_core.cuh"
+#include "conv_core.cuh"
 #include "pcen_core.cuh"
 #include "gl_core.cuh"
 #include "ts_core.cuh"
@@ -2184,6 +2185,202 @@ int kapre_sinc_resample(const kapre_sinc_plan* plan, const float* x_dev, const k
 int kapre_sinc_resample_backward(const kapre_sinc_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
                                  float* gx_dev, const kapre_wave_desc* gx_desc, double ratio, double offset, void* stream) {
     return kb_sinc_launch(plan, g_dev, g_desc, gx_dev, gx_desc, ratio, offset, 1, stream);
+}
+
+}  // extern "C"
+
+// ---- partitioned FFT convolution (conv_core.cuh) ---------------------------------------------------------
+__global__ void __launch_bounds__(KB_CONV_THREADS) kb_spec_conv_kernel(const __grid_constant__ KbConvParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_conv_cta(p, kb_smem, (int)blockIdx.x, (int)gridDim.x);
+}
+
+struct kapre_convolve_plan {
+    int B;                              // block size: STFT at n_fft 2B, window ones(B), hop B
+    DevInfo dev;
+    kapre_stft_plan* stft = nullptr;
+    kapre_istft_plan* istft = nullptr;  // n_fft = win_length = 2B, hop B, dual window ones(2B)
+};
+
+// Frames of a call: J = ceil(L / B) signal blocks, T = J + P - 1 output blocks, (T + 1) B untrimmed samples.
+static int kb_conv_geom(const kapre_convolve_plan* plan, long long L, long long P, int* J, int* T, int* out_len) {
+    if (L < 1) return kb_fail(KAPRE_E_INVALID, "signal length must be >= 1, got %lld", L);
+    if (P < 1) return kb_fail(KAPRE_E_INVALID, "filter spectrum must have >= 1 block, got P=%lld", P);
+    const long long j = (L + plan->B - 1) / plan->B, t = j + P - 1, n = (t + 1) * plan->B;
+    if (n > 0x7fffffffLL)
+        return kb_fail(KAPRE_E_INVALID, "%lld samples and %lld filter blocks of %d give %lld output samples, more than "
+                       "int32 holds", L, P, plan->B, n);
+    *J = (int)j; *T = (int)t; *out_len = (int)n;
+    return 0;
+}
+
+static long long kb_conv_spec_bytes(long long n_sig, long long frames, int B) {
+    return (n_sig * frames * (B + 1) * 8 + 255) / 256 * 256;
+}
+
+static kapre_spec_desc kb_conv_spec_desc(int C, int frames, int B) {
+    const long long F = B + 1;
+    return {(int64_t)C * frames * F, (int64_t)frames * F, F, 1};
+}
+
+// One launch of the per-bin multiply-accumulate over Bn x C sequences: To outputs from S a-frames and Tb b-frames.
+static int kb_conv_mac(const kapre_convolve_plan* plan, const void* a, const kapre_spec_desc* ad, int S, const void* b,
+                       const kapre_spec_desc* bd, int Tb, void* out, const kapre_spec_desc* od, int Bn, int C, int To,
+                       int correlate, cudaStream_t st) {
+    KbConvParams p{};
+    p.a = (const float2*)a; p.a_sb = ad->stride_b; p.a_sc = ad->stride_c; p.a_st = ad->stride_t; p.a_sf = ad->stride_f;
+    p.b = (const float2*)b; p.b_sb = bd->stride_b; p.b_sc = bd->stride_c; p.b_st = bd->stride_t; p.b_sf = bd->stride_f;
+    p.out = (float2*)out; p.o_sb = od->stride_b; p.o_sc = od->stride_c; p.o_st = od->stride_t; p.o_sf = od->stride_f;
+    p.Bn = Bn; p.C = C; p.F = plan->B + 1;
+    p.S = S; p.Tb = Tb; p.To = To;
+    p.correlate = correlate;
+    if (!kb_conv_setup(p, KB_CONV_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
+    int grid, rc;
+    if ((rc = kb_resident_grid(kb_spec_conv_kernel, KB_CONV_THREADS, KB_CONV_SMEM, p.n_tiles, plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_spec_conv_kernel, {.grid = grid, .block = KB_CONV_THREADS, .smem = KB_CONV_SMEM, .st = st,
+                                           .timed = true}, p);
+}
+
+static int kb_conv_check_wave(const kapre_wave_desc* d, const char* what) {
+    if (d->batch < 0 || d->channels < 0) return kb_fail(KAPRE_E_INVALID, "%s: negative size", what);
+    return 0;
+}
+
+extern "C" {
+
+int64_t kapre_convolve_block_size(int64_t ir_length) {
+    if (ir_length < 1) return kb_fail(KAPRE_E_INVALID, "filter length must be >= 1, got %lld", (long long)ir_length);
+    return kb_conv_block_size(ir_length);
+}
+
+int kapre_convolve_plan_create(int block, kapre_convolve_plan** out) {
+    if (!out) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (block != 128 && block != 256 && block != 512 && block != 1024)
+        return kb_fail(KAPRE_E_INVALID, "block size must be 128, 256, 512 or 1024, got %d", block);
+    kapre_convolve_plan* p = new kapre_convolve_plan();
+    p->B = block;
+    int rc = kb_dev_info(&p->dev);
+    if (rc) { delete p; return rc; }
+    const std::vector<float> ones(2 * block, 1.0f);
+    if ((rc = kapre_stft_plan_create(2 * block, block, block, ones.data(), &p->stft)) ||
+        (rc = kapre_istft_plan_create(2 * block, 2 * block, block, ones.data(), &p->istft))) {
+        kapre_convolve_plan_destroy(p);
+        return rc;
+    }
+    *out = p;
+    return 0;
+}
+
+void kapre_convolve_plan_destroy(kapre_convolve_plan* p) {
+    if (!p) return;
+    kapre_stft_plan_destroy(p->stft);
+    kapre_istft_plan_destroy(p->istft);
+    delete p;
+}
+
+int kapre_convolve_ir_spectrum(const kapre_convolve_plan* plan, const float* h_dev, const kapre_wave_desc* h_desc,
+                               void* H_dev, const kapre_spec_desc* H_desc, void* stream) {
+    if (!plan || !h_desc || !H_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (h_desc->length < 1) return kb_fail(KAPRE_E_INVALID, "filter length must be >= 1, got %d", h_desc->length);
+    int rc = kb_conv_check_wave(h_desc, "filter");
+    if (rc) return rc;
+    return kapre_stft_forward(plan->stft, h_dev, h_desc, 0, 1, KAPRE_OUT_COMPLEX, H_dev, H_desc, nullptr, nullptr,
+                              nullptr, stream);
+}
+
+int64_t kapre_convolve_workspace_bytes(const kapre_convolve_plan* plan, int batch, int channels, int length, int P) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (batch < 0 || channels < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    int J, T, n, rc;
+    if ((rc = kb_conv_geom(plan, length, P, &J, &T, &n))) return rc;
+    const long long sig = (long long)batch * channels;
+    return kb_conv_spec_bytes(sig, J, plan->B) + kb_conv_spec_bytes(sig, T, plan->B);
+}
+
+int kapre_convolve(const kapre_convolve_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, const void* H_dev,
+                   const kapre_spec_desc* H_desc, int P, float* y_dev, const kapre_wave_desc* y_desc, void* workspace_dev,
+                   void* stream) {
+    if (!plan || !x_desc || !H_desc || !y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
+    if ((rc = kb_conv_check_wave(x_desc, "signal"))) return rc;
+    int J, T, n;
+    if ((rc = kb_conv_geom(plan, x_desc->length, P, &J, &T, &n))) return rc;
+    if (y_desc->batch != x_desc->batch || y_desc->channels != x_desc->channels || y_desc->length != n)
+        return kb_fail(KAPRE_E_INVALID, "output must be %d x %d x %d samples, got %d x %d x %d", x_desc->batch,
+                       x_desc->channels, n, y_desc->batch, y_desc->channels, y_desc->length);
+    const int Bn = x_desc->batch, C = x_desc->channels;
+    if (Bn == 0 || C == 0) return 0;
+    if (!x_dev || !H_dev || !y_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    void* X = workspace_dev;
+    void* Y = (char*)workspace_dev + kb_conv_spec_bytes((long long)Bn * C, J, plan->B);
+    const kapre_spec_desc Xd = kb_conv_spec_desc(C, J, plan->B), Yd = kb_conv_spec_desc(C, T, plan->B);
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = kapre_stft_forward(plan->stft, x_dev, x_desc, 0, 1, KAPRE_OUT_COMPLEX, X, &Xd, nullptr, nullptr, nullptr,
+                                 stream)))
+        return rc;
+    if ((rc = kb_conv_mac(plan, H_dev, H_desc, P, X, &Xd, J, Y, &Yd, Bn, C, T, 0, st))) return rc;
+    return kapre_istft_inverse(plan->istft, Y, Bn, C, T, &Yd, y_dev, y_desc, stream);
+}
+
+int64_t kapre_convolve_backward_workspace_bytes(const kapre_convolve_plan* plan, int batch, int channels, int length,
+                                                int P) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (batch < 0 || channels < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    int J, T, n, rc;
+    if ((rc = kb_conv_geom(plan, length, P, &J, &T, &n))) return rc;
+    const long long sig = (long long)batch * channels;
+    const long long ola = length % plan->B ? (sig * J * plan->B * 4 + 255) / 256 * 256 : 0;
+    return kb_conv_spec_bytes(sig, T, plan->B) + kb_conv_spec_bytes(sig, J, plan->B) + ola;
+}
+
+int kapre_convolve_backward(const kapre_convolve_plan* plan, const float* gy_dev, const kapre_wave_desc* gy_desc,
+                            const void* H_dev, const kapre_spec_desc* H_desc, const void* X_dev,
+                            const kapre_spec_desc* X_desc, int P, float* gx_dev, const kapre_wave_desc* gx_desc,
+                            void* gH_dev, const kapre_spec_desc* gH_desc, void* workspace_dev, void* stream) {
+    if (!plan || !gy_desc || !gx_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (gx_dev && !H_desc) return kb_fail(KAPRE_E_INVALID, "the signal gradient needs H and its descriptor");
+    if (gH_dev && (!X_desc || !gH_desc)) return kb_fail(KAPRE_E_INVALID, "the filter gradient needs X and gH descriptors");
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
+    if ((rc = kb_conv_check_wave(gx_desc, "signal gradient"))) return rc;
+    int J, T, n;
+    if ((rc = kb_conv_geom(plan, gx_desc->length, P, &J, &T, &n))) return rc;
+    if (gy_desc->batch != gx_desc->batch || gy_desc->channels != gx_desc->channels || gy_desc->length != n)
+        return kb_fail(KAPRE_E_INVALID, "output gradient must be %d x %d x %d samples, got %d x %d x %d", gx_desc->batch,
+                       gx_desc->channels, n, gy_desc->batch, gy_desc->channels, gy_desc->length);
+    const int Bn = gx_desc->batch, C = gx_desc->channels;
+    if (Bn == 0 || C == 0 || (!gx_dev && !gH_dev)) return 0;
+    if (!gy_dev || !workspace_dev || (gx_dev && !H_dev) || (gH_dev && !X_dev))
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    const long long sig = (long long)Bn * C;
+    void* G = workspace_dev;
+    void* gX = (char*)workspace_dev + kb_conv_spec_bytes(sig, T, plan->B);
+    void* ola = (char*)gX + kb_conv_spec_bytes(sig, J, plan->B);
+    const kapre_spec_desc Gd = kb_conv_spec_desc(C, T, plan->B), gXd = kb_conv_spec_desc(C, J, plan->B);
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = kapre_istft_backward(plan->istft, gy_dev, gy_desc, Bn, C, T, G, &Gd, stream))) return rc;
+    if (gx_dev) {
+        if ((rc = kb_conv_mac(plan, H_dev, H_desc, P, G, &Gd, T, gX, &gXd, Bn, C, J, 1, st))) return rc;
+        if ((rc = kapre_stft_backward(plan->stft, gX, &gXd, Bn, C, J, 0, 1, gx_dev, gx_desc, ola, stream))) return rc;
+    }
+    if (gH_dev && (rc = kb_conv_mac(plan, X_dev, X_desc, J, G, &Gd, T, gH_dev, gH_desc, Bn, C, P, 1, st))) return rc;
+    return 0;
+}
+
+int kapre_convolve_ir_spectrum_backward(const kapre_convolve_plan* plan, const void* gH_dev, const kapre_spec_desc* gH_desc,
+                                        int P, float* gh_dev, const kapre_wave_desc* gh_desc, void* workspace_dev,
+                                        void* stream) {
+    if (!plan || !gH_desc || !gh_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (gh_desc->length < 1) return kb_fail(KAPRE_E_INVALID, "filter length must be >= 1, got %d", gh_desc->length);
+    int rc = kb_conv_check_wave(gh_desc, "filter gradient");
+    if (rc) return rc;
+    if ((gh_desc->length + (long long)plan->B - 1) / plan->B != P)
+        return kb_fail(KAPRE_E_INVALID, "a filter of %d taps has %d blocks of %d, got P=%d", gh_desc->length,
+                       (gh_desc->length + plan->B - 1) / plan->B, plan->B, P);
+    return kapre_stft_backward(plan->stft, gH_dev, gH_desc, gh_desc->batch, gh_desc->channels, P, 0, 1, gh_dev, gh_desc,
+                               workspace_dev, stream);
 }
 
 }  // extern "C"

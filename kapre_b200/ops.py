@@ -825,6 +825,189 @@ def sinc_resample_backward(g: torch.Tensor, ratio, offset, data_format, length):
     return gx
 
 
+class ConvolvePlan(_PerDevice):
+    """kapre_convolve_plan per CUDA device for one block size: the STFT (n_fft 2B, window ones(B), hop B) and the
+    inverse (dual window ones(2B)) of the partitioned convolution.  One instance per block size (``convolve_plan``)."""
+
+    def __init__(self, block):
+        self.block = int(block)
+        self._per_device = {}
+
+    _destroy = 'kapre_convolve_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_convolve_plan_create(self.block, out)
+
+
+_conv_plans = {}
+CONVOLVE_MODES = ('full', 'same', 'valid')
+
+
+def convolve_block_size(ir_length):
+    """The partition's block size B for a filter of ``ir_length`` taps (``kapre_convolve_block_size``)."""
+    b = int(N.lib().kapre_convolve_block_size(int(ir_length)))
+    if b < 0:
+        N.check(b)
+    return b
+
+
+def convolve_plan(block):
+    with _lock:
+        plan = _conv_plans.get(block)
+        if plan is None:
+            plan = _conv_plans[block] = ConvolvePlan(block)
+    return plan
+
+
+def convolve_span(length, ir_length, mode):
+    """(start, length) of torchaudio.functional.fftconvolve's ``mode`` inside the full convolution."""
+    full = length + ir_length - 1
+    if mode == 'full':
+        return 0, full
+    target = length if mode == 'same' else max(length, ir_length) - min(length, ir_length) + 1
+    return (full - target) // 2, target
+
+
+def _time_axis(data_format):
+    return 2 if data_format == _CH_FIRST_STR else 1
+
+
+def _spec_contiguous_desc(H, broadcast_b=False, broadcast_c=False):
+    """Descriptor of a contiguous (B, C, frames, F) complex tensor; a broadcast dimension gets stride 0."""
+    sb, sc, st, sf = H.stride()
+    return N.SpecDesc(0 if broadcast_b else sb, 0 if broadcast_c else sc, st, sf)
+
+
+def _conv_check(x, h, data_format):
+    """Shapes of ``convolve``'s operands: x (B, L, C) / (B, C, L); h (K,) or 3-D in x's format with batch in {1, B}
+    and channels in {1, C}.  Returns (h as a 3-D tensor, (B, C, L), (Bh, Ch, K))."""
+    if x.dim() != 3:
+        raise ValueError('convolve expects a 3-D signal batch, got shape %s' % (tuple(x.shape),))
+    B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == _CH_LAST_STR else tuple(x.shape)
+    if h.dim() == 1:
+        h = h.view(1, 1, -1) if data_format == _CH_FIRST_STR else h.view(1, -1, 1)
+    elif h.dim() != 3:
+        raise ValueError('the filter must be 1-D or 3-D, got shape %s' % (tuple(h.shape),))
+    Bh, Ch, K = (h.shape[0], h.shape[2], h.shape[1]) if data_format == _CH_LAST_STR else tuple(h.shape)
+    if Bh not in (1, B) or Ch not in (1, C):
+        raise ValueError('filter batch %d and channels %d must be 1 or the signal\'s (%d, %d)' % (Bh, Ch, B, C))
+    if L < 1 or K < 1:
+        raise ValueError('signal and filter need at least one sample, got %d and %d' % (L, K))
+    return h, (B, C, L), (Bh, Ch, K)
+
+
+def convolve_ir_spectrum(h, plan: ConvolvePlan, data_format):
+    """The block spectra H (Bh, Ch, P, B + 1) complex64 of a 3-D filter tensor in ``data_format`` (one launch)."""
+    if h.dtype != torch.float32:
+        h = h.float()
+    hd, (Bh, Ch, K) = _wave_desc(h, data_format)
+    P = -(-K // plan.block)
+    H = torch.empty((Bh, Ch, P, plan.block + 1), dtype=torch.complex64, device=h.device)
+    if H.numel():
+        N.check(N.lib().kapre_convolve_ir_spectrum(plan.handle(), _ptr(h), ctypes.byref(hd), _ptr(H),
+                                                   ctypes.byref(N.SpecDesc(*H.stride())), _stream_ptr()))
+    return H
+
+
+def _conv_workspace_bytes(plan, B, C, L, P, backward=False):
+    fn = N.lib().kapre_convolve_backward_workspace_bytes if backward else N.lib().kapre_convolve_workspace_bytes
+    n = int(fn(plan.handle(), B, C, L, P))
+    if n < 0:
+        N.check(n)
+    return n
+
+
+def convolve_full(x, H, plan: ConvolvePlan, data_format):
+    """x * h from the filter's block spectra H (``convolve_ir_spectrum``; batch and channels 1 broadcast): the
+    untrimmed (T + 1) B samples of ``kapre_convolve`` and the workspace, which begins with the signal spectra X."""
+    if x.dtype != torch.float32:
+        x = x.float()
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    P, blk = H.shape[2], plan.block
+    nbytes = _conv_workspace_bytes(plan, B, C, L, P)
+    T = -(-L // blk) + P - 1
+    y, yd = _wave_alloc(B, C, (T + 1) * blk, data_format, x.device)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    if y.numel():
+        Hd = _spec_contiguous_desc(H, H.shape[0] == 1, H.shape[1] == 1)
+        N.check(N.lib().kapre_convolve(plan.handle(), _ptr(x), ctypes.byref(xd), _ptr(H), ctypes.byref(Hd), P, _ptr(y),
+                                       ctypes.byref(yd), _ptr(ws), _stream_ptr()))
+    return y, ws
+
+
+def convolve_backward(g_full, H, X, plan: ConvolvePlan, data_format, length, want_x, want_h):
+    """Gradients of ``convolve_full`` given the gradient of its untrimmed output: (gx or None, per-(item, channel) gH
+    (B, C, P, B + 1) or None).  ``X``: the signal spectra ``convolve_full`` left in its workspace (for gH)."""
+    g_full = _raw(g_full.to(torch.float32))
+    gd, (B, C, _) = _wave_desc(g_full, data_format)
+    P, blk = H.shape[2], plan.block
+    gx, xd = _wave_alloc(B, C, int(length), data_format, g_full.device)
+    gH = torch.empty((B, C, P, blk + 1), dtype=torch.complex64, device=g_full.device) if want_h else None
+    ws = torch.empty(_conv_workspace_bytes(plan, B, C, int(length), P, backward=True), dtype=torch.uint8,
+                     device=g_full.device)
+    Hd = _spec_contiguous_desc(H, H.shape[0] == 1, H.shape[1] == 1)
+    Xd = N.SpecDesc(*X.stride()) if want_h else None
+    gHd = N.SpecDesc(*gH.stride()) if want_h else None
+    N.check(N.lib().kapre_convolve_backward(
+        plan.handle(), _ptr(g_full), ctypes.byref(gd), _ptr(H), ctypes.byref(Hd),
+        _ptr(X) if want_h else None, ctypes.byref(Xd) if want_h else None, P,
+        _ptr(gx) if want_x else None, ctypes.byref(xd), _ptr(gH) if want_h else None,
+        ctypes.byref(gHd) if want_h else None, _ptr(ws), _stream_ptr()))
+    return (gx if want_x else None), gH
+
+
+def convolve_ir_spectrum_backward(gH, plan: ConvolvePlan, ir_length):
+    """Gradient of ``convolve_ir_spectrum`` given gH (Bh, Ch, P, B + 1): a (Bh, Ch, K) channels_first filter gradient.
+    It is computed for the P B samples the blocks cover (no scratch needed) and cropped to K."""
+    gH = _raw(gH).contiguous()
+    Bh, Ch, P, _ = gH.shape
+    gh, hd = _wave_alloc(Bh, Ch, P * plan.block, _CH_FIRST_STR, gH.device)
+    N.check(N.lib().kapre_convolve_ir_spectrum_backward(plan.handle(), _ptr(gH), ctypes.byref(N.SpecDesc(*gH.stride())),
+                                                        P, _ptr(gh), ctypes.byref(hd), None, _stream_ptr()))
+    return gh[:, :, :int(ir_length)]
+
+
+def _crop(y, start, length, data_format):
+    return y.narrow(_time_axis(data_format), start, length)
+
+
+@_device_of_first_arg
+def convolve(x: torch.Tensor, h: torch.Tensor, mode='full', data_format=_CH_LAST_STR):
+    """``torchaudio.functional.fftconvolve`` along the time axis of x (B, L, C) / (B, C, L) with a filter h: (K,)
+    shared by every item and channel, or 3-D in x's format with batch in {1, B} and channels in {1, C} (1
+    broadcasts).  ``mode``: 'full' (L + K - 1 samples), 'same' (L) or 'valid' (max(L, K) - min(L, K) + 1); the
+    result may be a view of the untrimmed output.  Four launches: the filter's spectra, then ``kapre_convolve``'s
+    three.  Differentiable with respect to x and h."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and isinstance(h, torch.Tensor) and h.is_cuda):
+        raise N.KapreNativeError('convolve needs CUDA tensors')
+    if x.device != h.device:
+        raise ValueError('signal on %s, filter on %s' % (x.device, h.device))
+    if mode not in CONVOLVE_MODES:
+        raise ValueError('mode must be one of %s, got: %r' % (CONVOLVE_MODES, mode))
+    h3, (B, C, L), (Bh, Ch, K) = _conv_check(x, h, data_format)
+    plan = convolve_plan(convolve_block_size(K))
+    _conv_workspace_bytes(plan, B, C, L, -(-K // plan.block))      # size checks before anything is launched
+    if _wants_grad(x) or _wants_grad(h):
+        from . import autograd
+        return autograd.convolve(x, h, h3, plan, mode, data_format)
+    start, n = convolve_span(L, K, mode)
+    y, _ = convolve_full(x, convolve_ir_spectrum(h3, plan, data_format), plan, data_format)
+    return _crop(y, start, n, data_format)
+
+
+@_device_of_first_arg
+def convolve_spectrum(x: torch.Tensor, H: torch.Tensor, plan: ConvolvePlan, start, length, data_format=_CH_LAST_STR):
+    """``kapre_convolve`` with given filter spectra H (a constant: the gradient reaches x only), cropped to
+    [start, start + length) of the untrimmed output."""
+    if not x.is_cuda:
+        raise N.KapreNativeError('convolve needs a CUDA tensor')
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.convolve_spectrum(x, H, plan, start, length, data_format)
+    y, _ = convolve_full(x, H, plan, data_format)
+    return _crop(y, start, length, data_format)
+
+
 def _pcen_params(params, eps, device):
     """kapre_pcen_params over the four parameter tensors (gain, bias, power, smooth_coef): float32, 0-d (one value
     for every band) or 1-d (one per band), on ``device``."""

@@ -3,18 +3,19 @@
 (:365-447).  Same constructor arguments, validation and ``get_config`` keys; ``call`` runs CUDA
 kernels through the C ABI.  ``Resample`` (polyphase sample-rate conversion) has no counterpart in the
 reference, which expects audio to be resampled before it reaches the model; neither has ``Speed`` (speed perturbation by any
-real factor, band-limited interpolation)."""
+real factor, band-limited interpolation) or ``Convolve`` (convolution with long filters, partitioned FFT)."""
 from __future__ import annotations
 
 import math
 
 import numpy as np
+import torch
 
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
-__all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed']
+__all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve']
 
 
 def _resolve(fmt):
@@ -177,6 +178,40 @@ class Speed(Layer):
 
     _config_fields = (
         ('factor', 'factor'),
+        ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class Convolve(Layer):
+    """Convolution of waveforms with filters along the time axis (``torchaudio.transforms.Convolve``, i.e.
+    ``torchaudio.functional.fftconvolve``): ``call(x, h)`` with ``x`` ``(batch, time, ch)`` / ``(batch, ch, time)`` and
+    ``h`` either ``(K,)``, one filter for every item and channel, or 3-D in the same data format with batch 1 or
+    ``batch`` and channels 1 or ``ch`` (1 broadcasts).  ``mode``: 'full' (``time + K - 1`` samples), 'same' (``time``)
+    or 'valid' (``max(time, K) - min(time, K) + 1``), cropped from the full convolution as torchaudio does.
+
+    A uniformly partitioned overlap-add (``kapre_convolve``): the filter's block spectra, then the STFT of the signal,
+    one per-bin multiply-accumulate along the blocks and the inverse STFT, four launches in all.  The block size is a
+    function of ``K`` alone, so an output does not depend on the batch it came in.  Differentiable with respect to
+    ``x`` and ``h``."""
+
+    def __init__(self, mode='full', data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        if mode not in ops.CONVOLVE_MODES:
+            raise ValueError('mode must be one of %s, got: %r' % (ops.CONVOLVE_MODES, mode))
+        self.mode = mode
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+
+    def call(self, x, h):
+        if not (isinstance(h, torch.Tensor) and h.is_cuda):
+            h, _ = ops.to_device(h)
+        return ops.convolve(x, h, self.mode, self.data_format)
+
+    _config_fields = (
+        ('mode', 'mode'),
         ('data_format', 'data_format_str'),
     )
 
