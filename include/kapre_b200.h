@@ -336,6 +336,41 @@ int kapre_convolve_ir_spectrum_backward(const kapre_convolve_plan* plan, const v
                                         int P, float* gh_dev, const kapre_wave_desc* gh_desc, void* workspace_dev,
                                         void* stream);
 
+/* ---- IIR filters (torchaudio.functional.lfilter) ---------------------------------------------------
+ * Along the time axis of every (item, channel) column, with normalised coefficients (b / a0, a / a0):
+ *   y[t] = sum_{k=0..N} b[k] x[t-k] - sum_{k=1..N} a[k] y[t-k],   x, y = 0 before t = 0,
+ * then clamped to [-1, 1] with KAPRE_IIR_CLAMP.  KAPRE_IIR_REVERSE runs the filter in reverse time (sample t is
+ * read and written at L-1-t), which is filtfilt's second pass without a flip.  Order N <= 8
+ * (KAPRE_E_UNSUPPORTED above).  Coefficients: N + 1 consecutive floats per filter at b + i stride_b + c stride_c
+ * (a[0] is not read); a stride of 0 shares one filter over the batch or the channels.
+ * The kernel cuts time into chunks of 65 samples and carries the chunk states in float64 (DESIGN.md §IIR), so that
+ * y[t] depends on x[0..t] and the coefficients alone: not on the length, the batch, the strides or broadcasting.
+ * Four launches: the state-transition powers, the chunk states, the carry across blocks of 32 chunks, the output. */
+typedef struct {
+    const float* b;
+    const float* a;
+    int64_t b_stride_b, b_stride_c, a_stride_b, a_stride_c;
+    int order;
+} kapre_iir_coeffs;
+#define KAPRE_IIR_CLAMP 1
+#define KAPRE_IIR_REVERSE 2
+/* Scratch of kapre_lfilter and kapre_lfilter_backward.  < 0 on error: a negative size, an order outside [0, 8], or a
+ * workspace or chunk count beyond int64 / int32. */
+int64_t kapre_lfilter_workspace_bytes(int batch, int channels, int length, int order);
+/* y = lfilter(x).  x_desc and y_desc: same batch, channels and length, any strides; y must not alias x. */
+int kapre_lfilter(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_iir_coeffs* coeffs, int flags,
+                  float* y_dev, const kapre_wave_desc* y_desc, void* workspace_dev, void* stream);
+/* Gradients of kapre_lfilter (called with the forward's flags; KAPRE_IIR_CLAMP is ignored: the gradient is that of
+ * the unclamped output).  With v the all-pole recursion run the other way on gy,
+ *   gx[t] = sum_k b[k] v[t+k],   gb[k] = sum_t v[t] x[t-k],   ga[k] = -sum_t v[t] y[t-k]  (k >= 1, y unclamped).
+ * partials_dev (optional; needs x_dev and y_dev): (2 N + 1, batch, channels, ceil(length / 65)) float32, row k <= N
+ * the gb[k] sums per chunk, row N + k the ga[k] sums; the caller sums them (over broadcast axes too).  Four
+ * launches. */
+int kapre_lfilter_backward(const float* gy_dev, const kapre_wave_desc* gy_desc, const float* x_dev,
+                           const kapre_wave_desc* x_desc, const float* y_dev, const kapre_wave_desc* y_desc,
+                           const kapre_iir_coeffs* coeffs, int flags, float* gx_dev, const kapre_wave_desc* gx_desc,
+                           float* partials_dev, void* workspace_dev, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

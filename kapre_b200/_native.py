@@ -46,6 +46,14 @@ class FbInvCfg(Structure):
     _fields_ = [('n_iter', c_int), ('from_decibel', c_int), ('ref_value', c_float), ('amin', c_float)]
 
 
+class IirCoeffs(Structure):
+    _fields_ = [('b', c_void_p), ('a', c_void_p), ('b_stride_b', c_int64), ('b_stride_c', c_int64),
+                ('a_stride_b', c_int64), ('a_stride_c', c_int64), ('order', c_int)]
+
+
+IIR_CLAMP, IIR_REVERSE = 1, 2
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -117,6 +125,12 @@ SYMBOLS = [
                                         POINTER(SpecDesc), c_void_p, c_void_p]),
     ('kapre_convolve_ir_spectrum_backward', c_int, [c_void_p, c_void_p, POINTER(SpecDesc), c_int, c_void_p,
                                                     POINTER(WaveDesc), c_void_p, c_void_p]),
+    ('kapre_lfilter_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int]),
+    ('kapre_lfilter', c_int, [c_void_p, POINTER(WaveDesc), POINTER(IirCoeffs), c_int, c_void_p, POINTER(WaveDesc),
+                              c_void_p, c_void_p]),
+    ('kapre_lfilter_backward', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p,
+                                       POINTER(WaveDesc), POINTER(IirCoeffs), c_int, c_void_p, POINTER(WaveDesc),
+                                       c_void_p, c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

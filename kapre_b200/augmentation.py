@@ -2,7 +2,7 @@
 masking is one CUDA pass (``kapre_spec_augment``).  ``TimeStretch``: a phase vocoder, one CUDA scan over time
 (``kapre_time_stretch``).  ``PitchShift``: STFT, that phase vocoder, the inverse STFT and one band-limited
 interpolation (``kapre_sinc_resample``) back to the input length.  ``Reverb``: convolution with a room impulse response
-drawn from a bank (``kapre_convolve``)."""
+drawn from a bank (``kapre_convolve``).  ``RandomBiquad``: a biquad drawn per item (``kapre_lfilter``)."""
 from __future__ import annotations
 
 import numpy as np
@@ -307,4 +307,75 @@ class Reverb(Layer):
     def get_config(self):
         config = super().get_config()
         config.update({'rirs': self.bank.tolist(), 'seed': self.seed, 'data_format': self.data_format_original})
+        return config
+
+
+@register_keras_serializable(package='Kapre')
+class RandomBiquad(Layer):
+    """A random biquad per item (filter augmentation): ``kind`` one of ``backend.BIQUAD_KINDS``; per item the
+    frequency is drawn log-uniformly from ``freq_range`` (Hz, inside (0, sample_rate / 2)), ``Q`` uniformly from
+    ``Q_range`` and, for the equalizer, ``gain`` (dB) uniformly from ``gain_range``, with
+    ``np.random.default_rng(seed)``.  ``(batch, time, ch)`` / ``(batch, ch, time)`` in, the same shape out; every
+    channel of an item gets the item's filter, and the output is clamped to [-1, 1] as torchaudio's biquads do.
+
+    The coefficients are designed and normalised in float64 on the host and passed as one ``(batch, 1, 3)`` pair, so
+    a call is one ``kapre_lfilter`` (four launches).  ``last_choice`` records the draw as ``(freq, Q, gain)`` arrays.
+    The layer applies on every call (``Sequential`` passes no ``training`` flag); a captured graph
+    (``Sequential.capture``) replays the draw made when it was captured.  The gradient reaches the input."""
+
+    def __init__(self, kind, sample_rate, freq_range, Q_range=(0.707, 0.707), gain_range=(0.0, 0.0), seed=None,
+                 data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        if kind not in backend.BIQUAD_KINDS:
+            raise ValueError('kind must be one of %s, got: %r' % (backend.BIQUAD_KINDS, kind))
+        ranges = []
+        for name, r in (('freq_range', freq_range), ('Q_range', Q_range), ('gain_range', gain_range)):
+            r = tuple(float(v) for v in r)
+            if len(r) != 2 or not (np.isfinite(r[0]) and np.isfinite(r[1])) or r[0] > r[1]:
+                raise ValueError('%s must be a (low, high) pair of finite numbers, got: %r' % (name, r))
+            ranges.append(r)
+        # the ends of each range must make valid filters (biquad_coefficients checks them)
+        backend.biquad_coefficients(kind, sample_rate, [ranges[0][0], ranges[0][1]], [ranges[1][0], ranges[1][1]],
+                                    [ranges[2][0], ranges[2][1]])
+        self.kind, self.sample_rate = kind, sample_rate
+        self.freq_range, self.Q_range, self.gain_range = ranges
+        self.seed = seed
+        self.rng = np.random.default_rng(seed)
+        self.last_choice = None
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self._captured = []
+
+    def draw(self, batch):
+        """(freq, Q, gain) arrays of ``batch`` draws, in that order from the layer's generator."""
+        lo, hi = np.log(self.freq_range[0]), np.log(self.freq_range[1])
+        freq = np.exp(self.rng.uniform(lo, hi, size=batch))
+        Q = self.rng.uniform(self.Q_range[0], self.Q_range[1], size=batch)
+        gain = self.rng.uniform(self.gain_range[0], self.gain_range[1], size=batch)
+        return freq, Q, gain
+
+    def call(self, x):
+        if x.dim() != 3:
+            raise ValueError('RandomBiquad expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise N.KapreNativeError('RandomBiquad needs a CUDA tensor')
+        freq, Q, gain = self.draw(x.shape[0])
+        self.last_choice = (freq, Q, gain)
+        b, a = backend.biquad_coefficients(self.kind, self.sample_rate, freq, Q, gain)
+        host = torch.from_numpy(np.stack([b / a[:, :1], a / a[:, :1]]).astype(np.float32)).reshape(2, -1, 1, 3)
+        if torch.cuda.is_current_stream_capturing():
+            # the graph's copy node reads this pinned buffer on every replay: it is kept and never written again
+            host = host.pin_memory()
+            self._captured.append(host)
+        coef = host.to(x.device, non_blocking=True)
+        from .signal import lfilter
+        return lfilter(x, coef[1], coef[0], clamp=True, data_format=self.data_format)
+
+    def get_config(self):
+        config = super().get_config()
+        config.update({'kind': self.kind, 'sample_rate': self.sample_rate, 'freq_range': list(self.freq_range),
+                       'Q_range': list(self.Q_range), 'gain_range': list(self.gain_range), 'seed': self.seed,
+                       'data_format': self.data_format_original})
         return config

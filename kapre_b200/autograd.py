@@ -21,6 +21,9 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * Convolve, Reverb -> ``kapre_convolve_backward`` (correlations of the output spectra's gradient with the filter's and
   the signal's block spectra between the two transforms' adjoints) and ``kapre_convolve_ir_spectrum_backward``
 * PCEN            -> ``kapre_pcen_backward`` (reverse-time scan; input and parameter gradients)
+* lfilter, filtfilt, IIRFilter, Biquad, RandomBiquad -> ``kapre_lfilter_backward`` (the all-pole recursion run the
+  other way on the output gradient; input and normalised-coefficient gradients, the rest through torch's division
+  by a0)
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
@@ -341,6 +344,28 @@ class _Pcen(torch.autograd.Function):
         return (gE, *gp, None, None)
 
 
+class _Lfilter(torch.autograd.Function):
+    """The forward is the plain lfilter launch without the clamp (the caller clamps with torch.clamp); the output is
+    saved only when a coefficient needs its gradient, which is the only time the backward reads x and y."""
+
+    @staticmethod
+    def forward(ctx, x, b, a, flags, data_format):
+        y = ops.lfilter_forward(x, b, a, flags, data_format)
+        want = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
+        ctx.save_for_backward(x if want else None, y if want else None, b, a)
+        ctx.cfg = (flags, data_format, want)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x, y, b, a = ctx.saved_tensors
+        flags, data_format, want = ctx.cfg
+        gx, gb, ga = ops.lfilter_backward(gy, x, y, b, a, flags, data_format, want)
+        return (gx if ctx.needs_input_grad[0] else None, gb if ctx.needs_input_grad[1] else None,
+                ga if ctx.needs_input_grad[2] else None, None, None)
+
+
 class _TimeStretch(torch.autograd.Function):
     """The forward is the plain time-stretch launch; autograd saves its output, from which the backward takes the
     magnitude and phase gradients, so the forward writes nothing extra."""
@@ -430,6 +455,10 @@ def convolve_spectrum(x, H, plan, start, length, data_format):
 
 def pcen(E, params, eps, data_format):
     return _Pcen.apply(E.float(), *params, eps, data_format)
+
+
+def lfilter(x, b, a, flags, data_format):
+    return _Lfilter.apply(x.float(), b, a, flags, data_format)
 
 
 def time_stretch(X, rate, data_format):

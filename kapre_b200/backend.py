@@ -218,3 +218,45 @@ def filterbank_log(sample_rate: int, n_freq: int, n_bins: int = 84, bins_per_oct
     l1 = np.abs(basis).sum(axis=1, keepdims=True)
     l1 = np.where(l1 < np.finfo(np.float64).tiny, 1.0, l1)
     return np.ascontiguousarray((basis / l1).astype(_get_floatx()).T)
+
+
+BIQUAD_KINDS = ('lowpass', 'highpass', 'bandpass', 'bandreject', 'allpass', 'equalizer')
+
+
+def biquad_coefficients(kind: str, sample_rate, freq, Q=0.707, gain=0.0):
+    """(b, a): float64 arrays of shape (..., 3), not normalised, of torchaudio's biquad designs
+    (``lowpass_biquad``, ``highpass_biquad``, ``bandpass_biquad`` with ``const_skirt_gain=False``,
+    ``bandreject_biquad``, ``allpass_biquad``, ``equalizer_biquad``; the RBJ audio-EQ cookbook).  ``freq``, ``Q`` and
+    ``gain`` (dB, equalizer only) may be arrays of one shape, which gives one filter per element."""
+    if kind not in BIQUAD_KINDS:
+        raise ValueError('kind must be one of %s, got: %r' % (BIQUAD_KINDS, kind))
+    freq, Q, gain = np.broadcast_arrays(np.asarray(freq, np.float64), np.asarray(Q, np.float64),
+                                        np.asarray(gain, np.float64))
+    if not (np.isfinite(sample_rate) and sample_rate > 0):
+        raise ValueError('sample_rate must be positive, got: %r' % (sample_rate,))
+    if not (np.all(freq > 0) and np.all(freq < sample_rate / 2)):
+        raise ValueError('freq must lie in (0, sample_rate / 2), got: %r' % (freq,))
+    if not (np.all(Q > 0) and np.all(np.isfinite(Q))):
+        raise ValueError('Q must be positive and finite, got: %r' % (Q,))
+    if not np.all(np.isfinite(gain)):
+        raise ValueError('gain must be finite, got: %r' % (gain,))
+    w0 = 2 * np.pi * freq / sample_rate
+    alpha = np.sin(w0) / 2 / Q
+    c = np.cos(w0)
+    one = np.ones_like(w0)
+    a = [1 + alpha, -2 * c, 1 - alpha]
+    if kind == 'lowpass':
+        b = [(1 - c) / 2, 1 - c, (1 - c) / 2]
+    elif kind == 'highpass':
+        b = [(1 + c) / 2, -1 - c, (1 + c) / 2]
+    elif kind == 'bandpass':
+        b = [alpha, 0 * one, -alpha]
+    elif kind == 'bandreject':
+        b = [one, -2 * c, one]
+    elif kind == 'allpass':
+        b = [1 - alpha, -2 * c, 1 + alpha]
+    else:
+        A = np.exp(gain / 40.0 * np.log(10))
+        b = [1 + alpha * A, -2 * c, 1 - alpha * A]
+        a = [1 + alpha / A, -2 * c, 1 - alpha / A]
+    return np.stack(b, -1), np.stack(a, -1)

@@ -32,6 +32,7 @@
 #include "gl_core.cuh"
 #include "ts_core.cuh"
 #include "fbinv_core.cuh"
+#include "iir_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -2833,6 +2834,165 @@ int kapre_filterbank_invert(const kapre_fb_inverse_plan* plan, const kapre_fb_in
     int grid;
     if ((rc = kb_resident_grid(kb_fbi_kernel, KB_FBI_WARPS * 32, smem, tiles, plan->dev.sm_count, &grid))) return rc;
     return kb_launch(kb_fbi_kernel, {.grid = grid, .block = KB_FBI_WARPS * 32, .smem = smem, .st = (cudaStream_t)stream}, p);
+}
+
+}  // extern "C"
+
+// ---- IIR filters (iir_core.cuh) -------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(32) kb_iir_powers_kernel(const __grid_constant__ KbIirParams p) {
+    __shared__ double m[192];
+    kb_iir_powers_cta(p, m, (long long)blockIdx.x);
+}
+__global__ void __launch_bounds__(32) kb_iir_state_kernel(const __grid_constant__ KbIirParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_iir_state_cta(p, kb_smem, (long long)blockIdx.x);
+}
+__global__ void __launch_bounds__(128) kb_iir_carry_kernel(const __grid_constant__ KbIirParams p) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.n_cols) kb_iir_carry_col(p, i);
+}
+__global__ void __launch_bounds__(32) kb_iir_out_kernel(const __grid_constant__ KbIirParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_iir_out_cta(p, kb_smem, (long long)blockIdx.x);
+}
+
+static int64_t kb_iir_align(int64_t v) { return (v + 255) & ~(int64_t)255; }
+
+// Workspace sections: powers (one set per column at most), chunk end states, block carries.  -1: overflow.
+static int64_t kb_iir_ws(long long n_cols, int K, int nblk, int64_t* off_e, int64_t* off_blk) {
+    const double total = (double)n_cols * (KB_IIR_NPOW * 64 * 8 + (double)K * KB_IIR_N * 4 + (double)nblk * KB_IIR_N * 8);
+    if (total > 4.0e18) return -1;
+    const int64_t pw = kb_iir_align((int64_t)n_cols * KB_IIR_NPOW * 64 * 8);
+    const int64_t e = kb_iir_align((int64_t)n_cols * K * KB_IIR_N * 4);
+    *off_e = pw;
+    *off_blk = pw + e;
+    return pw + e + kb_iir_align((int64_t)n_cols * nblk * KB_IIR_N * 8);
+}
+
+static int kb_iir_check_sizes(int batch, int channels, int length, int order) {
+    if (batch < 0 || channels < 0 || length < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (order < 0) return kb_fail(KAPRE_E_INVALID, "order must be >= 0, got %d", order);
+    if (order > KB_IIR_N) return kb_fail(KAPRE_E_UNSUPPORTED, "IIR order %d is above the supported %d", order, KB_IIR_N);
+    const long long K = ((long long)length + KB_IIR_TC - 1) / KB_IIR_TC;
+    const long long nblk = (K + KB_IIR_W - 1) / KB_IIR_W;
+    if ((long long)batch * channels * nblk > 0x7fffffffLL || (long long)batch * channels > 0x7fffffffLL)
+        return kb_fail(KAPRE_E_INVALID, "too many IIR columns or blocks");
+    return 0;
+}
+
+static bool kb_iir_same_shape(const kapre_wave_desc* a, const kapre_wave_desc* b) {
+    return a->batch == b->batch && a->channels == b->channels && a->length == b->length;
+}
+
+// Fills everything but the data pointers; 1: nothing to do.
+static int kb_iir_prepare(KbIirParams& p, const kapre_wave_desc* xd, const kapre_iir_coeffs* cf, int flags,
+                          void* workspace_dev) {
+    if (!xd || !cf) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (flags & ~(KAPRE_IIR_CLAMP | KAPRE_IIR_REVERSE)) return kb_fail(KAPRE_E_INVALID, "unknown flags 0x%x", flags);
+    int rc = kb_iir_check_sizes(xd->batch, xd->channels, xd->length, cf->order);
+    if (rc) return rc;
+    if (cf->b_stride_b < 0 || cf->b_stride_c < 0 || cf->a_stride_b < 0 || cf->a_stride_c < 0)
+        return kb_fail(KAPRE_E_INVALID, "coefficient strides must be >= 0");
+    p.B = xd->batch; p.C = xd->channels; p.L = xd->length;
+    p.x_sb = xd->stride_b; p.x_sc = xd->stride_c; p.x_sl = xd->stride_l;
+    p.bc = cf->b; p.b_sb = cf->b_stride_b; p.b_sc = cf->b_stride_c;
+    p.ac = cf->a; p.a_sb = cf->a_stride_b; p.a_sc = cf->a_stride_c;
+    p.order = cf->order;
+    kb_iir_setup(p);
+    if (p.n_cols == 0 || p.L == 0) return 1;
+    if (!cf->b || !cf->a) return kb_fail(KAPRE_E_INVALID, "null coefficient pointer");
+    if (!workspace_dev) return kb_fail(KAPRE_E_INVALID, "null workspace");
+    int64_t off_e, off_blk;
+    if (kb_iir_ws(p.n_cols, p.K, p.nblk, &off_e, &off_blk) < 0) return kb_fail(KAPRE_E_INVALID, "IIR workspace overflows");
+    p.pw = (double*)workspace_dev;
+    p.e = (float*)((char*)workspace_dev + off_e);
+    p.blk = (double*)((char*)workspace_dev + off_blk);
+    return 0;
+}
+
+// The largest element offset + 1 of a wave descriptor (the bulk copies' bound), strides assumed >= 0 where they matter.
+static long long kb_iir_numel(const kapre_wave_desc* d) {
+    long long n = 1;
+    n += (long long)(d->batch - 1) * (d->stride_b > 0 ? d->stride_b : 0);
+    n += (long long)(d->channels - 1) * (d->stride_c > 0 ? d->stride_c : 0);
+    n += (long long)(d->length - 1) * (d->stride_l > 0 ? d->stride_l : 0);
+    return n;
+}
+
+static int kb_iir_launch(KbIirParams& p, const float* in, const kapre_wave_desc* in_d, cudaStream_t st) {
+    p.x = in;
+    p.x_numel = kb_iir_numel(in_d);
+    p.x_align = (unsigned)(((uintptr_t)in >> 2) & 3u);
+    const long long n_f = (long long)p.n_fb * p.n_fc, tiles = p.n_cols * p.nblk;
+    int rc;
+    if ((rc = kb_launch(kb_iir_powers_kernel, {.grid = (int)n_f, .block = 32, .st = st}, p))) return rc;
+    if ((rc = kb_launch(kb_iir_state_kernel, {.grid = (int)tiles, .block = 32, .smem = kb_iir_smem(0).total, .st = st,
+                                              .timed = true}, p)))
+        return rc;
+    if ((rc = kb_launch(kb_iir_carry_kernel, {.grid = (int)((p.n_cols + 127) / 128), .block = 128, .st = st}, p)))
+        return rc;
+    const int refs = p.bwd && p.part != nullptr;
+    return kb_launch(kb_iir_out_kernel, {.grid = (int)tiles, .block = 32, .smem = kb_iir_smem(refs).total, .st = st,
+                                         .timed = true}, p);
+}
+
+extern "C" {
+
+int64_t kapre_lfilter_workspace_bytes(int batch, int channels, int length, int order) {
+    int rc = kb_iir_check_sizes(batch, channels, length, order);
+    if (rc) return rc;
+    const int K = (int)(((long long)length + KB_IIR_TC - 1) / KB_IIR_TC);
+    int64_t off_e, off_blk;
+    const int64_t n = kb_iir_ws((long long)batch * channels, K, (K + KB_IIR_W - 1) / KB_IIR_W, &off_e, &off_blk);
+    if (n < 0) return kb_fail(KAPRE_E_INVALID, "IIR workspace overflows");
+    return n;
+}
+
+int kapre_lfilter(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_iir_coeffs* coeffs, int flags,
+                  float* y_dev, const kapre_wave_desc* y_desc, void* workspace_dev, void* stream) {
+    if (!y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbIirParams p{};
+    int rc = kb_iir_prepare(p, x_desc, coeffs, flags, workspace_dev);
+    if (rc < 0) return rc;
+    if (!kb_iir_same_shape(x_desc, y_desc)) return kb_fail(KAPRE_E_INVALID, "input and output shapes differ");
+    if (rc == 1) return 0;
+    if (!x_dev || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)x_dev == (const void*)y_dev) return kb_fail(KAPRE_E_INVALID, "lfilter cannot run in place");
+    p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_sl = y_desc->stride_l;
+    p.reverse = (flags & KAPRE_IIR_REVERSE) ? 1 : 0;
+    p.clamp = (flags & KAPRE_IIR_CLAMP) ? 1 : 0;
+    p.bwd = 0;
+    return kb_iir_launch(p, x_dev, x_desc, (cudaStream_t)stream);
+}
+
+int kapre_lfilter_backward(const float* gy_dev, const kapre_wave_desc* gy_desc, const float* x_dev,
+                           const kapre_wave_desc* x_desc, const float* y_dev, const kapre_wave_desc* y_desc,
+                           const kapre_iir_coeffs* coeffs, int flags, float* gx_dev, const kapre_wave_desc* gx_desc,
+                           float* partials_dev, void* workspace_dev, void* stream) {
+    if (!gx_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbIirParams p{};
+    int rc = kb_iir_prepare(p, gy_desc, coeffs, flags, workspace_dev);
+    if (rc < 0) return rc;
+    if (!kb_iir_same_shape(gy_desc, gx_desc)) return kb_fail(KAPRE_E_INVALID, "gradient shapes differ");
+    if (partials_dev) {
+        if (!x_desc || !y_desc) return kb_fail(KAPRE_E_INVALID, "coefficient gradients need x and y");
+        if (!kb_iir_same_shape(gy_desc, x_desc) || !kb_iir_same_shape(gy_desc, y_desc))
+            return kb_fail(KAPRE_E_INVALID, "x and y must have the gradient's shape");
+    }
+    if (rc == 1) return 0;      // no chunks: the partial sums are empty too
+    if (!gy_dev || !gx_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)gy_dev == (const void*)gx_dev) return kb_fail(KAPRE_E_INVALID, "lfilter backward cannot run in place");
+    if (partials_dev && (!x_dev || !y_dev)) return kb_fail(KAPRE_E_INVALID, "coefficient gradients need x and y");
+    p.y = gx_dev; p.y_sb = gx_desc->stride_b; p.y_sc = gx_desc->stride_c; p.y_sl = gx_desc->stride_l;
+    p.reverse = (flags & KAPRE_IIR_REVERSE) ? 0 : 1;       // the adjoint runs the other way
+    p.clamp = 0;
+    p.bwd = 1;
+    if (partials_dev) {
+        p.part = partials_dev;
+        p.xr = x_dev; p.xr_sb = x_desc->stride_b; p.xr_sc = x_desc->stride_c; p.xr_sl = x_desc->stride_l;
+        p.yr = y_dev; p.yr_sb = y_desc->stride_b; p.yr_sc = y_desc->stride_c; p.yr_sl = y_desc->stride_l;
+    }
+    return kb_iir_launch(p, gy_dev, gy_desc, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1008,6 +1008,129 @@ def convolve_spectrum(x: torch.Tensor, H: torch.Tensor, plan: ConvolvePlan, star
     return _crop(y, start, length, data_format)
 
 
+IIR_MAX_ORDER = 8
+
+
+def iir_check(x, b, a, data_format):
+    """Shapes of ``lfilter``'s operands: x (B, L, C) / (B, C, L); b and a of one shape, (N + 1,), (C, N + 1) or
+    (B, C, N + 1) with N <= 8.  Returns (B, C, L), (Bc, Cc, N + 1): the coefficients' batch and channels (1 when
+    shared)."""
+    if x.dim() != 3:
+        raise ValueError('lfilter expects a 3-D waveform batch, got shape %s' % (tuple(x.shape),))
+    B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == _CH_LAST_STR else tuple(x.shape)
+    if tuple(b.shape) != tuple(a.shape):
+        raise ValueError('a_coeffs %s and b_coeffs %s must have the same shape' % (tuple(a.shape), tuple(b.shape)))
+    if a.dim() == 1:
+        Bc, Cc = 1, 1
+    elif a.dim() == 2:
+        Bc, Cc = 1, a.shape[0]
+    elif a.dim() == 3:
+        Bc, Cc = a.shape[0], a.shape[1]
+    else:
+        raise ValueError('coefficients must be 1-D, 2-D or 3-D, got shape %s' % (tuple(a.shape),))
+    n = a.shape[-1]
+    if n < 1:
+        raise ValueError('coefficients need at least one value per filter')
+    if n - 1 > IIR_MAX_ORDER:
+        raise ValueError('IIR order %d is above the supported %d (at most %d coefficients)'
+                         % (n - 1, IIR_MAX_ORDER, IIR_MAX_ORDER + 1))
+    if a.dim() == 2 and Cc != C:
+        raise ValueError('2-D coefficients need one filter per channel: %d filters for %d channels' % (Cc, C))
+    if a.dim() == 3 and (Bc not in (1, B) or Cc not in (1, C)):
+        raise ValueError('3-D coefficients: batch %d and channels %d must be 1 or the waveform\'s (%d, %d)'
+                         % (Bc, Cc, B, C))
+    return (B, C, L), (Bc, Cc, n)
+
+
+def _iir_coeffs(b, a):
+    """kapre_iir_coeffs over normalised (Bc, Cc, N + 1) float32 tensors; a batch or channel axis of 1 is shared through
+    a zero stride."""
+    b = b.detach().to(torch.float32).contiguous()
+    a = a.detach().to(torch.float32).contiguous()
+    st = []
+    for t in (b, a):
+        st += [0 if t.shape[0] == 1 else t.stride(0), 0 if t.shape[1] == 1 else t.stride(1)]
+    return N.IirCoeffs(b.data_ptr(), a.data_ptr(), *st, int(a.shape[-1]) - 1), (b, a)
+
+
+def lfilter_workspace(B, C, L, order, device):
+    n = int(N.lib().kapre_lfilter_workspace_bytes(B, C, L, order))
+    if n < 0:
+        N.check(n)
+    return torch.empty(max(n, 1), dtype=torch.uint8, device=device)
+
+
+def lfilter_forward(x, b, a, flags, data_format):
+    """y = ``kapre_lfilter`` of x with normalised (Bc, Cc, N + 1) coefficients on x's device: four launches."""
+    x = _raw(x.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    y, yd = _wave_alloc(B, C, L, data_format, x.device)
+    if y.numel():
+        cf, keep = _iir_coeffs(b, a)
+        ws = lfilter_workspace(B, C, L, cf.order, x.device)
+        N.check(N.lib().kapre_lfilter(_ptr(x), ctypes.byref(xd), ctypes.byref(cf), int(flags), _ptr(y), ctypes.byref(yd),
+                                      _ptr(ws), _stream_ptr()))
+    return y
+
+
+def lfilter_backward(gy, x, y, b, a, flags, data_format, want_coeffs):
+    """Gradients of ``lfilter_forward`` (unclamped) at output gradient gy: (gx, gb, ga), gb and ga shaped like b and
+    a (summed over their shared axes; ga[..., 0] = 0) or None without ``want_coeffs``.  Four launches; x and y (the
+    unclamped output) are read only for the coefficient gradients.  The kernel writes per-(chunk, item, channel)
+    partial sums and torch adds them, so the result is deterministic."""
+    gy = _raw(gy.to(torch.float32))
+    gd, (B, C, L) = _wave_desc(gy, data_format)
+    gx, od = _wave_alloc(B, C, L, data_format, gy.device)
+    cf, keep = _iir_coeffs(b, a)
+    n = cf.order + 1
+    part = None
+    if want_coeffs:
+        K = -(-L // 65)
+        part = torch.empty((2 * n - 1, B, C, K), dtype=torch.float32, device=gy.device)
+        x = _raw(x.to(torch.float32))
+        xd, _ = _wave_desc(x, data_format)
+        yd, _ = _wave_desc(y, data_format)
+    if gx.numel():
+        ws = lfilter_workspace(B, C, L, cf.order, gy.device)
+        N.check(N.lib().kapre_lfilter_backward(
+            _ptr(gy), ctypes.byref(gd), _ptr(x) if want_coeffs else None, ctypes.byref(xd) if want_coeffs else None,
+            _ptr(y) if want_coeffs else None, ctypes.byref(yd) if want_coeffs else None, ctypes.byref(cf), int(flags),
+            _ptr(gx), ctypes.byref(od), _ptr(part) if want_coeffs else None, _ptr(ws), _stream_ptr()))
+    if not want_coeffs:
+        return gx, None, None
+    s = part.sum(dim=3) if part.shape[3] else torch.zeros(part.shape[:3], dtype=torch.float32, device=gy.device)
+    gb = s[:n].permute(1, 2, 0)                                                       # (B, C, N + 1)
+    ga = torch.cat([torch.zeros_like(s[:1]), s[n:]], 0).permute(1, 2, 0)
+    Bc, Cc = b.shape[0], b.shape[1]
+    if Bc == 1:
+        gb, ga = gb.sum(0, keepdim=True), ga.sum(0, keepdim=True)
+    if Cc == 1:
+        gb, ga = gb.sum(1, keepdim=True), ga.sum(1, keepdim=True)
+    return gx, gb, ga
+
+
+@_device_of_first_arg
+def lfilter(x, b, a, clamp=True, reverse=False, data_format=_CH_LAST_STR):
+    """IIR filter along the time axis of x (B, L, C) / (B, C, L) with normalised float32 coefficients b, a on x's
+    device, each (Bc, Cc, N + 1) with Bc in {1, B}, Cc in {1, C} (1 shares the filter).  ``reverse`` runs it in
+    reverse time.  Everything is validated before any launch.  Differentiable with respect to x, b and a: under
+    autograd the kernel writes the unclamped output and ``torch.clamp`` applies the clamp (the same bits)."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and b.is_cuda and a.is_cuda):
+        raise N.KapreNativeError('lfilter needs CUDA tensors')
+    if b.device != x.device or a.device != x.device:
+        raise ValueError('waveform on %s, coefficients on %s / %s' % (x.device, b.device, a.device))
+    if b.dim() != 3:
+        raise ValueError('normalised coefficients must be 3-D (batch, channels, order + 1)')
+    (B, C, L), (_, _, n) = iir_check(x, b, a, data_format)
+    lfilter_workspace(B, C, L, n - 1, x.device)            # size checks before anything is launched
+    flags = N.IIR_REVERSE if reverse else 0
+    if _wants_grad(x) or _wants_grad(b) or _wants_grad(a):
+        from . import autograd
+        y = autograd.lfilter(x, b, a, flags, data_format)
+        return torch.clamp(y, -1.0, 1.0) if clamp else y
+    return lfilter_forward(x, b, a, flags | (N.IIR_CLAMP if clamp else 0), data_format)
+
+
 def _pcen_params(params, eps, device):
     """kapre_pcen_params over the four parameter tensors (gain, bias, power, smooth_coef): float32, 0-d (one value
     for every band) or 1-d (one per band), on ``device``."""

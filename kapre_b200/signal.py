@@ -3,7 +3,8 @@
 (:365-447).  Same constructor arguments, validation and ``get_config`` keys; ``call`` runs CUDA
 kernels through the C ABI.  ``Resample`` (polyphase sample-rate conversion) has no counterpart in the
 reference, which expects audio to be resampled before it reaches the model; neither has ``Speed`` (speed perturbation by any
-real factor, band-limited interpolation) or ``Convolve`` (convolution with long filters, partitioned FFT)."""
+real factor, band-limited interpolation), ``Convolve`` (convolution with long filters, partitioned FFT) or the IIR
+filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan)."""
 from __future__ import annotations
 
 import math
@@ -15,7 +16,8 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
-__all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve']
+__all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
+           'Biquad']
 
 
 def _resolve(fmt):
@@ -212,6 +214,184 @@ class Convolve(Layer):
 
     _config_fields = (
         ('mode', 'mode'),
+        ('data_format', 'data_format_str'),
+    )
+
+
+def _coeff_tensor(c, name):
+    """A coefficient argument as a tensor (CPU or CUDA, autograd kept)."""
+    if isinstance(c, torch.Tensor):
+        return c
+    arr = np.asarray(c, np.float64)
+    if arr.dtype.kind not in 'fiu':
+        raise ValueError('%s must be numeric, got: %r' % (name, c))
+    return torch.from_numpy(np.ascontiguousarray(arr))
+
+
+def _normalised(x, a_coeffs, b_coeffs, data_format):
+    """(b / a0, a / a0) as 3-D float32 tensors on x's device, after every check: shapes (``ops.iir_check``) and, for
+    host coefficients, a0 != 0.  The division is a torch op, so autograd carries the gradient to raw a, b and a0."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise ops.N.KapreNativeError('lfilter needs a CUDA waveform')
+    a = _coeff_tensor(a_coeffs, 'a_coeffs')
+    b = _coeff_tensor(b_coeffs, 'b_coeffs')
+    _, (Bc, Cc, n) = ops.iir_check(x, b, a, data_format)
+    for t in (a, b):
+        if t.is_cuda and t.device != x.device:
+            raise ValueError('coefficients on %s, the waveform on %s' % (t.device, x.device))
+    if not a.is_cuda:
+        a0 = a.detach().reshape(-1, n)[:, 0]
+        if bool((a0 == 0).any()):
+            raise ValueError('a_coeffs[..., 0] must not be 0')
+        if not bool(torch.isfinite(a.detach()).all() and torch.isfinite(b.detach()).all()):
+            raise ValueError('coefficients must be finite')
+    a = a.to(device=x.device, dtype=torch.float32)
+    b = b.to(device=x.device, dtype=torch.float32)
+    a0 = a[..., :1]
+    return (b / a0).reshape(Bc, Cc, n), (a / a0).reshape(Bc, Cc, n)
+
+
+def lfilter(waveform, a_coeffs, b_coeffs, clamp=True, data_format='default'):
+    """``torchaudio.functional.lfilter`` along the time axis of ``waveform`` ``(batch, time, ch)`` /
+    ``(batch, ch, time)`` (a CUDA tensor), with torchaudio's argument order:
+
+        y[t] = (sum_{k=0..N} b[k] x[t-k] - sum_{k=1..N} a[k] y[t-k]) / a[0],   zero initial state,
+
+    then clamped to [-1, 1] when ``clamp``.  ``a_coeffs`` and ``b_coeffs`` have one shape: ``(N + 1,)`` (one filter),
+    ``(ch, N + 1)`` (one per channel, torchaudio's ``batching=True`` form) or ``(batch, ch, N + 1)`` with batch and
+    channels 1 or the waveform's (one per item and channel).  Order N <= 8.
+
+    The coefficients are divided by ``a[0]`` in float32 on the device, as torchaudio does, so the kernel sees
+    normalised float32 coefficients; ``a[0] == 0`` raises for host coefficients but is not checked for CUDA tensors
+    (that would synchronise), where it gives inf or NaN as in torchaudio.  Only stable filters are meaningful.  High
+    orders in direct form are fragile in float32 (rounding the denominator of an 8th-order Butterworth at 0.05 of
+    Nyquist makes it unstable), so prefer biquads or low orders for sharp filters.
+
+    Four launches (``kapre_lfilter``).  Differentiable with respect to the waveform and both coefficient tensors."""
+    fmt = _resolve(_unwrap_format(data_format))
+    b, a = _normalised(waveform, a_coeffs, b_coeffs, fmt)
+    return ops.lfilter(waveform, b, a, clamp=clamp, reverse=False, data_format=fmt)
+
+
+def filtfilt(waveform, a_coeffs, b_coeffs, clamp=True, data_format='default'):
+    """``torchaudio.functional.filtfilt``: ``lfilter`` without clamping, then ``lfilter`` in reverse time, then the
+    clamp; zero-phase, with no edge padding (unlike scipy's ``filtfilt``).  Arguments as ``lfilter``.  The reverse pass
+    runs the kernel backwards in time, so nothing is flipped or copied.  Eight launches."""
+    fmt = _resolve(_unwrap_format(data_format))
+    b, a = _normalised(waveform, a_coeffs, b_coeffs, fmt)
+    y = ops.lfilter(waveform, b, a, clamp=False, reverse=False, data_format=fmt)
+    return ops.lfilter(y, b, a, clamp=clamp, reverse=True, data_format=fmt)
+
+
+def _host_coeffs(b, a):
+    """Validated float64 host copies of a layer's coefficients (same shape, order <= 8, a0 != 0, finite)."""
+    b = np.asarray(b, np.float64)
+    a = np.asarray(a, np.float64)
+    if b.shape != a.shape or b.ndim not in (1, 2, 3) or b.shape[-1] < 1:
+        raise ValueError('b and a must have one 1-D, 2-D or 3-D shape, got %s and %s' % (b.shape, a.shape))
+    if b.shape[-1] - 1 > ops.IIR_MAX_ORDER:
+        raise ValueError('IIR order %d is above the supported %d' % (b.shape[-1] - 1, ops.IIR_MAX_ORDER))
+    if np.any(a[..., 0] == 0):
+        raise ValueError('a[..., 0] must not be 0')
+    if not (np.all(np.isfinite(a)) and np.all(np.isfinite(b))):
+        raise ValueError('coefficients must be finite')
+    return b, a
+
+
+@register_keras_serializable(package='Kapre')
+class IIRFilter(Layer):
+    """An IIR filter (``lfilter``) with fixed or trainable coefficients: ``(batch, time, ch)`` / ``(batch, ch, time)``
+    in, the same shape out.  ``b`` and ``a``: one shape, ``(N + 1,)``, ``(ch, N + 1)`` or ``(batch, ch, N + 1)`` as for
+    ``lfilter``, N <= 8, ``a[..., 0] != 0``.  They become the layer's weights on the first call: float32 tensors on
+    the input's device, raw (not normalised; the division by ``a[0]`` is part of every call), with
+    ``requires_grad = trainable``, so a learnable front end trains all of b and a.  Nothing keeps a trained filter
+    stable."""
+
+    def __init__(self, b, a, clamp=True, trainable=False, data_format='default', **kwargs):
+        super().__init__(trainable=trainable, **kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.b, self.a = _host_coeffs(b, a)
+        self.clamp = bool(clamp)
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+        self.built = False
+        self._weights = []
+
+    def build(self, device):
+        self._weights = [torch.tensor(v, dtype=torch.float32, device=device).requires_grad_(bool(self.trainable))
+                         for v in (self.b, self.a)]
+        self.built = True
+
+    @property
+    def weights(self):
+        """[b, a] once built (the first call), else []."""
+        return list(self._weights)
+
+    def count_params(self):
+        if not self.built:
+            raise ValueError('You tried to call `count_params` on layer %s, but the layer isn\'t built.' % self.name)
+        return sum(int(w.numel()) for w in self._weights)
+
+    def call(self, x):
+        if not self.built:
+            self.build(x.device)
+        elif self._weights[0].device != x.device:
+            raise ValueError('IIRFilter %s was built on %s and cannot run on %s' % (self.name, self._weights[0].device,
+                                                                                   x.device))
+        b, a = self._weights
+        return lfilter(x, a, b, clamp=self.clamp, data_format=self.data_format)
+
+    def get_config(self):
+        config = super().get_config()
+        config.update({'b': self.b.tolist(), 'a': self.a.tolist(), 'clamp': self.clamp,
+                       'data_format': self.data_format_str})
+        return config
+
+
+@register_keras_serializable(package='Kapre')
+class Biquad(Layer):
+    """A second-order filter of torchaudio's biquad family (``lowpass_biquad``, ``highpass_biquad``,
+    ``bandpass_biquad``, ``bandreject_biquad``, ``allpass_biquad``, ``equalizer_biquad``): ``kind`` one of
+    ``backend.BIQUAD_KINDS``, centre or cutoff ``freq`` in Hz at ``sample_rate``, quality factor ``Q`` and, for the
+    equalizer, ``gain`` in dB.  The coefficients are designed and normalised in float64 on the host
+    (``backend.biquad_coefficients``) and applied with ``lfilter`` (clamped to [-1, 1] when ``clamp``, as torchaudio's
+    helpers do).  ``(batch, time, ch)`` / ``(batch, ch, time)`` in, the same shape out; differentiable with respect to
+    the input."""
+
+    def __init__(self, kind, sample_rate, freq, Q=0.707, gain=0.0, clamp=True, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        b, a = backend.biquad_coefficients(kind, sample_rate, freq, Q, gain)
+        if b.ndim != 1:
+            raise ValueError('freq, Q and gain must be numbers')
+        self.kind, self.sample_rate, self.freq, self.Q, self.gain = kind, sample_rate, freq, Q, gain
+        self.clamp = bool(clamp)
+        self.b, self.a = b / a[0], a / a[0]
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+        self._coeffs = {}
+
+    def coefficients(self, device):
+        """(b, a) as float32 tensors on ``device`` (a[0] = 1), made on first use there."""
+        key = device.index if device.index is not None else torch.cuda.current_device()
+        c = self._coeffs.get(key)
+        if c is None:
+            c = self._coeffs[key] = tuple(torch.tensor(v, dtype=torch.float32, device=device) for v in (self.b, self.a))
+        return c
+
+    def call(self, x):
+        b, a = self.coefficients(x.device)
+        return lfilter(x, a, b, clamp=self.clamp, data_format=self.data_format)
+
+    _config_fields = (
+        ('kind', 'kind'),
+        ('sample_rate', 'sample_rate'),
+        ('freq', 'freq'),
+        ('Q', 'Q'),
+        ('gain', 'gain'),
+        ('clamp', 'clamp'),
         ('data_format', 'data_format_str'),
     )
 
