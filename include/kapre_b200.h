@@ -371,6 +371,60 @@ int kapre_lfilter_backward(const float* gy_dev, const kapre_wave_desc* gy_desc, 
                            const kapre_iir_coeffs* coeffs, int flags, float* gx_dev, const kapre_wave_desc* gx_desc,
                            float* partials_dev, void* workspace_dev, void* stream);
 
+/* ---- additive noise at a target SNR (torchaudio.functional.add_noise) -------------------------------------------
+ * For every (item, channel) column of x (L samples), noise n, snr in dB and valid length len:
+ *   Ex = sum_{t < len} x[t]^2,  En = sum_{t < len} n[t]^2,  s = sqrt(Ex / En) 10^(-snr / 20),  y[t] = x[t] + s n[t]
+ * for every t < L (noise is added past len too, as torchaudio does).  The mask is t < len, so len <= 0 counts no
+ * sample and len >= L every sample.  Ex, En and s are float64, s is rounded to float32 once and y = fmaf(s, n, x).
+ * One deviation from torchaudio: where En == 0 (or Ex == 0) s = 0 and y = x bit for bit, where torchaudio gives NaN
+ * for En == 0.  A NaN or inf in x or n makes that column non-finite.  The summation order depends on the column and
+ * the absolute sample index alone (segments of 4096 samples, a fixed tree per segment, the segments folded in order;
+ * no atomics), so an output's bits do not depend on the batch, the strides, the data format, broadcasting, or
+ * whether the noise comes from a tensor or a bank.  Two launches each way. */
+#define KAPRE_NOISE_TENSOR 0
+#define KAPRE_NOISE_BANK 1
+typedef struct {
+    int mode;                   /* KAPRE_NOISE_TENSOR or KAPRE_NOISE_BANK */
+    /* TENSOR: (batch, channels, length) with batch 1 or x's, channels 1 or x's and x's length; a batch or channel of 1
+     * (or a stride of 0) broadcasts without a copy. */
+    const float* noise;
+    kapre_wave_desc noise_desc;
+    /* BANK: bank_length floats of concatenated mono clips; per item (device arrays of batch int64) the clip's first
+     * sample `start`, its length `clip_len` and `offset`: n[b, c, t] = bank[start[b] + (offset[b] + t) mod clip_len[b]]
+     * for every channel, so short clips loop.  An item whose clip is empty or does not lie inside the bank reads
+     * zeros (so its output is its input). */
+    const float* bank;
+    int64_t bank_length;
+    const int64_t* start;
+    const int64_t* clip_len;
+    const int64_t* offset;
+} kapre_noise_source;
+/* snr (float32, required) and lengths (int32, optional: NULL means every sample counts) at
+ * ptr + b stride_b + c stride_c; a stride of 0 broadcasts. */
+typedef struct {
+    const float* snr;
+    int64_t snr_stride_b, snr_stride_c;
+    const int32_t* lengths;
+    int64_t lengths_stride_b, lengths_stride_c;
+} kapre_snr_desc;
+/* Scratch of kapre_add_noise and kapre_add_noise_backward: 16 bytes per (item, channel, 4096-sample segment), rounded
+ * up to 256.  < 0 on a negative size or an overflow. */
+int64_t kapre_add_noise_workspace_bytes(int batch, int channels, int length);
+/* y = x + s n.  y_desc: x's batch, channels and length, any strides; y must not be x or the noise.  stats_dev
+ * (optional): (batch, channels, 2) float64 (Ex, En) per column, which kapre_add_noise_backward reads. */
+int kapre_add_noise(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_noise_source* noise,
+                    const kapre_snr_desc* snr, float* y_dev, const kapre_wave_desc* y_desc, double* stats_dev,
+                    void* workspace_dev, void* stream);
+/* Gradients of kapre_add_noise given the output gradient g, x, the same noise, snr and lengths, and the stats the
+ * forward wrote.  With D = sum_{t < L} g[t] n[t] per column:
+ *   gx[t] = g[t] + [t < len] (D s / Ex) x[t],  gn[t] = s g[t] - [t < len] (D s / En) n[t],  gsnr = -D s ln(10) / 20,
+ * where every term through s is 0 where Ex == 0 or En == 0.  gx is required; gn (tensor noise only, x's full shape)
+ * and gsnr ((batch, channels) float32, contiguous) are written when not NULL.  Sum gn and gsnr over broadcast axes. */
+int kapre_add_noise_backward(const float* g_dev, const kapre_wave_desc* g_desc, const float* x_dev,
+                             const kapre_wave_desc* x_desc, const kapre_noise_source* noise, const kapre_snr_desc* snr,
+                             const double* stats_dev, float* gx_dev, const kapre_wave_desc* gx_desc, float* gn_dev,
+                             const kapre_wave_desc* gn_desc, float* gsnr_dev, void* workspace_dev, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

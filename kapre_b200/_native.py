@@ -54,6 +54,19 @@ class IirCoeffs(Structure):
 IIR_CLAMP, IIR_REVERSE = 1, 2
 
 
+class NoiseSource(Structure):
+    _fields_ = [('mode', c_int), ('noise', c_void_p), ('noise_desc', WaveDesc), ('bank', c_void_p),
+                ('bank_length', c_int64), ('start', c_void_p), ('clip_len', c_void_p), ('offset', c_void_p)]
+
+
+class SnrDesc(Structure):
+    _fields_ = [('snr', c_void_p), ('snr_stride_b', c_int64), ('snr_stride_c', c_int64), ('lengths', c_void_p),
+                ('lengths_stride_b', c_int64), ('lengths_stride_c', c_int64)]
+
+
+NOISE_TENSOR, NOISE_BANK = 0, 1
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -131,6 +144,12 @@ SYMBOLS = [
     ('kapre_lfilter_backward', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p,
                                        POINTER(WaveDesc), POINTER(IirCoeffs), c_int, c_void_p, POINTER(WaveDesc),
                                        c_void_p, c_void_p, c_void_p]),
+    ('kapre_add_noise_workspace_bytes', c_int64, [c_int, c_int, c_int]),
+    ('kapre_add_noise', c_int, [c_void_p, POINTER(WaveDesc), POINTER(NoiseSource), POINTER(SnrDesc), c_void_p,
+                                POINTER(WaveDesc), c_void_p, c_void_p, c_void_p]),
+    ('kapre_add_noise_backward', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), POINTER(NoiseSource),
+                                         POINTER(SnrDesc), c_void_p, c_void_p, POINTER(WaveDesc), c_void_p,
+                                         POINTER(WaveDesc), c_void_p, c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

@@ -2,7 +2,8 @@
 masking is one CUDA pass (``kapre_spec_augment``).  ``TimeStretch``: a phase vocoder, one CUDA scan over time
 (``kapre_time_stretch``).  ``PitchShift``: STFT, that phase vocoder, the inverse STFT and one band-limited
 interpolation (``kapre_sinc_resample``) back to the input length.  ``Reverb``: convolution with a room impulse response
-drawn from a bank (``kapre_convolve``).  ``RandomBiquad``: a biquad drawn per item (``kapre_lfilter``)."""
+drawn from a bank (``kapre_convolve``).  ``RandomBiquad``: a biquad drawn per item (``kapre_lfilter``).
+``BackgroundNoise``: a noise excerpt from a bank added at a drawn SNR (``kapre_add_noise``)."""
 from __future__ import annotations
 
 import numpy as np
@@ -378,4 +379,142 @@ class RandomBiquad(Layer):
         config.update({'kind': self.kind, 'sample_rate': self.sample_rate, 'freq_range': list(self.freq_range),
                        'Q_range': list(self.Q_range), 'gain_range': list(self.gain_range), 'seed': self.seed,
                        'data_format': self.data_format_original})
+        return config
+
+
+def prepare_noises(noises):
+    """The clips of a ``BackgroundNoise`` bank: ``noises`` is a 2-D array or a sequence of 1-D arrays of any lengths,
+    each non-empty, finite and not all zero (they are not rescaled: the SNR sets the level).  Returns the clips
+    concatenated as float32 and their lengths (int64)."""
+    if isinstance(noises, np.ndarray) and noises.ndim == 2:
+        rows = list(noises)
+    elif isinstance(noises, (np.ndarray, str, bytes)):
+        raise ValueError('noises must be a 2-D array or a list of 1-D arrays, got: %r' % (type(noises),))
+    else:
+        try:
+            rows = list(noises)
+        except TypeError:
+            raise ValueError('noises must be a 2-D array or a list of 1-D arrays, got: %r' % (type(noises),)) from None
+    if not rows:
+        raise ValueError('noises is empty')
+    out = []
+    for i, r in enumerate(rows):
+        r = np.asarray(r.detach().cpu() if hasattr(r, 'detach') else r)
+        if r.dtype.kind not in 'iuf' or r.ndim != 1 or r.size == 0:
+            raise ValueError('noise %d must be a non-empty 1-D array of numbers, got shape %s' % (i, r.shape))
+        r = r.astype(np.float32)
+        if not np.all(np.isfinite(r)):
+            raise ValueError('noise %d has non-finite samples' % i)
+        if not np.any(r != 0):
+            raise ValueError('noise %d is all zeros' % i)
+        out.append(r)
+    return np.concatenate(out), np.array([r.size for r in out], np.int64)
+
+
+@register_keras_serializable(package='Kapre')
+class BackgroundNoise(Layer):
+    """Background noise from a bank of clips at a random SNR (the noise step of speed perturbation -> reverberation ->
+    noise recipes, as with MUSAN): ``(batch, time, ch)`` / ``(batch, ch, time)`` in, the same shape out.  Item b gets
+    ``add_noise(x_b, n_b, snr_b)`` with ``n_b[t] = clip[(offset + t) mod len(clip)]`` for every channel, so a clip
+    shorter than the signal loops; the SNR is measured per channel, as ``signal.add_noise`` does, and a silent
+    excerpt leaves the item as it is.
+
+    ``call(x, noise_index=None, offset=None, snr=None, lengths=None)`` draws per item, in this order and with
+    ``np.random.default_rng(seed)``: the clips (uniformly), the offsets (uniformly in ``[0, len(clip))``) and the
+    SNRs (uniformly in ``snr_range``, dB).  Each argument (a number or ``batch`` values) replaces its draw, which is
+    then not made; ``lengths`` is passed to ``add_noise``.  ``last_choice = (index, offset, snr)`` records what was
+    applied.  The layer applies on every call, like ``Reverb``; a captured graph (``Sequential.capture``) replays
+    the draw made when it was captured.
+
+    The bank is uploaded on first use on a device and kept.  A call sends the per-item clip starts, lengths, offsets
+    and SNRs in one host-to-device copy and runs ``kapre_add_noise`` in bank mode (two launches): nothing is gathered.
+    The gradient reaches ``x`` only: the bank is a constant."""
+
+    def __init__(self, noises, snr_range=(0.0, 20.0), seed=None, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.bank, self.clip_len = prepare_noises(noises)
+        self.clip_start = np.concatenate([[0], np.cumsum(self.clip_len)[:-1]]).astype(np.int64)
+        r = tuple(float(v) for v in snr_range)
+        if len(r) != 2 or not (np.isfinite(r[0]) and np.isfinite(r[1])) or r[0] > r[1]:
+            raise ValueError('snr_range must be a (low, high) pair of finite numbers, got: %r' % (snr_range,))
+        self.snr_range = r
+        self.seed = seed
+        self.rng = np.random.default_rng(seed)
+        self.last_choice = None
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self._banks = {}
+        self._captured = []
+
+    def clips(self):
+        """The clips as a list of float32 arrays."""
+        return [self.bank[s:s + n] for s, n in zip(self.clip_start, self.clip_len)]
+
+    def bank_on(self, device):
+        """The flat bank on ``device``, uploaded on first use."""
+        key = device.index if device.index is not None else torch.cuda.current_device()
+        t = self._banks.get(key)
+        if t is None:
+            t = self._banks[key] = torch.from_numpy(self.bank).to(device)
+        return t
+
+    @staticmethod
+    def _override(name, v, batch, kind):
+        a = np.asarray(v)
+        if a.dtype.kind not in kind or a.ndim > 1 or (a.ndim == 1 and a.shape[0] != batch):
+            raise ValueError('%s must be a number or %d numbers, got: %r' % (name, batch, v))
+        return np.broadcast_to(a, (batch,)).copy()
+
+    def draw(self, batch, noise_index=None, offset=None, snr=None):
+        """(index, offset, snr) arrays of ``batch`` items: drawn in that order, or the validated overrides."""
+        n = len(self.clip_len)
+        if noise_index is None:
+            idx = self.rng.integers(0, n, size=batch)
+        else:
+            idx = self._override('noise_index', noise_index, batch, 'iu').astype(np.int64)
+            if np.any(idx < 0) or np.any(idx >= n):
+                raise ValueError('noise_index must lie in [0, %d), got: %r' % (n, noise_index))
+        if offset is None:
+            off = self.rng.integers(0, self.clip_len[idx])
+        else:
+            off = self._override('offset', offset, batch, 'iu').astype(np.int64)
+            if np.any(off < 0) or np.any(off >= self.clip_len[idx]):
+                raise ValueError('offset must lie in [0, clip length), got: %r' % (offset,))
+        if snr is None:
+            s = self.rng.uniform(self.snr_range[0], self.snr_range[1], size=batch)
+        else:
+            s = self._override('snr', snr, batch, 'iuf').astype(np.float64)
+            if not np.all(np.isfinite(s)):
+                raise ValueError('snr must be finite, got: %r' % (snr,))
+        return idx, np.asarray(off, np.int64), s
+
+    def call(self, x, noise_index=None, offset=None, snr=None, lengths=None):
+        if x.dim() != 3:
+            raise ValueError('BackgroundNoise expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise N.KapreNativeError('BackgroundNoise needs a CUDA tensor')
+        B = x.shape[0]
+        idx, off, s = self.draw(B, noise_index, offset, snr)
+        self.last_choice = (idx, off, s)
+        # one host buffer, one copy: rows start, clip length, offset, and the SNRs as float32 in the last row
+        host = torch.empty((4, B), dtype=torch.int64)
+        host[0] = torch.from_numpy(self.clip_start[idx])
+        host[1] = torch.from_numpy(self.clip_len[idx])
+        host[2] = torch.from_numpy(off)
+        host[3].view(torch.float32)[:B] = torch.from_numpy(s.astype(np.float32))
+        if torch.cuda.is_current_stream_capturing():
+            # the graph's copy node reads this pinned buffer on every replay: it is kept and never written again
+            host = host.pin_memory()
+            self._captured.append(host)
+        dev = host.to(x.device, non_blocking=True)
+        snr_d = dev[3].view(torch.float32)[:B].view(B, 1)
+        bank = (self.bank_on(x.device), dev[0], dev[1], dev[2])
+        return ops.add_noise(x, None, snr_d, lengths, self.data_format, bank=bank)
+
+    def get_config(self):
+        config = super().get_config()
+        config.update({'noises': [c.tolist() for c in self.clips()], 'snr_range': list(self.snr_range),
+                       'seed': self.seed, 'data_format': self.data_format_original})
         return config

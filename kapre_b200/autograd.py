@@ -24,6 +24,8 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * lfilter, filtfilt, IIRFilter, Biquad, RandomBiquad -> ``kapre_lfilter_backward`` (the all-pole recursion run the
   other way on the output gradient; input and normalised-coefficient gradients, the rest through torch's division
   by a0)
+* add_noise, BackgroundNoise -> ``kapre_add_noise_backward`` (a segment-sum pass over g n, then the input, noise and
+  snr gradients from the saved energies)
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
@@ -366,6 +368,29 @@ class _Lfilter(torch.autograd.Function):
                 ga if ctx.needs_input_grad[2] else None, None, None)
 
 
+class _AddNoise(torch.autograd.Function):
+    """The forward is the plain two-launch mix, which also writes the per-column energies (Ex, En) for the backward;
+    the noise is a tensor (differentiable) or a bank (a constant).  snr and the noise arrive as (B, C) / full-shape
+    broadcast views, so torch sums their gradients over the broadcast axes."""
+
+    @staticmethod
+    def forward(ctx, x, noise, snr, lengths, bank, data_format):
+        y, stats = ops.add_noise_forward(x, noise, bank, snr, lengths, data_format, True)
+        ctx.save_for_backward(x, noise, snr, lengths, stats)
+        ctx.cfg = (bank, data_format)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, noise, snr, lengths, stats = ctx.saved_tensors
+        bank, data_format = ctx.cfg
+        want_n = ctx.needs_input_grad[1] and noise is not None
+        gx, gn, gsnr = ops.add_noise_backward(g, x, noise, bank, snr, lengths, stats, data_format, want_n,
+                                              ctx.needs_input_grad[2])
+        return gx if ctx.needs_input_grad[0] else None, gn, gsnr, None, None, None
+
+
 class _TimeStretch(torch.autograd.Function):
     """The forward is the plain time-stretch launch; autograd saves its output, from which the backward takes the
     magnitude and phase gradients, so the forward writes nothing extra."""
@@ -479,3 +504,7 @@ def apply_filterbank(x, fb, data_format):
 
 def magnitude_to_decibel(x, ref_value, amin, dynamic_range):
     return _MagnitudeToDecibel.apply(x.float(), ref_value, amin, dynamic_range)
+
+
+def add_noise(x, noise, snr, lengths, bank, data_format):
+    return _AddNoise.apply(x.float(), noise, snr, lengths, bank, data_format)

@@ -18,7 +18,7 @@ import torch
 from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
-from .augmentation import RandomBiquad, Reverb, TimeStretch
+from .augmentation import BackgroundNoise, RandomBiquad, Reverb, TimeStretch
 from .signal import Biquad, IIRFilter, Resample, Speed
 from .time_frequency import (STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
                              MagnitudeToDecibel, Phase, get_registered_object)
@@ -106,10 +106,10 @@ class Sequential(Layer):
 
     def call(self, x):
         start = 0
-        # Leading waveform layers (Resample, Speed, Reverb and the IIR filters) run first, so that the STFT stack behind
-        # them still takes the fused launch.
+        # Leading waveform layers (Resample, Speed, Reverb, the IIR filters and BackgroundNoise) run first, so that the
+        # STFT stack behind them still takes the fused launch.
         while start < len(self.layers) and type(self.layers[start]) in (Resample, Speed, Reverb, IIRFilter, Biquad,
-                                                                        RandomBiquad):
+                                                                        RandomBiquad, BackgroundNoise):
             x = self.layers[start].call(x)
             start += 1
         fused = self._fused_prefix(start) if (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3) else None
@@ -252,7 +252,8 @@ class Sequential(Layer):
         """Freeze this model for one input shape into a CUDA graph (``CapturedSequential``): replaying it
         costs one graph launch instead of one kernel launch + Python / ctypes dispatch per layer, which is
         what bounds small batches (cfg1: 13 us of kernel under ~40 us of submission).  Random draws made on the
-        host (``Reverb``'s choice of responses, ``RandomBiquad``'s filters) are part of what is captured: every
+        host (``Reverb``'s choice of responses, ``RandomBiquad``'s filters, ``BackgroundNoise``'s clips, offsets and
+        SNRs) are part of what is captured: every
         replay reuses the draw made at capture time."""
         return CapturedSequential(self, example)
 

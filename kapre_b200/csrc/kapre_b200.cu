@@ -33,6 +33,7 @@
 #include "ts_core.cuh"
 #include "fbinv_core.cuh"
 #include "iir_core.cuh"
+#include "noise_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -2993,6 +2994,158 @@ int kapre_lfilter_backward(const float* gy_dev, const kapre_wave_desc* gy_desc, 
         p.yr = y_dev; p.yr_sb = y_desc->stride_b; p.yr_sc = y_desc->stride_c; p.yr_sl = y_desc->stride_l;
     }
     return kb_iir_launch(p, gy_dev, gy_desc, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+// ---- additive noise (noise_core.cuh) -------------------------------------------------------------------------------
+// Both passes wait for the previous kernel in the stream before touching data, so they may be launched with PDL.  Four
+// CTAs of four warps per SM: 128 registers, which hold a lane's batches of loads of every operand in flight at once.
+__global__ void __launch_bounds__(KB_NOISE_WARPS * 32, 4) kb_noise_sum_kernel(const __grid_constant__ KbNoiseParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long tile = (long long)blockIdx.x * KB_NOISE_WARPS + w;
+    if (tile < p.tiles) kb_noise_sum_tile(p, kb_smem + w * kb_noise_smem(kb_noise_cg_max(p)).total, tile);
+}
+__global__ void __launch_bounds__(KB_NOISE_WARPS * 32, 4) kb_noise_out_kernel(const __grid_constant__ KbNoiseParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long tile = (long long)blockIdx.x * KB_NOISE_WARPS + w;
+    if (tile < p.tiles) kb_noise_out_tile(p, kb_smem + w * kb_noise_smem(kb_noise_cg_max(p)).total, tile);
+}
+
+// Workspace bytes (the segment sums) of a shape; -1: a negative size or an overflow.
+static int64_t kb_noise_ws(int batch, int channels, int length) {
+    if (batch < 0 || channels < 0 || length < 0) return -1;
+    const long long nseg = ((long long)length + KB_NOISE_SEG - 1) / KB_NOISE_SEG;
+    const long long groups = ((long long)channels + KB_NOISE_G - 1) / KB_NOISE_G;
+    const double total = (double)batch * channels * nseg * 16.0;
+    if (total > 4.0e18 || (double)batch * groups * nseg / KB_NOISE_WARPS > 2147483647.0) return -1;
+    return ((int64_t)batch * channels * nseg * 16 + 255) & ~(int64_t)255;
+}
+
+static bool kb_noise_same_shape(const kapre_wave_desc* a, const kapre_wave_desc* b) {
+    return a->batch == b->batch && a->channels == b->channels && a->length == b->length;
+}
+
+static KbNoiseWave kb_noise_wave(const float* p, const kapre_wave_desc* d) {
+    KbNoiseWave w;
+    w.p = p;
+    w.sb = d->batch == 1 ? 0 : d->stride_b;
+    w.sc = d->channels == 1 ? 0 : d->stride_c;
+    w.sl = d->stride_l;
+    return w;
+}
+
+// Checks and fills everything the two directions share; 1: nothing to launch.
+static int kb_noise_prepare(KbNoiseParams& p, const kapre_wave_desc* xd, const kapre_noise_source* ns,
+                            const kapre_snr_desc* sd, void* workspace_dev) {
+    if (!xd || !ns || !sd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (kb_noise_ws(xd->batch, xd->channels, xd->length) < 0)
+        return kb_fail(KAPRE_E_INVALID, "add_noise: negative size or too many samples (%d, %d, %d)", xd->batch,
+                       xd->channels, xd->length);
+    if (ns->mode == KAPRE_NOISE_TENSOR) {
+        const kapre_wave_desc& nd = ns->noise_desc;
+        if ((nd.batch != 1 && nd.batch != xd->batch) || (nd.channels != 1 && nd.channels != xd->channels) ||
+            nd.length != xd->length)
+            return kb_fail(KAPRE_E_INVALID, "noise shape (%d, %d, %d) does not broadcast to (%d, %d, %d)", nd.batch,
+                           nd.channels, nd.length, xd->batch, xd->channels, xd->length);
+    } else if (ns->mode == KAPRE_NOISE_BANK) {
+        if (ns->bank_length < 0) return kb_fail(KAPRE_E_INVALID, "negative bank length");
+    } else {
+        return kb_fail(KAPRE_E_INVALID, "unknown noise mode %d", ns->mode);
+    }
+    p.B = xd->batch; p.C = xd->channels; p.L = xd->length;
+    kb_noise_setup(p);
+    if (p.tiles == 0) return 1;
+    if (!sd->snr) return kb_fail(KAPRE_E_INVALID, "null snr pointer");
+    if (ns->mode == KAPRE_NOISE_TENSOR && !ns->noise) return kb_fail(KAPRE_E_INVALID, "null noise pointer");
+    if (ns->mode == KAPRE_NOISE_BANK && (!ns->bank || !ns->start || !ns->clip_len || !ns->offset))
+        return kb_fail(KAPRE_E_INVALID, "null bank pointer");
+    if (!workspace_dev) return kb_fail(KAPRE_E_INVALID, "null workspace");
+    if (ns->mode == KAPRE_NOISE_TENSOR) {
+        p.n = kb_noise_wave(ns->noise, &ns->noise_desc);
+    } else {
+        p.bank = ns->bank; p.bank_numel = ns->bank_length;
+        p.start = (const long long*)ns->start; p.clip = (const long long*)ns->clip_len;
+        p.offset = (const long long*)ns->offset;
+    }
+    p.snr = sd->snr; p.snr_sb = sd->snr_stride_b; p.snr_sc = sd->snr_stride_c;
+    p.len = sd->lengths; p.len_sb = sd->lengths_stride_b; p.len_sc = sd->lengths_stride_c;
+    p.part = (double*)workspace_dev;
+    return 0;
+}
+
+static int kb_noise_launch(const KbNoiseParams& p, cudaStream_t st) {
+    const int grid = (int)((p.tiles + KB_NOISE_WARPS - 1) / KB_NOISE_WARPS);
+    const int smem = KB_NOISE_WARPS * kb_noise_smem(kb_noise_cg_max(p)).total;
+    int rc;
+    if ((rc = kb_launch(kb_noise_sum_kernel, {.grid = grid, .block = KB_NOISE_WARPS * 32, .smem = smem, .st = st,
+                                              .pdl = true}, p)))
+        return rc;
+    return kb_launch(kb_noise_out_kernel, {.grid = grid, .block = KB_NOISE_WARPS * 32, .smem = smem, .st = st,
+                                           .pdl = true}, p);
+}
+
+extern "C" {
+
+int64_t kapre_add_noise_workspace_bytes(int batch, int channels, int length) {
+    const int64_t n = kb_noise_ws(batch, channels, length);
+    if (n < 0) return kb_fail(KAPRE_E_INVALID, "add_noise: negative size or too many samples");
+    return n;
+}
+
+int kapre_add_noise(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_noise_source* noise,
+                    const kapre_snr_desc* snr, float* y_dev, const kapre_wave_desc* y_desc, double* stats_dev,
+                    void* workspace_dev, void* stream) {
+    if (!y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbNoiseParams p{};
+    int rc = kb_noise_prepare(p, x_desc, noise, snr, workspace_dev);
+    if (rc < 0) return rc;
+    if (!kb_noise_same_shape(x_desc, y_desc)) return kb_fail(KAPRE_E_INVALID, "input and output shapes differ");
+    if (rc == 1) return 0;
+    if (!x_dev || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)y_dev == (const void*)x_dev || (const void*)y_dev == (const void*)p.n.p)
+        return kb_fail(KAPRE_E_INVALID, "add_noise cannot run in place");
+    p.x = kb_noise_wave(x_dev, x_desc);
+    p.x.sb = x_desc->stride_b; p.x.sc = x_desc->stride_c;
+    p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_sl = y_desc->stride_l;
+    p.stats = stats_dev;
+    p.bwd = 0;
+    return kb_noise_launch(p, (cudaStream_t)stream);
+}
+
+int kapre_add_noise_backward(const float* g_dev, const kapre_wave_desc* g_desc, const float* x_dev,
+                             const kapre_wave_desc* x_desc, const kapre_noise_source* noise, const kapre_snr_desc* snr,
+                             const double* stats_dev, float* gx_dev, const kapre_wave_desc* gx_desc, float* gn_dev,
+                             const kapre_wave_desc* gn_desc, float* gsnr_dev, void* workspace_dev, void* stream) {
+    if (!x_desc || !gx_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbNoiseParams p{};
+    int rc = kb_noise_prepare(p, g_desc, noise, snr, workspace_dev);
+    if (rc < 0) return rc;
+    if (!kb_noise_same_shape(g_desc, x_desc) || !kb_noise_same_shape(g_desc, gx_desc))
+        return kb_fail(KAPRE_E_INVALID, "gradient and input shapes differ");
+    if (gn_dev) {
+        if (noise->mode != KAPRE_NOISE_TENSOR) return kb_fail(KAPRE_E_INVALID, "a noise bank has no gradient");
+        if (!gn_desc || !kb_noise_same_shape(g_desc, gn_desc))
+            return kb_fail(KAPRE_E_INVALID, "the noise gradient needs the input's shape");
+    }
+    if (rc == 1) return 0;
+    if (!g_dev || !x_dev || !gx_dev || !stats_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)gx_dev == (const void*)g_dev || (gn_dev && (const void*)gn_dev == (const void*)g_dev))
+        return kb_fail(KAPRE_E_INVALID, "add_noise backward cannot run in place");
+    p.x = kb_noise_wave(g_dev, g_desc);
+    p.x.sb = g_desc->stride_b; p.x.sc = g_desc->stride_c;
+    p.xr = kb_noise_wave(x_dev, x_desc);
+    p.xr.sb = x_desc->stride_b; p.xr.sc = x_desc->stride_c;
+    p.y = gx_dev; p.y_sb = gx_desc->stride_b; p.y_sc = gx_desc->stride_c; p.y_sl = gx_desc->stride_l;
+    if (gn_dev) { p.gn = gn_dev; p.gn_sb = gn_desc->stride_b; p.gn_sc = gn_desc->stride_c; p.gn_sl = gn_desc->stride_l; }
+    p.gsnr = gsnr_dev;
+    p.stats = const_cast<double*>(stats_dev);
+    p.bwd = 1;
+    return kb_noise_launch(p, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1131,6 +1131,143 @@ def lfilter(x, b, a, clamp=True, reverse=False, data_format=_CH_LAST_STR):
     return lfilter_forward(x, b, a, flags | (N.IIR_CLAMP if clamp else 0), data_format)
 
 
+def add_noise_workspace_bytes(B, C, L):
+    """``kapre_add_noise_workspace_bytes``; raises on a negative size or an overflow."""
+    n = int(N.lib().kapre_add_noise_workspace_bytes(B, C, L))
+    if n < 0:
+        N.check(n)
+    return n
+
+
+def add_noise_workspace(B, C, L, device):
+    return torch.empty(max(add_noise_workspace_bytes(B, C, L), 1), dtype=torch.uint8, device=device)
+
+
+def _noise_source(noise, bank, data_format):
+    """kapre_noise_source of a float32 noise tensor in ``data_format`` or of a bank (flat clips, start, clip_len,
+    offset), and the tensors it points into."""
+    if bank is not None:
+        flat, start, clip, offset = bank
+        return N.NoiseSource(N.NOISE_BANK, None, N.WaveDesc(), flat.data_ptr(), flat.numel(), start.data_ptr(),
+                             clip.data_ptr(), offset.data_ptr())
+    nd, _ = _wave_desc(noise, data_format)
+    return N.NoiseSource(N.NOISE_TENSOR, noise.data_ptr(), nd, None, 0, None, None, None)
+
+
+def _snr_desc(snr, lengths):
+    """kapre_snr_desc over (B, C) float32 snr and int32 lengths (or None) views; a stride of 0 broadcasts."""
+    if lengths is None:
+        return N.SnrDesc(snr.data_ptr(), snr.stride(0), snr.stride(1), None, 0, 0)
+    return N.SnrDesc(snr.data_ptr(), snr.stride(0), snr.stride(1), lengths.data_ptr(), lengths.stride(0),
+                     lengths.stride(1))
+
+
+def add_noise_forward(x, noise, bank, snr, lengths, data_format, want_stats):
+    """y = ``kapre_add_noise`` (two launches) and, with ``want_stats``, the (B, C, 2) float64 energies (Ex, En)."""
+    x = _raw(x.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    y, yd = _wave_alloc(B, C, L, data_format, x.device)
+    # every column's (Ex, En) is written by the tile of its first segment
+    stats = torch.empty((B, C, 2), dtype=torch.float64, device=x.device) if want_stats else None
+    if y.numel():
+        ws = add_noise_workspace(B, C, L, x.device)
+        src = _noise_source(noise, bank, data_format)
+        N.check(N.lib().kapre_add_noise(_ptr(x), ctypes.byref(xd), ctypes.byref(src), ctypes.byref(_snr_desc(snr, lengths)),
+                                        _ptr(y), ctypes.byref(yd), _ptr(stats) if want_stats else None, _ptr(ws),
+                                        _stream_ptr()))
+    return y, stats
+
+
+def add_noise_backward(g, x, noise, bank, snr, lengths, stats, data_format, want_noise, want_snr):
+    """Gradients of ``add_noise_forward`` at output gradient g: (gx, gn or None, gsnr (B, C) or None), per element
+    and column, two launches; the caller's autograd sums gn and gsnr over broadcast axes."""
+    g = _raw(g.to(torch.float32))
+    gd, (B, C, L) = _wave_desc(g, data_format)
+    xd, _ = _wave_desc(x, data_format)
+    gx, od = _wave_alloc(B, C, L, data_format, g.device)
+    gn, nd = _wave_alloc(B, C, L, data_format, g.device) if want_noise else (None, None)
+    gsnr = torch.zeros((B, C), dtype=torch.float32, device=g.device) if want_snr else None
+    if gx.numel():
+        ws = add_noise_workspace(B, C, L, g.device)
+        src = _noise_source(noise, bank, data_format)
+        N.check(N.lib().kapre_add_noise_backward(
+            _ptr(g), ctypes.byref(gd), _ptr(x), ctypes.byref(xd), ctypes.byref(src),
+            ctypes.byref(_snr_desc(snr, lengths)), _ptr(stats), _ptr(gx), ctypes.byref(od),
+            _ptr(gn) if want_noise else None, ctypes.byref(nd) if want_noise else None,
+            _ptr(gsnr) if want_snr else None, _ptr(ws), _stream_ptr()))
+    return gx, gn, gsnr
+
+
+def _per_column(v, B, C, dtype, device, name):
+    """A number, array or tensor broadcastable to (B, C) by torch's rules, on ``device`` (cast to ``dtype``)."""
+    if not isinstance(v, torch.Tensor):
+        a = np.asarray(v)
+        if a.dtype.kind not in 'iuf':
+            raise ValueError('%s must be real numbers, got: %r' % (name, v))
+        v = torch.from_numpy(np.ascontiguousarray(a))
+    if v.dtype == torch.bool or v.dtype.is_complex:
+        raise ValueError('%s must be real numbers, got dtype %s' % (name, v.dtype))
+    if v.dim() > 2 or any(n not in (1, m) for n, m in zip(v.shape[::-1], (C, B))):
+        raise ValueError('%s of shape %s does not broadcast to (batch, channels) = (%d, %d)'
+                         % (name, tuple(v.shape), B, C))
+    if v.is_cuda and v.device != device:
+        raise ValueError('%s on %s, the waveform on %s' % (name, v.device, device))
+    return v.to(device=device, dtype=dtype) if dtype is not None else v.to(device=device)
+
+
+def noise_check(x, noise, data_format):
+    """Shapes of ``add_noise``'s operands: x (B, L, C) / (B, C, L); noise 3-D in the same format with batch in {1, B},
+    channels in {1, C} and L samples.  Returns (B, C, L)."""
+    if x.dim() != 3:
+        raise ValueError('add_noise expects a 3-D waveform batch, got shape %s' % (tuple(x.shape),))
+    B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == _CH_LAST_STR else tuple(x.shape)
+    if noise is not None:
+        if noise.dim() != 3:
+            raise ValueError('the noise must be 3-D like the waveform, got shape %s' % (tuple(noise.shape),))
+        Bn, Cn, Ln = (noise.shape[0], noise.shape[2], noise.shape[1]) if data_format == _CH_LAST_STR \
+            else tuple(noise.shape)
+        if Bn not in (1, B) or Cn not in (1, C) or Ln != L:
+            raise ValueError('noise of shape %s does not match the waveform %s (batch and channels may be 1)'
+                             % (tuple(noise.shape), tuple(x.shape)))
+    return B, C, L
+
+
+@_device_of_first_arg
+def add_noise(x, noise, snr, lengths=None, data_format=_CH_LAST_STR, bank=None):
+    """``torchaudio.functional.add_noise`` per (item, channel) column of x (B, L, C) / (B, C, L) on the GPU:
+    ``y = x + s n`` with ``s = sqrt(Ex / En) 10^(-snr / 20)`` and the energies over ``t < lengths``; ``s = 0`` where
+    either energy is 0 (torchaudio gives NaN for silent noise).  ``noise``: 3-D in x's format with batch and channels
+    1 or x's (broadcast without a copy), or None with ``bank = (flat clips, start, clip_len, offset)`` (per-item int64
+    CUDA tensors; item b reads ``flat[start + (offset + t) mod clip_len]``).  ``snr`` and ``lengths``: numbers or
+    tensors broadcastable to (B, C) by torch's rules; lengths are clamped to [0, L] on the device, without a sync.
+    Everything is checked before any launch.  Two launches; differentiable with respect to x, a tensor noise and
+    snr."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise N.KapreNativeError('add_noise needs a CUDA waveform')
+    if noise is not None and not isinstance(noise, torch.Tensor):
+        noise = torch.as_tensor(np.asarray(noise, np.float32))
+    B, C, L = noise_check(x, noise, data_format)
+    if noise is not None:
+        if noise.is_cuda and noise.device != x.device:
+            raise ValueError('noise on %s, the waveform on %s' % (noise.device, x.device))
+        noise = noise.to(device=x.device, dtype=torch.float32)
+        noise = noise.expand(B, L, C) if data_format == _CH_LAST_STR else noise.expand(B, C, L)
+    elif bank is None:
+        raise ValueError('add_noise needs a noise tensor or a bank')
+    snr = _per_column(snr, B, C, torch.float32, x.device, 'snr').expand(B, C)
+    if lengths is not None:
+        lengths = _per_column(lengths, B, C, None, x.device, 'lengths')
+        if lengths.dtype.is_floating_point:
+            raise ValueError('lengths must be integers, got dtype %s' % (lengths.dtype,))
+        lengths = torch.clamp(lengths, 0, L).to(torch.int32).expand(B, C)
+    add_noise_workspace_bytes(B, C, L)                     # size checks before anything is launched
+    if _wants_grad(x) or _wants_grad(noise) or _wants_grad(snr):
+        from . import autograd
+        return autograd.add_noise(x, noise, snr, lengths, bank, data_format)
+    y, _ = add_noise_forward(x, noise, bank, snr, lengths, data_format, False)
+    return y
+
+
 def _pcen_params(params, eps, device):
     """kapre_pcen_params over the four parameter tensors (gain, bias, power, smooth_coef): float32, 0-d (one value
     for every band) or 1-d (one per band), on ``device``."""

@@ -4,7 +4,8 @@
 kernels through the C ABI.  ``Resample`` (polyphase sample-rate conversion) has no counterpart in the
 reference, which expects audio to be resampled before it reaches the model; neither has ``Speed`` (speed perturbation by any
 real factor, band-limited interpolation), ``Convolve`` (convolution with long filters, partitioned FFT) or the IIR
-filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan)."""
+filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan), or
+``add_noise`` (torchaudio's, with deterministic float64 energies)."""
 from __future__ import annotations
 
 import math
@@ -17,7 +18,7 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
-           'Biquad']
+           'Biquad', 'add_noise']
 
 
 def _resolve(fmt):
@@ -281,6 +282,25 @@ def filtfilt(waveform, a_coeffs, b_coeffs, clamp=True, data_format='default'):
     b, a = _normalised(waveform, a_coeffs, b_coeffs, fmt)
     y = ops.lfilter(waveform, b, a, clamp=False, reverse=False, data_format=fmt)
     return ops.lfilter(y, b, a, clamp=clamp, reverse=True, data_format=fmt)
+
+
+def add_noise(waveform, noise, snr, lengths=None, data_format='default'):
+    """``torchaudio.functional.add_noise`` on the GPU: per (item, channel) column,
+
+        y = x + s n,   s = sqrt(Ex / En) 10^(-snr / 20),   Ex = sum_{t < len} x[t]^2,   En = sum_{t < len} n[t]^2,
+
+    with noise added past ``len`` too, as torchaudio does.  ``waveform``: ``(batch, time, ch)`` / ``(batch, ch, time)``
+    (a CUDA tensor); ``noise``: the same shape, or batch and / or channels of 1 (broadcast without a copy); ``snr``
+    (dB) and ``lengths``: numbers or tensors broadcastable to ``(batch, ch)`` by torch's rules (``(batch, 1)`` for
+    one value per item).  The SNR is measured per channel, as torchaudio does.
+
+    The energies and ``s`` are float64 and summed in a fixed order (segments of 4096 samples, a fixed tree in each,
+    the segments in order), so an item's output does not depend on the batch, its position, the strides or the data
+    format.  One deliberate deviation: where the noise (or the signal) has zero energy over the valid samples, ``s`` is
+    0 and the output is the input bit for bit; torchaudio returns NaN there for silent noise.  Two launches;
+    differentiable with respect to ``waveform``, ``noise`` and ``snr`` (every term through ``s`` is 0 where an
+    energy is 0)."""
+    return ops.add_noise(waveform, noise, snr, lengths, _resolve(_unwrap_format(data_format)))
 
 
 def _host_coeffs(b, a):
