@@ -425,6 +425,59 @@ int kapre_add_noise_backward(const float* g_dev, const kapre_wave_desc* g_desc, 
                              const double* stats_dev, float* gx_dev, const kapre_wave_desc* gx_desc, float* gn_dev,
                              const kapre_wave_desc* gn_desc, float* gsnr_dev, void* workspace_dev, void* stream);
 
+/* ---- Kaldi-compatible features (torchaudio.compliance.kaldi.fbank / mfcc / spectrogram) -------------------
+ * Every (item, channel) column of a float32 waveform is framed, dithered, DC-removed, pre-emphasised, windowed,
+ * zero-padded to padded_window_size and transformed as torchaudio 2.11's functions do (one frame set per channel
+ * instead of one selected channel).  Output: (batch, channels, frames, bins) by element strides, with
+ *   fbank:        bins = num_mel_bins + use_energy   (energy first, or last with htk_compat)
+ *   mfcc:         bins = num_ceps
+ *   spectrogram:  bins = padded_window_size / 2 + 1
+ * Item b is computed as if cut to lengths[b] samples: its frame count is
+ *   snip_edges: 1 + (len - W) / shift, 0 when len < W;   otherwise (len + shift / 2) / shift, 0 when len < W,
+ * and 0 when len < min_length; frames past an item's count are written as 0.  padded_window_size must be one of
+ * 256, 512, 1024, 2048 (KAPRE_E_UNSUPPORTED otherwise).  Dither adds `dither` times a deterministic unit-variance
+ * value keyed by (seed, item, channel, frame, sample).  An item's output bits do not depend on the batch, its
+ * position, the strides, the data format or the launch shape. */
+enum { KAPRE_KALDI_FBANK = 0, KAPRE_KALDI_MFCC = 1, KAPRE_KALDI_SPECTROGRAM = 2 };
+typedef struct {
+    int kind;                           /* KAPRE_KALDI_* */
+    int window_size, window_shift;      /* samples: W >= 2, shift >= 1 */
+    int padded_window_size;             /* N >= W, a power of two in [256, 2048] */
+    int snip_edges;                     /* 0 or 1 */
+    int min_length;                     /* samples; shorter items have no frames */
+    int num_mel_bins;                   /* fbank / mfcc: 1 .. 256 */
+    int num_ceps;                       /* mfcc: 1 .. num_mel_bins */
+    int use_energy, htk_compat, raw_energy, use_power, use_log_fbank, remove_dc_offset, subtract_mean;
+    float preemphasis_coefficient;      /* [0, 1] */
+    float energy_floor;                 /* >= 0 */
+} kapre_kaldi_config;
+typedef struct kapre_kaldi_plan kapre_kaldi_plan;
+/* window_host: W floats.  banks_host (fbank / mfcc): num_mel_bins x (N / 2 + 1) row-major mel weights.  dct_host
+ * (mfcc): num_mel_bins x num_ceps, lifter applied (and c0's column scaled by sqrt 2 under htk_compat without
+ * use_energy).  Options must be finite; mfcc and spectrogram need use_power and mfcc use_log_fbank. */
+int kapre_kaldi_plan_create(const kapre_kaldi_config* cfg, const float* window_host, const float* banks_host,
+                            const float* dct_host, kapre_kaldi_plan** out);
+void kapre_kaldi_plan_destroy(kapre_kaldi_plan* plan);
+/* Frames of an item of `length` samples (< 0 on a negative length); bins per frame. */
+int kapre_kaldi_num_frames(const kapre_kaldi_plan* plan, int length);
+int kapre_kaldi_num_bins(const kapre_kaldi_plan* plan);
+/* Scratch of kapre_kaldi_features (backward = 0: none) or of kapre_kaldi_features_backward (the per-frame gradients
+ * and, with subtract_mean, the centred output gradient).  < 0 on a bad size or an overflow. */
+int64_t kapre_kaldi_workspace_bytes(const kapre_kaldi_plan* plan, int batch, int channels, int frames, int backward);
+/* y = features(x).  lengths_host (NULL: every item is x_desc->length long) holds each item's length in [0, length];
+ * lengths_dev holds the same values on the device.  frames must be the largest frame count of the batch.  One
+ * launch, two with subtract_mean. */
+int kapre_kaldi_features(const kapre_kaldi_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc,
+                         const int32_t* lengths_host, const int32_t* lengths_dev, int frames, float dither,
+                         uint64_t seed, float* y_dev, const kapre_spec_desc* y_desc, void* workspace_dev,
+                         void* stream);
+/* gx = the gradient of features(x) to x at output gradient gy, with the forward's dither (same dither and seed).
+ * Samples at or past an item's length get 0.  Two launches, three with subtract_mean. */
+int kapre_kaldi_features_backward(const kapre_kaldi_plan* plan, const float* gy_dev, const kapre_spec_desc* gy_desc,
+                                  const float* x_dev, const kapre_wave_desc* x_desc, const int32_t* lengths_host,
+                                  const int32_t* lengths_dev, int frames, float dither, uint64_t seed, float* gx_dev,
+                                  const kapre_wave_desc* gx_desc, void* workspace_dev, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

@@ -67,6 +67,14 @@ class SnrDesc(Structure):
 NOISE_TENSOR, NOISE_BANK = 0, 1
 
 
+class KaldiCfg(Structure):
+    _fields_ = [('kind', c_int), ('window_size', c_int), ('window_shift', c_int), ('padded_window_size', c_int),
+                ('snip_edges', c_int), ('min_length', c_int), ('num_mel_bins', c_int), ('num_ceps', c_int),
+                ('use_energy', c_int), ('htk_compat', c_int), ('raw_energy', c_int), ('use_power', c_int),
+                ('use_log_fbank', c_int), ('remove_dc_offset', c_int), ('subtract_mean', c_int),
+                ('preemphasis_coefficient', c_float), ('energy_floor', c_float)]
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -150,6 +158,16 @@ SYMBOLS = [
     ('kapre_add_noise_backward', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), POINTER(NoiseSource),
                                          POINTER(SnrDesc), c_void_p, c_void_p, POINTER(WaveDesc), c_void_p,
                                          POINTER(WaveDesc), c_void_p, c_void_p, c_void_p]),
+    ('kapre_kaldi_plan_create', c_int, [POINTER(KaldiCfg), c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
+    ('kapre_kaldi_plan_destroy', None, [c_void_p]),
+    ('kapre_kaldi_num_frames', c_int, [c_void_p, c_int]),
+    ('kapre_kaldi_num_bins', c_int, [c_void_p]),
+    ('kapre_kaldi_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
+    ('kapre_kaldi_features', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, c_void_p, c_int, c_float, c_uint64,
+                                     c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_kaldi_features_backward', c_int, [c_void_p, c_void_p, POINTER(SpecDesc), c_void_p, POINTER(WaveDesc),
+                                              c_void_p, c_void_p, c_int, c_float, c_uint64, c_void_p,
+                                              POINTER(WaveDesc), c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

@@ -26,6 +26,9 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
   by a0)
 * add_noise, BackgroundNoise -> ``kapre_add_noise_backward`` (a segment-sum pass over g n, then the input, noise and
   snr gradients from the saved energies)
+* kaldi_fbank, kaldi_mfcc, kaldi_spectrogram, KaldiFbank, KaldiMFCC, KaldiSpectrogram -> ``kapre_kaldi_features_backward``
+  (each frame's forward recomputed with the same dither and taken back to its samples, then a gather over the
+  frames covering every sample)
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
@@ -391,6 +394,26 @@ class _AddNoise(torch.autograd.Function):
         return gx if ctx.needs_input_grad[0] else None, gn, gsnr, None, None, None
 
 
+class _KaldiFeatures(torch.autograd.Function):
+    """The forward is the plain feature launch; only the waveform is saved, and the backward regenerates the dither
+    from (seed, item, channel, frame, sample)."""
+
+    @staticmethod
+    def forward(ctx, x, plan, lengths_h, lengths_d, data_format, dither, seed):
+        y = ops.kaldi_forward(x, plan, lengths_h, lengths_d, data_format, dither, seed)
+        ctx.save_for_backward(x)
+        ctx.cfg = (plan, lengths_h, lengths_d, data_format, dither, seed)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, = ctx.saved_tensors
+        plan, lengths_h, lengths_d, data_format, dither, seed = ctx.cfg
+        return ops.kaldi_backward(g, x, plan, lengths_h, lengths_d, data_format, dither, seed), None, None, None, \
+            None, None, None
+
+
 class _TimeStretch(torch.autograd.Function):
     """The forward is the plain time-stretch launch; autograd saves its output, from which the backward takes the
     magnitude and phase gradients, so the forward writes nothing extra."""
@@ -508,3 +531,7 @@ def magnitude_to_decibel(x, ref_value, amin, dynamic_range):
 
 def add_noise(x, noise, snr, lengths, bank, data_format):
     return _AddNoise.apply(x.float(), noise, snr, lengths, bank, data_format)
+
+
+def kaldi_features(x, plan, lengths_h, lengths_d, data_format, dither, seed):
+    return _KaldiFeatures.apply(x, plan, lengths_h, lengths_d, data_format, dither, seed)

@@ -260,3 +260,125 @@ def biquad_coefficients(kind: str, sample_rate, freq, Q=0.707, gain=0.0):
         b = [1 + alpha * A, -2 * c, 1 - alpha * A]
         a = [1 + alpha / A, -2 * c, 1 - alpha / A]
     return np.stack(b, -1), np.stack(a, -1)
+
+
+# ------------------------------------------------------------------------------- Kaldi features
+# Host constants of torchaudio.compliance.kaldi (2.11), restated in float64 NumPy: window properties and frame counts,
+# the feature windows, the mel banks with VTLN warping, and the DCT with the cepstral lifter.
+KALDI_WINDOWS = ('hamming', 'hanning', 'povey', 'rectangular', 'blackman')
+KALDI_PADDED_SIZES = (256, 512, 1024, 2048)
+
+
+def kaldi_window_properties(sample_frequency=16000.0, frame_shift=10.0, frame_length=25.0,
+                            round_to_power_of_two=True):
+    """(window_size, window_shift, padded_window_size) in samples, as torchaudio derives them from milliseconds."""
+    shift = int(sample_frequency * frame_shift * 0.001)
+    size = int(sample_frequency * frame_length * 0.001)
+    padded = (1 if size == 0 else 2 ** (size - 1).bit_length()) if round_to_power_of_two else size
+    return size, shift, padded
+
+
+def kaldi_num_frames(length, window_size, window_shift, snip_edges=True, min_length=0):
+    """Frames of an item of ``length`` samples (an int or an integer array): ``1 + (L - W) // shift`` with
+    snip_edges, else ``(L + shift // 2) // shift``; 0 when ``L < W`` (torchaudio refuses such items) or
+    ``L < min_length``."""
+    L = np.asarray(length, dtype=np.int64)
+    n = (1 + (L - window_size) // window_shift) if snip_edges else (L + window_shift // 2) // window_shift
+    n = np.where((L < window_size) | (L < min_length) | (L <= 0), 0, n)
+    return int(n) if n.ndim == 0 else n
+
+
+def kaldi_window(window_type, window_size, blackman_coeff=0.42):
+    """torchaudio's feature window of ``window_size`` samples (symmetric), float64."""
+    n = np.arange(window_size, dtype=np.float64)
+    if window_type in ('hanning', 'povey'):
+        w = 0.5 - 0.5 * np.cos(2.0 * np.pi * n / (window_size - 1)) if window_size > 1 else np.ones(1)
+        return w ** 0.85 if window_type == 'povey' else w
+    if window_type == 'hamming':
+        return 0.54 - 0.46 * np.cos(2.0 * np.pi * n / (window_size - 1)) if window_size > 1 else np.ones(1)
+    if window_type == 'rectangular':
+        return np.ones(window_size)
+    if window_type == 'blackman':
+        a = 2.0 * np.pi / (window_size - 1)
+        return blackman_coeff - 0.5 * np.cos(a * n) + (0.5 - blackman_coeff) * np.cos(2.0 * a * n)
+    raise ValueError('window_type must be one of %s, got %r' % (KALDI_WINDOWS, window_type))
+
+
+def _kaldi_mel(f):
+    return 1127.0 * np.log(1.0 + np.asarray(f, np.float64) / 700.0)
+
+
+def _kaldi_inv_mel(m):
+    return 700.0 * (np.exp(np.asarray(m, np.float64) / 1127.0) - 1.0)
+
+
+def _kaldi_vtln_warp_freq(vtln_low, vtln_high, low_freq, high_freq, warp, freq):
+    if not (vtln_low > low_freq and vtln_high < high_freq):
+        raise ValueError('vtln_low must be above low_freq and vtln_high below high_freq')
+    l = vtln_low * max(1.0, warp)
+    h = vtln_high * min(1.0, warp)
+    scale = 1.0 / warp
+    fl, fh = scale * l, scale * h
+    scale_left = (fl - low_freq) / (l - low_freq)
+    scale_right = (high_freq - fh) / (high_freq - h)
+    res = np.empty_like(freq)
+    after_h, before_h, before_l = freq >= h, freq < h, freq < l
+    outside = (freq < low_freq) | (freq > high_freq)
+    res[after_h] = high_freq + scale_right * (freq[after_h] - high_freq)
+    res[before_h] = scale * freq[before_h]
+    res[before_l] = low_freq + scale_left * (freq[before_l] - low_freq)
+    res[outside] = freq[outside]
+    return res
+
+
+def kaldi_mel_banks(num_bins, padded_window_size, sample_frequency, low_freq=20.0, high_freq=0.0, vtln_low=100.0,
+                    vtln_high=-500.0, vtln_warp=1.0):
+    """torchaudio's ``get_mel_banks`` in float64, with the zero Nyquist column: (num_bins, padded_window_size // 2 + 1).
+    ``high_freq <= 0`` and ``vtln_high < 0`` are offsets from the Nyquist frequency."""
+    if num_bins < 4:
+        raise ValueError('num_mel_bins must be at least 4, got %r' % (num_bins,))
+    nyquist = 0.5 * sample_frequency
+    if high_freq <= 0.0:
+        high_freq += nyquist
+    if not (0.0 <= low_freq < nyquist and 0.0 < high_freq <= nyquist and low_freq < high_freq):
+        raise ValueError('bad low_freq %r / high_freq %r for Nyquist %r' % (low_freq, high_freq, nyquist))
+    if vtln_high < 0.0:
+        vtln_high += nyquist
+    if vtln_warp != 1.0 and not (low_freq < vtln_low < high_freq and 0.0 < vtln_high < high_freq
+                                 and vtln_low < vtln_high):
+        raise ValueError('bad vtln_low %r / vtln_high %r for low_freq %r / high_freq %r'
+                         % (vtln_low, vtln_high, low_freq, high_freq))
+    n_fft_bins = padded_window_size // 2
+    mel_low, mel_high = _kaldi_mel(low_freq), _kaldi_mel(high_freq)
+    delta = (mel_high - mel_low) / (num_bins + 1)
+    b = np.arange(num_bins, dtype=np.float64)[:, None]
+    left, center, right = mel_low + b * delta, mel_low + (b + 1.0) * delta, mel_low + (b + 2.0) * delta
+    if vtln_warp != 1.0:
+        def warp(m):
+            return _kaldi_mel(_kaldi_vtln_warp_freq(vtln_low, vtln_high, low_freq, high_freq, vtln_warp,
+                                                    _kaldi_inv_mel(m)))
+        left, center, right = warp(left), warp(center), warp(right)
+    mel = _kaldi_mel(sample_frequency / padded_window_size * np.arange(n_fft_bins, dtype=np.float64))[None, :]
+    up = (mel - left) / (center - left)
+    down = (right - mel) / (right - center)
+    if vtln_warp == 1.0:
+        banks = np.maximum(0.0, np.minimum(up, down))
+    else:
+        banks = np.zeros_like(up)
+        ui = (mel > left) & (mel <= center)
+        di = (mel > center) & (mel < right)
+        banks[ui] = up[ui]
+        banks[di] = down[di]
+    return np.concatenate([banks, np.zeros((num_bins, 1))], axis=1)
+
+
+def kaldi_dct(num_ceps, num_mel_bins, cepstral_lifter=22.0):
+    """torchaudio's MFCC matrix (num_mel_bins, num_ceps), float64: the orthonormal DCT-II with the first column
+    sqrt(1 / num_mel_bins), times the lifter ``1 + 0.5 L sin(pi i / L)`` (none when ``cepstral_lifter == 0``)."""
+    n = np.arange(num_mel_bins, dtype=np.float64)[:, None]
+    k = np.arange(num_ceps, dtype=np.float64)[None, :]
+    d = np.cos(np.pi / num_mel_bins * (n + 0.5) * k) * np.sqrt(2.0 / num_mel_bins)
+    d[:, 0] = np.sqrt(1.0 / num_mel_bins)
+    if cepstral_lifter != 0.0:
+        d = d * (1.0 + 0.5 * cepstral_lifter * np.sin(np.pi * np.arange(num_ceps) / cepstral_lifter))[None, :]
+    return d

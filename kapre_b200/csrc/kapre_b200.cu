@@ -34,6 +34,7 @@
 #include "fbinv_core.cuh"
 #include "iir_core.cuh"
 #include "noise_core.cuh"
+#include "kaldi_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -3146,6 +3147,311 @@ int kapre_add_noise_backward(const float* g_dev, const kapre_wave_desc* g_desc, 
     p.stats = const_cast<double*>(stats_dev);
     p.bwd = 1;
     return kb_noise_launch(p, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+// ---- Kaldi-compatible features (kaldi_core.cuh) ----------------------------------------------------------------------
+// Persistent CTAs of four independent warps; one warp per job of 32 / Q frames.  The forward needs about 19 KB of
+// shared memory per warp (two CTAs per SM), the backward about 45 KB (one CTA per SM).
+template <int Q>
+__global__ void __launch_bounds__(KB_KALDI_WARPS * 32, 2) kb_kaldi_fwd_kernel(const __grid_constant__ KbKaldiParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    const int w = (int)(threadIdx.x >> 5);
+    const int per = kb_kaldi_smem(p.N, Q, p.n_mel, 0).total;
+    for (long long job = (long long)blockIdx.x * KB_KALDI_WARPS + w; job < p.jobs;
+         job += (long long)gridDim.x * KB_KALDI_WARPS)
+        kb_kaldi_fwd_job<Q>(p, kb_smem + w * per, job);
+}
+template <int Q>
+__global__ void __launch_bounds__(KB_KALDI_WARPS * 32, 1) kb_kaldi_bwd_kernel(const __grid_constant__ KbKaldiParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    const int w = (int)(threadIdx.x >> 5);
+    const int per = kb_kaldi_smem(p.N, Q, p.n_mel, 1).total;
+    for (long long job = (long long)blockIdx.x * KB_KALDI_WARPS + w; job < p.jobs;
+         job += (long long)gridDim.x * KB_KALDI_WARPS)
+        kb_kaldi_bwd_job<Q>(p, kb_smem + w * per, job);
+}
+__global__ void kb_kaldi_gather_kernel(const __grid_constant__ KbKaldiParams p, long long n) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n) kb_kaldi_gather_elem(p, e);
+}
+__global__ void kb_kaldi_cmn_kernel(const __grid_constant__ KbKaldiParams p, const float* in, kapre_spec_desc id,
+                                    float* out, kapre_spec_desc od, long long n) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n)
+        kb_kaldi_cmn_col(p, in, id.stride_b, id.stride_c, id.stride_t, id.stride_f, out, od.stride_b, od.stride_c,
+                         od.stride_t, od.stride_f, e);
+}
+
+struct kapre_kaldi_plan {
+    kapre_kaldi_config cfg;
+    int Q, K, P;
+    DevInfo dev;
+    void* block = nullptr;                          // every table in one allocation
+    const float* wh; const float* half; const float2* twp; const float2* twn;
+    const int* mlo; const int* mlen; const int* moff; const float* mw;
+    const int* klo; const int* klen; const int* kidx; const float* kw;
+    const float* dct;
+};
+
+static bool kb_finite(float v) { return kb_kaldi_finite(v); }
+
+static int kb_kaldi_check_cfg(const kapre_kaldi_config* c) {
+    if (c->kind < KAPRE_KALDI_FBANK || c->kind > KAPRE_KALDI_SPECTROGRAM)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: unknown feature kind %d", c->kind);
+    if (c->window_size < 2 || c->window_shift < 1 || c->min_length < 0)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: window size %d must be >= 2 and the shift %d >= 1", c->window_size,
+                       c->window_shift);
+    if (c->padded_window_size < c->window_size || (c->padded_window_size & 1))
+        return kb_fail(KAPRE_E_INVALID, "kaldi: padded window size %d must be even and >= the window size %d",
+                       c->padded_window_size, c->window_size);
+    const int n = c->padded_window_size;
+    if (n != 256 && n != 512 && n != 1024 && n != 2048)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "kaldi: padded window size %d is not supported (256, 512, 1024 or 2048)", n);
+    if (!kb_finite(c->preemphasis_coefficient) || c->preemphasis_coefficient < 0.0f ||
+        c->preemphasis_coefficient > 1.0f)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: preemphasis_coefficient must be in [0, 1]");
+    if (!kb_finite(c->energy_floor) || c->energy_floor < 0.0f)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: energy_floor must be finite and >= 0");
+    const int flags[] = {c->snip_edges, c->use_energy, c->htk_compat, c->raw_energy, c->use_power, c->use_log_fbank,
+                         c->remove_dc_offset, c->subtract_mean};
+    for (int f : flags)
+        if (f != 0 && f != 1) return kb_fail(KAPRE_E_INVALID, "kaldi: flags must be 0 or 1");
+    if (c->kind != KAPRE_KALDI_SPECTROGRAM && (c->num_mel_bins < 1 || c->num_mel_bins > KB_KALDI_MAX_MEL))
+        return kb_fail(KAPRE_E_INVALID, "kaldi: num_mel_bins %d must be in [1, %d]", c->num_mel_bins, KB_KALDI_MAX_MEL);
+    if (c->kind == KAPRE_KALDI_MFCC && (c->num_ceps < 1 || c->num_ceps > c->num_mel_bins))
+        return kb_fail(KAPRE_E_INVALID, "kaldi: num_ceps %d must be in [1, num_mel_bins]", c->num_ceps);
+    if (c->kind != KAPRE_KALDI_FBANK && !c->use_power)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: mfcc and spectrogram use the power spectrum");
+    if (c->kind == KAPRE_KALDI_MFCC && !c->use_log_fbank)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: mfcc takes the log mel energies");
+    return 0;
+}
+
+static KbKaldiParams kb_kaldi_params(const kapre_kaldi_plan* pl) {
+    const kapre_kaldi_config& c = pl->cfg;
+    KbKaldiParams p{};
+    p.W = c.window_size; p.H = c.window_shift; p.N = c.padded_window_size; p.Q = pl->Q;
+    p.snip = c.snip_edges; p.min_len = c.min_length;
+    p.kind = c.kind; p.n_mel = c.kind == KAPRE_KALDI_SPECTROGRAM ? 0 : c.num_mel_bins; p.n_ceps = c.num_ceps;
+    p.K = pl->K;
+    p.use_energy = c.use_energy; p.htk = c.htk_compat; p.raw_energy = c.raw_energy; p.use_power = c.use_power;
+    p.use_log = c.use_log_fbank; p.remove_dc = c.remove_dc_offset;
+    p.preemph = c.preemphasis_coefficient;
+    p.log_floor = c.energy_floor == 0.0f ? -INFINITY : (float)log((double)c.energy_floor);
+    p.wh = pl->wh; p.half = pl->half; p.twp = pl->twp; p.twn = pl->twn;
+    p.mlo = pl->mlo; p.mlen = pl->mlen; p.moff = pl->moff; p.mw = pl->mw;
+    p.klo = pl->klo; p.klen = pl->klen; p.kidx = pl->kidx; p.kw = pl->kw;
+    p.dct = pl->dct;
+    return p;
+}
+
+// Shape checks and per-call fields shared by both directions; 1: nothing to launch.
+static int kb_kaldi_prepare(KbKaldiParams& p, const kapre_kaldi_plan* pl, const kapre_wave_desc* xd,
+                            const int32_t* len_h, const int32_t* len_d, int frames, float dither, uint64_t seed) {
+    if (!pl || !xd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (xd->batch < 0 || xd->channels < 0 || xd->length < 0)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: negative size (%d, %d, %d)", xd->batch, xd->channels, xd->length);
+    if (!kb_finite(dither) || dither < 0.0f) return kb_fail(KAPRE_E_INVALID, "kaldi: dither must be finite and >= 0");
+    if (len_h && !len_d) return kb_fail(KAPRE_E_INVALID, "kaldi: lengths need their device copy");
+    p = kb_kaldi_params(pl);
+    p.B = xd->batch; p.C = xd->channels; p.L = xd->length;
+    int tmax = 0;
+    for (int b = 0; b < (len_h ? p.B : 1); ++b) {
+        const int l = len_h ? len_h[b] : p.L;
+        if (l < 0 || l > p.L) return kb_fail(KAPRE_E_INVALID, "kaldi: length %d of item %d is outside [0, %d]", l, b, p.L);
+        const int t = kb_kaldi_frames(l, p.W, p.H, p.snip, p.min_len);
+        tmax = t > tmax ? t : tmax;
+    }
+    if (p.B == 0) tmax = 0;
+    if (frames != tmax) return kb_fail(KAPRE_E_INVALID, "kaldi: frames %d, the batch has %d", frames, tmax);
+    if ((long long)frames * p.K > 2147483647LL || (long long)frames * p.W > 2147483647LL)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: frames x bins overflows int32");
+    p.T = frames;
+    p.len = len_h ? len_d : nullptr;
+    p.dither = dither; p.seed = (unsigned long long)seed;
+    const int FPW = 32 / p.Q;
+    p.jobs = (long long)p.B * p.C * ((p.T + FPW - 1) / FPW);
+    return p.jobs == 0 ? 1 : 0;
+}
+
+template <int Q>
+static int kb_kaldi_launch_q(const KbKaldiParams& p, int sm_count, cudaStream_t st) {
+    const int bwd = p.bwd;
+    const int smem = KB_KALDI_WARPS * kb_kaldi_smem(p.N, Q, p.n_mel, bwd).total;
+    const long long ctas = (p.jobs + KB_KALDI_WARPS - 1) / KB_KALDI_WARPS;
+    int grid = 0, rc;
+    if (bwd) {
+        if ((rc = kb_resident_grid(kb_kaldi_bwd_kernel<Q>, KB_KALDI_WARPS * 32, smem, ctas, sm_count, &grid))) return rc;
+        return kb_launch(kb_kaldi_bwd_kernel<Q>, {.grid = grid, .block = KB_KALDI_WARPS * 32, .smem = smem, .st = st}, p);
+    }
+    if ((rc = kb_resident_grid(kb_kaldi_fwd_kernel<Q>, KB_KALDI_WARPS * 32, smem, ctas, sm_count, &grid))) return rc;
+    return kb_launch(kb_kaldi_fwd_kernel<Q>, {.grid = grid, .block = KB_KALDI_WARPS * 32, .smem = smem, .st = st,
+                                              .timed = true}, p);
+}
+
+static int kb_kaldi_launch(const KbKaldiParams& p, int sm_count, cudaStream_t st) {
+    switch (p.Q) {
+        case 4: return kb_kaldi_launch_q<4>(p, sm_count, st);
+        case 8: return kb_kaldi_launch_q<8>(p, sm_count, st);
+        case 16: return kb_kaldi_launch_q<16>(p, sm_count, st);
+        default: return kb_kaldi_launch_q<32>(p, sm_count, st);
+    }
+}
+
+static int kb_kaldi_cmn(const KbKaldiParams& p, const float* in, const kapre_spec_desc& id, float* out,
+                        const kapre_spec_desc& od, cudaStream_t st) {
+    const long long n = (long long)p.B * p.C * p.K;
+    return kb_launch(kb_kaldi_cmn_kernel, {.grid = (int)((n + 255) / 256), .block = 256, .st = st}, p, in, id, out, od, n);
+}
+
+extern "C" {
+
+int kapre_kaldi_plan_create(const kapre_kaldi_config* cfg, const float* window_host, const float* banks_host,
+                            const float* dct_host, kapre_kaldi_plan** out) {
+    if (!cfg || !out || !window_host) return kb_fail(KAPRE_E_INVALID, "null argument");
+    *out = nullptr;
+    int rc = kb_kaldi_check_cfg(cfg);
+    if (rc) return rc;
+    const int W = cfg->window_size, N = cfg->padded_window_size, P = N / 2, Q = P / 32;
+    const bool mel = cfg->kind != KAPRE_KALDI_SPECTROGRAM;
+    const int M = mel ? cfg->num_mel_bins : 0;
+    if (mel && !banks_host) return kb_fail(KAPRE_E_INVALID, "kaldi: null mel banks");
+    if (cfg->kind == KAPRE_KALDI_MFCC && !dct_host) return kb_fail(KAPRE_E_INVALID, "kaldi: null DCT matrix");
+    KbKaldiTables t;
+    const int bad = kb_kaldi_tables(W, N, M, cfg->kind == KAPRE_KALDI_MFCC ? M * cfg->num_ceps : 0, window_host,
+                                    banks_host, dct_host, t);
+    if (bad) return kb_fail(KAPRE_E_INVALID, "kaldi: non-finite %s", bad == 1 ? "window" : bad == 2 ? "mel weight" : "DCT");
+    std::vector<float> &wh = t.wh, &half = t.half, &mw = t.mw, &kw = t.kw, &dct = t.dct;
+    std::vector<float2> &twp = t.twp, &twn = t.twn;
+    std::vector<int> &mlo = t.mlo, &mlen = t.mlen, &moff = t.moff, &klo = t.klo, &klen = t.klen, &kidx = t.kidx;
+    // one device block
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t o_wh = take(wh.size() * 4), o_half = take(half.size() * 4), o_twp = take(twp.size() * 8),
+                 o_twn = take(twn.size() * 8), o_mlo = take(mlo.size() * 4), o_mlen = take(mlen.size() * 4),
+                 o_moff = take(moff.size() * 4), o_mw = take(mw.size() * 4), o_klo = take(klo.size() * 4),
+                 o_klen = take(klen.size() * 4), o_kidx = take(kidx.size() * 4), o_kw = take(kw.size() * 4),
+                 o_dct = take(dct.size() * 4);
+    std::vector<char> host(off, 0);
+    auto put = [&](size_t o, const void* src, size_t bytes) { memcpy(host.data() + o, src, bytes); };
+    put(o_wh, wh.data(), wh.size() * 4); put(o_half, half.data(), half.size() * 4);
+    put(o_twp, twp.data(), twp.size() * 8); put(o_twn, twn.data(), twn.size() * 8);
+    put(o_mlo, mlo.data(), mlo.size() * 4); put(o_mlen, mlen.data(), mlen.size() * 4);
+    put(o_moff, moff.data(), moff.size() * 4); put(o_mw, mw.data(), mw.size() * 4);
+    put(o_klo, klo.data(), klo.size() * 4); put(o_klen, klen.data(), klen.size() * 4);
+    put(o_kidx, kidx.data(), kidx.size() * 4); put(o_kw, kw.data(), kw.size() * 4);
+    put(o_dct, dct.data(), dct.size() * 4);
+    kapre_kaldi_plan* pl = new kapre_kaldi_plan();
+    pl->cfg = *cfg;
+    pl->Q = Q; pl->P = P;
+    pl->K = cfg->kind == KAPRE_KALDI_FBANK ? M + cfg->use_energy
+          : cfg->kind == KAPRE_KALDI_MFCC ? cfg->num_ceps : P + 1;
+    if ((rc = kb_dev_info(&pl->dev))) { delete pl; return rc; }
+    if (cudaMalloc(&pl->block, off) != cudaSuccess) { delete pl; return kb_fail(KAPRE_E_NOMEM, "kaldi: plan allocation"); }
+    if (cudaMemcpy(pl->block, host.data(), off, cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaFree(pl->block); delete pl;
+        return kb_fail(KAPRE_E_CUDA, "kaldi: plan upload");
+    }
+    char* d = (char*)pl->block;
+    pl->wh = (const float*)(d + o_wh); pl->half = (const float*)(d + o_half);
+    pl->twp = (const float2*)(d + o_twp); pl->twn = (const float2*)(d + o_twn);
+    pl->mlo = (const int*)(d + o_mlo); pl->mlen = (const int*)(d + o_mlen); pl->moff = (const int*)(d + o_moff);
+    pl->mw = (const float*)(d + o_mw);
+    pl->klo = (const int*)(d + o_klo); pl->klen = (const int*)(d + o_klen); pl->kidx = (const int*)(d + o_kidx);
+    pl->kw = (const float*)(d + o_kw);
+    pl->dct = (const float*)(d + o_dct);
+    *out = pl;
+    return 0;
+}
+
+void kapre_kaldi_plan_destroy(kapre_kaldi_plan* plan) {
+    if (!plan) return;
+    cudaFree(plan->block);
+    delete plan;
+}
+
+int kapre_kaldi_num_frames(const kapre_kaldi_plan* plan, int length) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (length < 0) return kb_fail(KAPRE_E_INVALID, "negative length");
+    const kapre_kaldi_config& c = plan->cfg;
+    return kb_kaldi_frames(length, c.window_size, c.window_shift, c.snip_edges, c.min_length);
+}
+
+int kapre_kaldi_num_bins(const kapre_kaldi_plan* plan) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    return plan->K;
+}
+
+int64_t kapre_kaldi_workspace_bytes(const kapre_kaldi_plan* plan, int batch, int channels, int frames, int backward) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "kaldi: negative size");
+    if ((long long)frames * plan->K > 2147483647LL || (long long)frames * plan->cfg.window_size > 2147483647LL)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: frames x bins overflows int32");
+    if (!backward) return 0;
+    const double cols = (double)batch * channels * frames;
+    const double bytes = cols * plan->cfg.window_size * 4.0 + (plan->cfg.subtract_mean ? cols * plan->K * 4.0 : 0.0);
+    if (bytes > 4.0e18) return kb_fail(KAPRE_E_INVALID, "kaldi: workspace overflow");
+    const int64_t gf = ((int64_t)batch * channels * frames * plan->cfg.window_size * 4 + 255) & ~(int64_t)255;
+    const int64_t gc = plan->cfg.subtract_mean ? (int64_t)batch * channels * frames * plan->K * 4 : 0;
+    return gf + gc;
+}
+
+int kapre_kaldi_features(const kapre_kaldi_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc,
+                         const int32_t* lengths_host, const int32_t* lengths_dev, int frames, float dither,
+                         uint64_t seed, float* y_dev, const kapre_spec_desc* y_desc, void* workspace_dev,
+                         void* stream) {
+    (void)workspace_dev;
+    if (!y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbKaldiParams p;
+    int rc = kb_kaldi_prepare(p, plan, x_desc, lengths_host, lengths_dev, frames, dither, seed);
+    if (rc < 0) return rc;
+    if (rc == 1) return 0;
+    if (!x_dev || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_sl = x_desc->stride_l;
+    p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_st = y_desc->stride_t;
+    p.y_sk = y_desc->stride_f;
+    p.bwd = 0;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = kb_kaldi_launch(p, plan->dev.sm_count, st))) return rc;
+    if (plan->cfg.subtract_mean) return kb_kaldi_cmn(p, y_dev, *y_desc, y_dev, *y_desc, st);
+    return 0;
+}
+
+int kapre_kaldi_features_backward(const kapre_kaldi_plan* plan, const float* gy_dev, const kapre_spec_desc* gy_desc,
+                                  const float* x_dev, const kapre_wave_desc* x_desc, const int32_t* lengths_host,
+                                  const int32_t* lengths_dev, int frames, float dither, uint64_t seed, float* gx_dev,
+                                  const kapre_wave_desc* gx_desc, void* workspace_dev, void* stream) {
+    if (!gy_desc || !gx_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbKaldiParams p;
+    int rc = kb_kaldi_prepare(p, plan, x_desc, lengths_host, lengths_dev, frames, dither, seed);
+    if (rc < 0) return rc;
+    if (gx_desc->batch != x_desc->batch || gx_desc->channels != x_desc->channels || gx_desc->length != x_desc->length)
+        return kb_fail(KAPRE_E_INVALID, "kaldi: the gradient needs the waveform's shape");
+    const long long n = (long long)p.B * p.C * p.L;
+    if (n == 0) return 0;
+    if (!x_dev || !gx_dev || (p.jobs > 0 && (!gy_dev || !workspace_dev)))
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_sl = x_desc->stride_l;
+    p.gx = gx_dev; p.gx_sb = gx_desc->stride_b; p.gx_sc = gx_desc->stride_c; p.gx_sl = gx_desc->stride_l;
+    p.gf = (float*)workspace_dev;
+    p.bwd = 1;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (p.jobs > 0) {
+        p.g = gy_dev; p.g_sb = gy_desc->stride_b; p.g_sc = gy_desc->stride_c; p.g_st = gy_desc->stride_t;
+        p.g_sk = gy_desc->stride_f;
+        if (plan->cfg.subtract_mean) {
+            float* gc = (float*)((char*)workspace_dev +
+                                 (((int64_t)p.B * p.C * p.T * p.W * 4 + 255) & ~(int64_t)255));
+            kapre_spec_desc cd;
+            cd.stride_f = 1; cd.stride_t = p.K; cd.stride_c = (int64_t)p.T * p.K; cd.stride_b = cd.stride_c * p.C;
+            if ((rc = kb_kaldi_cmn(p, gy_dev, *gy_desc, gc, cd, st))) return rc;
+            p.g = gc; p.g_sb = cd.stride_b; p.g_sc = cd.stride_c; p.g_st = cd.stride_t; p.g_sk = cd.stride_f;
+        }
+        if ((rc = kb_kaldi_launch(p, plan->dev.sm_count, st))) return rc;
+    }
+    return kb_launch(kb_kaldi_gather_kernel, {.grid = (int)((n + 255) / 256), .block = 256, .st = st}, p, n);
 }
 
 }  // extern "C"

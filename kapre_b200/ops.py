@@ -1486,3 +1486,190 @@ def concat_frequency_map_backward(g: torch.Tensor, data_format):
     if gx.numel():
         N.check(N.lib().kapre_concat_frequency_map_backward(_ptr(g), _ptr(gx), B, C1 - 1, T, F, int(cl), _stream_ptr()))
     return gx
+
+
+# ------------------------------------------------------------------------------- Kaldi features
+KALDI_COMMON = dict(blackman_coeff=0.42, dither=0.0, energy_floor=1.0, frame_length=25.0, frame_shift=10.0,
+                    min_duration=0.0, preemphasis_coefficient=0.97, raw_energy=True, remove_dc_offset=True,
+                    round_to_power_of_two=True, sample_frequency=16000.0, snip_edges=True, subtract_mean=False,
+                    window_type='povey')
+_KALDI_MEL = dict(high_freq=0.0, htk_compat=False, low_freq=20.0, num_mel_bins=23, use_energy=False, vtln_high=-500.0,
+                  vtln_low=100.0, vtln_warp=1.0)
+# torchaudio.compliance.kaldi's keywords and defaults per function (without `channel`: every channel is computed)
+KALDI_DEFAULTS = {
+    'fbank': dict(KALDI_COMMON, **_KALDI_MEL, use_log_fbank=True, use_power=True),
+    'mfcc': dict(KALDI_COMMON, **_KALDI_MEL, cepstral_lifter=22.0, num_ceps=13),
+    'spectrogram': dict(KALDI_COMMON),
+}
+_KALDI_KIND = {'fbank': 0, 'mfcc': 1, 'spectrogram': 2}
+
+
+def kaldi_options(kind, **kwargs):
+    """torchaudio's keywords for ``kind`` ('fbank', 'mfcc', 'spectrogram') with their defaults filled in; raises on an
+    unknown keyword or a non-finite number."""
+    if kind not in KALDI_DEFAULTS:
+        raise ValueError('kind must be one of %s, got %r' % (tuple(KALDI_DEFAULTS), kind))
+    unknown = set(kwargs) - set(KALDI_DEFAULTS[kind])
+    if unknown:
+        raise TypeError('kaldi %s got unknown keyword(s) %s' % (kind, sorted(unknown)))
+    o = dict(KALDI_DEFAULTS[kind], **kwargs)
+    for k, v in o.items():
+        if isinstance(v, float) and not math.isfinite(v):
+            raise ValueError('%s must be finite, got %r' % (k, v))
+    return o
+
+
+class KaldiPlan(_PerDevice):
+    """kapre_kaldi_plan per CUDA device for one set of options (as ``kaldi_options`` returns them): the window, the
+    mel banks (VTLN included) and the DCT with the lifter are built here in float64 and held by the plan."""
+
+    def __init__(self, kind, options):
+        from . import backend
+        o = dict(options)
+        self.kind, self.options = kind, o
+        W, H, Np = backend.kaldi_window_properties(o['sample_frequency'], o['frame_shift'], o['frame_length'],
+                                                   o['round_to_power_of_two'])
+        if W < 2 or H < 1:
+            raise ValueError('window size %d and shift %d (samples) must be >= 2 and >= 1' % (W, H))
+        if Np not in backend.KALDI_PADDED_SIZES:
+            raise N.KapreNativeError('kaldi %s: padded window size %d is not supported; the supported sizes are %s '
+                                     '(round_to_power_of_two=True with a window of 129 to 2048 samples)'
+                                     % (kind, Np, ', '.join(map(str, backend.KALDI_PADDED_SIZES))))
+        if not 0.0 <= o['preemphasis_coefficient'] <= 1.0:
+            raise ValueError('preemphasis_coefficient must be in [0, 1]')
+        if o['dither'] < 0.0:
+            raise ValueError('dither must be >= 0')
+        if o['energy_floor'] < 0.0:
+            raise ValueError('energy_floor must be >= 0')
+        self.W, self.H, self.N = W, H, Np
+        self.window = backend.kaldi_window(o['window_type'], W, o['blackman_coeff']).astype(np.float32)
+        M, n_ceps, banks, dct = 0, 0, None, None
+        if kind != 'spectrogram':
+            M = int(o['num_mel_bins'])
+            banks = np.ascontiguousarray(backend.kaldi_mel_banks(
+                M, Np, o['sample_frequency'], o['low_freq'], o['high_freq'], o['vtln_low'], o['vtln_high'],
+                o['vtln_warp']), dtype=np.float32)
+        if kind == 'mfcc':
+            n_ceps = int(o['num_ceps'])
+            if n_ceps > M:
+                raise ValueError('num_ceps %d cannot be larger than num_mel_bins %d' % (n_ceps, M))
+            d = backend.kaldi_dct(n_ceps, M, o['cepstral_lifter'])
+            if o['htk_compat'] and not o['use_energy']:
+                d[:, 0] *= math.sqrt(2.0)
+            dct = np.ascontiguousarray(d, dtype=np.float32)
+        self.banks, self.dct = banks, dct
+        self.min_length = int(math.ceil(o['min_duration'] * o['sample_frequency'])) if o['min_duration'] > 0 else 0
+        self.cfg = N.KaldiCfg(_KALDI_KIND[kind], W, H, Np, int(bool(o['snip_edges'])), self.min_length, M, n_ceps,
+                              int(bool(o.get('use_energy', False))), int(bool(o.get('htk_compat', False))),
+                              int(bool(o['raw_energy'])), int(bool(o.get('use_power', True))),
+                              int(bool(o.get('use_log_fbank', True))), int(bool(o['remove_dc_offset'])),
+                              int(bool(o['subtract_mean'])), float(o['preemphasis_coefficient']),
+                              float(o['energy_floor']))
+        self.K = M + int(bool(o.get('use_energy', False))) if kind == 'fbank' else (n_ceps if kind == 'mfcc'
+                                                                                    else Np // 2 + 1)
+        self._per_device = {}
+
+    _destroy = 'kapre_kaldi_plan_destroy'
+
+    def _create(self, lib, out):
+        def p(a):
+            return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
+        return lib.kapre_kaldi_plan_create(ctypes.byref(self.cfg), p(self.window), p(self.banks), p(self.dct), out)
+
+    def num_frames(self, length):
+        from . import backend
+        return backend.kaldi_num_frames(length, self.W, self.H, self.cfg.snip_edges, self.min_length)
+
+
+_kaldi_plans = {}
+
+
+def kaldi_plan(kind, options):
+    key = (kind, tuple(sorted((k, v) for k, v in options.items() if k != 'dither')))
+    with _lock:
+        p = _kaldi_plans.get(key)
+    if p is None:
+        p = KaldiPlan(kind, options)
+        with _lock:
+            p = _kaldi_plans.setdefault(key, p)
+    return p
+
+
+def _kaldi_lengths(lengths, B, L, device):
+    """(host int32 array, device int32 tensor) of per-item lengths in [0, L], or (None, None)."""
+    if lengths is None:
+        return None, None
+    if isinstance(lengths, torch.Tensor):
+        if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+            raise ValueError('lengths must be integers, got dtype %s' % (lengths.dtype,))
+        h = lengths.detach().to('cpu').numpy()
+    else:
+        h = np.asarray(lengths)
+        if h.dtype.kind not in 'iu':
+            raise ValueError('lengths must be integers, got %r' % (lengths,))
+    h = np.ascontiguousarray(h.reshape(-1), dtype=np.int64)
+    if h.shape != (B,):
+        raise ValueError('lengths must have shape (batch,) = (%d,), got %s' % (B, h.shape))
+    if (h < 0).any() or (h > L).any():
+        raise ValueError('lengths must be in [0, %d], got %s' % (L, h))
+    h = h.astype(np.int32)
+    return h, torch.from_numpy(h).to(device)
+
+
+def kaldi_forward(x, plan: KaldiPlan, lengths_h, lengths_d, data_format, dither, seed):
+    """(B, L, C) / (B, C, L) float32 -> (B, T, K, C) / (B, C, T, K) features: one launch (two with subtract_mean)."""
+    x = _raw(x.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    T = int(plan.num_frames(lengths_h).max()) if lengths_h is not None and B else (plan.num_frames(L) if B else 0)
+    y, yd = _spec_alloc(B, C, T, plan.K, data_format, torch.float32, x.device)
+    if y.numel():
+        h = plan.handle()
+        N.check(N.lib().kapre_kaldi_workspace_bytes(h, B, C, T, 0))
+        lp = lengths_h.ctypes.data_as(ctypes.c_void_p) if lengths_h is not None else None
+        N.check(N.lib().kapre_kaldi_features(h, _ptr(x), ctypes.byref(xd), lp,
+                                             _ptr(lengths_d) if lengths_d is not None else None, T, float(dither),
+                                             int(seed) & 0xFFFFFFFFFFFFFFFF, _ptr(y), ctypes.byref(yd), None,
+                                             _stream_ptr()))
+    return y
+
+
+def kaldi_backward(gy, x, plan: KaldiPlan, lengths_h, lengths_d, data_format, dither, seed):
+    """Gradient of ``kaldi_forward`` to x: two launches (three with subtract_mean)."""
+    gy = _raw(gy.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    gd, (_, _, T, _) = _spec_desc(gy, data_format)
+    gx, od = _wave_alloc(B, C, L, data_format, x.device)
+    if gx.numel():
+        h = plan.handle()
+        n = int(N.lib().kapre_kaldi_workspace_bytes(h, B, C, T, 1))
+        if n < 0:
+            N.check(n)
+        ws = torch.empty(max(n, 1), dtype=torch.uint8, device=x.device)
+        lp = lengths_h.ctypes.data_as(ctypes.c_void_p) if lengths_h is not None else None
+        N.check(N.lib().kapre_kaldi_features_backward(
+            h, _ptr(gy), ctypes.byref(gd), _ptr(x), ctypes.byref(xd), lp,
+            _ptr(lengths_d) if lengths_d is not None else None, T, float(dither), int(seed) & 0xFFFFFFFFFFFFFFFF,
+            _ptr(gx), ctypes.byref(od), _ptr(ws), _stream_ptr()))
+    return gx
+
+
+@_device_of_first_arg
+def kaldi_features(x, plan: KaldiPlan, lengths=None, data_format=_CH_LAST_STR, dither=0.0, seed=0):
+    """Kaldi features of every (item, channel) of a float32 CUDA waveform (B, L, C) / (B, C, L) under ``plan``:
+    (B, T, K, C) / (B, C, T, K), T the largest frame count of the batch, frames past an item's count 0.
+    Differentiable with respect to x; requiring grad changes neither the bits nor the launch count."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise N.KapreNativeError('kaldi features need a CUDA waveform')
+    if x.dim() != 3:
+        raise ValueError('kaldi features expect a 3-D waveform batch, got shape %s' % (tuple(x.shape),))
+    if x.dtype != torch.float32:
+        raise ValueError('kaldi features take a float32 waveform, got %s' % (x.dtype,))
+    dither = float(dither)
+    if not math.isfinite(dither) or dither < 0.0:
+        raise ValueError('dither must be finite and >= 0, got %r' % (dither,))
+    B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == _CH_LAST_STR else tuple(x.shape)
+    lh, ld = _kaldi_lengths(lengths, B, L, x.device)
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.kaldi_features(x, plan, lh, ld, data_format, dither, seed)
+    return kaldi_forward(x, plan, lh, ld, data_format, dither, seed)

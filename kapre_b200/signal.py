@@ -18,7 +18,7 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
-           'Biquad', 'add_noise']
+           'Biquad', 'add_noise', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram']
 
 
 def _resolve(fmt):
@@ -449,3 +449,33 @@ class LogmelToMFCC(Layer):
         return ops.apply_filterbank(log_melgrams, fb, self.data_format)
 
     _config_fields = (('n_mfccs', 'n_mfccs'), ('data_format', 'data_format_str'))
+
+
+def _kaldi(kind, waveform, lengths, data_format, seed, kwargs):
+    o = ops.kaldi_options(kind, **kwargs)
+    fmt = _resolve(_unwrap_format(data_format))
+    if fmt not in (_CH_FIRST_STR, _CH_LAST_STR):
+        raise ValueError('Unknown data_format: %r' % (data_format,))
+    return ops.kaldi_features(waveform, ops.kaldi_plan(kind, o), lengths, fmt, o['dither'], seed)
+
+
+def kaldi_fbank(waveform, lengths=None, data_format='default', seed=0, **kwargs):
+    """``torchaudio.compliance.kaldi.fbank`` on the GPU for a batch: every keyword of torchaudio's function with its
+    default, except ``channel`` (every channel is computed).  ``waveform``: float32 ``(batch, time, ch)`` /
+    ``(batch, ch, time)`` CUDA tensor; returns ``(batch, frames, bins, ch)`` / ``(batch, ch, frames, bins)`` with
+    ``bins = num_mel_bins + use_energy``.  ``lengths`` (``(batch,)`` integers, samples): item b is computed as if cut
+    to ``lengths[b]`` and its frames past its own count are 0; ``frames`` is the largest count.  Dither is a
+    deterministic function of ``(seed, item, channel, frame, sample)``.  The padded window must be 256, 512, 1024 or
+    2048 samples.  One launch (two with ``subtract_mean``); differentiable with respect to ``waveform``."""
+    return _kaldi('fbank', waveform, lengths, data_format, seed, kwargs)
+
+
+def kaldi_mfcc(waveform, lengths=None, data_format='default', seed=0, **kwargs):
+    """``torchaudio.compliance.kaldi.mfcc`` on the GPU for a batch (``num_ceps`` bins); see ``kaldi_fbank``."""
+    return _kaldi('mfcc', waveform, lengths, data_format, seed, kwargs)
+
+
+def kaldi_spectrogram(waveform, lengths=None, data_format='default', seed=0, **kwargs):
+    """``torchaudio.compliance.kaldi.spectrogram`` on the GPU for a batch (``padded_window_size // 2 + 1`` bins);
+    see ``kaldi_fbank``."""
+    return _kaldi('spectrogram', waveform, lengths, data_format, seed, kwargs)

@@ -23,7 +23,7 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
 __all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
-           'PCEN', 'GriffinLim', 'InverseFilterbank']
+           'PCEN', 'GriffinLim', 'InverseFilterbank', 'KaldiFbank', 'KaldiMFCC', 'KaldiSpectrogram']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -634,3 +634,68 @@ class InverseFilterbank(Layer):
         ('db_amin', 'db_amin'),
         ('data_format', 'data_format_original'),
     )
+
+
+class _KaldiLayer(Layer):
+    """torchaudio.compliance.kaldi features of a batch as a layer: torchaudio's keywords (without ``channel``) and
+    ``data_format``.  ``call(x, lengths=None, training=False)``: dither (``dither`` > 0) is applied only with
+    ``training=True``, from a seed drawn per call from ``np.random.default_rng(seed)`` and recorded in
+    ``last_choice``; ``Sequential`` passes no ``training`` flag, so a captured graph never dithers."""
+
+    _kind = None
+
+    def __init__(self, data_format='default', seed=None, **kwargs):
+        keys = ops.KALDI_DEFAULTS[self._kind]
+        kaldi = {k: kwargs.pop(k) for k in list(kwargs) if k in keys}
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.options = ops.kaldi_options(self._kind, **kaldi)
+        for k, v in self.options.items():
+            setattr(self, k, v)
+        self.plan = ops.kaldi_plan(self._kind, self.options)
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self.seed = seed
+        self.rng = np.random.default_rng(seed)
+        self.last_choice = None
+
+    def __call__(self, x, lengths=None, training=None, **kwargs):
+        t, was_host = ops.to_device(x)
+        if was_host:
+            with torch.no_grad():
+                return ops.to_host(self.call(t, lengths=lengths, training=training))
+        return self.call(t, lengths=lengths, training=training)
+
+    def call(self, x, lengths=None, training=False):
+        dither, seed = 0.0, 0
+        if training and self.options['dither'] > 0.0:
+            dither = self.options['dither']
+            seed = int(self.rng.integers(0, 2 ** 63))
+            self.last_choice = seed
+        return ops.kaldi_features(x, self.plan, lengths, self.data_format, dither, seed)
+
+    @property
+    def _config_fields(self):
+        return tuple((k, k) for k in ops.KALDI_DEFAULTS[self._kind]) + (
+            ('data_format', 'data_format_original'), ('seed', 'seed'))
+
+
+@register_keras_serializable(package='Kapre')
+class KaldiFbank(_KaldiLayer):
+    """``torchaudio.compliance.kaldi.fbank`` per (item, channel): ``(batch, time, ch)`` / ``(batch, ch, time)`` ->
+    ``(batch, frames, num_mel_bins + use_energy, ch)`` / ``(batch, ch, frames, num_mel_bins + use_energy)``."""
+    _kind = 'fbank'
+
+
+@register_keras_serializable(package='Kapre')
+class KaldiMFCC(_KaldiLayer):
+    """``torchaudio.compliance.kaldi.mfcc`` per (item, channel): ``num_ceps`` bins per frame."""
+    _kind = 'mfcc'
+
+
+@register_keras_serializable(package='Kapre')
+class KaldiSpectrogram(_KaldiLayer):
+    """``torchaudio.compliance.kaldi.spectrogram`` per (item, channel): ``padded_window_size // 2 + 1`` bins per
+    frame."""
+    _kind = 'spectrogram'
