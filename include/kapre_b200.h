@@ -425,6 +425,30 @@ int kapre_add_noise_backward(const float* g_dev, const kapre_wave_desc* g_desc, 
                              const double* stats_dev, float* gx_dev, const kapre_wave_desc* gx_desc, float* gn_dev,
                              const kapre_wave_desc* gn_desc, float* gsnr_dev, void* workspace_dev, void* stream);
 
+/* ---- gated loudness (torchaudio.functional.loudness, ITU-R BS.1770-4) -------------------------------------------
+ * On the K-weighted signal y (batch, channels <= 5, length): per item of valid length len (lengths_dev, int32 per
+ * item on the device, clamped to [0, length]; NULL: every sample counts), blocks [j step, j step + gate) for
+ * j <= (len - gate) / step (none when len < gate), e_cj = mean of y_c^2 over block j, E_j = sum_c g_c e_cj with
+ * g = (1, 1, 1, 1.41, 1.41), l_j = -0.691 + 10 log10(E_j); J1 = {j : l_j > -70}; Gamma = -0.691 +
+ * 10 log10(mean_{J1} E_j) - 10; J2 = {j in J1 : l_j > Gamma}; LKFS = -0.691 + 10 log10(mean_{J2} E_j), float64
+ * throughout and rounded once to float32.  An empty J2 gives -inf (torchaudio gives NaN); a non-finite block energy
+ * gives NaN.  Sums run in a fixed order that depends on the item and the absolute sample index alone, so an item's
+ * result does not depend on the batch, its position, the strides, the data format or its samples past len.  K-weight
+ * with two kapre_lfilter calls first (see INTEGRATION.md). */
+/* Scratch of kapre_loudness (the return value) and, in *stats_bytes (may be NULL), the size of its stats buffer, which
+ * kapre_loudness_backward reads.  < 0 on a bad size (channels outside [1, 5], gate < 1, step outside [1, gate]) or an
+ * overflow. */
+int64_t kapre_loudness_workspace_bytes(int batch, int channels, int length, int gate, int step, int64_t* stats_bytes);
+/* out_dev: batch float32 LKFS.  Two launches (one when length < gate). */
+int kapre_loudness(const float* y_dev, const kapre_wave_desc* y_desc, const int32_t* lengths_dev, int gate, int step,
+                   float* out_dev, void* stats_dev, void* workspace_dev, void* stream);
+/* gy = the gradient of kapre_loudness with respect to y at output gradient gl_dev (batch float32), given the stats
+ * the forward wrote:  gy[t] = gl (20 / ln 10) g_c y[t] n(t) / (E2 |J2| gate), n(t) the J2 blocks covering t; exactly 0
+ * where n(t) = 0 and for -inf items.  gy_desc: y's shape, any strides, not y.  One launch. */
+int kapre_loudness_backward(const float* gl_dev, const float* y_dev, const kapre_wave_desc* y_desc,
+                            const int32_t* lengths_dev, int gate, int step, const void* stats_dev, float* gy_dev,
+                            const kapre_wave_desc* gy_desc, void* stream);
+
 /* ---- Kaldi-compatible features (torchaudio.compliance.kaldi.fbank / mfcc / spectrogram) -------------------
  * Every (item, channel) column of a float32 waveform is framed, dithered, DC-removed, pre-emphasised, windowed,
  * zero-padded to padded_window_size and transformed as torchaudio 2.11's functions do (one frame set per channel

@@ -158,6 +158,11 @@ SYMBOLS = [
     ('kapre_add_noise_backward', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), POINTER(NoiseSource),
                                          POINTER(SnrDesc), c_void_p, c_void_p, POINTER(WaveDesc), c_void_p,
                                          POINTER(WaveDesc), c_void_p, c_void_p, c_void_p]),
+    ('kapre_loudness_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int, c_int, POINTER(c_int64)]),
+    ('kapre_loudness', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                               c_void_p]),
+    ('kapre_loudness_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, c_int, c_int, c_void_p,
+                                        c_void_p, POINTER(WaveDesc), c_void_p]),
     ('kapre_kaldi_plan_create', c_int, [POINTER(KaldiCfg), c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
     ('kapre_kaldi_plan_destroy', None, [c_void_p]),
     ('kapre_kaldi_num_frames', c_int, [c_void_p, c_int]),

@@ -3,7 +3,8 @@ masking is one CUDA pass (``kapre_spec_augment``).  ``TimeStretch``: a phase voc
 (``kapre_time_stretch``).  ``PitchShift``: STFT, that phase vocoder, the inverse STFT and one band-limited
 interpolation (``kapre_sinc_resample``) back to the input length.  ``Reverb``: convolution with a room impulse response
 drawn from a bank (``kapre_convolve``).  ``RandomBiquad``: a biquad drawn per item (``kapre_lfilter``).
-``BackgroundNoise``: a noise excerpt from a bank added at a drawn SNR (``kapre_add_noise``)."""
+``BackgroundNoise``: a noise excerpt from a bank added at a drawn SNR (``kapre_add_noise``).  ``LoudnessNormalization``:
+a gain to a drawn loudness target (``kapre_lfilter`` and ``kapre_loudness``)."""
 from __future__ import annotations
 
 import numpy as np
@@ -517,4 +518,70 @@ class BackgroundNoise(Layer):
         config = super().get_config()
         config.update({'noises': [c.tolist() for c in self.clips()], 'snr_range': list(self.snr_range),
                        'seed': self.seed, 'data_format': self.data_format_original})
+        return config
+
+
+@register_keras_serializable(package='Kapre')
+class LoudnessNormalization(Layer):
+    """Loudness normalisation to a target per item (EBU R128's -23 LUFS, streaming's -14, or a random target per
+    example): ``(batch, time, ch)`` / ``(batch, ch, time)`` in (ch <= 5), the same shape out, each item scaled by
+    ``10^((target - L) / 20)`` with L its BS.1770 loudness (``signal.loudness``).  Items whose L is not finite
+    (silent, shorter than one 400 ms block, or with a non-finite sample) come back unchanged.  Nothing limits peaks.
+
+    ``call(x, lufs=None, lengths=None)`` draws the targets uniformly from ``lufs_range`` with
+    ``np.random.default_rng(seed)``; ``lufs`` (a number or ``batch`` values) replaces the draw, which is then not made.
+    ``lengths`` is passed to ``loudness``.  ``last_choice`` records the targets.  The gain is formed on the device with
+    no sync; a captured graph (``Sequential.capture``) replays the draw made when it was captured.  The gradient
+    reaches ``x``, through the gain as well."""
+
+    def __init__(self, sample_rate, lufs_range=(-23.0, -23.0), seed=None, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        backend.k_weighting_coefficients(sample_rate)           # validates the rate
+        r = tuple(float(v) for v in lufs_range)
+        if len(r) != 2 or not (np.isfinite(r[0]) and np.isfinite(r[1])) or r[0] > r[1]:
+            raise ValueError('lufs_range must be a (low, high) pair of finite numbers, got: %r' % (lufs_range,))
+        self.sample_rate = sample_rate
+        self.lufs_range = r
+        self.seed = seed
+        self.rng = np.random.default_rng(seed)
+        self.last_choice = None
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self._captured = []
+
+    def draw(self, batch, lufs=None):
+        """``batch`` targets in LUFS: drawn, or the validated override."""
+        if lufs is None:
+            return self.rng.uniform(self.lufs_range[0], self.lufs_range[1], size=batch)
+        t = BackgroundNoise._override('lufs', lufs, batch, 'iuf').astype(np.float64)
+        if not np.all(np.isfinite(t)):
+            raise ValueError('lufs must be finite, got: %r' % (lufs,))
+        return t
+
+    def call(self, x, lufs=None, lengths=None):
+        if x.dim() != 3:
+            raise ValueError('LoudnessNormalization expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise N.KapreNativeError('LoudnessNormalization needs a CUDA tensor')
+        B = x.shape[0]
+        target = self.draw(B, lufs)
+        self.last_choice = target
+        host = torch.from_numpy(target.astype(np.float32))
+        if torch.cuda.is_current_stream_capturing():
+            # the graph's copy node reads this pinned buffer on every replay: it is kept and never written again
+            host = host.pin_memory()
+            self._captured.append(host)
+        t = host.to(x.device, non_blocking=True)
+        L = ops.loudness(x, self.sample_rate, lengths, self.data_format)
+        # a non-finite L gives the exponent 0 (gain 1), and no gradient flows into it
+        L = torch.where(torch.isfinite(L), L, t)
+        gain = torch.pow(10.0, (t - L) / 20.0)
+        return x * gain.view(B, 1, 1)
+
+    def get_config(self):
+        config = super().get_config()
+        config.update({'sample_rate': self.sample_rate, 'lufs_range': list(self.lufs_range), 'seed': self.seed,
+                       'data_format': self.data_format_original})
         return config

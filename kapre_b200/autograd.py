@@ -26,6 +26,8 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
   by a0)
 * add_noise, BackgroundNoise -> ``kapre_add_noise_backward`` (a segment-sum pass over g n, then the input, noise and
   snr gradients from the saved energies)
+* loudness, Loudness, LoudnessNormalization -> ``kapre_loudness_backward`` (gL (20 / ln 10) g_c y n(t) / (E2 |J2| G)
+  from the saved gate decisions), then the two lfilter gradients of the K-weighting
 * kaldi_fbank, kaldi_mfcc, kaldi_spectrogram, KaldiFbank, KaldiMFCC, KaldiSpectrogram -> ``kapre_kaldi_features_backward``
   (each frame's forward recomputed with the same dither and taken back to its samples, then a gather over the
   frames covering every sample)
@@ -394,6 +396,25 @@ class _AddNoise(torch.autograd.Function):
         return gx if ctx.needs_input_grad[0] else None, gn, gsnr, None, None, None
 
 
+class _Loudness(torch.autograd.Function):
+    """Over the K-weighted signal y (the two lfilter calls before it have their own autograd): the forward is the plain
+    two-launch measurement, whose stats (E2, |J2| and the J2 decisions) the one-launch backward reads."""
+
+    @staticmethod
+    def forward(ctx, y, lengths, G, S, data_format):
+        out, stats = ops.loudness_forward(y, lengths, G, S, data_format)
+        ctx.save_for_backward(y, lengths, stats)
+        ctx.cfg = (G, S, data_format)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        y, lengths, stats = ctx.saved_tensors
+        G, S, data_format = ctx.cfg
+        return ops.loudness_backward(g, y, lengths, G, S, stats, data_format), None, None, None, None
+
+
 class _KaldiFeatures(torch.autograd.Function):
     """The forward is the plain feature launch; only the waveform is saved, and the backward regenerates the dither
     from (seed, item, channel, frame, sample)."""
@@ -531,6 +552,10 @@ def magnitude_to_decibel(x, ref_value, amin, dynamic_range):
 
 def add_noise(x, noise, snr, lengths, bank, data_format):
     return _AddNoise.apply(x.float(), noise, snr, lengths, bank, data_format)
+
+
+def loudness(y, lengths, G, S, data_format):
+    return _Loudness.apply(y, lengths, G, S, data_format)
 
 
 def kaldi_features(x, plan, lengths_h, lengths_d, data_format, dither, seed):

@@ -262,6 +262,23 @@ def biquad_coefficients(kind: str, sample_rate, freq, Q=0.707, gain=0.0):
     return np.stack(b, -1), np.stack(a, -1)
 
 
+def k_weighting_coefficients(sample_rate):
+    """The two filters of ITU-R BS.1770's K-weighting as ``torchaudio.functional.loudness`` designs them: ((b, a) of
+    ``treble_biquad(sample_rate, 4.0, 1500.0, 1 / sqrt(2))``, (b, a) of ``highpass_biquad(sample_rate, 38.0, 0.5)``),
+    float64 arrays of length 3, not normalised.  ``sample_rate`` must be above 3000 Hz, so that the shelf's 1500 Hz lies
+    below the Nyquist frequency."""
+    if not (isinstance(sample_rate, (int, float, np.integer, np.floating)) and np.isfinite(sample_rate)
+            and sample_rate > 3000):
+        raise ValueError('sample_rate must be a number above 3000 Hz, got: %r' % (sample_rate,))
+    w0 = 2 * np.pi * 1500.0 / sample_rate
+    alpha = np.sin(w0) / 2 / (1 / np.sqrt(2))
+    A = np.exp(4.0 / 40 * np.log(10))
+    t1, t2, t3 = 2 * np.sqrt(A) * alpha, (A - 1) * np.cos(w0), (A + 1) * np.cos(w0)
+    shelf = (np.array([A * ((A + 1) + t2 + t1), -2 * A * ((A - 1) + t3), A * ((A + 1) + t2 - t1)]),
+             np.array([(A + 1) - t2 + t1, 2 * ((A - 1) - t3), (A + 1) - t2 - t1]))
+    return shelf, biquad_coefficients('highpass', sample_rate, 38.0, 0.5)
+
+
 # ------------------------------------------------------------------------------- Kaldi features
 # Host constants of torchaudio.compliance.kaldi (2.11), restated in float64 NumPy: window properties and frame counts,
 # the feature windows, the mel banks with VTLN warping, and the DCT with the cepstral lifter.

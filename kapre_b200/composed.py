@@ -18,7 +18,7 @@ import torch
 from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
-from .augmentation import BackgroundNoise, RandomBiquad, Reverb, TimeStretch
+from .augmentation import BackgroundNoise, LoudnessNormalization, RandomBiquad, Reverb, TimeStretch
 from .signal import Biquad, IIRFilter, Resample, Speed
 from .time_frequency import (STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
                              MagnitudeToDecibel, Phase, get_registered_object)
@@ -106,10 +106,11 @@ class Sequential(Layer):
 
     def call(self, x):
         start = 0
-        # Leading waveform layers (Resample, Speed, Reverb, the IIR filters and BackgroundNoise) run first, so that the
-        # STFT stack behind them still takes the fused launch.
+        # Leading waveform layers (Resample, Speed, Reverb, the IIR filters, LoudnessNormalization and BackgroundNoise)
+        # run first, so that the STFT stack behind them still takes the fused launch.
         while start < len(self.layers) and type(self.layers[start]) in (Resample, Speed, Reverb, IIRFilter, Biquad,
-                                                                        RandomBiquad, BackgroundNoise):
+                                                                        RandomBiquad, LoudnessNormalization,
+                                                                        BackgroundNoise):
             x = self.layers[start].call(x)
             start += 1
         fused = self._fused_prefix(start) if (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3) else None

@@ -35,6 +35,7 @@
 #include "iir_core.cuh"
 #include "noise_core.cuh"
 #include "kaldi_core.cuh"
+#include "loudness_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -3452,6 +3453,113 @@ int kapre_kaldi_features_backward(const kapre_kaldi_plan* plan, const float* gy_
         if ((rc = kb_kaldi_launch(p, plan->dev.sm_count, st))) return rc;
     }
     return kb_launch(kb_kaldi_gather_kernel, {.grid = (int)((n + 255) / 256), .block = 256, .st = st}, p, n);
+}
+
+}  // extern "C"
+
+// ---- gated loudness (loudness_core.cuh) ----------------------------------------------------------------------------
+// Every pass waits for the previous kernel in the stream before touching data, so all three may be launched with PDL.
+__global__ void __launch_bounds__(KB_LOUD_WARPS * 32) kb_loud_energy_kernel(const __grid_constant__ KbLoudParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long tile = (long long)blockIdx.x * KB_LOUD_WARPS + w;
+    if (tile < p.tiles) kb_loud_energy_tile(p, kb_smem + w * kb_loud_smem().total, tile);
+}
+__global__ void __launch_bounds__(KB_LOUD_WARPS * 32) kb_loud_gate_kernel(const __grid_constant__ KbLoudParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long b = (long long)blockIdx.x * KB_LOUD_WARPS + w;
+    if (b < p.B) kb_loud_gate_tile(p, kb_smem + w * kb_loud_smem().total, b);
+}
+__global__ void __launch_bounds__(KB_LOUD_WARPS * 32) kb_loud_bwd_kernel(const __grid_constant__ KbLoudParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long tile = (long long)blockIdx.x * KB_LOUD_WARPS + w;
+    if (tile < p.tiles) kb_loud_bwd_tile(p, kb_smem + w * kb_loud_smem().total, tile);
+}
+
+// Checks a shape and fills the geometry; the workspace (piece sums) and stats ((E2, |J2|) per item, then one decision
+// byte per block) sizes, or -1 on a bad argument or an overflow.
+static int kb_loud_geometry(KbLoudParams& p, int batch, int channels, int length, int gate, int step, int64_t* ws,
+                            int64_t* stats) {
+    if (batch < 0 || channels < 1 || channels > KB_LOUD_MAXC || length < 0 || gate < 1 || step < 1 || step > gate)
+        return -1;
+    p.B = batch; p.C = channels; p.L = length; p.G = gate; p.S = step;
+    kb_loud_setup(p);
+    const double w = (double)batch * p.K * 2 * channels * 8.0, s = (double)batch * (16.0 + p.Jmax);
+    const double tiles = (double)batch * (p.Kb > p.K ? p.Kb : p.K);
+    if (w > 4.0e18 || s > 4.0e18 || tiles / KB_LOUD_WARPS > 2147483647.0) return -1;
+    *ws = ((int64_t)batch * p.K * 2 * channels * 8 + 255) & ~(int64_t)255;
+    *stats = ((int64_t)batch * 16 + (int64_t)batch * p.Jmax + 255) & ~(int64_t)255;
+    return 0;
+}
+
+static int kb_loud_launch(void (*kernel)(KbLoudParams), long long work, const KbLoudParams& p, cudaStream_t st) {
+    return kb_launch(kernel, {.grid = (int)((work + KB_LOUD_WARPS - 1) / KB_LOUD_WARPS), .block = KB_LOUD_WARPS * 32,
+                              .smem = KB_LOUD_WARPS * kb_loud_smem().total, .st = st, .pdl = true}, p);
+}
+
+extern "C" {
+
+int64_t kapre_loudness_workspace_bytes(int batch, int channels, int length, int gate, int step, int64_t* stats_bytes) {
+    KbLoudParams p{};
+    int64_t ws = 0, stats = 0;
+    if (kb_loud_geometry(p, batch, channels, length, gate, step, &ws, &stats) < 0)
+        return kb_fail(KAPRE_E_INVALID, "loudness: bad size (%d, %d, %d), gate %d or step %d, or an overflow", batch,
+                       channels, length, gate, step);
+    if (stats_bytes) *stats_bytes = stats;
+    return ws;
+}
+
+int kapre_loudness(const float* y_dev, const kapre_wave_desc* y_desc, const int32_t* lengths_dev, int gate, int step,
+                   float* out_dev, void* stats_dev, void* workspace_dev, void* stream) {
+    if (!y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbLoudParams p{};
+    int64_t ws = 0, stats = 0;
+    if (kb_loud_geometry(p, y_desc->batch, y_desc->channels, y_desc->length, gate, step, &ws, &stats) < 0)
+        return kb_fail(KAPRE_E_INVALID, "loudness: bad size (%d, %d, %d), gate %d or step %d, or an overflow",
+                       y_desc->batch, y_desc->channels, y_desc->length, gate, step);
+    if (p.B == 0) return 0;
+    if (!out_dev || !stats_dev || (p.K && (!y_dev || !workspace_dev)))
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_sl = y_desc->stride_l;
+    p.len = lengths_dev;
+    p.out = out_dev;
+    p.part = (double*)workspace_dev;
+    p.stats = (double*)stats_dev;
+    p.mask = (unsigned char*)stats_dev + (int64_t)p.B * 16;
+    p.tiles = (long long)p.B * p.K;
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if (p.tiles && (rc = kb_loud_launch(kb_loud_energy_kernel, p.tiles, p, st))) return rc;
+    return kb_loud_launch(kb_loud_gate_kernel, p.B, p, st);
+}
+
+int kapre_loudness_backward(const float* gl_dev, const float* y_dev, const kapre_wave_desc* y_desc,
+                            const int32_t* lengths_dev, int gate, int step, const void* stats_dev, float* gy_dev,
+                            const kapre_wave_desc* gy_desc, void* stream) {
+    if (!y_desc || !gy_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbLoudParams p{};
+    int64_t ws = 0, stats = 0;
+    if (kb_loud_geometry(p, y_desc->batch, y_desc->channels, y_desc->length, gate, step, &ws, &stats) < 0)
+        return kb_fail(KAPRE_E_INVALID, "loudness: bad size (%d, %d, %d), gate %d or step %d, or an overflow",
+                       y_desc->batch, y_desc->channels, y_desc->length, gate, step);
+    if (gy_desc->batch != p.B || gy_desc->channels != p.C || gy_desc->length != p.L)
+        return kb_fail(KAPRE_E_INVALID, "gradient and signal shapes differ");
+    p.tiles = (long long)p.B * p.Kb;
+    if (p.tiles == 0) return 0;
+    if (!gl_dev || !y_dev || !stats_dev || !gy_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)gy_dev == (const void*)y_dev) return kb_fail(KAPRE_E_INVALID, "loudness backward cannot run in place");
+    p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_sl = y_desc->stride_l;
+    p.len = lengths_dev;
+    p.gl = gl_dev;
+    p.gy = gy_dev; p.g_sb = gy_desc->stride_b; p.g_sc = gy_desc->stride_c; p.g_sl = gy_desc->stride_l;
+    p.stats = (double*)const_cast<void*>(stats_dev);
+    p.mask = (unsigned char*)const_cast<void*>(stats_dev) + (int64_t)p.B * 16;
+    return kb_loud_launch(kb_loud_bwd_kernel, p.tiles, p, (cudaStream_t)stream);
 }
 
 }  // extern "C"

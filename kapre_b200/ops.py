@@ -1268,6 +1268,107 @@ def add_noise(x, noise, snr, lengths=None, data_format=_CH_LAST_STR, bank=None):
     return y
 
 
+LOUDNESS_MAX_CHANNELS = 5
+_k_weighting = {}
+
+
+def loudness_geometry(sample_rate):
+    """(G, S): the 400 ms gate and its 75 %-overlap step in samples, rounded as torchaudio rounds them."""
+    G = int(round(0.4 * sample_rate))
+    return G, int(round(G * 0.25))
+
+
+def k_weighting(sample_rate, device):
+    """The K-weighting's two normalised filters as ((b, a), (b, a)) float32 (1, 1, 3) tensors on ``device``, made once
+    per (device, rate): nothing is copied to the device on later calls, so a call can be captured in a CUDA graph."""
+    from .backend import k_weighting_coefficients
+    key = (device.index if device.index is not None else torch.cuda.current_device(), float(sample_rate))
+    c = _k_weighting.get(key)
+    if c is None:
+        c = tuple(tuple(torch.tensor(v, dtype=torch.float32, device=device).reshape(1, 1, 3) for v in (b / a[0], a / a[0]))
+                  for b, a in k_weighting_coefficients(sample_rate))
+        _k_weighting[key] = c
+    return c
+
+
+def loudness_sizes(B, C, L, G, S):
+    """(workspace bytes, stats bytes) of ``kapre_loudness``; raises on a bad size or an overflow."""
+    stats = ctypes.c_int64(0)
+    n = int(N.lib().kapre_loudness_workspace_bytes(B, C, L, G, S, ctypes.byref(stats)))
+    if n < 0:
+        N.check(n)
+    return n, int(stats.value)
+
+
+def loudness_forward(y, lengths, G, S, data_format):
+    """(LKFS (B,) float32, stats) of the K-weighted y: ``kapre_loudness``, two launches."""
+    y = _raw(y.to(torch.float32))
+    yd, (B, C, L) = _wave_desc(y, data_format)
+    nw, ns = loudness_sizes(B, C, L, G, S)
+    out = torch.empty(B, dtype=torch.float32, device=y.device)
+    stats = torch.empty(max(ns, 1), dtype=torch.uint8, device=y.device)
+    if B:
+        ws = torch.empty(max(nw, 1), dtype=torch.uint8, device=y.device)
+        N.check(N.lib().kapre_loudness(_ptr(y), ctypes.byref(yd), _ptr(lengths) if lengths is not None else None, G, S,
+                                       _ptr(out), _ptr(stats), _ptr(ws), _stream_ptr()))
+    return out, stats
+
+
+def loudness_backward(gl, y, lengths, G, S, stats, data_format):
+    """The gradient of ``loudness_forward`` with respect to y at output gradient gl (B,): one launch."""
+    y = _raw(y.to(torch.float32))
+    yd, (B, C, L) = _wave_desc(y, data_format)
+    gl = gl.to(torch.float32).contiguous()
+    gy, gd = _wave_alloc(B, C, L, data_format, y.device)
+    if gy.numel():
+        N.check(N.lib().kapre_loudness_backward(_ptr(gl), _ptr(y), ctypes.byref(yd),
+                                                _ptr(lengths) if lengths is not None else None, G, S, _ptr(stats),
+                                                _ptr(gy), ctypes.byref(gd), _stream_ptr()))
+    return gy
+
+
+def _item_lengths(lengths, B, L, device):
+    """A number or (B,) integers as (B,) int32 on ``device``, clamped to [0, L] there (no sync)."""
+    if not isinstance(lengths, torch.Tensor):
+        a = np.asarray(lengths)
+        if a.dtype.kind not in 'iu':
+            raise ValueError('lengths must be integers, got: %r' % (lengths,))
+        lengths = torch.as_tensor(a)
+    if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+        raise ValueError('lengths must be integers, got dtype %s' % (lengths.dtype,))
+    if lengths.dim() > 1 or (lengths.dim() == 1 and lengths.shape[0] != B):
+        raise ValueError('lengths must be a number or (batch,) = (%d,) values, got shape %s' % (B, tuple(lengths.shape)))
+    if lengths.is_cuda and lengths.device != device:
+        raise ValueError('lengths on %s, the waveform on %s' % (lengths.device, device))
+    return torch.clamp(lengths.to(device), 0, L).to(torch.int32).expand(B).contiguous()
+
+
+@_device_of_first_arg
+def loudness(x, sample_rate, lengths=None, data_format=_CH_LAST_STR):
+    """``torchaudio.functional.loudness`` per item of x (B, L, C) / (B, C, L), C <= 5: the K-weighting as two
+    ``kapre_lfilter`` calls with the clamp (four launches each), then ``kapre_loudness`` (two launches).  Everything is
+    checked before any launch.  Differentiable with respect to x."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise N.KapreNativeError('loudness needs a CUDA waveform')
+    if x.dim() != 3:
+        raise ValueError('loudness expects a 3-D waveform batch, got shape %s' % (tuple(x.shape),))
+    B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == _CH_LAST_STR else tuple(x.shape)
+    if not 1 <= C <= LOUDNESS_MAX_CHANNELS:
+        raise ValueError('loudness supports 1 to %d channels, got %d' % (LOUDNESS_MAX_CHANNELS, C))
+    (b1, a1), (b2, a2) = k_weighting(sample_rate, x.device)
+    G, S = loudness_geometry(sample_rate)
+    if lengths is not None:
+        lengths = _item_lengths(lengths, B, L, x.device)
+    loudness_sizes(B, C, L, G, S)                           # size checks before anything is launched
+    lfilter_workspace(B, C, L, 2, x.device)
+    y = lfilter(x, b1, a1, clamp=True, data_format=data_format)
+    y = lfilter(y, b2, a2, clamp=True, data_format=data_format)
+    if _wants_grad(y):
+        from . import autograd
+        return autograd.loudness(y, lengths, G, S, data_format)
+    return loudness_forward(y, lengths, G, S, data_format)[0]
+
+
 def _pcen_params(params, eps, device):
     """kapre_pcen_params over the four parameter tensors (gain, bias, power, smooth_coef): float32, 0-d (one value
     for every band) or 1-d (one per band), on ``device``."""

@@ -5,7 +5,8 @@ kernels through the C ABI.  ``Resample`` (polyphase sample-rate conversion) has 
 reference, which expects audio to be resampled before it reaches the model; neither has ``Speed`` (speed perturbation by any
 real factor, band-limited interpolation), ``Convolve`` (convolution with long filters, partitioned FFT) or the IIR
 filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan), or
-``add_noise`` (torchaudio's, with deterministic float64 energies)."""
+``add_noise`` (torchaudio's, with deterministic float64 energies), or ``loudness`` and ``Loudness`` (torchaudio's
+BS.1770 gated loudness, with per-item lengths)."""
 from __future__ import annotations
 
 import math
@@ -18,7 +19,7 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
-           'Biquad', 'add_noise', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram']
+           'Biquad', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram']
 
 
 def _resolve(fmt):
@@ -301,6 +302,51 @@ def add_noise(waveform, noise, snr, lengths=None, data_format='default'):
     differentiable with respect to ``waveform``, ``noise`` and ``snr`` (every term through ``s`` is 0 where an
     energy is 0)."""
     return ops.add_noise(waveform, noise, snr, lengths, _resolve(_unwrap_format(data_format)))
+
+
+def loudness(waveform, sample_rate, lengths=None, data_format='default'):
+    """``torchaudio.functional.loudness`` (ITU-R BS.1770-4 gated loudness, LKFS) per item of ``waveform``
+    ``(batch, time, ch)`` / ``(batch, ch, time)`` (a CUDA tensor, ch <= 5), as a ``(batch,)`` float32 tensor.
+
+    The K-weighting is torchaudio's: ``treble_biquad(sample_rate, 4.0, 1500.0, 1 / sqrt(2))`` then
+    ``highpass_biquad(sample_rate, 38.0, 0.5)``, each clamped to [-1, 1] as torchaudio's biquads do.  The 400 ms
+    blocks step by 100 ms (rounded as torchaudio rounds them), with the absolute gate at -70 LKFS and the relative
+    gate 10 LU below, and the channel weights (1, 1, 1, 1.41, 1.41).  ``sample_rate`` must be above 3000 Hz.
+    ``lengths``: a number or ``(batch,)`` integers; item b is measured as if cut to ``lengths[b]`` samples (clamped to
+    [0, time] on the device, without a sync).
+
+    The block energies and gates are float64 in a fixed order, so an item's result does not depend on the batch, its
+    position, the strides or the data format.  Deliberate deviations from torchaudio: an item whose blocks are all
+    gated out (silence, fewer samples than one block, or no samples) gives ``-inf`` and a gradient of 0, where
+    torchaudio gives NaN or raises; a non-finite sample that reaches a block makes that item NaN and no other.
+
+    Ten launches: two ``kapre_lfilter`` calls of four, then ``kapre_loudness``'s energy and gate passes.  The filter
+    coefficients are uploaded once per device and rate, so a call can be captured in a CUDA graph.  Differentiable
+    with respect to ``waveform``."""
+    return ops.loudness(waveform, sample_rate, lengths, _resolve(_unwrap_format(data_format)))
+
+
+@register_keras_serializable(package='Kapre')
+class Loudness(Layer):
+    """``torchaudio.transforms.Loudness`` as a layer: ``(batch, time, ch)`` / ``(batch, ch, time)`` in (ch <= 5), the
+    ``(batch,)`` loudness in LKFS out (``loudness``).  ``call(x, lengths=None)``."""
+
+    def __init__(self, sample_rate, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        backend.k_weighting_coefficients(sample_rate)           # validates the rate
+        self.sample_rate = sample_rate
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+
+    def call(self, x, lengths=None):
+        return ops.loudness(x, self.sample_rate, lengths, self.data_format)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'),
+        ('data_format', 'data_format_str'),
+    )
 
 
 def _host_coeffs(b, a):
