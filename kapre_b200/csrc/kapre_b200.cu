@@ -141,9 +141,10 @@ static int kb_resident_threads(long long* threads) {
 
 // Grid of a persistent kernel whose CTAs loop over `tiles`: what fits on the device at once (a CTA that waited for a
 // slot would start its share of the tiles late), and no more CTAs than tiles.  The shared-memory attribute is set
-// first because the occupancy query needs it above 48 KiB.
+// first because the occupancy query needs it above 48 KiB.  The launch is reported as "<name> grid=G tiles=T"
+// (kapre_last_launch_info), which tells whether a CTA walks more than one tile.
 template <typename K>
-static int kb_resident_grid(K kernel, int block, int smem, long long tiles, int sm_count, int* grid) {
+static int kb_resident_grid(K kernel, const char* name, int block, int smem, long long tiles, int sm_count, int* grid) {
     int rc = kb_set_smem(kernel, smem);
     if (rc) return rc;
     int per_sm = 0;
@@ -151,6 +152,9 @@ static int kb_resident_grid(K kernel, int block, int smem, long long tiles, int 
     if (per_sm < 1) per_sm = 1;
     const long long cap = (long long)sm_count * per_sm;
     *grid = (int)(tiles < cap ? tiles : cap);
+    char buf[96];
+    snprintf(buf, sizeof(buf), "%s grid=%d tiles=%lld", name, *grid, tiles);
+    g_launch_info = buf;
     return 0;
 }
 
@@ -2027,7 +2031,7 @@ static int kb_resample_launch(const kapre_resample_plan* plan, const float* x_de
     if (!kb_resample_setup(p, KB_RESAMPLE_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
     const int smem = kb_resample_smem(p.up, p.Kp, p.NT, p.down, p.G);
     int grid, rc;
-    if ((rc = kb_resident_grid(kb_resample_kernel, KB_RESAMPLE_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
+    if ((rc = kb_resident_grid(kb_resample_kernel, "resample", KB_RESAMPLE_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
         return rc;
     return kb_launch(kb_resample_kernel, {.grid = grid, .block = KB_RESAMPLE_THREADS, .smem = smem,
                                           .st = (cudaStream_t)stream, .timed = true}, p);
@@ -2150,7 +2154,7 @@ static int kb_sinc_launch(const kapre_sinc_plan* plan, const float* x_dev, const
     if (!kb_sinc_setup(p, step, off, s, gain, plan->integral, KB_SINC_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
     const int smem = kb_sinc_smem(p.NT, step, p.nw, p.G);
     int grid, rc;
-    if ((rc = kb_resident_grid(kb_sinc_resample_kernel, KB_SINC_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
+    if ((rc = kb_resident_grid(kb_sinc_resample_kernel, "sinc", KB_SINC_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
         return rc;
     return kb_launch(kb_sinc_resample_kernel, {.grid = grid, .block = KB_SINC_THREADS, .smem = smem,
                                                .st = (cudaStream_t)stream, .timed = true}, p);
@@ -2240,7 +2244,7 @@ static int kb_conv_mac(const kapre_convolve_plan* plan, const void* a, const kap
     p.correlate = correlate;
     if (!kb_conv_setup(p, KB_CONV_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
     int grid, rc;
-    if ((rc = kb_resident_grid(kb_spec_conv_kernel, KB_CONV_THREADS, KB_CONV_SMEM, p.n_tiles, plan->dev.sm_count, &grid)))
+    if ((rc = kb_resident_grid(kb_spec_conv_kernel, "spec_conv", KB_CONV_THREADS, KB_CONV_SMEM, p.n_tiles, plan->dev.sm_count, &grid)))
         return rc;
     return kb_launch(kb_spec_conv_kernel, {.grid = grid, .block = KB_CONV_THREADS, .smem = KB_CONV_SMEM, .st = st,
                                            .timed = true}, p);
@@ -2325,7 +2329,11 @@ int kapre_convolve(const kapre_convolve_plan* plan, const float* x_dev, const ka
                                  stream)))
         return rc;
     if ((rc = kb_conv_mac(plan, H_dev, H_desc, P, X, &Xd, J, Y, &Yd, Bn, C, T, 0, st))) return rc;
-    return kapre_istft_inverse(plan->istft, Y, Bn, C, T, &Yd, y_dev, y_desc, stream);
+    // the launch report names the multiply-accumulate (the persistent launch) before the inverse STFT's
+    const std::string mac = g_launch_info;
+    if ((rc = kapre_istft_inverse(plan->istft, Y, Bn, C, T, &Yd, y_dev, y_desc, stream))) return rc;
+    g_launch_info = mac + "; " + g_launch_info;
+    return 0;
 }
 
 int64_t kapre_convolve_backward_workspace_bytes(const kapre_convolve_plan* plan, int batch, int channels, int length,
@@ -2365,11 +2373,17 @@ int kapre_convolve_backward(const kapre_convolve_plan* plan, const float* gy_dev
     const kapre_spec_desc Gd = kb_conv_spec_desc(C, T, plan->B), gXd = kb_conv_spec_desc(C, J, plan->B);
     cudaStream_t st = (cudaStream_t)stream;
     if ((rc = kapre_istft_backward(plan->istft, gy_dev, gy_desc, Bn, C, T, G, &Gd, stream))) return rc;
+    std::string macs;   // the launch report: the multiply-accumulates, signal gradient's first
     if (gx_dev) {
         if ((rc = kb_conv_mac(plan, H_dev, H_desc, P, G, &Gd, T, gX, &gXd, Bn, C, J, 1, st))) return rc;
+        macs = g_launch_info;
         if ((rc = kapre_stft_backward(plan->stft, gX, &gXd, Bn, C, J, 0, 1, gx_dev, gx_desc, ola, stream))) return rc;
     }
-    if (gH_dev && (rc = kb_conv_mac(plan, X_dev, X_desc, J, G, &Gd, T, gH_dev, gH_desc, Bn, C, P, 1, st))) return rc;
+    if (gH_dev) {
+        if ((rc = kb_conv_mac(plan, X_dev, X_desc, J, G, &Gd, T, gH_dev, gH_desc, Bn, C, P, 1, st))) return rc;
+        macs += (macs.empty() ? "" : "; ") + g_launch_info;
+    }
+    g_launch_info = macs;
     return 0;
 }
 
@@ -2835,7 +2849,7 @@ int kapre_filterbank_invert(const kapre_fb_inverse_plan* plan, const kapre_fb_in
     if (tiles > 0x7fffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many frames");
     const int smem = kb_fbi_smem_layout(plan->n_freq, plan->n_bands, p.R).total;
     int grid;
-    if ((rc = kb_resident_grid(kb_fbi_kernel, KB_FBI_WARPS * 32, smem, tiles, plan->dev.sm_count, &grid))) return rc;
+    if ((rc = kb_resident_grid(kb_fbi_kernel, "fbinv", KB_FBI_WARPS * 32, smem, tiles, plan->dev.sm_count, &grid))) return rc;
     return kb_launch(kb_fbi_kernel, {.grid = grid, .block = KB_FBI_WARPS * 32, .smem = smem, .st = (cudaStream_t)stream}, p);
 }
 
@@ -3284,10 +3298,10 @@ static int kb_kaldi_launch_q(const KbKaldiParams& p, int sm_count, cudaStream_t 
     const long long ctas = (p.jobs + KB_KALDI_WARPS - 1) / KB_KALDI_WARPS;
     int grid = 0, rc;
     if (bwd) {
-        if ((rc = kb_resident_grid(kb_kaldi_bwd_kernel<Q>, KB_KALDI_WARPS * 32, smem, ctas, sm_count, &grid))) return rc;
+        if ((rc = kb_resident_grid(kb_kaldi_bwd_kernel<Q>, "kaldi_bwd", KB_KALDI_WARPS * 32, smem, ctas, sm_count, &grid))) return rc;
         return kb_launch(kb_kaldi_bwd_kernel<Q>, {.grid = grid, .block = KB_KALDI_WARPS * 32, .smem = smem, .st = st}, p);
     }
-    if ((rc = kb_resident_grid(kb_kaldi_fwd_kernel<Q>, KB_KALDI_WARPS * 32, smem, ctas, sm_count, &grid))) return rc;
+    if ((rc = kb_resident_grid(kb_kaldi_fwd_kernel<Q>, "kaldi_fwd", KB_KALDI_WARPS * 32, smem, ctas, sm_count, &grid))) return rc;
     return kb_launch(kb_kaldi_fwd_kernel<Q>, {.grid = grid, .block = KB_KALDI_WARPS * 32, .smem = smem, .st = st,
                                               .timed = true}, p);
 }

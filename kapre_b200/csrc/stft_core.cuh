@@ -94,11 +94,81 @@ static inline float kb_fdividef(float a, float b) { return a / b; }
 static inline float kb_ldg(const float* p) { return *p; }
 static inline void kb_atomic_max_u32(unsigned int* p, unsigned int v) { if (v > *p) *p = v; }
 static inline unsigned int kb_f2u(float f) { unsigned int u; std::memcpy(&u, &f, 4); return u; }
-// async staging primitives: the emulation copies synchronously and barriers are no-ops
+// Async staging primitives: a host model of the mbarrier protocol that checks how a body uses it.  An 8-byte KbBar in
+// emulated shared memory cannot hold the model's state, so it lives in a table keyed by the barrier's address.  A bulk
+// copy fills its destination with NaN and is performed only by the wait that completes its phase, so a read of the
+// buffer before that wait, or a new copy into a buffer still being read, changes the output.  Every misuse the
+// hardware would turn into a fault, a hang or a silent race counts as a violation (kb_emu_async_violations).  The
+// model checks one ordering only, a copy that lands late: a copy landing early, so that a generic store into its
+// destination before the wait would be lost, is not modelled, and neither is fence.proxy.async.
+#include <map>
 typedef unsigned long long KbBar;
-static inline void kb_bar_init(KbBar*, int) {}
-static inline void kb_bulk_g2s(void* dst, const void* src, int bytes, KbBar*) { std::memcpy(dst, src, bytes); }
-static inline void kb_bar_wait(KbBar*, unsigned) {}
+struct KbEmuCopy { void* dst; const void* src; int bytes; };
+struct KbEmuBar {
+    unsigned long long phase = 0;           // completed phases
+    int count = 0;                          // arrivals per phase (mbarrier.init)
+    int arrived = 0;                        // arrivals in the current phase
+    std::vector<KbEmuCopy> pending;         // bulk copies of the current phase
+};
+struct KbEmuAsync {
+    std::map<const KbBar*, KbEmuBar> bars;
+    long long violations = 0;
+};
+inline KbEmuAsync& kb_emu_async() { static KbEmuAsync s; return s; }
+static inline void kb_bar_init(KbBar* b, int count) {
+    KbEmuAsync& s = kb_emu_async();
+    KbEmuBar& m = s.bars[b];
+    if (!m.pending.empty()) ++s.violations;     // re-initialised while a copy into shared memory is in flight
+    m = KbEmuBar{};
+    m.count = count;
+}
+static inline void kb_bulk_g2s(void* dst, const void* src, int bytes, KbBar* bar) {
+    KbEmuAsync& s = kb_emu_async();
+    const auto it = s.bars.find(bar);
+    const bool aligned = ((uintptr_t)dst & 15u) == 0 && ((uintptr_t)src & 15u) == 0 && (bytes & 15) == 0;
+    const bool sized = bytes > 0 && bytes < (1 << 20);
+    // with count arrivals per phase, one more arrive.expect_tx would complete a phase nobody waits for
+    const bool accepts = it != s.bars.end() && it->second.arrived < it->second.count;
+    if (!aligned || !sized || !accepts) ++s.violations;
+    if (!sized || it == s.bars.end()) return;
+    ++it->second.arrived;
+    it->second.pending.push_back({dst, src, bytes});
+    const unsigned nan = 0x7fc0deadu;
+    for (int i = 0; i + 4 <= bytes; i += 4) std::memcpy(static_cast<char*>(dst) + i, &nan, 4);
+}
+// mbarrier.try_wait.parity: returns once the phase with parity `parity` has completed.  The body's phases run one
+// after another for all threads, so a wait never has to wait for a copy issued after it: a wait that finds its phase
+// current with copies pending completes it (performs the copies), one that finds it current with nothing pending
+// would hang, and one that finds it complete while copies of the current phase are pending, or that names the phase
+// before the first (which the hardware reports as complete; no body here relies on that), has the wrong parity.
+static inline void kb_bar_wait(KbBar* bar, unsigned parity) {
+    KbEmuAsync& s = kb_emu_async();
+    const auto it = s.bars.find(bar);
+    if (it == s.bars.end()) { ++s.violations; return; }
+    KbEmuBar& m = it->second;
+    if ((m.phase & 1u) != (parity & 1u)) {
+        if (m.phase == 0 || !m.pending.empty()) ++s.violations;
+        return;
+    }
+    if (m.pending.empty() || m.arrived < m.count) { ++s.violations; return; }
+    for (const KbEmuCopy& c : m.pending) std::memcpy(c.dst, c.src, (size_t)c.bytes);
+    m.pending.clear();
+    m.arrived = 0;
+    ++m.phase;
+}
+// Exported by every emulation library (each is one translation unit that includes this header): the violations since
+// the last reset, plus one per barrier that still has copies in flight (a CTA that exits before its copies land).
+extern "C" __attribute__((used)) inline long long kb_emu_async_violations(void) {
+    const KbEmuAsync& s = kb_emu_async();
+    long long n = s.violations;
+    for (const auto& kv : s.bars) n += kv.second.pending.empty() ? 0 : 1;
+    return n;
+}
+extern "C" __attribute__((used)) inline void kb_emu_async_reset(void) {
+    KbEmuAsync& s = kb_emu_async();
+    s.bars.clear();
+    s.violations = 0;
+}
 #else
 #define KB_PHASE_BEGIN { const int tid = threadIdx.x; KbThreadRegs& R = kb_regs;
 #define KB_PHASE_END }
@@ -775,9 +845,7 @@ __device__ __forceinline__ void kb_stft_cta(const KbStftParams& p, char* smem, i
 
         // ---- wait for this tile's samples -----------------------------------------------------
         if (tp.bulk) {
-#if !defined(KB_HOST_EMU)
             kb_bar_wait(bar, par);
-#endif
             par ^= 1u;
         }
         {

@@ -436,6 +436,73 @@ void kb_emu_db_tail(const float* x, float* out, long long n, float amin, float d
     for (long long i = 0; i < n; ++i) out[i] = db_mul * kb_log2(kb_floor_keepnan(x[i], amin)) - db_sub;
 }
 
+// The host model of the async staging primitives (stft_core.cuh) against known misuses, each on a private buffer.
+// Returns a bit per case that the model caught: 0 wrong parity, 1 read before the wait (the read sees the NaN fill),
+// 2 second arrive.expect_tx in one phase, 3 misaligned destination, source or size, 4 size 0 or >= 2^20, 5 wait that
+// would hang, 6 re-initialisation with a copy in flight, 7 exit with a copy in flight; bit 8: three phases of the
+// correct protocol land their data with no violation.  Leaves the model reset.
+int kb_emu_async_selftest() {
+    alignas(16) static float src[64];
+    alignas(16) static float dst[68];
+    alignas(16) static KbBar bar;
+    for (int i = 0; i < 64; ++i) src[i] = (float)i;
+    int flagged = 0;
+    auto after = [&](int bit, auto&& play) {
+        kb_emu_async_reset();
+        play();
+        if (kb_emu_async_violations() > 0) flagged |= 1 << bit;
+        kb_emu_async_reset();
+    };
+    after(0, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 64, &bar); kb_bar_wait(&bar, 1); kb_bar_wait(&bar, 0); });
+    {
+        kb_emu_async_reset();
+        kb_bar_init(&bar, 1);
+        kb_bulk_g2s(dst, src, 64, &bar);
+        const float early = dst[3];
+        kb_bar_wait(&bar, 0);
+        if (std::isnan(early) && dst[3] == 3.0f && kb_emu_async_violations() == 0) flagged |= 1 << 1;
+        kb_emu_async_reset();
+    }
+    after(2, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 32, &bar); kb_bulk_g2s(dst + 8, src + 8, 32, &bar);
+                   kb_bar_wait(&bar, 0); });
+    {
+        int caught = 0;
+        after(3, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst + 1, src, 64, &bar); kb_bar_wait(&bar, 0); });
+        caught += (flagged >> 3) & 1; flagged &= ~(1 << 3);
+        after(3, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src + 2, 64, &bar); kb_bar_wait(&bar, 0); });
+        caught += (flagged >> 3) & 1; flagged &= ~(1 << 3);
+        after(3, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 60, &bar); kb_bar_wait(&bar, 0); });
+        caught += (flagged >> 3) & 1; flagged &= ~(1 << 3);
+        if (caught == 3) flagged |= 1 << 3;
+    }
+    {
+        int caught = 0;
+        after(4, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 0, &bar); });
+        caught += (flagged >> 4) & 1; flagged &= ~(1 << 4);
+        after(4, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 1 << 20, &bar); });
+        caught += (flagged >> 4) & 1; flagged &= ~(1 << 4);
+        if (caught == 2) flagged |= 1 << 4;
+    }
+    after(5, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 64, &bar); kb_bar_wait(&bar, 0); kb_bar_wait(&bar, 1);
+                   kb_bar_wait(&bar, 1); });
+    after(6, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 64, &bar); kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 64, &bar);
+                   kb_bar_wait(&bar, 0); });
+    after(7, [&] { kb_bar_init(&bar, 1); kb_bulk_g2s(dst, src, 64, &bar); });
+    {
+        kb_emu_async_reset();
+        kb_bar_init(&bar, 1);
+        bool ok = true;
+        for (int k = 0; k < 3; ++k) {
+            kb_bulk_g2s(dst + 4 * k, src + 16 * k, 64, &bar);
+            for (unsigned w = 0; w < 4; ++w) kb_bar_wait(&bar, (unsigned)k & 1u);   // every thread of a phase waits
+            for (int i = 0; i < 16; ++i) ok = ok && dst[4 * k + i] == src[16 * k + i];
+        }
+        if (ok && kb_emu_async_violations() == 0) flagged |= 1 << 8;
+        kb_emu_async_reset();
+    }
+    return flagged;
+}
+
 // kb_atan2 (the Phase outputs' polynomial atan2) on arrays, for the accuracy test
 void kb_emu_atan2(const float* y, const float* x, float* out, long long n) {
     for (long long i = 0; i < n; ++i) out[i] = kb_atan2(y[i], x[i]);

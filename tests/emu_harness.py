@@ -25,12 +25,39 @@ def _needs_build():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
+class Checked:
+    """An emulation library whose every call is checked against the host model of the async staging primitives
+    (stft_core.cuh): the model is reset before the call and must count no violation after it.  `raw` is the
+    unchecked library."""
+
+    def __init__(self, lib):
+        lib.kb_emu_async_violations.restype = ctypes.c_longlong
+        self.raw = lib
+
+    def __getattr__(self, name):
+        fn = getattr(self.raw, name)
+
+        def call(*args):
+            self.raw.kb_emu_async_reset()
+            out = fn(*args)
+            n = self.raw.kb_emu_async_violations()
+            assert n == 0, '%s: %d violations of the async staging protocol' % (name, n)
+            return out
+        return call
+
+
+_lib_handle = None
+
+
 def load():
-    if _needs_build():
-        os.makedirs(os.path.dirname(_OUT), exist_ok=True)
-        subprocess.check_call(['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-DKB_HOST_EMU',
-                               '-Wno-unknown-pragmas', '-o', _OUT, _SRC])
-    return ctypes.CDLL(_OUT)
+    global _lib_handle
+    if _lib_handle is None:
+        if _needs_build():
+            os.makedirs(os.path.dirname(_OUT), exist_ok=True)
+            subprocess.check_call(['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-DKB_HOST_EMU',
+                                   '-Wno-unknown-pragmas', '-o', _OUT, _SRC])
+        _lib_handle = Checked(ctypes.CDLL(_OUT))
+    return _lib_handle
 
 
 def _fp(a):

@@ -18,6 +18,7 @@ import scipy.signal
 
 import conv_ref as CR
 import emu_harness as EH
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_conv.cpp')
@@ -45,7 +46,7 @@ def _lib():
         lib.kb_emu_spec_conv.argtypes = [P, P, I, P, P, I, P, P, I, I, I, I, I, I, I]
         lib.kb_emu_conv_block_size.restype = ctypes.c_longlong
         lib.kb_emu_conv_block_size.argtypes = [ctypes.c_longlong]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

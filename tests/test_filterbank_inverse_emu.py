@@ -24,6 +24,7 @@ import pytest
 
 import fbinv_ref as FR
 import oracle
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_fbinv.cpp')
@@ -53,7 +54,7 @@ def _lib():
         lib.kb_emu_fbi_tables.argtypes = [P, I, I, P, P, P]
         lib.kb_emu_fbi_pick_r.argtypes = [I, I, I]
         lib.kb_emu_fbi.argtypes = [P, I, I, P, P, I, I, I, I, I, F, F, P, P, I, I]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

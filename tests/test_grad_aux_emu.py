@@ -20,6 +20,7 @@ import torch
 import grad_ref as R
 import grad_ref_adjacent as RA
 from oracle import reference as ref
+from emu_harness import Checked
 
 LL = ctypes.c_longlong
 FMTS = ('channels_first', 'channels_last')
@@ -49,7 +50,7 @@ def _lib():
         lib = ctypes.CDLL(out)
         lib.kb_emu_pad_index.restype = ctypes.c_longlong
         lib.kb_emu_pad_index.argtypes = [ctypes.c_longlong, ctypes.c_longlong, ctypes.c_int]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

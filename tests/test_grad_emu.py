@@ -14,6 +14,7 @@ import torch
 import emu_harness as E
 import grad_ref as R
 from oracle import reference as ref
+from emu_harness import Checked
 
 LL = ctypes.c_longlong
 FMTS = ('channels_first', 'channels_last')
@@ -44,7 +45,7 @@ def _grad_lib():
             subprocess.check_call(['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-DKB_HOST_EMU', '-Wno-unknown-pragmas',
                                    '-o', tmp, _GRAD_SRC])
             os.replace(tmp, out)
-        _grad_lib_handle = ctypes.CDLL(out)
+        _grad_lib_handle = Checked(ctypes.CDLL(out))
     return _grad_lib_handle
 
 

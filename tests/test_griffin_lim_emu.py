@@ -17,6 +17,7 @@ import pytest
 import torch
 
 import gl_ref as GR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_gl.cpp')
@@ -47,7 +48,7 @@ def _lib():
         lib.kb_emu_gl_u.argtypes = [ctypes.c_ulonglong, ctypes.c_longlong]
         lib.kb_emu_gl_u.restype = ctypes.c_float
         lib.kb_emu_gl_phasor.argtypes = [ctypes.c_float, P, P]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

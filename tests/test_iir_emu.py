@@ -16,6 +16,7 @@ import scipy.signal
 import torch
 
 import iir_ref as IR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_iir.cpp')
@@ -42,7 +43,7 @@ def _lib():
         I, P, LL = ctypes.c_int, ctypes.c_void_p, ctypes.c_longlong
         lib.kb_emu_lfilter.argtypes = [P, P, P, P, P, P, P, I, I, I, I, I, I, P, P, P, P, I, I, LL]
         lib.kb_emu_iir_powers.argtypes = [P, I, P]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

@@ -17,6 +17,7 @@ import torchaudio.compliance.kaldi as TK
 
 import kaldi_ref as R
 from kapre_b200 import backend, ops
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_kaldi.cpp')
@@ -39,7 +40,7 @@ def _lib():
             subprocess.check_call(['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-DKB_HOST_EMU', '-Wno-unknown-pragmas',
                                    '-o', tmp, _SRC])
             os.replace(tmp, out)
-        _lib_handle = ctypes.CDLL(out)
+        _lib_handle = Checked(ctypes.CDLL(out))
     return _lib_handle
 
 

@@ -15,6 +15,7 @@ import pytest
 import torch
 
 import loudness_ref as LR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_loudness.cpp')
@@ -43,7 +44,7 @@ def _lib():
         lib.kb_emu_loudness.argtypes = [P, P, P, I, I, I, I, I, P, P, P, P, I]
         lib.kb_emu_loudness_backward.argtypes = [P, P, P, P, I, I, I, I, I, P, P, P, P, I]
         lib.kb_emu_loudness_geometry.argtypes = [I, I, I, P]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

@@ -15,6 +15,7 @@ import pytest
 import torch
 
 import noise_ref as NR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_noise.cpp')
@@ -41,7 +42,7 @@ def _lib():
         P, I, LL = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong
         lib.kb_emu_add_noise.argtypes = [P, P, P, LL, P, P, P, P, P, P, P, P, P, I, I, I, I, P, P, P, I]
         lib.kb_emu_noise_consts.argtypes = [P]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

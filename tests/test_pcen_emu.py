@@ -24,6 +24,7 @@ import pytest
 import torch
 
 import pcen_ref as PR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_pcen.cpp')
@@ -55,7 +56,7 @@ def _lib():
         lib.kb_emu_pcen_backward.argtypes = [P, P, P, P, P, P, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                              P, P, ctypes.c_float, ctypes.c_int, P, P, P]
         lib.kb_emu_pcen_chunks.argtypes = [ctypes.c_longlong, ctypes.c_int, ctypes.c_longlong]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

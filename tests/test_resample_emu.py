@@ -17,6 +17,7 @@ import pytest
 import torch
 
 import resample_ref as RR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_resample.cpp')
@@ -45,7 +46,7 @@ def _lib():
                                         ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                         ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_int,
                                         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 
@@ -53,9 +54,9 @@ def _fp(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
-def emu_resample(x, fmt, up, down, h32, gain=None, length=None, NT=64, n_cta=3):
+def emu_resample(x, fmt, up, down, h32, gain=None, length=None, NT=64, n_cta=3, bulk=None):
     """Run the kernel body on the NumPy array `x` ((B, L, C) channels_last or (B, C, L), any strides, possibly a view
-    into a larger buffer) with the library's choice of channel grouping and loader."""
+    into a larger buffer) with the library's choice of channel grouping and loader unless overridden."""
     if fmt == CL:
         B, L, C = x.shape
         sb, sl, sc = (s // 4 for s in x.strides)
@@ -70,10 +71,11 @@ def emu_resample(x, fmt, up, down, h32, gain=None, length=None, NT=64, n_cta=3):
     ys = np.array([y.strides[0], y.strides[2], y.strides[1]] if fmt == CL else [s for s in y.strides], np.int64) // 4
     xs = np.array([sb, sc, sl], np.int64)
     G = C if (1 < C <= 256 and abs(sc) < abs(sl)) else 1           # kb_resample_launch's choice
-    bulk = int((G == 1 and sl == 1) or (G == C and sc == 1 and sl == C))
+    can_bulk = int((G == 1 and sl == 1) or (G == C and sc == 1 and sl == C))
     h32 = np.ascontiguousarray(h32, np.float32)
     rc = _lib().kb_emu_resample(x.ctypes.data, _fp(xs), numel, B, C, L, _fp(y), _fp(ys), Lo, up, down, _fp(h32), h32.size,
-                                float(up if gain is None else gain), G, NT, 256, n_cta, bulk)
+                                float(up if gain is None else gain), G, NT, 256, n_cta,
+                                can_bulk if bulk is None else int(bulk and can_bulk))
     assert rc == 0
     return y
 

@@ -17,6 +17,7 @@ import pytest
 import torch
 
 import sinc_ref as SR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_sinc.cpp')
@@ -51,7 +52,7 @@ def _lib():
         lib.kb_emu_sinc_h.argtypes = [D]
         lib.kb_emu_sinc_table.argtypes = [P]
         lib.kb_emu_sinc_smem.argtypes = [I, D, I, I]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 

@@ -21,6 +21,7 @@ import pytest
 import torch
 
 import time_stretch_ref as TR
+from emu_harness import Checked
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, 'emu', 'kb_emu_ts.cpp')
@@ -52,7 +53,7 @@ def _lib():
         lib.kb_emu_ts.argtypes = [P, P, I, I, I, I, D, I, P, P]
         lib.kb_emu_ts_backward.argtypes = [P, P, P, P, P, P, I, I, I, I, D, I, P, P]
         lib.kb_emu_ts_chunks.argtypes = [ctypes.c_longlong, I, ctypes.c_longlong]
-        _lib_handle = lib
+        _lib_handle = Checked(lib)
     return _lib_handle
 
 
