@@ -502,6 +502,48 @@ int kapre_kaldi_features_backward(const kapre_kaldi_plan* plan, const float* gy_
                                   const int32_t* lengths_dev, int frames, float dither, uint64_t seed, float* gx_dev,
                                   const kapre_wave_desc* gx_desc, void* workspace_dev, void* stream);
 
+/* ---- constant-Q transform (multirate, modelled on librosa's cqt / vqt) ------------------------------------------
+ * Octave i = 0 .. n_oct - 1 (n_oct = ceil(n_bins / bins_per_octave), octave 0 the top one) holds the bins
+ * [max(0, n_bins - (i + 1) B), n_bins - i B) and reads pyramid level y_i: y_0 = x, y_{i+1} = resample_poly(y_i, 1, 2)
+ * with the decimation filter given to the plan (L_{i+1} = ceil(L_i / 2)), hop h_i = hop_length / 2^i.  With octave i's
+ * table T (one row of taps[i] complex taps per bin, the scale and the conjugate folded in),
+ *   C[k, m] = sum_{j < taps[i]} y_i[m h_i + j - taps[i] / 2] T_k[j],   y_i = 0 outside [0, L_i),  m < 1 + length / hop
+ * as one float32 dot product per output with j ascending, so an output's bits depend on (item, channel, octave,
+ * frame, bin) alone: not on the batch, its position, the strides or the launch shape. */
+#define KAPRE_CQT_MAX_OCTAVES 12
+#define KAPRE_CQT_MAX_TAPS 2048
+typedef struct {
+    int n_bins, bins_per_octave;
+    int hop_length;                       /* a multiple of 2^(n_oct - 1) */
+    int taps[KAPRE_CQT_MAX_OCTAVES];      /* row length of octave i's table, 1 .. KAPRE_CQT_MAX_TAPS */
+} kapre_cqt_config;
+typedef struct kapre_cqt_plan kapre_cqt_plan;
+/* taps_host: octave 0's table, then octave 1's, ..., each (bins of the octave) x taps[i] complex64 (float pairs),
+ * bins ascending.  decim_taps_host: the odd, symmetric 2:1 decimation filter (kapre_resample_plan_create(1, 2, ...)).
+ * Every octave with taps[i] <= KAPRE_CQT_MAX_TAPS fits the kernel's shared-memory staging at any hop;
+ * KAPRE_E_UNSUPPORTED when the octaves need more than 256 (octave, bin group) segments, a group being the bins whose
+ * taps fit 32 KB (kapre_b200.backend.cqt_geometry computes the count). */
+int kapre_cqt_plan_create(const kapre_cqt_config* cfg, const float* taps_host, const float* decim_taps_host,
+                          int n_decim_taps, kapre_cqt_plan** out);
+void kapre_cqt_plan_destroy(kapre_cqt_plan* plan);
+/* 1 + length / hop_length (< 0 on a negative length). */
+int kapre_cqt_num_frames(const kapre_cqt_plan* plan, int length);
+/* Device scratch of kapre_cqt (backward = 0: pyramid levels 1 .. n_oct - 1) or of kapre_cqt_backward (backward = 1:
+ * the adjoint's levels and their decimation adjoints).  < 0 on a bad size or an overflow. */
+int64_t kapre_cqt_workspace_bytes(const kapre_cqt_plan* plan, int batch, int channels, int length, int backward);
+/* out = C (complex64, magnitude = 0) or |C| (float32, magnitude = 1), (batch, channels, frames, n_bins) by element
+ * strides.  The pyramid is left in workspace_dev (kapre_cqt_workspace_bytes(..., 0) bytes).  n_oct - 1 resampling
+ * launches and one transform launch. */
+int kapre_cqt(const kapre_cqt_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, int magnitude,
+              void* out_dev, const kapre_spec_desc* out_desc, void* workspace_dev, void* stream);
+/* gx = the gradient of kapre_cqt to x at output gradient g: Re(A^H g) for complex g (torch's dL/dRe + i dL/dIm), or
+ * in magnitude mode the same at g C / |C| (0 where |C| = 0), C recomputed from x and the pyramid the forward left in
+ * fwd_workspace_dev (unused in complex mode).  workspace_dev: kapre_cqt_workspace_bytes(..., 1) bytes.  Lowest
+ * octave first, 2 n_oct - 1 launches: n_oct adjoint gathers and n_oct - 1 resampling adjoints. */
+int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc,
+                       const void* fwd_workspace_dev, const void* g_dev, const kapre_spec_desc* g_desc, int magnitude,
+                       float* gx_dev, const kapre_wave_desc* gx_desc, void* workspace_dev, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

@@ -75,6 +75,14 @@ class KaldiCfg(Structure):
                 ('preemphasis_coefficient', c_float), ('energy_floor', c_float)]
 
 
+CQT_MAX_OCTAVES = 12
+
+
+class CqtCfg(Structure):
+    _fields_ = [('n_bins', c_int), ('bins_per_octave', c_int), ('hop_length', c_int),
+                ('taps', c_int * CQT_MAX_OCTAVES)]
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -173,6 +181,13 @@ SYMBOLS = [
     ('kapre_kaldi_features_backward', c_int, [c_void_p, c_void_p, POINTER(SpecDesc), c_void_p, POINTER(WaveDesc),
                                               c_void_p, c_void_p, c_int, c_float, c_uint64, c_void_p,
                                               POINTER(WaveDesc), c_void_p, c_void_p]),
+    ('kapre_cqt_plan_create', c_int, [POINTER(CqtCfg), c_void_p, c_void_p, c_int, POINTER(c_void_p)]),
+    ('kapre_cqt_plan_destroy', None, [c_void_p]),
+    ('kapre_cqt_num_frames', c_int, [c_void_p, c_int]),
+    ('kapre_cqt_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
+    ('kapre_cqt', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_int, c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_cqt_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, c_void_p, POINTER(SpecDesc), c_int,
+                                   c_void_p, POINTER(WaveDesc), c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

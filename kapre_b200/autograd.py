@@ -31,6 +31,9 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * kaldi_fbank, kaldi_mfcc, kaldi_spectrogram, KaldiFbank, KaldiMFCC, KaldiSpectrogram -> ``kapre_kaldi_features_backward``
   (each frame's forward recomputed with the same dither and taken back to its samples, then a gather over the
   frames covering every sample)
+* CQT (and its fused ``CQT -> Magnitude``) -> ``kapre_cqt_backward`` (per octave, lowest first, a gather of the
+  filters' adjoint over the frames covering each sample plus the decimator's adjoint of the octave below; the
+  magnitude mode recomputes C from the saved pyramid)
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
@@ -435,6 +438,22 @@ class _KaldiFeatures(torch.autograd.Function):
             None, None, None
 
 
+class _Cqt(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, plan, input_data_format, output_data_format, magnitude):
+        y, ws = ops.cqt_forward(x, plan, input_data_format, output_data_format, magnitude)
+        ctx.save_for_backward(x, ws if magnitude else None)
+        ctx.cfg = (plan, input_data_format, output_data_format, magnitude)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, ws = ctx.saved_tensors
+        plan, idf, odf, magnitude = ctx.cfg
+        return ops.cqt_backward(g, x, ws, plan, idf, odf, magnitude), None, None, None, None
+
+
 class _TimeStretch(torch.autograd.Function):
     """The forward is the plain time-stretch launch; autograd saves its output, from which the backward takes the
     magnitude and phase gradients, so the forward writes nothing extra."""
@@ -560,3 +579,7 @@ def loudness(y, lengths, G, S, data_format):
 
 def kaldi_features(x, plan, lengths_h, lengths_d, data_format, dither, seed):
     return _KaldiFeatures.apply(x, plan, lengths_h, lengths_d, data_format, dither, seed)
+
+
+def cqt(x, plan, input_data_format, output_data_format, magnitude):
+    return _Cqt.apply(x, plan, input_data_format, output_data_format, magnitude)

@@ -399,3 +399,102 @@ def kaldi_dct(num_ceps, num_mel_bins, cepstral_lifter=22.0):
     if cepstral_lifter != 0.0:
         d = d * (1.0 + 0.5 * cepstral_lifter * np.sin(np.pi * np.arange(num_ceps) / cepstral_lifter))[None, :]
     return d
+
+
+# ---- constant-Q transform ---------------------------------------------------------------------------------------
+CQT_C1 = 32.70319566257483      # C1 in Hz, the default lowest bin
+CQT_MAX_OCTAVES = 12            # octaves one launch covers (KAPRE_CQT_MAX_OCTAVES)
+CQT_MAX_TAPS = 2048             # longest filter of an octave at its own rate (KAPRE_CQT_MAX_TAPS)
+CQT_MAX_SEGMENTS = 256          # (octave, bin group) segments of one plan (KB_CQT_MAX_SEGS)
+CQT_GROUP_BYTES = 32 * 1024     # a bin group's complex64 taps (KB_CQT_TAB_BYTES)
+
+
+def cqt_segments(taps, octave_bins):
+    """Forward (octave, bin group) segments of a plan whose octave i has ``octave_bins[i]`` bins and ``taps[i]`` taps
+    per bin: groups of an even number of bins whose taps fit CQT_GROUP_BYTES, at most 256 bins (kb_cqt_fwd_group)."""
+    n = 0
+    for N, nk in zip(taps, octave_bins):
+        gk = min((CQT_GROUP_BYTES // (8 * N)) & ~1, (nk + 1) & ~1, 256)
+        n += -(-nk // gk)
+    return n
+
+
+def cqt_frequencies(n_bins: int, f_min: Optional[float] = None, bins_per_octave: int = 12) -> np.ndarray:
+    """Centre frequencies ``f_k = f_min 2^(k / bins_per_octave)`` of the CQT bins, float64 (``f_min`` default C1)."""
+    f_min = CQT_C1 if f_min is None else float(f_min)
+    return f_min * 2.0 ** (np.arange(int(n_bins), dtype=np.float64) / int(bins_per_octave))
+
+
+def cqt_geometry(sample_rate, hop_length, f_min=None, n_bins=84, bins_per_octave=12, filter_scale=1.0, gamma=0.0):
+    """Validated geometry of a multirate CQT / VQT: dict with ``freqs``, ``lengths`` (the real full-rate filter
+    lengths l_k = Q sr / (f_k + gamma / alpha)), ``alpha``, ``Q``, ``n_octaves`` and ``octaves``, a list of
+    (first bin, end bin) per octave, top octave first.  Raises ValueError on a configuration the transform rejects."""
+    for name, v in (('sample_rate', sample_rate), ('hop_length', hop_length), ('n_bins', n_bins),
+                    ('bins_per_octave', bins_per_octave), ('filter_scale', filter_scale)):
+        if isinstance(v, bool) or not np.isfinite(float(v)) or float(v) <= 0:
+            raise ValueError('%s must be positive, got %r' % (name, v))
+    for name, v in (('hop_length', hop_length), ('n_bins', n_bins), ('bins_per_octave', bins_per_octave)):
+        if int(v) != v:
+            raise ValueError('%s must be an integer, got %r' % (name, v))
+    if f_min is not None and not (np.isfinite(float(f_min)) and float(f_min) > 0):
+        raise ValueError('f_min must be positive, got %r' % (f_min,))
+    if not (np.isfinite(float(gamma)) and float(gamma) >= 0):
+        raise ValueError('gamma must be >= 0, got %r' % (gamma,))
+    sr, h, n, B = float(sample_rate), int(hop_length), int(n_bins), int(bins_per_octave)
+    freqs = cqt_frequencies(n, f_min, B)
+    r = 2.0 ** (1.0 / B)
+    alpha = (r * r - 1.0) / (r * r + 1.0)
+    Q = float(filter_scale) / alpha
+    n_oct = -(-n // B)
+    f_max = freqs[-1]
+    edge = f_max + (alpha * f_max + float(gamma)) / 2.0
+    if edge >= sr / 2.0:
+        raise ValueError('the top band edge %.1f Hz (f_max + (alpha f_max + gamma) / 2) is at or above the Nyquist '
+                         'frequency %.1f Hz: reduce n_bins or f_min' % (edge, sr / 2.0))
+    if n_oct > CQT_MAX_OCTAVES:
+        raise ValueError('%d octaves exceed the kernel limit of %d octaves per transform' % (n_oct, CQT_MAX_OCTAVES))
+    if h % (1 << (n_oct - 1)):
+        raise ValueError('hop_length %d must be a multiple of 2^(n_octaves - 1) = %d for %d octaves'
+                         % (h, 1 << (n_oct - 1), n_oct))
+    lengths = Q * sr / (freqs + float(gamma) / alpha)
+    octaves = [(max(0, n - (i + 1) * B), n - i * B) for i in range(n_oct)]
+    for i, (k0, _) in enumerate(octaves):
+        N = int(np.ceil(lengths[k0] / 2.0 ** i))
+        if N > CQT_MAX_TAPS:
+            raise ValueError('the filter of bin %d is %d taps long at octave %d\'s rate, over the kernel limit of %d '
+                             'taps: raise f_min, n_bins or sample_rate, or lower filter_scale' % (k0, N, i, CQT_MAX_TAPS))
+    taps = [int(np.ceil(lengths[k0] / 2.0 ** i)) for i, (k0, _) in enumerate(octaves)]
+    segs = cqt_segments(taps, [k1 - k0 for k0, k1 in octaves])
+    if segs > CQT_MAX_SEGMENTS:
+        raise ValueError('%d (octave, bin group) segments exceed the kernel limit of %d (a group holds the bins whose '
+                         'taps fit %d bytes): lower bins_per_octave or filter_scale' % (segs, CQT_MAX_SEGMENTS,
+                                                                                       CQT_GROUP_BYTES))
+    return dict(freqs=freqs, lengths=lengths, alpha=alpha, Q=Q, n_octaves=n_oct, octaves=octaves)
+
+
+def cqt_filters(sample_rate, f_min=None, n_bins=84, bins_per_octave=12, filter_scale=1.0, gamma=0.0, scale=True):
+    """Per-octave complex128 tap tables of the multirate CQT, top octave first.  Octave i's table T has shape
+    (bins in the octave, N_i) with N_i = ceil(l_k0 / 2^i) the length of its longest (lowest) filter, and
+        T[k, j] = s_k conj(psi_k[j - N_i // 2]),   psi_k[n] = w[n + N // 2] exp(2 pi i f_k n / sr_i) / sum(w)
+    for n in [-(N // 2), N - N // 2), N = ceil(l_k / 2^i), w the periodic Hann window of N points, 0 elsewhere;
+    s_k = sqrt(l_k) with ``scale``, else l_k.  Then C[k, m] = sum_j y_i[m h_i + j - N_i // 2] T[k, j]."""
+    g = cqt_geometry(sample_rate, 1 << (-(-int(n_bins) // int(bins_per_octave)) - 1), f_min, n_bins,
+                     bins_per_octave, filter_scale, gamma)
+    sr = float(sample_rate)
+    out = []
+    for i, (k0, k1) in enumerate(g['octaves']):
+        sr_i = sr / 2.0 ** i
+        Ni = int(np.ceil(g['lengths'][k0] / 2.0 ** i))
+        half = Ni // 2
+        T = np.zeros((k1 - k0, Ni), dtype=np.complex128)
+        for kk, k in enumerate(range(k0, k1)):
+            lk = g['lengths'][k]
+            N = int(np.ceil(lk / 2.0 ** i))
+            j = np.arange(N, dtype=np.float64)
+            w = 0.5 - 0.5 * np.cos(2.0 * np.pi * j / N)
+            nn = j - N // 2
+            psi = w * np.exp(2j * np.pi * g['freqs'][k] * nn / sr_i) / w.sum()
+            s = np.sqrt(lk) if scale else lk
+            T[kk, half - N // 2:half - N // 2 + N] = s * np.conj(psi)
+        out.append(T)
+    return out

@@ -20,12 +20,12 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .augmentation import BackgroundNoise, LoudnessNormalization, RandomBiquad, Reverb, TimeStretch
 from .signal import Biquad, IIRFilter, Resample, Speed
-from .time_frequency import (STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
+from .time_frequency import (CQT, STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
                              MagnitudeToDecibel, Phase, get_registered_object)
 
 __all__ = ['CapturedSequential', 'Sequential', 'StftMagPhase', 'get_stft_magnitude_layer', 'get_melspectrogram_layer',
-           'get_log_frequency_spectrogram_layer', 'get_perfectly_reconstructing_stft_istft', 'get_stft_mag_phase',
-           'get_time_stretch_layer', 'get_inverse_melspectrogram_layer']
+           'get_log_frequency_spectrogram_layer', 'get_cqt_layer', 'get_perfectly_reconstructing_stft_istft',
+           'get_stft_mag_phase', 'get_time_stretch_layer', 'get_inverse_melspectrogram_layer']
 
 
 _streams = {}
@@ -113,8 +113,13 @@ class Sequential(Layer):
                                                                         BackgroundNoise):
             x = self.layers[start].call(x)
             start += 1
-        fused = self._fused_prefix(start) if (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3) else None
-        if fused is not None:
+        on_device = isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3
+        fused = self._fused_prefix(start) if on_device else None
+        if on_device and fused is None and self.fuse and len(self.layers) > start + 1 \
+                and type(self.layers[start]) is CQT and type(self.layers[start + 1]) is Magnitude:
+            x = self.layers[start].call(x, magnitude=True)      # CQT -> Magnitude: one launch writes |C|
+            start += 2
+        elif fused is not None:
             n, mode, stft, fbl, dbl = fused
             db = None
             if dbl is not None:
@@ -377,6 +382,23 @@ def get_log_frequency_spectrogram_layer(input_shape=None, n_fft=2048, win_length
               'bins_per_octave': log_bins_per_octave, 'f_min': log_f_min, 'spread': log_spread}
     stftm_to_loggram = ApplyFilterbank(type='log', filterbank_kwargs=kwargs, data_format=output_data_format)
     layers = [waveform_to_stft, Magnitude(), stftm_to_loggram]
+    if return_decibel:
+        layers.append(MagnitudeToDecibel(ref_value=db_ref_value, amin=db_amin, dynamic_range=db_dynamic_range))
+    return Sequential(layers, name=name)
+
+
+def get_cqt_layer(input_shape=None, sample_rate=22050, hop_length=512, f_min=None, n_bins=84, bins_per_octave=12,
+                  filter_scale=1.0, gamma=0.0, scale=True, return_decibel=False, db_amin=1e-5, db_ref_value=1.0,
+                  db_dynamic_range=80.0, input_data_format='default', output_data_format='default', name='cqt'):
+    """``Sequential([CQT, Magnitude, (MagnitudeToDecibel)])``: the constant-Q counterpart of
+    ``get_log_frequency_spectrogram_layer``, with a long window for the low bins and a short one for the high bins.
+    Called on a CUDA tensor, CQT and Magnitude run as one fused launch (after the pyramid's decimations)."""
+    backend.validate_data_format_str(input_data_format)
+    backend.validate_data_format_str(output_data_format)
+    kwargs = {} if input_shape is None else {'input_shape': input_shape}
+    layers = [CQT(**kwargs, sample_rate=sample_rate, hop_length=hop_length, f_min=f_min, n_bins=n_bins,
+                  bins_per_octave=bins_per_octave, filter_scale=filter_scale, gamma=gamma, scale=scale,
+                  input_data_format=input_data_format, output_data_format=output_data_format), Magnitude()]
     if return_decibel:
         layers.append(MagnitudeToDecibel(ref_value=db_ref_value, amin=db_amin, dynamic_range=db_dynamic_range))
     return Sequential(layers, name=name)

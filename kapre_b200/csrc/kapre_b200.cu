@@ -36,6 +36,7 @@
 #include "noise_core.cuh"
 #include "kaldi_core.cuh"
 #include "loudness_core.cuh"
+#include "cqt_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -3574,6 +3575,231 @@ int kapre_loudness_backward(const float* gl_dev, const float* y_dev, const kapre
     p.stats = (double*)const_cast<void*>(stats_dev);
     p.mask = (unsigned char*)const_cast<void*>(stats_dev) + (int64_t)p.B * 16;
     return kb_loud_launch(kb_loud_bwd_kernel, p.tiles, p, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+// ---- constant-Q transform (cqt_core.cuh) ------------------------------------------------------------------------------
+__global__ void __launch_bounds__(KB_CQT_THREADS) kb_cqt_fwd_kernel(const __grid_constant__ KbCqtParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_cqt_fwd_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_CQT_BWD_THREADS) kb_cqt_bwd_kernel(const __grid_constant__ KbCqtParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_cqt_bwd_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+
+struct kapre_cqt_plan {
+    kapre_cqt_config cfg;
+    KbCqtParams geo;                        // octaves and segments (per-call fields unset)
+    DevInfo dev;
+    float2* tab = nullptr;
+    float2* btab = nullptr;
+    kapre_resample_plan* rs = nullptr;      // the 2:1 decimator
+};
+
+static const int KB_CQT_FWD_SMEM = KB_CQT_TAB_BYTES + KB_CQT_SPAN_FLOATS * 4;
+
+// Level i's length: L_0 = length, L_{i+1} = ceil(L_i / 2).
+static long long kb_cqt_level_len(long long L, int i) {
+    for (int k = 0; k < i; ++k) L = (L + 1) / 2;
+    return L;
+}
+
+// Float offsets, 256 B aligned, of the pyramid levels 1 .. n_oct-1 (forward workspace), or (backward workspace) of the
+// adjoint's levels 1 .. n_oct-1 and its resampling adjoints at levels 0 .. n_oct-2.  Returns the total in bytes.
+static int64_t kb_cqt_layout(int n_oct, long long bc, long long L, int backward, int64_t* lvl, int64_t* glvl,
+                             int64_t* rlvl) {
+    int64_t off = 0;
+    auto take = [&](long long n) { const int64_t o = off; off += (n * 4 + 255) / 256 * 64; return o; };
+    if (!backward)
+        for (int i = 1; i < n_oct; ++i) lvl[i] = take(bc * kb_cqt_level_len(L, i));
+    else {
+        for (int i = 1; i < n_oct; ++i) glvl[i] = take(bc * kb_cqt_level_len(L, i));
+        for (int i = 0; i + 1 < n_oct; ++i) rlvl[i] = take(bc * kb_cqt_level_len(L, i));
+    }
+    return off * 4;
+}
+
+static int kb_cqt_check_shape(const kapre_cqt_plan* plan, const kapre_wave_desc* xd) {
+    if (!plan || !xd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (xd->batch < 0 || xd->channels < 0 || xd->length < 0)
+        return kb_fail(KAPRE_E_INVALID, "cqt: negative size (%d, %d, %d)", xd->batch, xd->channels, xd->length);
+    if ((double)xd->batch * xd->channels * (xd->length + 1.0) * 3.0 > 4.0e18)
+        return kb_fail(KAPRE_E_INVALID, "cqt: size overflow");
+    int cur = -1;
+    KB_CUDA(cudaGetDevice(&cur));
+    if (cur != plan->dev.device)
+        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    return 0;
+}
+
+// Common fields: levels (level 0 = x, the others contiguous (B, C, L_i) in the workspace) and sizes.
+static KbCqtParams kb_cqt_params(const kapre_cqt_plan* plan, const float* x, const kapre_wave_desc* xd, float* ws) {
+    KbCqtParams p = plan->geo;
+    p.B = xd->batch; p.C = xd->channels;
+    p.M = 1 + xd->length / plan->cfg.hop_length;
+    p.tab = plan->tab; p.btab = plan->btab;
+    int64_t lvl[KB_CQT_MAX_OCT], g[KB_CQT_MAX_OCT], r[KB_CQT_MAX_OCT];
+    kb_cqt_layout(p.n_oct, (long long)p.B * p.C, xd->length, 0, lvl, g, r);
+    for (int i = 0; i < p.n_oct; ++i) {
+        KbCqtOct& o = p.oct[i];
+        o.L = (int)kb_cqt_level_len(xd->length, i);
+        if (i == 0) { o.y = x; o.y_sb = xd->stride_b; o.y_sc = xd->stride_c; o.y_sl = xd->stride_l; }
+        else { o.y = ws + lvl[i]; o.y_sb = (long long)p.C * o.L; o.y_sc = o.L; o.y_sl = 1; }
+    }
+    return p;
+}
+
+static kapre_wave_desc kb_cqt_level_desc(int B, int C, int L) {
+    kapre_wave_desc d;
+    d.batch = B; d.channels = C; d.length = L;
+    d.stride_b = (int64_t)C * L; d.stride_c = L; d.stride_l = 1;
+    return d;
+}
+
+extern "C" {
+
+int kapre_cqt_plan_create(const kapre_cqt_config* cfg, const float* taps_host, const float* decim_taps_host,
+                          int n_decim_taps, kapre_cqt_plan** out) {
+    if (!cfg || !taps_host || !decim_taps_host || !out) return kb_fail(KAPRE_E_INVALID, "null argument");
+    *out = nullptr;
+    if (cfg->n_bins < 1 || cfg->bins_per_octave < 1 || cfg->hop_length < 1)
+        return kb_fail(KAPRE_E_INVALID, "cqt: n_bins %d, bins_per_octave %d and hop_length %d must be positive",
+                       cfg->n_bins, cfg->bins_per_octave, cfg->hop_length);
+    const int n_oct = (cfg->n_bins + cfg->bins_per_octave - 1) / cfg->bins_per_octave;
+    if (n_oct > KAPRE_CQT_MAX_OCTAVES)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "cqt: %d octaves exceed the limit of %d", n_oct, KAPRE_CQT_MAX_OCTAVES);
+    if (cfg->hop_length % (1 << (n_oct - 1)))
+        return kb_fail(KAPRE_E_INVALID, "cqt: hop_length %d must be a multiple of 2^(octaves - 1) = %d",
+                       cfg->hop_length, 1 << (n_oct - 1));
+    for (int i = 0; i < n_oct; ++i)
+        if (cfg->taps[i] < 1 || cfg->taps[i] > KAPRE_CQT_MAX_TAPS)
+            return kb_fail(cfg->taps[i] < 1 ? KAPRE_E_INVALID : KAPRE_E_UNSUPPORTED,
+                           "cqt: octave %d's filters of %d taps exceed the limit of %d taps", i, cfg->taps[i],
+                           KAPRE_CQT_MAX_TAPS);
+    kapre_cqt_plan* pl = new kapre_cqt_plan();
+    pl->cfg = *cfg;
+    std::vector<float2> tab, btab;
+    const int bad = kb_cqt_build(cfg->n_bins, cfg->bins_per_octave, cfg->hop_length, cfg->taps, taps_host, pl->geo,
+                                 tab, btab);
+    int rc = 0;
+    if (bad) {
+        delete pl;
+        return kb_fail(KAPRE_E_UNSUPPORTED, "cqt: octave %d takes the transform past the kernel's limit of %d (octave, bin "
+                       "group) segments (a group holds the bins whose taps fit %d B)", bad - 1, KB_CQT_MAX_SEGS,
+                       KB_CQT_TAB_BYTES);
+    }
+    for (const float2& v : tab)
+        if (!std::isfinite(v.x) || !std::isfinite(v.y)) { delete pl; return kb_fail(KAPRE_E_INVALID, "cqt: non-finite tap"); }
+    if ((rc = kb_dev_info(&pl->dev)) || (rc = kb_upload(tab, &pl->tab)) || (rc = kb_upload(btab, &pl->btab)) ||
+        (rc = kapre_resample_plan_create(1, 2, decim_taps_host, n_decim_taps, &pl->rs))) {
+        kapre_cqt_plan_destroy(pl);
+        return rc;
+    }
+    *out = pl;
+    return 0;
+}
+
+void kapre_cqt_plan_destroy(kapre_cqt_plan* plan) {
+    if (!plan) return;
+    cudaFree(plan->tab);
+    cudaFree(plan->btab);
+    kapre_resample_plan_destroy(plan->rs);
+    delete plan;
+}
+
+int kapre_cqt_num_frames(const kapre_cqt_plan* plan, int length) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (length < 0) return kb_fail(KAPRE_E_INVALID, "negative length");
+    return 1 + length / plan->cfg.hop_length;
+}
+
+int64_t kapre_cqt_workspace_bytes(const kapre_cqt_plan* plan, int batch, int channels, int length, int backward) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (batch < 0 || channels < 0 || length < 0) return kb_fail(KAPRE_E_INVALID, "cqt: negative size");
+    if ((double)batch * channels * (length + 1.0) * 3.0 > 4.0e18) return kb_fail(KAPRE_E_INVALID, "cqt: size overflow");
+    int64_t a[KB_CQT_MAX_OCT], b[KB_CQT_MAX_OCT], c[KB_CQT_MAX_OCT];
+    return kb_cqt_layout(plan->geo.n_oct, (long long)batch * channels, length, backward ? 1 : 0, a, b, c);
+}
+
+int kapre_cqt(const kapre_cqt_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, int magnitude,
+              void* out_dev, const kapre_spec_desc* out_desc, void* workspace_dev, void* stream) {
+    int rc = kb_cqt_check_shape(plan, x_desc);
+    if (rc) return rc;
+    if (!out_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (magnitude != 0 && magnitude != 1) return kb_fail(KAPRE_E_INVALID, "cqt: magnitude must be 0 or 1");
+    if ((long long)x_desc->batch * x_desc->channels == 0) return 0;
+    if (!x_dev || !out_dev || (plan->geo.n_oct > 1 && !workspace_dev)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    KbCqtParams p = kb_cqt_params(plan, x_dev, x_desc, (float*)workspace_dev);
+    p.n_threads = KB_CQT_THREADS;
+    p.mag = magnitude;
+    p.out = out_dev; p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t;
+    p.o_sk = out_desc->stride_f;
+    if (!kb_cqt_setup(p)) return kb_fail(KAPRE_E_INVALID, "cqt: too many tiles");
+    const cudaStream_t st = (cudaStream_t)stream;
+    for (int i = 1; i < p.n_oct; ++i) {
+        const KbCqtOct& a = p.oct[i - 1];
+        const kapre_wave_desc ad = i == 1 ? *x_desc : kb_cqt_level_desc(p.B, p.C, a.L);
+        const kapre_wave_desc yd = kb_cqt_level_desc(p.B, p.C, p.oct[i].L);
+        if (yd.length == 0) continue;
+        if ((rc = kb_resample_launch(plan->rs, a.y, &ad, const_cast<float*>(p.oct[i].y), &yd, stream))) return rc;
+    }
+    int grid;
+    if ((rc = kb_resident_grid(kb_cqt_fwd_kernel, "cqt_fwd", KB_CQT_THREADS, KB_CQT_FWD_SMEM, p.jobs,
+                               plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_cqt_fwd_kernel, {.grid = grid, .block = KB_CQT_THREADS, .smem = KB_CQT_FWD_SMEM, .st = st,
+                                         .timed = true}, p);
+}
+
+int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc,
+                       const void* fwd_workspace_dev, const void* g_dev, const kapre_spec_desc* g_desc, int magnitude,
+                       float* gx_dev, const kapre_wave_desc* gx_desc, void* workspace_dev, void* stream) {
+    int rc = kb_cqt_check_shape(plan, x_desc);
+    if (rc) return rc;
+    if (!g_desc || !gx_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (magnitude != 0 && magnitude != 1) return kb_fail(KAPRE_E_INVALID, "cqt: magnitude must be 0 or 1");
+    if (gx_desc->batch != x_desc->batch || gx_desc->channels != x_desc->channels || gx_desc->length != x_desc->length)
+        return kb_fail(KAPRE_E_INVALID, "cqt: the gradient needs the waveform's shape");
+    const long long bc = (long long)x_desc->batch * x_desc->channels;
+    if (bc * x_desc->length == 0) return 0;
+    const int n_oct = plan->geo.n_oct;
+    if (!g_dev || !gx_dev || (n_oct > 1 && !workspace_dev) || (magnitude && (!x_dev || (n_oct > 1 && !fwd_workspace_dev))))
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    KbCqtParams p = kb_cqt_params(plan, x_dev, x_desc, (float*)const_cast<void*>(fwd_workspace_dev));
+    p.n_threads = KB_CQT_BWD_THREADS;
+    p.mag = magnitude;
+    p.g = g_dev; p.g_sb = g_desc->stride_b; p.g_sc = g_desc->stride_c; p.g_st = g_desc->stride_t;
+    p.g_sk = g_desc->stride_f;
+    int64_t lvl[KB_CQT_MAX_OCT], glvl[KB_CQT_MAX_OCT], rlvl[KB_CQT_MAX_OCT];
+    kb_cqt_layout(n_oct, bc, x_desc->length, 1, lvl, glvl, rlvl);
+    float* ws = (float*)workspace_dev;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int smem = kb_cqt_bwd_smem();
+    // lowest octave first: g_i = adjoint_i(G) + R^T g_{i+1}
+    for (int i = n_oct - 1; i >= 0; --i) {
+        const KbCqtOct& o = p.oct[i];
+        if (o.L == 0) continue;
+        p.bo = i;
+        p.add = nullptr;
+        if (i + 1 < n_oct && p.oct[i + 1].L > 0) {
+            const kapre_wave_desc gd = kb_cqt_level_desc(p.B, p.C, p.oct[i + 1].L);
+            const kapre_wave_desc rd = kb_cqt_level_desc(p.B, p.C, o.L);
+            if ((rc = kapre_resample_backward(plan->rs, ws + glvl[i + 1], &gd, ws + rlvl[i], &rd, stream))) return rc;
+            p.add = ws + rlvl[i];
+        }
+        if (i == 0) { p.gy = gx_dev; p.gy_sb = gx_desc->stride_b; p.gy_sc = gx_desc->stride_c; p.gy_sl = gx_desc->stride_l; }
+        else { p.gy = ws + glvl[i]; p.gy_sb = (long long)p.C * o.L; p.gy_sc = o.L; p.gy_sl = 1; }
+        const long long tiles = bc * ((o.L + o.TS - 1) / o.TS);
+        int grid;
+        if ((rc = kb_resident_grid(kb_cqt_bwd_kernel, "cqt_bwd", KB_CQT_BWD_THREADS, smem, tiles, plan->dev.sm_count,
+                                   &grid)))
+            return rc;
+        if ((rc = kb_launch(kb_cqt_bwd_kernel, {.grid = grid, .block = KB_CQT_BWD_THREADS, .smem = smem, .st = st}, p)))
+            return rc;
+    }
+    return 0;
 }
 
 }  // extern "C"

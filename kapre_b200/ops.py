@@ -1774,3 +1774,83 @@ def kaldi_features(x, plan: KaldiPlan, lengths=None, data_format=_CH_LAST_STR, d
         from . import autograd
         return autograd.kaldi_features(x, plan, lh, ld, data_format, dither, seed)
     return kaldi_forward(x, plan, lh, ld, data_format, dither, seed)
+
+
+# ------------------------------------------------------------------------------- constant-Q transform
+class CqtPlan(_PerDevice):
+    """kapre_cqt_plan per CUDA device for one CQT configuration: the per-octave tap tables (``backend.cqt_filters``,
+    float64, rounded here once to complex64) and the 2:1 decimation filter ``resample_filter(1, 2)``."""
+
+    def __init__(self, sample_rate, hop_length, f_min=None, n_bins=84, bins_per_octave=12, filter_scale=1.0,
+                 gamma=0.0, scale=True):
+        from . import backend
+        from .signal import resample_filter
+        self.geometry = backend.cqt_geometry(sample_rate, hop_length, f_min, n_bins, bins_per_octave, filter_scale,
+                                             gamma)
+        self.hop_length, self.n_bins, self.bins_per_octave = int(hop_length), int(n_bins), int(bins_per_octave)
+        self.n_octaves = self.geometry['n_octaves']
+        self.tables = [t.astype(np.complex64) for t in backend.cqt_filters(sample_rate, f_min, n_bins, bins_per_octave,
+                                                                           filter_scale, gamma, scale)]
+        self.decimator = resample_filter(1, 2)
+        taps = [t.shape[1] for t in self.tables] + [0] * (N.CQT_MAX_OCTAVES - len(self.tables))
+        self.cfg = N.CqtCfg(self.n_bins, self.bins_per_octave, self.hop_length, (ctypes.c_int * N.CQT_MAX_OCTAVES)(*taps))
+        self._flat = np.ascontiguousarray(np.concatenate([t.reshape(-1) for t in self.tables]))
+        self._per_device = {}
+
+    _destroy = 'kapre_cqt_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_cqt_plan_create(ctypes.byref(self.cfg), self._flat.ctypes.data_as(ctypes.c_void_p),
+                                         self.decimator.ctypes.data_as(ctypes.c_void_p), self.decimator.size, out)
+
+    def num_frames(self, length):
+        return 1 + int(length) // self.hop_length
+
+    def workspace(self, B, C, L, backward, device):
+        n = int(N.lib().kapre_cqt_workspace_bytes(self.handle(), B, C, L, int(backward)))
+        if n < 0:
+            N.check(n)
+        return torch.empty(max((n + 3) // 4, 1), dtype=torch.float32, device=device)
+
+
+def cqt_forward(x, plan: CqtPlan, input_data_format, output_data_format, magnitude):
+    """(B, L, C) / (B, C, L) float32 -> (B, M, n_bins, C) / (B, C, M, n_bins) complex64 (or float32 |C|), and the
+    workspace holding the pyramid: n_octaves - 1 resampling launches and one transform launch."""
+    x = _raw(x.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, input_data_format)
+    out, od = _spec_alloc(B, C, plan.num_frames(L), plan.n_bins, output_data_format,
+                          torch.float32 if magnitude else torch.complex64, x.device)
+    ws = plan.workspace(B, C, L, False, x.device)
+    if out.numel():
+        N.check(N.lib().kapre_cqt(plan.handle(), _ptr(x), ctypes.byref(xd), int(bool(magnitude)), _ptr(out),
+                                  ctypes.byref(od), _ptr(ws), _stream_ptr()))
+    return out, ws
+
+
+def cqt_backward(g, x, fwd_ws, plan: CqtPlan, input_data_format, output_data_format, magnitude):
+    """Gradient of ``cqt_forward`` to x: 2 n_octaves - 1 launches.  ``fwd_ws``: the forward's pyramid (magnitude mode)."""
+    g = _raw(g.to(torch.float32 if magnitude else torch.complex64))
+    x = _raw(x.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, input_data_format)
+    gd, _ = _spec_desc(g, output_data_format)
+    gx, gxd = _wave_alloc(B, C, L, input_data_format, x.device)
+    if gx.numel():
+        ws = plan.workspace(B, C, L, True, x.device)
+        N.check(N.lib().kapre_cqt_backward(plan.handle(), _ptr(x), ctypes.byref(xd),
+                                           _ptr(fwd_ws) if fwd_ws is not None else None, _ptr(g), ctypes.byref(gd),
+                                           int(bool(magnitude)), _ptr(gx), ctypes.byref(gxd), _ptr(ws), _stream_ptr()))
+    return gx
+
+
+@_device_of_first_arg
+def cqt(x, plan: CqtPlan, input_data_format=_CH_LAST_STR, output_data_format=_CH_LAST_STR, magnitude=False):
+    """Constant-Q transform of a float32 CUDA waveform batch under ``plan`` (see ``time_frequency.CQT``).
+    Differentiable with respect to x; requiring grad changes neither the bits nor the launch count."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise N.KapreNativeError('cqt needs a CUDA waveform')
+    if x.dim() != 3:
+        raise ValueError('cqt expects a 3-D waveform batch, got shape %s' % (tuple(x.shape),))
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.cqt(x, plan, input_data_format, output_data_format, magnitude)
+    return cqt_forward(x, plan, input_data_format, output_data_format, magnitude)[0]

@@ -23,7 +23,7 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
 __all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
-           'PCEN', 'GriffinLim', 'InverseFilterbank', 'KaldiFbank', 'KaldiMFCC', 'KaldiSpectrogram']
+           'PCEN', 'GriffinLim', 'InverseFilterbank', 'KaldiFbank', 'KaldiMFCC', 'KaldiSpectrogram', 'CQT']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -699,3 +699,60 @@ class KaldiSpectrogram(_KaldiLayer):
     """``torchaudio.compliance.kaldi.spectrogram`` per (item, channel): ``padded_window_size // 2 + 1`` bins per
     frame."""
     _kind = 'spectrogram'
+
+
+@register_keras_serializable(package='Kapre')
+class CQT(Layer):
+    """Constant-Q transform, modelled on librosa's multirate ``cqt`` (``gamma > 0``: ``vqt``).
+
+    ``(batch, time, ch)`` / ``(batch, ch, time)`` float32 waveforms -> complex64 ``(batch, frames, n_bins, ch)`` /
+    ``(batch, ch, frames, n_bins)``, bins in ascending frequency, ``frames = 1 + time // hop_length``, frame m centred on
+    sample ``m hop_length``.  Bin k has centre ``f_k = f_min 2^(k / bins_per_octave)`` (``f_min`` default C1) and a
+    periodic-Hann complex filter of ``l_k = Q sample_rate / (f_k + gamma / alpha)`` samples, ``Q = filter_scale /
+    alpha``, ``alpha = (r^2 - 1) / (r^2 + 1)``, ``r = 2^(1 / bins_per_octave)``, with unit L1 norm; outputs are scaled
+    by ``sqrt(l_k)`` (``scale=True``) or ``l_k``.  Each octave is computed at its own rate on a 2:1 polyphase pyramid
+    (``scipy.signal.resample_poly(y, 1, 2)``), as an exact time-domain inner product per output.  The decimator's
+    response is within 0.25 % of 1 up to 0.2 cycles per sample and below -56 dB from 0.3 on, and every octave's
+    bins sit in the same digital band, so with the top band below 0.4 ``sample_rate`` the lower octaves see its flat
+    passband.  ``hop_length`` must be a multiple of ``2^(n_octaves - 1)``.  Followed by ``Magnitude()`` in a
+    ``Sequential`` it runs as one fused launch writing ``|C|``."""
+
+    def __init__(self, sample_rate=22050, hop_length=512, f_min=None, n_bins=84, bins_per_octave=12, filter_scale=1.0,
+                 gamma=0.0, scale=True, input_data_format='default', output_data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        for data_format in (input_data_format, output_data_format):
+            backend.validate_data_format_str(data_format)
+        input_data_format = _unwrap_format(input_data_format)
+        output_data_format = _unwrap_format(output_data_format)
+        backend.cqt_geometry(sample_rate, hop_length, f_min, n_bins, bins_per_octave, filter_scale, gamma)
+        self.sample_rate, self.hop_length, self.f_min = sample_rate, hop_length, f_min
+        self.n_bins, self.bins_per_octave = n_bins, bins_per_octave
+        self.filter_scale, self.gamma, self.scale = filter_scale, gamma, scale
+        self.input_data_format_original = input_data_format
+        self.output_data_format_original = output_data_format
+        self.input_data_format = _resolve(input_data_format)
+        self.output_data_format = _resolve(output_data_format)
+        self._plan = None
+
+    @property
+    def plan(self) -> ops.CqtPlan:
+        if self._plan is None:
+            self._plan = ops.CqtPlan(self.sample_rate, self.hop_length, self.f_min, self.n_bins, self.bins_per_octave,
+                                     self.filter_scale, self.gamma, self.scale)
+        return self._plan
+
+    def call(self, x, magnitude=False):
+        return ops.cqt(x, self.plan, self.input_data_format, self.output_data_format, magnitude)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'),
+        ('hop_length', 'hop_length'),
+        ('f_min', 'f_min'),
+        ('n_bins', 'n_bins'),
+        ('bins_per_octave', 'bins_per_octave'),
+        ('filter_scale', 'filter_scale'),
+        ('gamma', 'gamma'),
+        ('scale', 'scale'),
+        ('input_data_format', 'input_data_format_original'),
+        ('output_data_format', 'output_data_format_original'),
+    )
