@@ -544,6 +544,61 @@ int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kap
                        const void* fwd_workspace_dev, const void* g_dev, const kapre_spec_desc* g_desc, int magnitude,
                        float* gx_dev, const kapre_wave_desc* gx_desc, void* workspace_dev, void* stream);
 
+/* ---- pitch tracking: YIN and probabilistic YIN (modelled on librosa's yin / pyin) -----------------------------------
+ * Frame m of each (item, channel) row holds the samples [m hop - pad, m hop - pad + frame_length), pad =
+ * frame_length / 2 with `center` (zeros outside the signal), m < kapre_pitch_num_frames.  With x the frame and W the
+ * window, d(tau) = sum_{j=1..W} (x[j] - x[j + tau])^2 and the CMNDF c(tau) = d(tau) / (mean_{k<=tau} d(k) + 2^-126)
+ * for min_period <= tau <= max_period.  Every output's bits depend on (item, channel, frame) alone. */
+#define KAPRE_PITCH_MAX_FRAME 8192
+#define KAPRE_PITCH_MAX_THRESHOLDS 1024
+#define KAPRE_PITCH_MAX_BINS 8192
+#define KAPRE_PITCH_MAX_BAND 8192
+typedef struct {
+    float sample_rate;
+    int frame_length, win_length, hop_length, center;
+    int min_period, max_period;           /* 1 <= min_period, min_period + 2 <= max_period < frame_length - win_length */
+    double trough_threshold;              /* YIN */
+    /* pYIN (kapre_pyin only) */
+    int n_thresholds, n_pitch, band_width;
+    float log_stay, log_switch;           /* log(1 - switch_prob), log(switch_prob) */
+    float log_init_voiced, log_init_unvoiced;
+    float fill_na;
+} kapre_pitch_config;
+/* float64 host tables of pYIN (rounded to float32 on upload, except the edges).  cmax = (n + 1) / 2, n =
+ * max_period - min_period + 1, is the most troughs a frame can hold. */
+typedef struct {
+    const double* beta_probs;             /* n_thresholds: Bcdf(i / n) - Bcdf((i - 1) / n), i = 1 .. n */
+    const double* boltzmann_pow;          /* cmax + 1: e^{-lambda r} */
+    const double* boltzmann_norm;         /* cmax + 1: (1 - e^{-lambda}) / (1 - e^{-lambda N}) (entry 0 unused) */
+    const double* no_trough_bonus;        /* n_thresholds + 1: no_trough_prob (beta_1 + ... + beta_k) */
+    const double* period_edges;           /* n_pitch - 1: the period at the upper edge of bin m (descending) */
+    const double* freqs;                  /* n_pitch: the bins' frequencies */
+    const double* log_triangle;           /* band_width: log of the triangle taps */
+    const double* log_row_norm;           /* n_pitch: -log(sum of row i's taps inside [0, n_pitch)) */
+} kapre_pitch_tables;
+/* Element strides (batch, channel, frame) of a per-frame output. */
+typedef struct {
+    int64_t stride_b, stride_c, stride_t;
+} kapre_frames_desc;
+typedef struct kapre_pitch_plan kapre_pitch_plan;
+/* tables = NULL: a YIN-only plan.  KAPRE_E_UNSUPPORTED past the KAPRE_PITCH_MAX_* limits. */
+int kapre_pitch_plan_create(const kapre_pitch_config* cfg, const kapre_pitch_tables* tables, kapre_pitch_plan** out);
+void kapre_pitch_plan_destroy(kapre_pitch_plan* plan);
+/* max(0, 1 + (length + 2 pad - frame_length) / hop_length) (< 0 on a negative length). */
+int kapre_pitch_num_frames(const kapre_pitch_plan* plan, int length);
+/* Device scratch of kapre_pyin: the candidate lists and the Viterbi backpointers (2 n_pitch uint16 per frame). */
+int64_t kapre_pitch_workspace_bytes(const kapre_pitch_plan* plan, int batch, int channels, int length);
+/* f0 = sr / (min_period + k + shift) of YIN's trough k (first below trough_threshold, else the first global minimum),
+ * NaN on frames holding a non-finite sample.  cmndf_dev (nullable): c(min_period + k) at (b, c, frame, k).  One launch. */
+int kapre_yin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* f0_dev,
+              const kapre_frames_desc* f0_desc, float* cmndf_dev, const kapre_spec_desc* cmndf_desc, void* stream);
+/* pYIN's Viterbi-decoded f0 (fill_na on unvoiced frames), voiced flag (uint8) and voiced probability, all three with
+ * the strides of out_desc.  A row with a non-finite sample in any frame gives fill_na, 0 and NaN throughout.  Two
+ * launches. */
+int kapre_pyin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* f0_dev,
+               uint8_t* voiced_flag_dev, float* voiced_prob_dev, const kapre_frames_desc* out_desc, float* cmndf_dev,
+               const kapre_spec_desc* cmndf_desc, void* workspace_dev, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

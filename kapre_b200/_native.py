@@ -83,6 +83,23 @@ class CqtCfg(Structure):
                 ('taps', c_int * CQT_MAX_OCTAVES)]
 
 
+class PitchCfg(Structure):
+    _fields_ = [('sample_rate', c_float), ('frame_length', c_int), ('win_length', c_int), ('hop_length', c_int),
+                ('center', c_int), ('min_period', c_int), ('max_period', c_int), ('trough_threshold', ctypes.c_double),
+                ('n_thresholds', c_int), ('n_pitch', c_int), ('band_width', c_int), ('log_stay', c_float),
+                ('log_switch', c_float), ('log_init_voiced', c_float), ('log_init_unvoiced', c_float),
+                ('fill_na', c_float)]
+
+
+class PitchTables(Structure):
+    _fields_ = [(name, c_void_p) for name in ('beta_probs', 'boltzmann_pow', 'boltzmann_norm', 'no_trough_bonus',
+                                              'period_edges', 'freqs', 'log_triangle', 'log_row_norm')]
+
+
+class FramesDesc(Structure):
+    _fields_ = [('stride_b', c_int64), ('stride_c', c_int64), ('stride_t', c_int64)]
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -188,6 +205,14 @@ SYMBOLS = [
     ('kapre_cqt', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_int, c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),
     ('kapre_cqt_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, c_void_p, POINTER(SpecDesc), c_int,
                                    c_void_p, POINTER(WaveDesc), c_void_p, c_void_p]),
+    ('kapre_pitch_plan_create', c_int, [POINTER(PitchCfg), POINTER(PitchTables), POINTER(c_void_p)]),
+    ('kapre_pitch_plan_destroy', None, [c_void_p]),
+    ('kapre_pitch_num_frames', c_int, [c_void_p, c_int]),
+    ('kapre_pitch_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int]),
+    ('kapre_yin', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, POINTER(FramesDesc), c_void_p,
+                          POINTER(SpecDesc), c_void_p]),
+    ('kapre_pyin', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, c_void_p, c_void_p, POINTER(FramesDesc),
+                           c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

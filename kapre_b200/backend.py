@@ -7,6 +7,7 @@ Same public names, argument meaning and error behaviour as the reference
 """
 from __future__ import annotations
 
+import math
 from typing import Callable, Optional, Union
 
 import numpy as np
@@ -498,3 +499,173 @@ def cqt_filters(sample_rate, f_min=None, n_bins=84, bins_per_octave=12, filter_s
             T[kk, half - N // 2:half - N // 2 + N] = s * np.conj(psi)
         out.append(T)
     return out
+
+
+# ---- pitch tracking (YIN / pYIN) --------------------------------------------------------------------------------
+PITCH_MAX_FRAME = 8192          # KAPRE_PITCH_MAX_FRAME: the staged frame and its CMNDF fit one CTA
+PITCH_MAX_THRESHOLDS = 1024     # KAPRE_PITCH_MAX_THRESHOLDS
+PITCH_MAX_BINS = 8192           # KAPRE_PITCH_MAX_BINS: the Viterbi scores of 2 n_pitch states fit shared memory
+PITCH_MAX_BAND = 8192           # KAPRE_PITCH_MAX_BAND
+PITCH_TINY = 2.0 ** -126
+
+
+def _positive(name, v, integer=False):
+    if isinstance(v, bool) or not np.isfinite(float(v)) or float(v) <= 0:
+        raise ValueError('%s must be positive, got %r' % (name, v))
+    if integer and int(v) != v:
+        raise ValueError('%s must be an integer, got %r' % (name, v))
+
+
+def pitch_geometry(sample_rate, fmin, fmax, frame_length=2048, win_length=None, hop_length=None, center=True):
+    """Validated framing of YIN / pYIN: dict with ``frame_length``, ``win_length``, ``hop_length``, ``pad`` (leading
+    zeros), ``min_period = floor(sr / fmax)``, ``max_period = min(ceil(sr / fmin), frame_length - win_length - 1)``
+    and ``n_lags``.  Raises ValueError on a configuration the kernels reject."""
+    _positive('sample_rate', sample_rate)
+    _positive('frame_length', frame_length, True)
+    F = int(frame_length)
+    W = F // 2 if win_length is None else win_length
+    h = F // 4 if hop_length is None else hop_length
+    _positive('win_length', W, True)
+    _positive('hop_length', h, True)
+    W, h = int(W), int(h)
+    for name, v in (('fmin', fmin), ('fmax', fmax)):
+        if isinstance(v, bool) or not np.isfinite(float(v)):
+            raise ValueError('%s must be finite, got %r' % (name, v))
+    sr, fmin, fmax = float(sample_rate), float(fmin), float(fmax)
+    if fmin <= 0:
+        raise ValueError('fmin must be positive, got %r' % fmin)
+    if fmin >= fmax:
+        raise ValueError('fmin %r must be below fmax %r' % (fmin, fmax))
+    if fmax > sr / 2:
+        raise ValueError('fmax %r is above the Nyquist frequency %r' % (fmax, sr / 2))
+    if not isinstance(center, (bool, np.bool_)):
+        raise ValueError('center must be a bool, got %r' % (center,))
+    if W >= F:
+        raise ValueError('win_length %d must be below frame_length %d' % (W, F))
+    if F > PITCH_MAX_FRAME:
+        raise ValueError('frame_length %d exceeds the kernel limit of %d samples' % (F, PITCH_MAX_FRAME))
+    min_p = int(np.floor(sr / fmax))
+    max_p = min(int(np.ceil(sr / fmin)), F - W - 1)
+    if min_p < 1:
+        raise ValueError('min_period floor(sr / fmax) = %d is below 1' % min_p)
+    if max_p - min_p + 1 < 3:
+        raise ValueError('the lag range [%d, %d] holds fewer than 3 lags: lower fmin or win_length, raise fmax or '
+                         'frame_length' % (min_p, max_p))
+    return dict(frame_length=F, win_length=W, hop_length=h, pad=F // 2 if center else 0, center=bool(center),
+                min_period=min_p, max_period=max_p, n_lags=max_p - min_p + 1, sample_rate=sr, fmin=fmin, fmax=fmax)
+
+
+def beta_cdf(x, a, b):
+    """Regularised incomplete beta function I_x(a, b) in float64 (the Beta(a, b) CDF), by the continued fraction of
+    the incomplete beta function (modified Lentz), on the side where it converges fast."""
+    x = np.asarray(x, dtype=np.float64)
+    a, b = float(a), float(b)
+    lbeta = math.lgamma(a) + math.lgamma(b) - math.lgamma(a + b)
+
+    def cf(x, a, b):
+        tiny = 1e-300
+        c, d = 1.0, 1.0 - (a + b) * x / (a + 1.0)
+        d = 1.0 / (d if abs(d) > tiny else tiny)
+        f = d
+        for m in range(1, 10000):
+            m2 = 2 * m
+            num = m * (b - m) * x / ((a + m2 - 1.0) * (a + m2))
+            for k in (0, 1):
+                d = 1.0 + num * d
+                d = 1.0 / (d if abs(d) > tiny else tiny)
+                c = 1.0 + num / c
+                c = c if abs(c) > tiny else tiny
+                f *= c * d
+                if k == 0:
+                    num = -(a + m) * (a + b + m) * x / ((a + m2) * (a + m2 + 1.0))
+            if abs(c * d - 1.0) < 1e-16:
+                break
+        return f
+
+    out = np.empty(x.shape, dtype=np.float64)
+    for idx, v in np.ndenumerate(x):
+        v = float(v)
+        if v <= 0.0:
+            out[idx] = 0.0
+        elif v >= 1.0:
+            out[idx] = 1.0
+        else:
+            front = math.exp(a * math.log(v) + b * math.log1p(-v) - lbeta)
+            if v < (a + 1.0) / (a + b + 2.0):
+                out[idx] = front * cf(v, a, b) / a
+            else:
+                out[idx] = 1.0 - front * cf(1.0 - v, b, a) / b
+    return out
+
+
+def triangle_window(w):
+    """``scipy.signal.windows.triang(w)`` (symmetric) in numpy."""
+    w = int(w)
+    n = np.arange(1, (w + 1) // 2 + 1, dtype=np.float64)
+    half = 2.0 * n / (w + 1.0) if w % 2 else (2.0 * n - 1.0) / w
+    return np.concatenate([half, half[-2::-1]]) if w % 2 else np.concatenate([half, half[::-1]])
+
+
+def pyin_geometry(geometry, n_thresholds=100, beta_parameters=(2, 18), boltzmann_parameter=2, resolution=0.1,
+                  max_transition_rate=35.92, switch_prob=0.01, no_trough_prob=0.01):
+    """pYIN's sizes on top of ``pitch_geometry``: ``bins_per_semitone = ceil(1 / resolution)``, ``n_pitch``, the
+    transition band width ``band_width = round(max_transition_rate 12 h / sr) bins_per_semitone + 1`` and ``n_states
+    = 2 n_pitch``.  Raises ValueError on parameters the kernels reject."""
+    _positive('n_thresholds', n_thresholds, True)
+    _positive('resolution', resolution)
+    _positive('max_transition_rate', max_transition_rate)
+    _positive('boltzmann_parameter', boltzmann_parameter)
+    if len(beta_parameters) != 2:
+        raise ValueError('beta_parameters must be a pair, got %r' % (beta_parameters,))
+    for v in beta_parameters:
+        _positive('beta_parameters', v)
+    for name, v in (('switch_prob', switch_prob), ('no_trough_prob', no_trough_prob)):
+        if isinstance(v, bool) or not (0.0 <= float(v) <= 1.0):
+            raise ValueError('%s must lie in [0, 1], got %r' % (name, v))
+    if resolution >= 1:
+        raise ValueError('resolution must be below 1 semitone, got %r' % (resolution,))
+    if int(n_thresholds) > PITCH_MAX_THRESHOLDS:
+        raise ValueError('%d thresholds exceed the kernel limit of %d' % (n_thresholds, PITCH_MAX_THRESHOLDS))
+    g = geometry
+    bps = int(np.ceil(1.0 / float(resolution)))
+    n_pitch = int(np.floor(12 * bps * np.log2(g['fmax'] / g['fmin']))) + 1
+    band = int(np.round(float(max_transition_rate) * 12 * g['hop_length'] / g['sample_rate'])) * bps + 1
+    if 2 * n_pitch > 65535:
+        raise ValueError('%d HMM states exceed the 65535 that uint16 backpointers address' % (2 * n_pitch))
+    if n_pitch > PITCH_MAX_BINS:
+        raise ValueError('%d pitch bins exceed the kernel limit of %d: raise resolution or narrow [fmin, fmax]'
+                         % (n_pitch, PITCH_MAX_BINS))
+    if band > PITCH_MAX_BAND:
+        raise ValueError('a transition band of %d bins exceeds the kernel limit of %d' % (band, PITCH_MAX_BAND))
+    return dict(n_thresholds=int(n_thresholds), beta_parameters=tuple(float(v) for v in beta_parameters),
+                boltzmann_parameter=float(boltzmann_parameter), bins_per_semitone=bps, n_pitch=n_pitch,
+                band_width=band, n_states=2 * n_pitch, switch_prob=float(switch_prob),
+                no_trough_prob=float(no_trough_prob))
+
+
+def pyin_tables(geometry, pyin):
+    """float64 tables of pYIN (see kapre_pitch_tables in include/kapre_b200.h) as a dict of arrays."""
+    g, q = geometry, pyin
+    nt = q['n_thresholds']
+    cdf = beta_cdf(np.arange(nt + 1, dtype=np.float64) / nt, *q['beta_parameters'])
+    beta = np.diff(cdf)
+    cmax = (g['n_lags'] + 1) // 2
+    lam = q['boltzmann_parameter']
+    r = np.arange(cmax + 1, dtype=np.float64)
+    bpow = np.exp(-lam * r)
+    bnorm = np.zeros(cmax + 1)
+    bnorm[1:] = -np.expm1(-lam) / -np.expm1(-lam * r[1:])
+    bonus = q['no_trough_prob'] * np.concatenate([[0.0], np.cumsum(beta)])
+    B = 12 * q['bins_per_semitone']
+    m = np.arange(q['n_pitch'], dtype=np.float64)
+    freqs = g['fmin'] * 2.0 ** (m / B)
+    edges = g['sample_rate'] / (g['fmin'] * 2.0 ** ((m[:-1] + 0.5) / B))
+    w = q['band_width']
+    tri = triangle_window(w)
+    n = q['n_pitch']
+    rows = np.zeros(n)
+    for i in range(n):
+        j0, j1 = max(0, i - w // 2), min(n, i - w // 2 + w)
+        rows[i] = tri[j0 - i + w // 2:j1 - i + w // 2].sum()
+    return dict(beta_probs=beta, boltzmann_pow=bpow, boltzmann_norm=bnorm, no_trough_bonus=bonus,
+                period_edges=edges, freqs=freqs, log_triangle=np.log(tri), log_row_norm=-np.log(rows))

@@ -37,6 +37,7 @@
 #include "kaldi_core.cuh"
 #include "loudness_core.cuh"
 #include "cqt_core.cuh"
+#include "pitch_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -3800,6 +3801,236 @@ int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kap
             return rc;
     }
     return 0;
+}
+
+}  // extern "C"
+
+// ---- pitch tracking (pitch_core.cuh) ------------------------------------------------------------------------------
+__global__ void __launch_bounds__(KB_PITCH_THREADS) kb_pitch_kernel(const __grid_constant__ KbPitchParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_pitch_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_VIT_THREADS) kb_viterbi_kernel(const __grid_constant__ KbVitParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_vit_cta(p, kb_smem, reinterpret_cast<float*>(kb_smem) + 6 * p.n + p.w + 4, blockIdx.x, gridDim.x);
+}
+
+struct kapre_pitch_plan {
+    kapre_pitch_config cfg;
+    KbPitchParams geo;                      // tiling and tables (per-call fields unset)
+    KbVitParams vit;
+    DevInfo dev;
+    std::vector<void*> bufs;                // device tables
+};
+
+template <typename T>
+static int kb_pitch_upload(kapre_pitch_plan* pl, const double* src, size_t n, const T** dst) {
+    std::vector<T> h(n);
+    for (size_t i = 0; i < n; ++i) {
+        h[i] = (T)src[i];
+        if (!std::isfinite((double)h[i])) return kb_fail(KAPRE_E_INVALID, "pitch: non-finite table entry");
+    }
+    T* d = nullptr;
+    int rc = kb_upload(h, &d);
+    if (d) pl->bufs.push_back(d);
+    *dst = d;
+    return rc;
+}
+
+static int kb_pitch_frames(const kapre_pitch_config& c, long long length) {
+    const long long lp = length + (c.center ? 2LL * (c.frame_length / 2) : 0);
+    return lp < c.frame_length ? 0 : (int)(1 + (lp - c.frame_length) / c.hop_length);
+}
+
+static int kb_pitch_check_shape(const kapre_pitch_plan* plan, const kapre_wave_desc* xd) {
+    if (!plan || !xd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (xd->batch < 0 || xd->channels < 0 || xd->length < 0)
+        return kb_fail(KAPRE_E_INVALID, "pitch: negative size (%d, %d, %d)", xd->batch, xd->channels, xd->length);
+    int cur = -1;
+    KB_CUDA(cudaGetDevice(&cur));
+    if (cur != plan->dev.device)
+        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    return 0;
+}
+
+// The difference-function launch of kapre_yin (pyin = 0) and kapre_pyin.
+static int kb_pitch_launch(const kapre_pitch_plan* plan, const float* x, const kapre_wave_desc* xd, float* out,
+                           const kapre_frames_desc* od, float* cm, const kapre_spec_desc* cd, void* ws, cudaStream_t st) {
+    KbPitchParams p = plan->geo;
+    p.B = xd->batch; p.C = xd->channels; p.L = xd->length;
+    p.M = kb_pitch_frames(plan->cfg, xd->length);
+    p.x = x; p.x_sb = xd->stride_b; p.x_sc = xd->stride_c; p.x_sl = xd->stride_l;
+    p.out = out; p.o_sb = od->stride_b; p.o_sc = od->stride_c; p.o_st = od->stride_t;
+    p.cm = cm;
+    if (cm) { p.c_sb = cd->stride_b; p.c_sc = cd->stride_c; p.c_st = cd->stride_t; p.c_sk = cd->stride_f; }
+    if (p.pyin) {
+        const long long fr = (long long)p.B * p.C * p.M;
+        char* w = (char*)ws;
+        p.cand_n = (int*)w;
+        p.cand_p = (float*)(w + (fr * 4 + 255) / 256 * 256);
+        p.cand_bin = (unsigned short*)((char*)p.cand_p + (fr * p.cmax * 4 + 255) / 256 * 256);
+    }
+    if (!kb_pitch_setup(p)) return kb_fail(KAPRE_E_INVALID, "pitch: too many tiles");
+    int grid, rc;
+    if ((rc = kb_resident_grid(kb_pitch_kernel, "pitch", KB_PITCH_THREADS, p.smem, p.jobs, plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_pitch_kernel, {.grid = grid, .block = KB_PITCH_THREADS, .smem = p.smem, .st = st,
+                                       .timed = true}, p);
+}
+
+static int64_t kb_pitch_ws_layout(const kapre_pitch_plan* plan, long long rows, int M, int64_t* bp_off) {
+    const long long fr = rows * M;
+    int64_t off = (fr * 4 + 255) / 256 * 256;
+    off += (fr * plan->geo.cmax * 4 + 255) / 256 * 256;
+    off += (fr * plan->geo.cmax * 2 + 255) / 256 * 256;
+    *bp_off = off;
+    return off + fr * 2LL * plan->cfg.n_pitch * 2;
+}
+
+extern "C" {
+
+int kapre_pitch_plan_create(const kapre_pitch_config* cfg, const kapre_pitch_tables* tab, kapre_pitch_plan** out) {
+    if (!cfg || !out) return kb_fail(KAPRE_E_INVALID, "null argument");
+    *out = nullptr;
+    const kapre_pitch_config& c = *cfg;
+    if (!(c.sample_rate > 0.0f) || c.frame_length < 2 || c.win_length < 1 || c.hop_length < 1 ||
+        c.win_length >= c.frame_length || c.min_period < 1 || c.max_period < c.min_period + 2 ||
+        c.max_period > c.frame_length - c.win_length - 1)
+        return kb_fail(KAPRE_E_INVALID, "pitch: bad geometry (frame %d, window %d, hop %d, periods %d .. %d)",
+                       c.frame_length, c.win_length, c.hop_length, c.min_period, c.max_period);
+    if (c.frame_length > KAPRE_PITCH_MAX_FRAME)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "pitch: frame_length %d exceeds the limit of %d", c.frame_length,
+                       KAPRE_PITCH_MAX_FRAME);
+    if (tab) {
+        if (c.n_thresholds < 1 || c.n_pitch < 1 || c.band_width < 1)
+            return kb_fail(KAPRE_E_INVALID, "pyin: n_thresholds, n_pitch and band_width must be positive");
+        if (c.n_thresholds > KAPRE_PITCH_MAX_THRESHOLDS || c.n_pitch > KAPRE_PITCH_MAX_BINS ||
+            c.band_width > KAPRE_PITCH_MAX_BAND)
+            return kb_fail(KAPRE_E_UNSUPPORTED, "pyin: %d thresholds, %d pitch bins or a band of %d exceed the limits "
+                           "(%d, %d, %d)", c.n_thresholds, c.n_pitch, c.band_width, KAPRE_PITCH_MAX_THRESHOLDS,
+                           KAPRE_PITCH_MAX_BINS, KAPRE_PITCH_MAX_BAND);
+        if (!tab->beta_probs || !tab->boltzmann_pow || !tab->boltzmann_norm || !tab->no_trough_bonus ||
+            (c.n_pitch > 1 && !tab->period_edges) || !tab->freqs || !tab->log_triangle || !tab->log_row_norm)
+            return kb_fail(KAPRE_E_INVALID, "pyin: null table");
+    }
+    kapre_pitch_plan* pl = new kapre_pitch_plan();
+    pl->cfg = c;
+    KbPitchParams& g = pl->geo;
+    g = KbPitchParams{};
+    g.F = c.frame_length; g.W = c.win_length; g.h = c.hop_length; g.pad = c.center ? c.frame_length / 2 : 0;
+    g.min_p = c.min_period; g.max_p = c.max_period;
+    g.sr = c.sample_rate; g.thresh = c.trough_threshold;
+    g.pyin = tab ? 1 : 0;
+    g.n_thr = tab ? c.n_thresholds : 0;
+    g.n_pitch = tab ? c.n_pitch : 0;
+    if (!kb_pitch_tiling(g)) {
+        delete pl;
+        return kb_fail(KAPRE_E_UNSUPPORTED, "pitch: one frame does not fit the kernel's shared memory");
+    }
+    int rc = kb_dev_info(&pl->dev);
+    if (!rc && g.smem > pl->dev.smem_optin) rc = kb_fail(KAPRE_E_UNSUPPORTED, "pitch: %d B of shared memory", g.smem);
+    if (!rc && tab) {
+        KbVitParams& v = pl->vit;
+        v = KbVitParams{};
+        v.n = c.n_pitch; v.w = c.band_width; v.half = c.band_width / 2;
+        v.cmax = g.cmax;
+        v.ls = c.log_stay; v.lw = c.log_switch; v.lpv = c.log_init_voiced; v.lpu = c.log_init_unvoiced;
+        v.fill = c.fill_na;
+        v.nt = (c.n_pitch + 31) / 32 * 32;
+        if (v.nt > KB_VIT_THREADS) v.nt = KB_VIT_THREADS;
+        if (kb_vit_smem(v.n, v.w) > pl->dev.smem_optin)
+            rc = kb_fail(KAPRE_E_UNSUPPORTED, "pyin: %d pitch bins and a band of %d need %d B of shared memory", v.n,
+                         v.w, kb_vit_smem(v.n, v.w));
+        const double* edges = tab->period_edges;
+        std::vector<double> one(1, 0.0);
+        if (c.n_pitch == 1) edges = one.data();
+        if (!rc) rc = kb_pitch_upload<float>(pl, tab->beta_probs, c.n_thresholds, &g.beta);
+        if (!rc) rc = kb_pitch_upload<float>(pl, tab->boltzmann_pow, g.cmax + 1, &g.bpow);
+        if (!rc) rc = kb_pitch_upload<float>(pl, tab->boltzmann_norm, g.cmax + 1, &g.bnorm);
+        if (!rc) rc = kb_pitch_upload<float>(pl, tab->no_trough_bonus, c.n_thresholds + 1, &g.bonus);
+        if (!rc) rc = kb_pitch_upload<double>(pl, edges, c.n_pitch > 1 ? c.n_pitch - 1 : 1, &g.edges);
+        if (!rc) rc = kb_pitch_upload<float>(pl, tab->freqs, c.n_pitch, &v.freq);
+        if (!rc) rc = kb_pitch_upload<float>(pl, tab->log_triangle, c.band_width, &v.ltri);
+        if (!rc) rc = kb_pitch_upload<float>(pl, tab->log_row_norm, c.n_pitch, &v.lnorm);
+    }
+    if (rc) {
+        kapre_pitch_plan_destroy(pl);
+        return rc;
+    }
+    *out = pl;
+    return 0;
+}
+
+void kapre_pitch_plan_destroy(kapre_pitch_plan* plan) {
+    if (!plan) return;
+    for (void* b : plan->bufs) cudaFree(b);
+    delete plan;
+}
+
+int kapre_pitch_num_frames(const kapre_pitch_plan* plan, int length) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (length < 0) return kb_fail(KAPRE_E_INVALID, "negative length");
+    return kb_pitch_frames(plan->cfg, length);
+}
+
+int64_t kapre_pitch_workspace_bytes(const kapre_pitch_plan* plan, int batch, int channels, int length) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (batch < 0 || channels < 0 || length < 0) return kb_fail(KAPRE_E_INVALID, "pitch: negative size");
+    if (!plan->geo.pyin) return 0;
+    int64_t bp;
+    return kb_pitch_ws_layout(plan, (long long)batch * channels, kb_pitch_frames(plan->cfg, length), &bp);
+}
+
+int kapre_yin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* f0_dev,
+              const kapre_frames_desc* f0_desc, float* cmndf_dev, const kapre_spec_desc* cmndf_desc, void* stream) {
+    int rc = kb_pitch_check_shape(plan, x_desc);
+    if (rc) return rc;
+    if (!f0_desc || (cmndf_dev && !cmndf_desc)) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if ((long long)x_desc->batch * x_desc->channels * kb_pitch_frames(plan->cfg, x_desc->length) == 0) return 0;
+    if (!x_dev || !f0_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    KbPitchParams geo = plan->geo;
+    if (geo.pyin) {   // a pYIN plan also serves YIN: the same tiling without the pYIN scratch
+        kapre_pitch_plan tmp;
+        tmp.cfg = plan->cfg; tmp.dev = plan->dev; tmp.geo = geo;
+        tmp.geo.pyin = 0;
+        tmp.geo.n_thr = 0;
+        kb_pitch_tiling(tmp.geo);
+        return kb_pitch_launch(&tmp, x_dev, x_desc, f0_dev, f0_desc, cmndf_dev, cmndf_desc, nullptr,
+                               (cudaStream_t)stream);
+    }
+    return kb_pitch_launch(plan, x_dev, x_desc, f0_dev, f0_desc, cmndf_dev, cmndf_desc, nullptr, (cudaStream_t)stream);
+}
+
+int kapre_pyin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* f0_dev,
+               uint8_t* voiced_flag_dev, float* voiced_prob_dev, const kapre_frames_desc* out_desc, float* cmndf_dev,
+               const kapre_spec_desc* cmndf_desc, void* workspace_dev, void* stream) {
+    int rc = kb_pitch_check_shape(plan, x_desc);
+    if (rc) return rc;
+    if (!plan->geo.pyin) return kb_fail(KAPRE_E_INVALID, "pyin: the plan was created without pYIN tables");
+    if (!out_desc || (cmndf_dev && !cmndf_desc)) return kb_fail(KAPRE_E_INVALID, "null argument");
+    const int M = kb_pitch_frames(plan->cfg, x_desc->length);
+    const long long rows = (long long)x_desc->batch * x_desc->channels;
+    if (rows * M == 0) return 0;
+    if (!x_dev || !f0_dev || !voiced_flag_dev || !voiced_prob_dev || !workspace_dev)
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = kb_pitch_launch(plan, x_dev, x_desc, voiced_prob_dev, out_desc, cmndf_dev, cmndf_desc, workspace_dev, st)))
+        return rc;
+    KbVitParams v = plan->vit;
+    int64_t bp;
+    kb_pitch_ws_layout(plan, rows, M, &bp);
+    char* w = (char*)workspace_dev;
+    v.M = M; v.C = x_desc->channels; v.rows = rows;
+    v.cand_n = (const int*)w;
+    v.cand_p = (const float*)(w + (rows * M * 4 + 255) / 256 * 256);
+    v.cand_bin = (const unsigned short*)((const char*)v.cand_p + (rows * M * plan->geo.cmax * 4 + 255) / 256 * 256);
+    v.bp = (unsigned short*)(w + bp);
+    v.vp = voiced_prob_dev; v.f0 = f0_dev; v.flag = voiced_flag_dev;
+    v.o_sb = out_desc->stride_b; v.o_sc = out_desc->stride_c; v.o_st = out_desc->stride_t;
+    const int smem = kb_vit_smem(v.n, v.w);
+    int grid;
+    if ((rc = kb_resident_grid(kb_viterbi_kernel, "viterbi", v.nt, smem, rows, plan->dev.sm_count, &grid))) return rc;
+    return kb_launch(kb_viterbi_kernel, {.grid = grid, .block = v.nt, .smem = smem, .st = st, .timed = true}, v);
 }
 
 }  // extern "C"

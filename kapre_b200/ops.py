@@ -1854,3 +1854,123 @@ def cqt(x, plan: CqtPlan, input_data_format=_CH_LAST_STR, output_data_format=_CH
         from . import autograd
         return autograd.cqt(x, plan, input_data_format, output_data_format, magnitude)
     return cqt_forward(x, plan, input_data_format, output_data_format, magnitude)[0]
+
+
+# ------------------------------------------------------------------------------- pitch tracking (YIN / pYIN)
+class PitchPlan(_PerDevice):
+    """kapre_pitch_plan per CUDA device for one YIN configuration (``backend.pitch_geometry``), or with ``pyin`` (a
+    dict of ``backend.pyin_geometry``'s keyword arguments) one pYIN configuration, whose float64 tables
+    (``backend.pyin_tables``) are uploaded once per device."""
+
+    def __init__(self, sample_rate, fmin, fmax, frame_length=2048, win_length=None, hop_length=None, center=True,
+                 trough_threshold=0.1, pyin=None, fill_na=float('nan')):
+        from . import backend
+        self.geometry = g = backend.pitch_geometry(sample_rate, fmin, fmax, frame_length, win_length, hop_length,
+                                                   center)
+        if isinstance(trough_threshold, bool) or not np.isfinite(float(trough_threshold)):
+            raise ValueError('trough_threshold must be finite, got %r' % (trough_threshold,))
+        self.pyin = None
+        self.n_lags = g['n_lags']
+        n_thr = n_pitch = band = 0
+        ls = lw = lpv = lpu = 0.0
+        self._tables = None
+        if pyin is not None:
+            self.pyin = q = backend.pyin_geometry(g, **pyin)
+            t = {k: np.ascontiguousarray(v, dtype=np.float64) for k, v in backend.pyin_tables(g, q).items()}
+            self._tables = t
+            self._tab = N.PitchTables(*[t[name].ctypes.data_as(ctypes.c_void_p) for name, _ in N.PitchTables._fields_])
+            n_thr, n_pitch, band = q['n_thresholds'], q['n_pitch'], q['band_width']
+            tiny = backend.PITCH_TINY
+            ls, lw = np.log(1.0 - q['switch_prob'] + tiny), np.log(q['switch_prob'] + tiny)
+            lpv, lpu = np.log(tiny), np.log(1.0 / n_pitch + tiny)
+        self.fill_na = float(fill_na)
+        self.cfg = N.PitchCfg(g['sample_rate'], g['frame_length'], g['win_length'], g['hop_length'], int(g['center']),
+                              g['min_period'], g['max_period'], float(trough_threshold), n_thr, n_pitch, band, ls, lw,
+                              lpv, lpu, self.fill_na)
+        self._per_device = {}
+
+    _destroy = 'kapre_pitch_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_pitch_plan_create(ctypes.byref(self.cfg), ctypes.byref(self._tab) if self.pyin else None, out)
+
+    def num_frames(self, length):
+        g = self.geometry
+        lp = int(length) + 2 * g['pad']
+        return 0 if lp < g['frame_length'] else 1 + (lp - g['frame_length']) // g['hop_length']
+
+    def workspace(self, B, C, L, device):
+        n = int(N.lib().kapre_pitch_workspace_bytes(self.handle(), B, C, L))
+        if n < 0:
+            N.check(n)
+        return torch.empty(max((n + 3) // 4, 1), dtype=torch.float32, device=device)
+
+
+def _frames_alloc(B, C, M, data_format, dtype, device):
+    if data_format == _CH_LAST_STR:
+        y = torch.empty((B, M, C), dtype=dtype, device=device)
+        sb, st, sc = y.stride()
+    else:
+        y = torch.empty((B, C, M), dtype=dtype, device=device)
+        sb, sc, st = y.stride()
+    return y, N.FramesDesc(sb, sc, st)
+
+
+def _pitch_input(x, name):
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise N.KapreNativeError('%s needs a CUDA waveform' % name)
+    if x.dim() != 3:
+        raise ValueError('%s expects a 3-D waveform batch, got shape %s' % (name, tuple(x.shape)))
+    if x.dtype != torch.float32:
+        raise ValueError('%s expects float32 samples, got %s' % (name, x.dtype))
+    return x.detach()
+
+
+def _cmndf_desc(cmndf, B, C, M, plan):
+    """The (B, C, frames, n_lags) float32 CUDA tensor the caller passed for the CMNDF, or None."""
+    if cmndf is None:
+        return None, None
+    if (not isinstance(cmndf, torch.Tensor) or not cmndf.is_cuda or cmndf.dtype != torch.float32
+            or tuple(cmndf.shape) != (B, C, M, plan.n_lags)):
+        raise ValueError('cmndf must be a float32 CUDA tensor of shape %s' % ((B, C, M, plan.n_lags),))
+    return cmndf, N.SpecDesc(*cmndf.stride())
+
+
+@_device_of_first_arg
+def yin(x, plan: PitchPlan, data_format=_CH_LAST_STR, cmndf=None):
+    """YIN f0 of a float32 CUDA waveform batch (``(B, L, C)`` channels_last or ``(B, C, L)``) under ``plan``, as
+    ``(B, frames, C)`` / ``(B, C, frames)`` float32 (see ``signal.yin``).  ``cmndf`` (optional): a ``(B, C, frames,
+    n_lags)`` float32 tensor that also receives the CMNDF at lags min_period .. max_period.  One launch.  Not
+    differentiable: the output carries no ``grad_fn``."""
+    x = _pitch_input(x, 'yin')
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    M = plan.num_frames(L)
+    f0, fd = _frames_alloc(B, C, M, data_format, torch.float32, x.device)
+    cm, cd = _cmndf_desc(cmndf, B, C, M, plan)
+    if f0.numel():
+        N.check(N.lib().kapre_yin(plan.handle(), _ptr(x), ctypes.byref(xd), _ptr(f0), ctypes.byref(fd),
+                                  _ptr(cm) if cm is not None else None, ctypes.byref(cd) if cd is not None else None,
+                                  _stream_ptr()))
+    return f0
+
+
+@_device_of_first_arg
+def pyin(x, plan: PitchPlan, data_format=_CH_LAST_STR, cmndf=None):
+    """pYIN of a float32 CUDA waveform batch under a pYIN ``plan``: ``(f0, voiced_flag, voiced_prob)``, each ``(B,
+    frames, C)`` / ``(B, C, frames)`` (float32, bool, float32; see ``signal.pyin``).  ``cmndf`` as in ``yin``.  Two
+    launches.  Not differentiable: the outputs carry no ``grad_fn``."""
+    if plan.pyin is None:
+        raise ValueError('pyin needs a PitchPlan made with pyin parameters')
+    x = _pitch_input(x, 'pyin')
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    M = plan.num_frames(L)
+    f0, fd = _frames_alloc(B, C, M, data_format, torch.float32, x.device)
+    flag, _ = _frames_alloc(B, C, M, data_format, torch.bool, x.device)
+    vp, _ = _frames_alloc(B, C, M, data_format, torch.float32, x.device)
+    cm, cd = _cmndf_desc(cmndf, B, C, M, plan)
+    if f0.numel():
+        ws = plan.workspace(B, C, L, x.device)
+        N.check(N.lib().kapre_pyin(plan.handle(), _ptr(x), ctypes.byref(xd), _ptr(f0), _ptr(flag), _ptr(vp),
+                                   ctypes.byref(fd), _ptr(cm) if cm is not None else None,
+                                   ctypes.byref(cd) if cd is not None else None, _ptr(ws), _stream_ptr()))
+    return f0, flag, vp

@@ -6,7 +6,8 @@ reference, which expects audio to be resampled before it reaches the model; neit
 real factor, band-limited interpolation), ``Convolve`` (convolution with long filters, partitioned FFT) or the IIR
 filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan), or
 ``add_noise`` (torchaudio's, with deterministic float64 energies), or ``loudness`` and ``Loudness`` (torchaudio's
-BS.1770 gated loudness, with per-item lengths)."""
+BS.1770 gated loudness, with per-item lengths), or the pitch trackers ``yin``, ``pyin``, ``YIN`` and ``PYIN``
+(librosa's)."""
 from __future__ import annotations
 
 import math
@@ -19,7 +20,8 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
-           'Biquad', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram']
+           'Biquad', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
+           'YIN', 'PYIN']
 
 
 def _resolve(fmt):
@@ -525,3 +527,140 @@ def kaldi_spectrogram(waveform, lengths=None, data_format='default', seed=0, **k
     """``torchaudio.compliance.kaldi.spectrogram`` on the GPU for a batch (``padded_window_size // 2 + 1`` bins);
     see ``kaldi_fbank``."""
     return _kaldi('spectrogram', waveform, lengths, data_format, seed, kwargs)
+
+
+# ---- pitch tracking -------------------------------------------------------------------------------------------
+_PYIN_DEFAULTS = dict(n_thresholds=100, beta_parameters=(2, 18), boltzmann_parameter=2, resolution=0.1,
+                      max_transition_rate=35.92, switch_prob=0.01, no_trough_prob=0.01)
+_pitch_plans = {}
+
+
+def _pitch_plan(sample_rate, fmin, fmax, frame_length, win_length, hop_length, center, trough_threshold, pyin=None,
+                fill_na=float('nan')):
+    """One PitchPlan per configuration (so a call uploads nothing after the first and can be captured)."""
+    key = (float(sample_rate), float(fmin), float(fmax), frame_length, win_length, hop_length, bool(center),
+           float(trough_threshold), None if pyin is None else tuple(sorted((k, v if not isinstance(v, list) else
+                                                                            tuple(v)) for k, v in pyin.items())),
+           repr(float(fill_na)))
+    plan = _pitch_plans.get(key)
+    if plan is None:
+        plan = ops.PitchPlan(sample_rate, fmin, fmax, frame_length, win_length, hop_length, center, trough_threshold,
+                             pyin, fill_na)
+        _pitch_plans[key] = plan
+    return plan
+
+
+def yin(waveform, sample_rate, fmin, fmax, frame_length=2048, win_length=None, hop_length=None, trough_threshold=0.1,
+        center=True, data_format='default'):
+    """YIN fundamental frequency (Hz) per frame of ``waveform`` ``(batch, time, ch)`` / ``(batch, ch, time)`` (a
+    float32 CUDA tensor), as ``(batch, frames, ch)`` / ``(batch, ch, frames)`` float32; modelled on ``librosa.yin``.
+
+    Frame m holds samples [m h - F / 2, m h + F / 2) with ``center`` (zeros outside the signal; librosa 0.10's
+    ``pad_mode='constant'``, the only pad mode), else [m h, m h + F); frames = 1 + (L_pad - F) // h.  With W =
+    ``win_length`` (default F // 2), h = ``hop_length`` (default F // 4) and x the frame,
+
+        d(tau) = sum_{j=1..W} (x[j] - x[j + tau])^2,   c(tau) = d(tau) / (mean_{k<=tau} d(k) + 2^-126)
+
+    for tau in [floor(sr / fmax), min(ceil(sr / fmin), F - W - 1)].  The first trough of c below
+    ``trough_threshold`` is chosen, else the first global minimum, refined by a parabolic shift; f0 = sr / period.
+    Unlike librosa, no autocorrelation or energy term is flushed to zero below 1e-6, so quiet signals behave as loud
+    ones.  A frame holding a non-finite sample gives NaN; no other frame changes.  An output's bits depend on its
+    (item, channel, frame) alone.
+
+    One launch.  f0 comes from a discrete choice, so it has no gradient: an input that requires grad is accepted
+    and the output carries no ``grad_fn``."""
+    fmt = _resolve(_unwrap_format(data_format))
+    plan = _pitch_plan(sample_rate, fmin, fmax, frame_length, win_length, hop_length, center, trough_threshold)
+    return ops.yin(waveform, plan, fmt)
+
+
+def pyin(waveform, sample_rate, fmin, fmax, frame_length=2048, win_length=None, hop_length=None, n_thresholds=100,
+         beta_parameters=(2, 18), boltzmann_parameter=2, resolution=0.1, max_transition_rate=35.92, switch_prob=0.01,
+         no_trough_prob=0.01, fill_na=float('nan'), center=True, data_format='default'):
+    """Probabilistic YIN (modelled on ``librosa.pyin``): ``(f0, voiced_flag, voiced_prob)``, each ``(batch, frames,
+    ch)`` / ``(batch, ch, frames)`` (float32, bool, float32).  Framing and CMNDF as ``yin``.
+
+    Each trough of the CMNDF gets the probability sum_i Boltzmann(rank among the troughs below s_i) beta_i over the
+    thresholds s_i = i / n_thresholds with beta_i the Beta(``beta_parameters``) mass of (s_{i-1}, s_i]; the first
+    global-minimum trough also gets ``no_trough_prob`` times the mass of the thresholds at or below it.  Troughs map
+    to pitch bins of ``resolution`` semitones from ``fmin``; the voiced observation of a bin is the **sum** of its
+    troughs' probabilities (librosa keeps the last one), ``voiced_prob = min(sum, 1)``, and each unvoiced state
+    observes (1 - voiced_prob) / n_pitch.  A Viterbi decode over 2 n_pitch states (voiced, then unvoiced) with a
+    triangular transition band of ``max_transition_rate`` semitones per second and ``switch_prob`` gives the path;
+    f0 is the bin frequency on voiced frames and ``fill_na`` elsewhere.  Log probabilities are log(p + 2^-126) and
+    transitions outside the band are excluded (librosa gives them log(tiny)).  A non-finite sample makes its whole
+    (item, channel) row ``fill_na``, unvoiced and NaN; no other row changes.
+
+    Two launches: the CMNDF with the trough probabilities, then the Viterbi decode.  No gradient: an input that
+    requires grad is accepted and the outputs carry no ``grad_fn``."""
+    fmt = _resolve(_unwrap_format(data_format))
+    q = dict(n_thresholds=n_thresholds, beta_parameters=tuple(beta_parameters), boltzmann_parameter=boltzmann_parameter,
+             resolution=resolution, max_transition_rate=max_transition_rate, switch_prob=switch_prob,
+             no_trough_prob=no_trough_prob)
+    plan = _pitch_plan(sample_rate, fmin, fmax, frame_length, win_length, hop_length, center, 0.1, q, fill_na)
+    return ops.pyin(waveform, plan, fmt)
+
+
+@register_keras_serializable(package='Kapre')
+class YIN(Layer):
+    """``yin`` as a layer: ``(batch, time, ch)`` / ``(batch, ch, time)`` in, ``(batch, frames, ch)`` / ``(batch, ch,
+    frames)`` f0 out.  Same arguments as ``yin`` (without the waveform)."""
+
+    def __init__(self, sample_rate, fmin, fmax, frame_length=2048, win_length=None, hop_length=None,
+                 trough_threshold=0.1, center=True, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.sample_rate, self.fmin, self.fmax = sample_rate, fmin, fmax
+        self.frame_length, self.win_length, self.hop_length = frame_length, win_length, hop_length
+        self.trough_threshold, self.center = trough_threshold, center
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+        self.plan = _pitch_plan(sample_rate, fmin, fmax, frame_length, win_length, hop_length, center,
+                                trough_threshold)
+
+    def call(self, x):
+        return ops.yin(x, self.plan, self.data_format)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'), ('fmin', 'fmin'), ('fmax', 'fmax'), ('frame_length', 'frame_length'),
+        ('win_length', 'win_length'), ('hop_length', 'hop_length'), ('trough_threshold', 'trough_threshold'),
+        ('center', 'center'), ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class PYIN(Layer):
+    """``pyin`` as a layer: the waveform in, ``(f0, voiced_flag, voiced_prob)`` out.  Same arguments as ``pyin``."""
+
+    def __init__(self, sample_rate, fmin, fmax, frame_length=2048, win_length=None, hop_length=None, n_thresholds=100,
+                 beta_parameters=(2, 18), boltzmann_parameter=2, resolution=0.1, max_transition_rate=35.92,
+                 switch_prob=0.01, no_trough_prob=0.01, fill_na=float('nan'), center=True, data_format='default',
+                 **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.sample_rate, self.fmin, self.fmax = sample_rate, fmin, fmax
+        self.frame_length, self.win_length, self.hop_length = frame_length, win_length, hop_length
+        self.n_thresholds, self.beta_parameters = n_thresholds, tuple(beta_parameters)
+        self.boltzmann_parameter, self.resolution = boltzmann_parameter, resolution
+        self.max_transition_rate, self.switch_prob = max_transition_rate, switch_prob
+        self.no_trough_prob, self.fill_na, self.center = no_trough_prob, fill_na, center
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+        q = dict(n_thresholds=n_thresholds, beta_parameters=self.beta_parameters,
+                 boltzmann_parameter=boltzmann_parameter, resolution=resolution,
+                 max_transition_rate=max_transition_rate, switch_prob=switch_prob, no_trough_prob=no_trough_prob)
+        self.plan = _pitch_plan(sample_rate, fmin, fmax, frame_length, win_length, hop_length, center, 0.1, q, fill_na)
+
+    def call(self, x):
+        return ops.pyin(x, self.plan, self.data_format)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'), ('fmin', 'fmin'), ('fmax', 'fmax'), ('frame_length', 'frame_length'),
+        ('win_length', 'win_length'), ('hop_length', 'hop_length'), ('n_thresholds', 'n_thresholds'),
+        ('beta_parameters', 'beta_parameters'), ('boltzmann_parameter', 'boltzmann_parameter'),
+        ('resolution', 'resolution'), ('max_transition_rate', 'max_transition_rate'), ('switch_prob', 'switch_prob'),
+        ('no_trough_prob', 'no_trough_prob'), ('fill_na', 'fill_na'), ('center', 'center'),
+        ('data_format', 'data_format_str'),
+    )
