@@ -599,6 +599,65 @@ int kapre_pyin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wav
                uint8_t* voiced_flag_dev, float* voiced_prob_dev, const kapre_frames_desc* out_desc, float* cmndf_dev,
                const kapre_spec_desc* cmndf_desc, void* workspace_dev, void* stream);
 
+/* ---- chroma features (modelled on librosa's chroma_stft, chroma_cqt, chroma_cens and estimate_tuning) -------------
+ * A chroma plan holds n_tables filterbank tables W (n_chroma x n_bins each), optionally the CENS smoothing taps and
+ * optionally the tuning estimate's geometry.  For every frame of a (item, channel) row of a spectrogram s (any element
+ * strides (b, c, t, k)), y_j = sum_k W[j][k] s_k in ascending k (float32), entries below the threshold are set to 0
+ * and the frame is normalised; a frame whose length is below FLT_MIN is left as it is.  An output's bits depend on
+ * (item, channel, frame, chroma) and the item's table alone. */
+#define KAPRE_CHROMA_MAX_CHROMA 64
+#define KAPRE_CHROMA_MAX_BINS 4097
+#define KAPRE_CHROMA_MAX_TUNING_BINS 1000
+#define KAPRE_CHROMA_MAX_SMOOTH 514
+enum { KAPRE_CHROMA_IN_LINEAR = 0, KAPRE_CHROMA_IN_SQUARE = 1, KAPRE_CHROMA_IN_COMPLEX = 2 };
+enum { KAPRE_CHROMA_NORM_NONE = 0, KAPRE_CHROMA_NORM_INF = 1, KAPRE_CHROMA_NORM_L1 = 2, KAPRE_CHROMA_NORM_L2 = 3 };
+typedef struct {
+    int n_chroma, n_bins, n_tables;       /* n_tables = 0: a plan for the tuning estimate alone */
+    const double* tables;                 /* n_tables x n_chroma x n_bins, rounded to float32 on upload */
+    int n_smooth;                         /* CENS smoothing taps (0: no CENS) */
+    const double* smooth;
+    int n_tuning_bins;                    /* residual histogram bins (0: no tuning estimate) */
+    const double* tuning_edges;           /* n_tuning_bins + 1, ascending */
+    int peak_lo, peak_hi;                 /* piptrack's bins [peak_lo, peak_hi), 1 <= peak_lo, peak_hi < n_bins */
+    float sample_rate, n_fft;             /* pitch = (k + shift) sample_rate / n_fft */
+    double bins_per_octave;               /* of the residual */
+} kapre_chroma_plan_desc;
+typedef struct {
+    int in_mode;                          /* KAPRE_CHROMA_IN_*: s = x, x^2 (float x) or |x| (complex64 x) */
+    int norm;                             /* KAPRE_CHROMA_NORM_* */
+    int has_threshold;
+    float threshold;
+} kapre_chroma_config;
+typedef struct kapre_chroma_plan kapre_chroma_plan;
+int kapre_chroma_plan_create(const kapre_chroma_plan_desc* desc, kapre_chroma_plan** out);
+void kapre_chroma_plan_destroy(kapre_chroma_plan* plan);
+/* The chroma (batch, channels, frames, n_chroma) at out_desc's strides.  table_dev (nullable, device int per item):
+ * the table of each item, else table 0.  One launch. */
+int kapre_chroma(const kapre_chroma_plan* plan, const kapre_chroma_config* cfg, const void* x_dev,
+                 const kapre_spec_desc* x_desc, int batch, int channels, int frames, const int* table_dev, float* out_dev,
+                 const kapre_spec_desc* out_desc, void* stream);
+/* Gradient of kapre_chroma to x (float, or complex64 for KAPRE_CHROMA_IN_COMPLEX) at gx_desc's strides, given the
+ * output gradient g.  Through the normalisation (norm inf: to the first index of the maximum), the threshold, W and the
+ * input mode (2 x g, or g x / |x| with 0 at x = 0).  One launch. */
+int kapre_chroma_backward(const kapre_chroma_plan* plan, const kapre_chroma_config* cfg, const void* x_dev,
+                          const kapre_spec_desc* x_desc, int batch, int channels, int frames, const int* table_dev,
+                          const float* g_dev, const kapre_spec_desc* g_desc, void* gx_dev, const kapre_spec_desc* gx_desc,
+                          void* stream);
+int64_t kapre_chroma_cens_workspace_bytes(const kapre_chroma_plan* plan, int batch, int channels, int frames);
+/* CENS: threshold 0, L1 normalisation and quantisation (one launch), then the smoothing along time with zeros outside
+ * the row and the L2 normalisation (a second launch). */
+int kapre_chroma_cens(const kapre_chroma_plan* plan, int in_mode, const void* x_dev, const kapre_spec_desc* x_desc,
+                      int batch, int channels, int frames, float* out_dev, const kapre_spec_desc* out_desc,
+                      void* workspace_dev, void* stream);
+int64_t kapre_chroma_tuning_workspace_bytes(const kapre_chroma_plan* plan, int batch, int channels, int frames);
+/* librosa's estimate_tuning per item over all its channels from a power (KAPRE_CHROMA_IN_SQUARE of |X|) or given
+ * (KAPRE_CHROMA_IN_LINEAR) spectrogram: tuning_dev (double per item) and table_dev (int per item: the index of the
+ * tuning's edge, n_tuning_bins for an item without peaks).  Seven launches and two memsets whatever the data; nothing
+ * is read back to the host. */
+int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float* x_dev, const kapre_spec_desc* x_desc,
+                        int batch, int channels, int frames, double* tuning_dev, int* table_dev, void* workspace_dev,
+                        void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

@@ -100,6 +100,21 @@ class FramesDesc(Structure):
     _fields_ = [('stride_b', c_int64), ('stride_c', c_int64), ('stride_t', c_int64)]
 
 
+class ChromaPlanDesc(Structure):
+    _fields_ = [('n_chroma', c_int), ('n_bins', c_int), ('n_tables', c_int), ('tables', c_void_p),
+                ('n_smooth', c_int), ('smooth', c_void_p), ('n_tuning_bins', c_int), ('tuning_edges', c_void_p),
+                ('peak_lo', c_int), ('peak_hi', c_int), ('sample_rate', c_float), ('n_fft', c_float),
+                ('bins_per_octave', ctypes.c_double)]
+
+
+class ChromaCfg(Structure):
+    _fields_ = [('in_mode', c_int), ('norm', c_int), ('has_threshold', c_int), ('threshold', c_float)]
+
+
+CHROMA_IN_LINEAR, CHROMA_IN_SQUARE, CHROMA_IN_COMPLEX = range(3)
+CHROMA_NORM_NONE, CHROMA_NORM_INF, CHROMA_NORM_L1, CHROMA_NORM_L2 = range(4)
+
+
 class DbCfg(Structure):
     _fields_ = [('ref_value', c_float), ('amin', c_float), ('dynamic_range', c_float)]
 
@@ -213,6 +228,18 @@ SYMBOLS = [
                           POINTER(SpecDesc), c_void_p]),
     ('kapre_pyin', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, c_void_p, c_void_p, POINTER(FramesDesc),
                            c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_chroma_plan_create', c_int, [POINTER(ChromaPlanDesc), POINTER(c_void_p)]),
+    ('kapre_chroma_plan_destroy', None, [c_void_p]),
+    ('kapre_chroma', c_int, [c_void_p, POINTER(ChromaCfg), c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_void_p,
+                             c_void_p, POINTER(SpecDesc), c_void_p]),
+    ('kapre_chroma_backward', c_int, [c_void_p, POINTER(ChromaCfg), c_void_p, POINTER(SpecDesc), c_int, c_int, c_int,
+                                      c_void_p, c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p]),
+    ('kapre_chroma_cens_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int]),
+    ('kapre_chroma_cens', c_int, [c_void_p, c_int, c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_void_p,
+                                  POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_chroma_tuning_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int]),
+    ('kapre_chroma_tuning', c_int, [c_void_p, c_int, c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

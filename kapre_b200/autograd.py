@@ -34,6 +34,9 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * CQT (and its fused ``CQT -> Magnitude``) -> ``kapre_cqt_backward`` (per octave, lowest first, a gather of the
   filters' adjoint over the frames covering each sample plus the decimator's adjoint of the octave below; the
   magnitude mode recomputes C from the saved pyramid)
+* chroma_stft, chroma_cqt, ChromaSTFT, ChromaCQT -> ``kapre_chroma_backward`` (y = W s recomputed, the gradient
+  taken back through the normalisation and the threshold, then W^T and the input's square or modulus), then the STFT
+  magnitude or CQT magnitude backward; the tuning estimate is a constant
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
@@ -454,6 +457,21 @@ class _Cqt(torch.autograd.Function):
         return ops.cqt_backward(g, x, ws, plan, idf, odf, magnitude), None, None, None, None
 
 
+class _Chroma(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, plan, cfg, data_format, table):
+        ctx.save_for_backward(x, table)
+        ctx.cfg = (plan, cfg, data_format)
+        return ops.chroma_forward(x, plan, cfg, data_format, table)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, table = ctx.saved_tensors
+        plan, cfg, data_format = ctx.cfg
+        return ops.chroma_backward(g, x, plan, cfg, data_format, table), None, None, None, None
+
+
 class _TimeStretch(torch.autograd.Function):
     """The forward is the plain time-stretch launch; autograd saves its output, from which the backward takes the
     magnitude and phase gradients, so the forward writes nothing extra."""
@@ -583,3 +601,7 @@ def kaldi_features(x, plan, lengths_h, lengths_d, data_format, dither, seed):
 
 def cqt(x, plan, input_data_format, output_data_format, magnitude):
     return _Cqt.apply(x, plan, input_data_format, output_data_format, magnitude)
+
+
+def chroma(x, plan, cfg, data_format, table):
+    return _Chroma.apply(x, plan, cfg, data_format, table)

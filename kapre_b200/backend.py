@@ -669,3 +669,128 @@ def pyin_tables(geometry, pyin):
         rows[i] = tri[j0 - i + w // 2:j1 - i + w // 2].sum()
     return dict(beta_probs=beta, boltzmann_pow=bpow, boltzmann_norm=bnorm, no_trough_bonus=bonus,
                 period_edges=edges, freqs=freqs, log_triangle=np.log(tri), log_row_norm=-np.log(rows))
+
+
+# ---- chroma -----------------------------------------------------------------------------------------------------------
+CHROMA_MAX_CHROMA = 64          # KAPRE_CHROMA_MAX_CHROMA
+CHROMA_MAX_NFFT = 8192          # n_fft / 2 + 1 <= KAPRE_CHROMA_MAX_BINS
+CHROMA_MAX_TUNING_BINS = 1000   # KAPRE_CHROMA_MAX_TUNING_BINS
+CHROMA_MAX_SMOOTH = 512         # win_len_smooth + 2 <= KAPRE_CHROMA_MAX_SMOOTH
+CHROMA_NORMS = {None: 0, np.inf: 1, 1: 2, 2: 3}   # KAPRE_CHROMA_NORM_*
+
+
+def chroma_norm_code(norm):
+    """``norm`` (``inf``, 1, 2 or None) as the library's normalisation code; ValueError otherwise."""
+    if norm is None:
+        return 0
+    if isinstance(norm, bool) or not isinstance(norm, (int, float, np.integer, np.floating)):
+        raise ValueError('norm must be inf, 1, 2 or None, got %r' % (norm,))
+    if float(norm) == np.inf:
+        return 1
+    if float(norm) in (1.0, 2.0):
+        return 2 if float(norm) == 1.0 else 3
+    raise ValueError('norm must be inf, 1, 2 or None, got %r' % (norm,))
+
+
+def _check_n_chroma(n_chroma):
+    if isinstance(n_chroma, bool) or int(n_chroma) != n_chroma or not 1 <= int(n_chroma) <= CHROMA_MAX_CHROMA:
+        raise ValueError('n_chroma must be an integer in [1, %d], got %r' % (CHROMA_MAX_CHROMA, n_chroma))
+    return int(n_chroma)
+
+
+def _check_n_fft(n_fft):
+    if isinstance(n_fft, bool) or int(n_fft) != n_fft or not 2 <= int(n_fft) <= CHROMA_MAX_NFFT:
+        raise ValueError('n_fft must be an integer in [2, %d], got %r' % (CHROMA_MAX_NFFT, n_fft))
+    return int(n_fft)
+
+
+def chroma_filterbank(sample_rate, n_fft, n_chroma=12, tuning=0.0, ctroct=5.0, octwidth=2.0, base_c=True):
+    """librosa's ``filters.chroma``: the float64 (n_chroma, n_fft // 2 + 1) weights of the STFT bins per pitch class.
+    Gaussian bumps around each pitch class (2 D / binwidth), each column of unit L2 norm, then weighted by a Gaussian
+    over octaves centred on ``ctroct`` of width ``octwidth`` (none when None), rows rolled so that C comes first with
+    ``base_c``.  ``tuning`` is in fractions of a chroma bin: A440 becomes 440 2^(tuning / n_chroma)."""
+    n_chroma = _check_n_chroma(n_chroma)
+    n_fft = _check_n_fft(n_fft)
+    sr = float(sample_rate)
+    if not (np.isfinite(sr) and sr > 0):
+        raise ValueError('sample_rate must be positive, got %r' % (sample_rate,))
+    if not np.isfinite(float(tuning)):
+        raise ValueError('tuning must be finite, got %r' % (tuning,))
+    f = np.linspace(0, sr, n_fft, endpoint=False)[1:]
+    a440 = 440.0 * 2.0 ** (float(tuning) / n_chroma)
+    frqbins = n_chroma * np.log2(f / (a440 / 16.0))
+    frqbins = np.concatenate(([frqbins[0] - 1.5 * n_chroma], frqbins))
+    binwidth = np.concatenate((np.maximum(frqbins[1:] - frqbins[:-1], 1.0), [1.0]))
+    D = np.subtract.outer(frqbins, np.arange(0, n_chroma, dtype='d')).T
+    half = np.round(float(n_chroma) / 2)
+    D = np.remainder(D + half + 10 * n_chroma, n_chroma) - half
+    wts = np.exp(-0.5 * (2 * D / np.tile(binwidth, (n_chroma, 1))) ** 2)
+    wts = wts / np.sqrt(np.sum(wts ** 2, axis=0, keepdims=True))
+    if octwidth is not None:
+        wts = wts * np.tile(np.exp(-0.5 * (((frqbins / n_chroma - float(ctroct)) / float(octwidth)) ** 2)),
+                            (n_chroma, 1))
+    if base_c:
+        wts = np.roll(wts, -3 * (n_chroma // 12), axis=0)
+    return np.ascontiguousarray(wts[:, :n_fft // 2 + 1], dtype=np.float64)
+
+
+def hz_to_midi(f):
+    return 12.0 * (np.log2(np.asarray(f, dtype=np.float64)) - np.log2(440.0)) + 69.0
+
+
+def cq_to_chroma(n_input, bins_per_octave=12, n_chroma=12, f_min=None, base_c=True):
+    """librosa's ``filters.cq_to_chroma`` (without ``window``): the float64 (n_chroma, n_input) 0/1 matrix that merges
+    ``bins_per_octave / n_chroma`` adjacent CQT bins into each chroma, rolled so that the bin of ``f_min`` (default C1)
+    lands on its pitch class (C first with ``base_c``, else A).  ValueError unless ``bins_per_octave`` is a multiple
+    of ``n_chroma``."""
+    n_chroma = _check_n_chroma(n_chroma)
+    n_input, bpo = int(n_input), int(bins_per_octave)
+    if bpo < 1 or n_input < 1:
+        raise ValueError('n_input and bins_per_octave must be positive')
+    if bpo % n_chroma:
+        raise ValueError('bins_per_octave=%d must be an integer multiple of n_chroma=%d' % (bpo, n_chroma))
+    n_merge = bpo // n_chroma
+    f_min = CQT_C1 if f_min is None else float(f_min)
+    m = np.repeat(np.eye(n_chroma), n_merge, axis=1)
+    m = np.roll(m, -int(n_merge // 2), axis=1)
+    m = np.tile(m, int(np.ceil(float(n_input) / bpo)))[:, :n_input]
+    midi0 = np.mod(hz_to_midi(f_min), 12)
+    roll = int(np.round((midi0 - (0 if base_c else 9)) * (n_chroma / 12.0)))
+    return np.ascontiguousarray(np.roll(m, roll, axis=0), dtype=np.float64)
+
+
+def tuning_edges(resolution=0.01):
+    """The residual histogram edges of ``estimate_tuning``: ``linspace(-0.5, 0.5, ceil(1 / resolution) + 1)``;
+    ValueError unless 0 < resolution <= 1 with at most CHROMA_MAX_TUNING_BINS bins."""
+    r = float(resolution)
+    if isinstance(resolution, bool) or not (np.isfinite(r) and 0.0 < r <= 1.0):
+        raise ValueError('resolution must be in (0, 1], got %r' % (resolution,))
+    n = int(np.ceil(1.0 / r))
+    if n > CHROMA_MAX_TUNING_BINS:
+        raise ValueError('resolution %r gives %d histogram bins, over the limit of %d' % (resolution, n,
+                                                                                        CHROMA_MAX_TUNING_BINS))
+    return np.linspace(-0.5, 0.5, n + 1)
+
+
+def piptrack_bins(sample_rate, n_fft, fmin=150.0, fmax=4000.0):
+    """[lo, hi): the STFT bins piptrack searches, ``fmin <= f_k < min(fmax, sr / 2)`` with librosa's
+    ``fft_frequencies`` (``numpy.fft.rfftfreq``)."""
+    sr = float(sample_rate)
+    f = np.fft.rfftfreq(int(n_fft), 1.0 / sr)
+    k = np.nonzero((fmin <= f) & (f < min(float(fmax), sr / 2.0)))[0]
+    if k.size == 0:
+        return 1, 1
+    return max(int(k[0]), 1), min(int(k[-1]) + 1, int(n_fft) // 2)
+
+
+def cens_window(win_len_smooth=41):
+    """The CENS smoothing taps ``hann(win_len_smooth + 2, symmetric) / sum`` (float64); None or 0: the single tap 1."""
+    if win_len_smooth is None or win_len_smooth == 0:
+        return np.ones(1)
+    if isinstance(win_len_smooth, bool) or int(win_len_smooth) != win_len_smooth or not \
+            1 <= int(win_len_smooth) <= CHROMA_MAX_SMOOTH:
+        raise ValueError('win_len_smooth must be None or an integer in [0, %d], got %r'
+                         % (CHROMA_MAX_SMOOTH, win_len_smooth))
+    n = int(win_len_smooth) + 2
+    w = 0.5 - 0.5 * np.cos(2.0 * np.pi * np.arange(n) / (n - 1))
+    return w / w.sum()

@@ -38,6 +38,7 @@
 #include "loudness_core.cuh"
 #include "cqt_core.cuh"
 #include "pitch_core.cuh"
+#include "chroma_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -4031,6 +4032,281 @@ int kapre_pyin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wav
     int grid;
     if ((rc = kb_resident_grid(kb_viterbi_kernel, "viterbi", v.nt, smem, rows, plan->dev.sm_count, &grid))) return rc;
     return kb_launch(kb_viterbi_kernel, {.grid = grid, .block = v.nt, .smem = smem, .st = st, .timed = true}, v);
+}
+
+}  // extern "C"
+
+// ---- chroma features (chroma_core.cuh) ----------------------------------------------------------------------------
+__global__ void __launch_bounds__(KB_CH_THREADS) kb_chroma_kernel(const __grid_constant__ KbChromaParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_chroma_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_CH_THREADS) kb_chroma_bwd_kernel(const __grid_constant__ KbChromaParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_chroma_bwd_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_CH_THREADS) kb_tune_peak_kernel(const __grid_constant__ KbTuneParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_tune_peak_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_CH_THREADS) kb_tune_sel_kernel(const __grid_constant__ KbTuneParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_tune_sel_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_CH_THREADS) kb_tune_argmax_kernel(const __grid_constant__ KbTuneParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_tune_argmax_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_CH_THREADS) kb_cens_kernel(const __grid_constant__ KbCensParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_cens_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+
+struct kapre_chroma_plan {
+    kapre_chroma_plan_desc d;
+    DevInfo dev;
+    float* W = nullptr;                   // n_tables x n_chroma x n_bins
+    float* smooth = nullptr;
+    double* edges = nullptr;
+};
+
+static int kb_chroma_check(const kapre_chroma_plan* plan, const void* x, const kapre_spec_desc* xd, int B, int C, int M,
+                           const void* out, const kapre_spec_desc* od) {
+    if (!plan || !xd || !od) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (B < 0 || C < 0 || M < 0) return kb_fail(KAPRE_E_INVALID, "chroma: negative size (%d, %d, %d)", B, C, M);
+    int cur = -1;
+    KB_CUDA(cudaGetDevice(&cur));
+    if (cur != plan->dev.device)
+        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    if ((long long)B * C * M && (!x || !out)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    return 0;
+}
+
+static int kb_chroma_params(const kapre_chroma_plan* plan, const kapre_chroma_config* cfg, const void* x,
+                            const kapre_spec_desc* xd, int B, int C, int M, const int* tab, KbChromaParams* out) {
+    if (!cfg) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (plan->d.n_tables < 1) return kb_fail(KAPRE_E_INVALID, "chroma: the plan has no filterbank table");
+    if (cfg->in_mode < 0 || cfg->in_mode > 2 || cfg->norm < 0 || cfg->norm > 3)
+        return kb_fail(KAPRE_E_INVALID, "chroma: bad input mode %d or norm %d", cfg->in_mode, cfg->norm);
+    KbChromaParams p{};
+    p.NC = plan->d.n_chroma; p.K = plan->d.n_bins;
+    p.in_mode = cfg->in_mode; p.norm = cfg->norm; p.has_thr = cfg->has_threshold; p.thr = cfg->threshold;
+    p.W = plan->W; p.tab = tab;
+    kb_chroma_tiling(p);
+    p.B = B; p.C = C; p.M = M;
+    p.x = x; p.x_sb = xd->stride_b; p.x_sc = xd->stride_c; p.x_st = xd->stride_t; p.x_sk = xd->stride_f;
+    if (!kb_chroma_setup(p)) return kb_fail(KAPRE_E_INVALID, "chroma: too many tiles");
+    *out = p;
+    return 0;
+}
+
+static int kb_chroma_fwd_launch(const kapre_chroma_plan* plan, const KbChromaParams& p, cudaStream_t st) {
+    const int smem = kb_chroma_smem(p.NC, p.G, p.TF);
+    int grid, rc;
+    if ((rc = kb_resident_grid(kb_chroma_kernel, "chroma", KB_CH_THREADS, smem, p.jobs, plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_chroma_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = smem, .st = st, .timed = true}, p);
+}
+
+static int64_t kb_tune_ws(const kapre_chroma_plan* plan, long long B, long long rows, long long M, int64_t* off) {
+    const long long cap = (plan->d.peak_hi - plan->d.peak_lo + 1) / 2;
+    int64_t o = 0;
+    off[0] = o; o += (B * 1024 * 4 + 255) / 256 * 256;                         // radix histograms
+    off[1] = o; o += (B * plan->d.n_tuning_bins * 4 + 255) / 256 * 256;         // residual histograms
+    off[2] = o; o += (B * 4 + 255) / 256 * 256;                                 // smallest mag above the lower rank
+    off[3] = o; o += (rows * M * cap * 4 + 255) / 256 * 256;                    // peak mags
+    off[4] = o; o += (rows * M * cap * 4 + 255) / 256 * 256;                    // peak pitches
+    return o;
+}
+
+extern "C" {
+
+int kapre_chroma_plan_create(const kapre_chroma_plan_desc* desc, kapre_chroma_plan** out) {
+    if (!desc || !out) return kb_fail(KAPRE_E_INVALID, "null argument");
+    *out = nullptr;
+    const kapre_chroma_plan_desc& d = *desc;
+    if (d.n_chroma < 1 || d.n_chroma > KAPRE_CHROMA_MAX_CHROMA)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "chroma: n_chroma %d outside [1, %d]", d.n_chroma, KAPRE_CHROMA_MAX_CHROMA);
+    if (d.n_bins < 1 || d.n_bins > KAPRE_CHROMA_MAX_BINS || d.n_tables < 0 || (d.n_tables && !d.tables))
+        return kb_fail(KAPRE_E_INVALID, "chroma: bad table (%d bins, %d tables)", d.n_bins, d.n_tables);
+    if (d.n_smooth < 0 || d.n_smooth > KAPRE_CHROMA_MAX_SMOOTH || (d.n_smooth && !d.smooth))
+        return kb_fail(KAPRE_E_INVALID, "chroma: bad smoothing window of %d taps", d.n_smooth);
+    if (d.n_tuning_bins < 0 || d.n_tuning_bins > KAPRE_CHROMA_MAX_TUNING_BINS || (d.n_tuning_bins && !d.tuning_edges))
+        return kb_fail(KAPRE_E_INVALID, "chroma: bad tuning histogram of %d bins", d.n_tuning_bins);
+    if (d.n_tuning_bins && (d.peak_lo < 1 || d.peak_hi > d.n_bins - 1 || d.peak_hi <= d.peak_lo ||
+                            !(d.sample_rate > 0.0f) || !(d.n_fft > 0.0f) || !(d.bins_per_octave > 0.0)))
+        return kb_fail(KAPRE_E_INVALID, "chroma: bad peak range [%d, %d) of %d bins", d.peak_lo, d.peak_hi, d.n_bins);
+    kapre_chroma_plan* pl = new kapre_chroma_plan();
+    pl->d = d;
+    pl->d.tables = nullptr; pl->d.smooth = nullptr; pl->d.tuning_edges = nullptr;
+    int rc = kb_dev_info(&pl->dev);
+    if (!rc && d.n_tables) {
+        const size_t n = (size_t)d.n_tables * d.n_chroma * d.n_bins;
+        std::vector<float> h(n);
+        for (size_t i = 0; i < n; ++i) h[i] = (float)d.tables[i];
+        rc = kb_upload(h, &pl->W);
+    }
+    if (!rc && d.n_smooth) {
+        std::vector<float> h(d.smooth, d.smooth + d.n_smooth);
+        rc = kb_upload(h, &pl->smooth);
+    }
+    if (!rc && d.n_tuning_bins) {
+        std::vector<double> h(d.tuning_edges, d.tuning_edges + d.n_tuning_bins + 1);
+        rc = kb_upload(h, &pl->edges);
+    }
+    if (rc) {
+        kapre_chroma_plan_destroy(pl);
+        return rc;
+    }
+    *out = pl;
+    return 0;
+}
+
+void kapre_chroma_plan_destroy(kapre_chroma_plan* plan) {
+    if (!plan) return;
+    cudaFree(plan->W);
+    cudaFree(plan->smooth);
+    cudaFree(plan->edges);
+    delete plan;
+}
+
+int kapre_chroma(const kapre_chroma_plan* plan, const kapre_chroma_config* cfg, const void* x_dev,
+                 const kapre_spec_desc* x_desc, int batch, int channels, int frames, const int* table_dev, float* out_dev,
+                 const kapre_spec_desc* out_desc, void* stream) {
+    int rc = kb_chroma_check(plan, x_dev, x_desc, batch, channels, frames, out_dev, out_desc);
+    if (rc) return rc;
+    KbChromaParams p;
+    if ((rc = kb_chroma_params(plan, cfg, x_dev, x_desc, batch, channels, frames, table_dev, &p))) return rc;
+    if (!p.jobs) return 0;
+    p.out = out_dev; p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t;
+    p.o_sk = out_desc->stride_f;
+    return kb_chroma_fwd_launch(plan, p, (cudaStream_t)stream);
+}
+
+int kapre_chroma_backward(const kapre_chroma_plan* plan, const kapre_chroma_config* cfg, const void* x_dev,
+                          const kapre_spec_desc* x_desc, int batch, int channels, int frames, const int* table_dev,
+                          const float* g_dev, const kapre_spec_desc* g_desc, void* gx_dev, const kapre_spec_desc* gx_desc,
+                          void* stream) {
+    int rc = kb_chroma_check(plan, x_dev, x_desc, batch, channels, frames, gx_dev, gx_desc);
+    if (rc) return rc;
+    if (!g_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbChromaParams p;
+    if ((rc = kb_chroma_params(plan, cfg, x_dev, x_desc, batch, channels, frames, table_dev, &p))) return rc;
+    if (!p.jobs) return 0;
+    if (!g_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.g = g_dev; p.g_sb = g_desc->stride_b; p.g_sc = g_desc->stride_c; p.g_st = g_desc->stride_t;
+    p.g_sk = g_desc->stride_f;
+    p.gx = gx_dev; p.gx_sb = gx_desc->stride_b; p.gx_sc = gx_desc->stride_c; p.gx_st = gx_desc->stride_t;
+    p.gx_sk = gx_desc->stride_f;
+    const int smem = kb_chroma_smem(p.NC, p.G, p.TF);
+    int grid;
+    if ((rc = kb_resident_grid(kb_chroma_bwd_kernel, "chroma_bwd", KB_CH_THREADS, smem, p.jobs, plan->dev.sm_count,
+                               &grid)))
+        return rc;
+    return kb_launch(kb_chroma_bwd_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = smem,
+                                            .st = (cudaStream_t)stream}, p);
+}
+
+int64_t kapre_chroma_cens_workspace_bytes(const kapre_chroma_plan* plan, int batch, int channels, int frames) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "chroma: negative size");
+    return (int64_t)batch * channels * frames * plan->d.n_chroma * 4;
+}
+
+int kapre_chroma_cens(const kapre_chroma_plan* plan, int in_mode, const void* x_dev, const kapre_spec_desc* x_desc,
+                      int batch, int channels, int frames, float* out_dev, const kapre_spec_desc* out_desc,
+                      void* workspace_dev, void* stream) {
+    int rc = kb_chroma_check(plan, x_dev, x_desc, batch, channels, frames, out_dev, out_desc);
+    if (rc) return rc;
+    if (plan->d.n_smooth < 1) return kb_fail(KAPRE_E_INVALID, "chroma_cens: the plan has no smoothing window");
+    const kapre_chroma_config cfg = {in_mode, KAPRE_CHROMA_NORM_L1, 1, 0.0f};
+    KbChromaParams p;
+    if ((rc = kb_chroma_params(plan, &cfg, x_dev, x_desc, batch, channels, frames, nullptr, &p))) return rc;
+    if (!p.jobs) return 0;
+    if (!workspace_dev) return kb_fail(KAPRE_E_INVALID, "null workspace");
+    const int NC = plan->d.n_chroma;
+    p.cens = 1;
+    p.out = (float*)workspace_dev;
+    p.o_sc = (long long)frames * NC; p.o_sb = channels * p.o_sc; p.o_st = NC; p.o_sk = 1;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = kb_chroma_fwd_launch(plan, p, st))) return rc;
+    KbCensParams c{};
+    c.NC = NC; c.N = plan->d.n_smooth; c.w = plan->smooth;
+    c.B = batch; c.C = channels; c.M = frames;
+    c.tiles = ((long long)frames + KB_CH_SMOOTH_TF - 1) / KB_CH_SMOOTH_TF;
+    c.jobs = (long long)batch * channels * c.tiles;
+    c.q = (const float*)workspace_dev;
+    c.out = out_dev; c.o_sb = out_desc->stride_b; c.o_sc = out_desc->stride_c; c.o_st = out_desc->stride_t;
+    c.o_sk = out_desc->stride_f;
+    const int smem = kb_cens_smem(NC, c.N);
+    if (smem > plan->dev.smem_optin) return kb_fail(KAPRE_E_UNSUPPORTED, "chroma_cens: %d B of shared memory", smem);
+    int grid;
+    if ((rc = kb_resident_grid(kb_cens_kernel, "cens", KB_CH_THREADS, smem, c.jobs, plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_cens_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = smem, .st = st}, c);
+}
+
+int64_t kapre_chroma_tuning_workspace_bytes(const kapre_chroma_plan* plan, int batch, int channels, int frames) {
+    if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
+    if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "chroma: negative size");
+    if (!plan->d.n_tuning_bins) return kb_fail(KAPRE_E_INVALID, "chroma: the plan has no tuning estimate");
+    int64_t off[5];
+    return kb_tune_ws(plan, batch, (long long)batch * channels, frames, off);
+}
+
+int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float* x_dev, const kapre_spec_desc* x_desc,
+                        int batch, int channels, int frames, double* tuning_dev, int* table_dev, void* workspace_dev,
+                        void* stream) {
+    int rc = kb_chroma_check(plan, x_dev, x_desc, batch, channels, frames, tuning_dev, x_desc);
+    if (rc) return rc;
+    if (!plan->d.n_tuning_bins) return kb_fail(KAPRE_E_INVALID, "chroma: the plan has no tuning estimate");
+    if (in_mode != KAPRE_CHROMA_IN_LINEAR && in_mode != KAPRE_CHROMA_IN_SQUARE)
+        return kb_fail(KAPRE_E_INVALID, "estimate_tuning: bad input mode %d", in_mode);
+    if (batch == 0) return 0;
+    if (!tuning_dev || !table_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    const cudaStream_t st = (cudaStream_t)stream;
+    KbTuneParams p{};
+    const kapre_chroma_plan_desc& d = plan->d;
+    p.K = d.n_bins; p.lo = d.peak_lo; p.hi = d.peak_hi; p.cap = (d.peak_hi - d.peak_lo + 1) / 2;
+    p.in_mode = in_mode; p.sr = d.sample_rate; p.nfft = d.n_fft; p.bpo = d.bins_per_octave;
+    p.nres = d.n_tuning_bins; p.edges = plan->edges;
+    p.B = batch; p.C = channels; p.M = frames;
+    p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_st = x_desc->stride_t;
+    p.x_sk = x_desc->stride_f;
+    int64_t off[5];
+    kb_tune_ws(plan, batch, (long long)batch * channels, frames, off);
+    char* w = (char*)workspace_dev;
+    p.hist = (unsigned*)(w + off[0]); p.res = (unsigned*)(w + off[1]); p.above = (unsigned*)(w + off[2]);
+    p.mag = (float*)(w + off[3]); p.pitch = (float*)(w + off[4]);
+    p.tuning = tuning_dev; p.tab = table_dev;
+    KB_CUDA(cudaMemsetAsync(w, 0, (size_t)off[2], st));
+    KB_CUDA(cudaMemsetAsync(w + off[2], 0xff, (size_t)batch * 4, st));
+    const long long rows = (long long)batch * channels;
+    int grid;
+    if (frames > 0) {
+        p.tiles = ((long long)frames + KB_CH_PEAK_TF - 1) / KB_CH_PEAK_TF;
+        p.jobs = rows * p.tiles;
+        if ((rc = kb_resident_grid(kb_tune_peak_kernel, "tune_peak", KB_CH_THREADS, kb_tune_peak_smem(), p.jobs,
+                                   plan->dev.sm_count, &grid)))
+            return rc;
+        if ((rc = kb_launch(kb_tune_peak_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = kb_tune_peak_smem(),
+                                                  .st = st}, p)))
+            return rc;
+        p.tiles = ((long long)frames + KB_CH_SEL_TF - 1) / KB_CH_SEL_TF;
+        p.jobs = rows * p.tiles;
+        if ((rc = kb_resident_grid(kb_tune_sel_kernel, "tune_select", KB_CH_THREADS, kb_tune_sel_smem(), p.jobs,
+                                   plan->dev.sm_count, &grid)))
+            return rc;
+        for (p.pass = 1; p.pass <= 5; ++p.pass)
+            if ((rc = kb_launch(kb_tune_sel_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = kb_tune_sel_smem(),
+                                                     .st = st}, p)))
+                return rc;
+    }
+    if ((rc = kb_resident_grid(kb_tune_argmax_kernel, "tune_argmax", KB_CH_THREADS, 2 * KB_CH_THREADS * 4, batch,
+                               plan->dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_tune_argmax_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = 2 * KB_CH_THREADS * 4,
+                                             .st = st}, p);
 }
 
 }  // extern "C"

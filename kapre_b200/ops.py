@@ -1974,3 +1974,126 @@ def pyin(x, plan: PitchPlan, data_format=_CH_LAST_STR, cmndf=None):
                                    ctypes.byref(fd), _ptr(cm) if cm is not None else None,
                                    ctypes.byref(cd) if cd is not None else None, _ptr(ws), _stream_ptr()))
     return f0, flag, vp
+
+
+# ------------------------------------------------------------------------------- chroma
+class ChromaPlan(_PerDevice):
+    """kapre_chroma_plan per CUDA device: ``tables``, float64 (n_tables, n_chroma, n_bins) filterbanks (rounded once
+    to float32 on upload), optionally the CENS smoothing taps ``smooth`` and the tuning estimate's geometry ``tuning``
+    (a dict of ``edges``, ``lo``, ``hi``, ``sample_rate``, ``n_fft`` and ``bins_per_octave``)."""
+
+    def __init__(self, tables, smooth=None, tuning=None, n_chroma=None, n_bins=None):
+        if tables is None:
+            self.tables = np.zeros((0, int(n_chroma), int(n_bins)))
+        else:
+            self.tables = np.ascontiguousarray(tables, dtype=np.float64)
+        if self.tables.ndim != 3:
+            raise ValueError('chroma tables must be (n_tables, n_chroma, n_bins)')
+        self.n_tables, self.n_chroma, self.n_bins = self.tables.shape
+        self.smooth = None if smooth is None else np.ascontiguousarray(smooth, dtype=np.float64)
+        self.tuning = tuning
+        self._edges = None
+        nres, lo, hi, sr, nfft, bpo = 0, 0, 0, 0.0, 0.0, 0.0
+        if tuning is not None:
+            self._edges = np.ascontiguousarray(tuning['edges'], dtype=np.float64)
+            nres = self._edges.size - 1
+            lo, hi = tuning['lo'], tuning['hi']
+            sr, nfft, bpo = tuning['sample_rate'], tuning['n_fft'], tuning['bins_per_octave']
+        vp = lambda a: None if a is None else a.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
+        self.desc = N.ChromaPlanDesc(self.n_chroma, self.n_bins, self.n_tables, vp(self.tables) if self.n_tables
+                                     else None, 0 if self.smooth is None else self.smooth.size, vp(self.smooth), nres,
+                                     vp(self._edges), lo, hi, sr, nfft, bpo)
+        self._per_device = {}
+
+    _destroy = 'kapre_chroma_plan_destroy'
+
+    def _create(self, lib, out):
+        return lib.kapre_chroma_plan_create(ctypes.byref(self.desc), out)
+
+
+def _chroma_input(x, plan: ChromaPlan, data_format, complex_ok):
+    """The spectrogram input of a chroma op: (tensor, its SpecDesc, (B, C, M)); its bins must match the plan."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise N.KapreNativeError('chroma needs a CUDA spectrogram')
+    if x.dim() != 4:
+        raise ValueError('chroma expects a 4-D spectrogram batch, got shape %s' % (tuple(x.shape),))
+    if x.dtype == torch.complex64 and not complex_ok:
+        raise ValueError('this chroma input must be real')
+    if x.dtype not in (torch.float32, torch.complex64):
+        raise ValueError('chroma expects float32 (or complex64) input, got %s' % (x.dtype,))
+    x = _raw(x)
+    xd, (B, C, M, K) = _spec_desc(x, data_format)
+    if K != plan.n_bins:
+        raise ValueError('the chroma filterbank expects %d bins, the input has %d' % (plan.n_bins, K))
+    return x, xd, (B, C, M)
+
+
+def chroma_forward(x, plan: ChromaPlan, cfg, data_format, table=None):
+    x, xd, (B, C, M) = _chroma_input(x, plan, data_format, True)
+    out, od = _spec_alloc(B, C, M, plan.n_chroma, data_format, torch.float32, x.device)
+    if out.numel():
+        N.check(N.lib().kapre_chroma(plan.handle(), ctypes.byref(cfg), _ptr(x), ctypes.byref(xd), B, C, M,
+                                     _ptr(table) if table is not None else None, _ptr(out), ctypes.byref(od),
+                                     _stream_ptr()))
+    return out
+
+
+def chroma_backward(g, x, plan: ChromaPlan, cfg, data_format, table=None):
+    x, xd, (B, C, M) = _chroma_input(x, plan, data_format, True)
+    g = _raw(g.to(torch.float32))
+    gd, _ = _spec_desc(g, data_format)
+    gx, gxd = _spec_alloc(B, C, M, plan.n_bins, data_format, x.dtype, x.device)
+    if gx.numel():
+        N.check(N.lib().kapre_chroma_backward(plan.handle(), ctypes.byref(cfg), _ptr(x), ctypes.byref(xd), B, C, M,
+                                              _ptr(table) if table is not None else None, _ptr(g), ctypes.byref(gd),
+                                              _ptr(gx), ctypes.byref(gxd), _stream_ptr()))
+    return gx
+
+
+@_device_of_first_arg
+def chroma(x, plan: ChromaPlan, in_mode, norm, threshold=None, data_format=_CH_LAST_STR, table=None):
+    """Chroma of a CUDA spectrogram batch ``(B, M, K, C)`` / ``(B, C, M, K)`` under ``plan``: float32 ``(B, M,
+    n_chroma, C)`` / ``(B, C, M, n_chroma)``.  ``in_mode``: ``N.CHROMA_IN_*`` (the input as it is, squared, or the
+    modulus of complex64); ``norm``: ``N.CHROMA_NORM_*``; ``table``: an int32 CUDA tensor of one filterbank index per
+    item (else table 0).  One launch.  Differentiable with respect to x; ``table`` is a constant."""
+    cfg = N.ChromaCfg(int(in_mode), int(norm), int(threshold is not None),
+                      0.0 if threshold is None else float(threshold))
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.chroma(x, plan, cfg, data_format, table)
+    return chroma_forward(x, plan, cfg, data_format, table)
+
+
+@_device_of_first_arg
+def chroma_cens(x, plan: ChromaPlan, in_mode, data_format=_CH_LAST_STR):
+    """CENS of a CUDA spectrogram batch under a plan with smoothing taps: the L1-normalised chroma (threshold 0)
+    quantised, smoothed along time and L2-normalised.  Two launches.  No gradient: the output carries no
+    ``grad_fn``."""
+    x, xd, (B, C, M) = _chroma_input(x.detach(), plan, data_format, True)
+    out, od = _spec_alloc(B, C, M, plan.n_chroma, data_format, torch.float32, x.device)
+    if out.numel():
+        n = int(N.lib().kapre_chroma_cens_workspace_bytes(plan.handle(), B, C, M))
+        if n < 0:
+            N.check(n)
+        ws = torch.empty(max(n // 4, 1), dtype=torch.float32, device=x.device)
+        N.check(N.lib().kapre_chroma_cens(plan.handle(), int(in_mode), _ptr(x), ctypes.byref(xd), B, C, M, _ptr(out),
+                                          ctypes.byref(od), _ptr(ws), _stream_ptr()))
+    return out
+
+
+@_device_of_first_arg
+def chroma_tuning(x, plan: ChromaPlan, in_mode, data_format=_CH_LAST_STR):
+    """librosa's ``estimate_tuning`` per item of a CUDA spectrogram batch (power with ``N.CHROMA_IN_SQUARE`` of a
+    magnitude, or as given with ``N.CHROMA_IN_LINEAR``): ``(tuning, table)``, a float64 ``(B,)`` tensor and the int32
+    index of each item's filterbank table.  Seven launches; nothing is read back to the host.  No gradient."""
+    x, xd, (B, C, M) = _chroma_input(x.detach(), plan, data_format, False)
+    tuning = torch.empty(B, dtype=torch.float64, device=x.device)
+    table = torch.empty(B, dtype=torch.int32, device=x.device)
+    if B:
+        n = int(N.lib().kapre_chroma_tuning_workspace_bytes(plan.handle(), B, C, M))
+        if n < 0:
+            N.check(n)
+        ws = torch.empty(max((n + 3) // 4, 1), dtype=torch.float32, device=x.device)
+        N.check(N.lib().kapre_chroma_tuning(plan.handle(), int(in_mode), _ptr(x), ctypes.byref(xd), B, C, M,
+                                            _ptr(tuning), _ptr(table), _ptr(ws), _stream_ptr()))
+    return tuning, table

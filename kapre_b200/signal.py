@@ -7,6 +7,7 @@ real factor, band-limited interpolation), ``Convolve`` (convolution with long fi
 filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan), or
 ``add_noise`` (torchaudio's, with deterministic float64 energies), or ``loudness`` and ``Loudness`` (torchaudio's
 BS.1770 gated loudness, with per-item lengths), or the pitch trackers ``yin``, ``pyin``, ``YIN`` and ``PYIN``
+(librosa's), or the chroma features ``chroma_stft``, ``chroma_cqt``, ``chroma_cens`` and ``estimate_tuning``
 (librosa's)."""
 from __future__ import annotations
 
@@ -21,7 +22,7 @@ from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
            'Biquad', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
-           'YIN', 'PYIN']
+           'YIN', 'PYIN', 'chroma_stft', 'chroma_cqt', 'chroma_cens', 'estimate_tuning']
 
 
 def _resolve(fmt):
@@ -664,3 +665,218 @@ class PYIN(Layer):
         ('no_trough_prob', 'no_trough_prob'), ('fill_na', 'fill_na'), ('center', 'center'),
         ('data_format', 'data_format_str'),
     )
+
+
+# ---- chroma ------------------------------------------------------------------------------------------------------------
+_chroma_plans = {}
+
+
+def _cached(key, make):
+    plan = _chroma_plans.get(key)
+    if plan is None:
+        plan = make()
+        _chroma_plans[key] = plan
+    return plan
+
+
+def _stft_chroma_plans(sample_rate, n_fft, hop_length, window_name, n_chroma, tuning, ctroct, octwidth, base_c,
+                       bins_per_octave=None, resolution=0.01, tables=True):
+    """(StftPlan, ChromaPlan) of one chroma_stft / estimate_tuning configuration.  ``tuning=None``: one table per
+    left edge of the tuning grid plus one for 0.0 (items without peaks), and the tuning estimate."""
+    n_fft = backend._check_n_fft(n_fft)
+    n_chroma = backend._check_n_chroma(n_chroma)
+    if isinstance(hop_length, bool) or int(hop_length) != hop_length or int(hop_length) < 1:
+        raise ValueError('hop_length must be a positive integer, got %r' % (hop_length,))
+    hop_length = int(hop_length)
+    sr = float(sample_rate)
+    if not (np.isfinite(sr) and sr > 0):
+        raise ValueError('sample_rate must be positive, got %r' % (sample_rate,))
+    stft = _cached(('stft', n_fft, hop_length, window_name),
+                   lambda: ops.StftPlan(n_fft, n_fft, hop_length, backend.get_window_fn(window_name)(n_fft)))
+    fb = dict(ctroct=ctroct, octwidth=octwidth, base_c=bool(base_c))
+    if tuning is not None:
+        t = float(tuning)
+        key = ('chroma', sr, n_fft, n_chroma, t, ctroct, octwidth, bool(base_c))
+        return stft, _cached(key, lambda: ops.ChromaPlan(
+            backend.chroma_filterbank(sr, n_fft, n_chroma, t, **fb)[None]))
+    bpo = n_chroma if bins_per_octave is None else bins_per_octave
+    if isinstance(bpo, bool) or not (np.isfinite(float(bpo)) and float(bpo) > 0):
+        raise ValueError('bins_per_octave must be positive, got %r' % (bins_per_octave,))
+    edges = backend.tuning_edges(resolution)
+    lo, hi = backend.piptrack_bins(sr, n_fft)
+    est = dict(edges=edges, lo=lo, hi=hi, sample_rate=sr, n_fft=float(n_fft), bins_per_octave=float(bpo))
+    if not tables:
+        key = ('tuning', sr, n_fft, float(bpo), float(resolution))
+        return stft, _cached(key, lambda: ops.ChromaPlan(None, tuning=est, n_chroma=1, n_bins=n_fft // 2 + 1))
+    key = ('chroma_est', sr, n_fft, n_chroma, float(resolution), ctroct, octwidth, bool(base_c))
+
+    def make():
+        grid = [backend.chroma_filterbank(sr, n_fft, n_chroma, e, **fb) for e in edges[:-1]]
+        grid.append(backend.chroma_filterbank(sr, n_fft, n_chroma, 0.0, **fb))
+        return ops.ChromaPlan(np.stack(grid), tuning=est)
+    return stft, _cached(key, make)
+
+
+def _centred_magnitude(waveform, stft, fmt, center):
+    """|STFT| of ``waveform`` with ``n_fft // 2`` zeros on each side when ``center``: a pad in front of the fused
+    STFT-magnitude launch, differentiable through both."""
+    if not (isinstance(waveform, torch.Tensor) and waveform.is_cuda):
+        raise ops.N.KapreNativeError('chroma needs a CUDA waveform')
+    if waveform.dim() != 3:
+        raise ValueError('expected a 3-D waveform batch, got shape %s' % (tuple(waveform.shape),))
+    x = waveform.to(torch.float32)
+    if center:
+        h = stft.n_fft // 2
+        x = torch.nn.functional.pad(x, (0, 0, h, h) if fmt == _CH_LAST_STR else (h, h))
+    return ops.stft_forward(x, stft, fmt, fmt, False, False, ops.N.OUT_MAG)
+
+
+def _spectrogram_arg(S, name, fmt, bins, allow_complex=False):
+    if not (isinstance(S, torch.Tensor) and S.is_cuda):
+        raise ops.N.KapreNativeError('%s must be a CUDA tensor' % name)
+    if S.dim() != 4:
+        raise ValueError('%s must be 4-D, got shape %s' % (name, tuple(S.shape)))
+    K = S.shape[2] if fmt == _CH_LAST_STR else S.shape[3]
+    if K != bins:
+        raise ValueError('%s has %d bins, expected %d' % (name, K, bins))
+    if not (S.dtype == torch.float32 or (allow_complex and S.dtype == torch.complex64)):
+        raise ValueError('%s must be float32%s, got %s' % (name, ' or complex64' if allow_complex else '', S.dtype))
+    return S
+
+
+def chroma_stft(waveform=None, sample_rate=22050, S=None, norm=np.inf, n_fft=2048, hop_length=512, win_length=None,
+                window_name=None, center=True, tuning=None, n_chroma=12, ctroct=5.0, octwidth=2.0, base_c=True,
+                data_format='default'):
+    """Chroma of a power spectrogram (modelled on ``librosa.feature.chroma_stft``): float32 ``(batch, frames,
+    n_chroma, ch)`` / ``(batch, ch, frames, n_chroma)``.
+
+    From ``waveform`` (``(batch, time, ch)`` / ``(batch, ch, time)`` float32 CUDA), S = |STFT|^2 with the periodic
+    Hann window (``window_name``) of ``n_fft`` samples every ``hop_length``, unnormalised; with ``center`` the signal
+    first gets ``n_fft // 2`` zeros on each side (librosa's ``pad_mode='constant'``), giving ``1 + time // hop``
+    frames.  ``win_length`` must be None or ``n_fft``.  ``S`` (instead of a waveform): a power spectrogram in this
+    library's layout, used as given.  The chroma is ``normalize(W @ S, norm)`` with W =
+    ``backend.chroma_filterbank(sample_rate, n_fft, n_chroma, tuning, ctroct, octwidth, base_c)``; ``norm`` is inf,
+    1, 2 or None, and a frame whose length is below FLT_MIN is left as it is.
+
+    ``tuning=None`` estimates each item's tuning from S (``estimate_tuning`` with ``bins_per_octave=n_chroma``) on
+    the device: the plan holds a table per edge of the tuning grid and the projection reads each item's index, so
+    nothing is synchronised with the host and the call can be captured in a CUDA graph; the result equals
+    ``chroma_stft(tuning=t_i)`` item by item, bit for bit.
+
+    Launches: the STFT magnitude and the projection (2), plus 7 with ``tuning=None``; from ``S`` only the chroma
+    launches.  Differentiable with respect to the waveform and ``S``; the tuning estimate is a constant."""
+    fmt = _resolve(_unwrap_format(data_format))
+    code = backend.chroma_norm_code(norm)
+    if win_length is not None and win_length != n_fft:
+        raise ValueError('win_length must be None or n_fft=%r, got %r: the STFT does not centre a shorter window'
+                         % (n_fft, win_length))
+    if (waveform is None) == (S is None):
+        raise ValueError('pass exactly one of waveform and S')
+    stft, plan = _stft_chroma_plans(sample_rate, n_fft, hop_length, window_name, n_chroma, tuning, ctroct, octwidth,
+                                    base_c)
+    if S is None:
+        X = _centred_magnitude(waveform, stft, fmt, center)
+        mode = ops.N.CHROMA_IN_SQUARE
+    else:
+        X = _spectrogram_arg(S, 'S', fmt, n_fft // 2 + 1)
+        mode = ops.N.CHROMA_IN_LINEAR
+    table = None
+    if tuning is None:
+        table = ops.chroma_tuning(X, plan, mode, fmt)[1]
+    return ops.chroma(X, plan, mode, code, None, fmt, table)
+
+
+def estimate_tuning(waveform=None, sample_rate=22050, S=None, n_fft=2048, hop_length=None, resolution=0.01,
+                    bins_per_octave=12, data_format='default'):
+    """librosa's ``estimate_tuning`` per item (over all its channels) on the device: a float64 ``(batch,)`` CUDA
+    tensor of tunings in fractions of a bin of ``bins_per_octave``, in [-0.5, 0.5).
+
+    piptrack's peaks (``fmin=150``, ``fmax=min(4000, sr / 2)``, ``threshold=0.1``) of S, from ``waveform`` the
+    centred |STFT| (``power=1``, hop ``n_fft // 4`` by default) or the given ``S`` (the library's layout); the peaks
+    with magnitude at or above their exact median; the residual ``mod(bins_per_octave log2(pitch / 27.5), 1)`` in
+    [-0.5, 0.5) binned over ``linspace(-0.5, 0.5, ceil(1 / resolution) + 1)``; the left edge of the first fullest
+    bin.  An item without peaks gives 0.0, and a frame holding a non-finite bin has no peaks.  Launches: the STFT
+    magnitude (from a waveform) and 7, whatever the data; nothing is read back.  No gradient: an input that requires
+    grad is accepted and the output carries no ``grad_fn``."""
+    fmt = _resolve(_unwrap_format(data_format))
+    if (waveform is None) == (S is None):
+        raise ValueError('pass exactly one of waveform and S')
+    n_fft = backend._check_n_fft(n_fft)
+    hop = n_fft // 4 if hop_length is None else hop_length
+    stft, plan = _stft_chroma_plans(sample_rate, n_fft, hop, None, 1, None, 5.0, 2.0, True, bins_per_octave,
+                                    resolution, tables=False)
+    with torch.no_grad():
+        if S is None:
+            X = _centred_magnitude(waveform.detach(), stft, fmt, True)
+        else:
+            X = _spectrogram_arg(S, 'S', fmt, n_fft // 2 + 1).detach()
+        return ops.chroma_tuning(X, plan, ops.N.CHROMA_IN_LINEAR, fmt)[0]
+
+
+def _cqt_chroma_plans(sample_rate, hop_length, f_min, tuning, n_chroma, n_octaves, bins_per_octave, base_c, smooth):
+    n_chroma = backend._check_n_chroma(n_chroma)
+    for name, v in (('n_octaves', n_octaves), ('bins_per_octave', bins_per_octave)):
+        if isinstance(v, bool) or int(v) != v or int(v) < 1:
+            raise ValueError('%s must be a positive integer, got %r' % (name, v))
+    if isinstance(tuning, bool) or tuning is None or not np.isfinite(float(tuning)):
+        raise ValueError('tuning must be a finite number (per-item tuning needs a CQT plan per item), got %r'
+                         % (tuning,))
+    bpo, n_bins = int(bins_per_octave), int(n_octaves) * int(bins_per_octave)
+    fmin = backend.CQT_C1 if f_min is None else float(f_min)
+    m = backend.cq_to_chroma(n_bins, bpo, n_chroma, fmin, base_c)
+    ftuned = fmin * 2.0 ** (float(tuning) / bpo)
+    cqt = _cached(('cqt', float(sample_rate), int(hop_length), ftuned, n_bins, bpo),
+                  lambda: ops.CqtPlan(sample_rate, hop_length, ftuned, n_bins, bpo))
+    taps = None if smooth is False else backend.cens_window(smooth)
+    key = ('cq_chroma', n_bins, bpo, n_chroma, fmin, bool(base_c), None if taps is None else tuple(taps))
+    return cqt, _cached(key, lambda: ops.ChromaPlan(m[None], smooth=taps))
+
+
+def _cq_magnitude(waveform, C, cqt, fmt):
+    if (waveform is None) == (C is None):
+        raise ValueError('pass exactly one of waveform and C')
+    if C is None:
+        return ops.cqt(waveform, cqt, fmt, fmt, True), ops.N.CHROMA_IN_LINEAR
+    C = _spectrogram_arg(C, 'C', fmt, cqt.n_bins, allow_complex=True)
+    return C, ops.N.CHROMA_IN_COMPLEX if C.dtype == torch.complex64 else ops.N.CHROMA_IN_LINEAR
+
+
+def chroma_cqt(waveform=None, sample_rate=22050, C=None, hop_length=512, f_min=None, norm=np.inf, threshold=0.0,
+               tuning=0.0, n_chroma=12, n_octaves=7, bins_per_octave=36, base_c=True, data_format='default'):
+    """Constant-Q chroma (modelled on ``librosa.feature.chroma_cqt``): float32 ``(batch, frames, n_chroma, ch)`` /
+    ``(batch, ch, frames, n_chroma)``.
+
+    C = |CQT| of ``n_octaves * bins_per_octave`` bins from ``f_min 2^(tuning / bins_per_octave)`` (``f_min`` default
+    C1; see ``time_frequency.CQT``), or the given ``C`` (complex64, or float32 |C|, in the CQT's layout).  The chroma
+    is ``normalize(threshold(M @ C), norm)`` with M = ``backend.cq_to_chroma`` (``bins_per_octave`` a multiple of
+    ``n_chroma``), entries below ``threshold`` set to 0 (None: no threshold).  ``tuning`` is a number: librosa's
+    ``None`` would need a CQT plan per item.  Launches: the CQT's (7 at the defaults) and 1; from ``C`` only the
+    chroma launch.  Differentiable with respect to the waveform and ``C``."""
+    fmt = _resolve(_unwrap_format(data_format))
+    code = backend.chroma_norm_code(norm)
+    if threshold is not None and not np.isfinite(float(threshold)):
+        raise ValueError('threshold must be finite or None, got %r' % (threshold,))
+    cqt, plan = _cqt_chroma_plans(sample_rate, hop_length, f_min, tuning, n_chroma, n_octaves, bins_per_octave,
+                                  base_c, False)
+    X, mode = _cq_magnitude(waveform, C, cqt, fmt)
+    return ops.chroma(X, plan, mode, code, threshold, fmt)
+
+
+def chroma_cens(waveform=None, sample_rate=22050, C=None, hop_length=512, f_min=None, tuning=0.0, n_chroma=12,
+                n_octaves=7, bins_per_octave=36, base_c=True, norm=2, win_len_smooth=41, data_format='default'):
+    """Chroma energy normalised statistics (modelled on ``librosa.feature.chroma_cens``): ``chroma_cqt`` with no
+    normalisation, L1-normalised per frame, quantised to ``0.25 #{s in (0.4, 0.2, 0.1, 0.05) : v > s}``, smoothed
+    along time by ``hann(win_len_smooth + 2, symmetric) / sum`` centred with zeros outside the signal
+    (``scipy.ndimage.convolve(mode='constant')``; None or 0: no smoothing) and normalised with ``norm`` (2).  A NaN
+    chroma stays NaN through the quantisation (librosa's would become 0), so it reaches only the frames whose smoothing
+    window holds it.  Launches: the CQT's and 2.  No gradient: an input that requires grad is accepted and the output
+    carries no ``grad_fn``."""
+    fmt = _resolve(_unwrap_format(data_format))
+    if backend.chroma_norm_code(norm) != 3:
+        raise ValueError('chroma_cens supports norm=2 only, got %r' % (norm,))
+    cqt, plan = _cqt_chroma_plans(sample_rate, hop_length, f_min, tuning, n_chroma, n_octaves, bins_per_octave,
+                                  base_c, win_len_smooth)
+    with torch.no_grad():
+        X, mode = _cq_magnitude(None if waveform is None else waveform.detach(),
+                                None if C is None else C.detach(), cqt, fmt)
+        return ops.chroma_cens(X, plan, mode, fmt)

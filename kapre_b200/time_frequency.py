@@ -23,7 +23,8 @@ from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
 __all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
-           'PCEN', 'GriffinLim', 'InverseFilterbank', 'KaldiFbank', 'KaldiMFCC', 'KaldiSpectrogram', 'CQT']
+           'PCEN', 'GriffinLim', 'InverseFilterbank', 'KaldiFbank', 'KaldiMFCC', 'KaldiSpectrogram', 'CQT',
+           'ChromaSTFT', 'ChromaCQT', 'ChromaCENS']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -755,4 +756,104 @@ class CQT(Layer):
         ('scale', 'scale'),
         ('input_data_format', 'input_data_format_original'),
         ('output_data_format', 'output_data_format_original'),
+    )
+
+
+class _ChromaLayer(Layer):
+    """A chroma function of ``signal`` as a layer: the waveform in, the chroma out.  The constructor takes the
+    function's keyword arguments (without the waveform and the precomputed spectrogram), checks them and builds the
+    plans on the host."""
+    _fn = None
+
+    def __init__(self, data_format, args, **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        self.data_format_str = _unwrap_format(data_format)
+        self._kw = args
+        for k, v in args.items():
+            setattr(self, k, v)
+        self._check()
+
+    def call(self, x):
+        from . import signal
+        return getattr(signal, self._fn)(x, data_format=self.data_format_str, **self._kw)
+
+
+@register_keras_serializable(package='Kapre')
+class ChromaSTFT(_ChromaLayer):
+    """``signal.chroma_stft`` as a layer: ``(batch, time, ch)`` / ``(batch, ch, time)`` waveforms in, ``(batch,
+    frames, n_chroma, ch)`` / ``(batch, ch, frames, n_chroma)`` chroma out.  Same arguments."""
+    _fn = 'chroma_stft'
+
+    def __init__(self, sample_rate=22050, norm=np.inf, n_fft=2048, hop_length=512, win_length=None, window_name=None,
+                 center=True, tuning=None, n_chroma=12, ctroct=5.0, octwidth=2.0, base_c=True, data_format='default',
+                 **kwargs):
+        super().__init__(data_format, dict(sample_rate=sample_rate, norm=norm, n_fft=n_fft, hop_length=hop_length,
+                                           win_length=win_length, window_name=window_name, center=center,
+                                           tuning=tuning, n_chroma=n_chroma, ctroct=ctroct, octwidth=octwidth,
+                                           base_c=base_c), **kwargs)
+
+    def _check(self):
+        from . import signal
+        backend.chroma_norm_code(self.norm)
+        if self.win_length is not None and self.win_length != self.n_fft:
+            raise ValueError('win_length must be None or n_fft=%r, got %r' % (self.n_fft, self.win_length))
+        signal._stft_chroma_plans(self.sample_rate, self.n_fft, self.hop_length, self.window_name, self.n_chroma,
+                                  self.tuning, self.ctroct, self.octwidth, self.base_c)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'), ('norm', 'norm'), ('n_fft', 'n_fft'), ('hop_length', 'hop_length'),
+        ('win_length', 'win_length'), ('window_name', 'window_name'), ('center', 'center'), ('tuning', 'tuning'),
+        ('n_chroma', 'n_chroma'), ('ctroct', 'ctroct'), ('octwidth', 'octwidth'), ('base_c', 'base_c'),
+        ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class ChromaCQT(_ChromaLayer):
+    """``signal.chroma_cqt`` as a layer (waveforms in, chroma out).  Same arguments."""
+    _fn = 'chroma_cqt'
+
+    def __init__(self, sample_rate=22050, hop_length=512, f_min=None, norm=np.inf, threshold=0.0, tuning=0.0,
+                 n_chroma=12, n_octaves=7, bins_per_octave=36, base_c=True, data_format='default', **kwargs):
+        super().__init__(data_format, dict(sample_rate=sample_rate, hop_length=hop_length, f_min=f_min, norm=norm,
+                                           threshold=threshold, tuning=tuning, n_chroma=n_chroma, n_octaves=n_octaves,
+                                           bins_per_octave=bins_per_octave, base_c=base_c), **kwargs)
+
+    def _check(self):
+        from . import signal
+        backend.chroma_norm_code(self.norm)
+        signal._cqt_chroma_plans(self.sample_rate, self.hop_length, self.f_min, self.tuning, self.n_chroma,
+                                 self.n_octaves, self.bins_per_octave, self.base_c, False)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'), ('hop_length', 'hop_length'), ('f_min', 'f_min'), ('norm', 'norm'),
+        ('threshold', 'threshold'), ('tuning', 'tuning'), ('n_chroma', 'n_chroma'), ('n_octaves', 'n_octaves'),
+        ('bins_per_octave', 'bins_per_octave'), ('base_c', 'base_c'), ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class ChromaCENS(_ChromaLayer):
+    """``signal.chroma_cens`` as a layer (waveforms in, CENS out).  Same arguments."""
+    _fn = 'chroma_cens'
+
+    def __init__(self, sample_rate=22050, hop_length=512, f_min=None, tuning=0.0, n_chroma=12, n_octaves=7,
+                 bins_per_octave=36, base_c=True, norm=2, win_len_smooth=41, data_format='default', **kwargs):
+        super().__init__(data_format, dict(sample_rate=sample_rate, hop_length=hop_length, f_min=f_min, tuning=tuning,
+                                           n_chroma=n_chroma, n_octaves=n_octaves, bins_per_octave=bins_per_octave,
+                                           base_c=base_c, norm=norm, win_len_smooth=win_len_smooth), **kwargs)
+
+    def _check(self):
+        from . import signal
+        if backend.chroma_norm_code(self.norm) != 3:
+            raise ValueError('chroma_cens supports norm=2 only, got %r' % (self.norm,))
+        signal._cqt_chroma_plans(self.sample_rate, self.hop_length, self.f_min, self.tuning, self.n_chroma,
+                                 self.n_octaves, self.bins_per_octave, self.base_c, self.win_len_smooth)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'), ('hop_length', 'hop_length'), ('f_min', 'f_min'), ('tuning', 'tuning'),
+        ('n_chroma', 'n_chroma'), ('n_octaves', 'n_octaves'), ('bins_per_octave', 'bins_per_octave'),
+        ('base_c', 'base_c'), ('norm', 'norm'), ('win_len_smooth', 'win_len_smooth'),
+        ('data_format', 'data_format_str'),
     )
