@@ -217,7 +217,7 @@ __device__ __forceinline__ void kb_dft_cta(const KbDftParams& p, char* smem, int
                         if (p.mode == KB_OUT_COMPLEX)
                             reinterpret_cast<float2*>(p.out)[o] = make_float2(ar[f], ai[f]);
                         else
-                            reinterpret_cast<float*>(p.out)[o] = kb_sqrt(ar[f] * ar[f] + ai[f] * ai[f]);
+                            reinterpret_cast<float*>(p.out)[o] = kb_cabs(ar[f], ai[f]);
                     }
                 }
             }

@@ -120,7 +120,7 @@ KB_HD int kb_chroma_smem(int NC, int G, int TF) {
 KB_CH_FN float kb_chroma_in(const KbChromaParams& p, long long o) {
     if (p.in_mode == KB_CH_IN_COMPLEX) {
         const float2 c = reinterpret_cast<const float2*>(p.x)[o];
-        return sqrtf(fmaf(c.x, c.x, c.y * c.y));
+        return kb_cabs<true>(c.x, c.y);
     }
     const float v = reinterpret_cast<const float*>(p.x)[o];
     return p.in_mode == KB_CH_IN_SQUARE ? kb_ch_mul(v, v) : v;
@@ -256,7 +256,7 @@ KB_CH_FN void kb_chroma_bwd_cta(const KbChromaParams& p, char* smem, long long c
                 const long long gb = (row / p.C) * p.g_sb + (row % p.C) * p.g_sc + m * p.g_st;
                 float dot = 0.0f;
                 for (int j = 0; j < NC; ++j) dot = fmaf(p.g[gb + j * p.g_sk], kb_chroma_thr(yr[j], p.has_thr, p.thr), dot);
-                const float l2 = len * len;
+                const float dl = (dot / len) / len;   // dot / len^2: len^2 itself leaves the float range below 2^-63
                 for (int j = 0; j < NC; ++j) {
                     const float gj = p.g[gb + j * p.g_sk];
                     const float v = kb_chroma_thr(yr[j], p.has_thr, p.thr);
@@ -266,9 +266,9 @@ KB_CH_FN void kb_chroma_bwd_cta(const KbChromaParams& p, char* smem, long long c
                     } else {
                         const float sg = v > 0.0f ? 1.0f : (v < 0.0f ? -1.0f : 0.0f);
                         gv = gj / len;
-                        if (p.norm == KB_CH_NORM_L1) gv = gv - sg * (dot / l2);
-                        else if (p.norm == KB_CH_NORM_L2) gv = gv - v * (dot / (l2 * len));
-                        else if (j == imax) gv = gv - sg * (dot / l2);
+                        if (p.norm == KB_CH_NORM_L1) gv = gv - sg * dl;
+                        else if (p.norm == KB_CH_NORM_L2) gv = gv - v * (dl / len);
+                        else if (j == imax) gv = gv - sg * dl;
                     }
                     yr[j] = (p.has_thr && yr[j] < p.thr) ? 0.0f : gv;
                 }
@@ -300,9 +300,10 @@ KB_CH_FN void kb_chroma_bwd_cta(const KbChromaParams& p, char* smem, long long c
                 const long long go = gxb + m * p.gx_st + (long long)(k0 + kk) * p.gx_sk;
                 if (p.in_mode == KB_CH_IN_COMPLEX) {
                     const float2 c = reinterpret_cast<const float2*>(p.x)[xo];
-                    const float a = sqrtf(fmaf(c.x, c.x, c.y * c.y));
-                    const float r = a > 0.0f ? s / a : 0.0f;
-                    reinterpret_cast<float2*>(p.gx)[go] = make_float2(r * c.x, r * c.y);
+                    // s (C / |C|): s / |C| overflows for a tiny C whose s scales as 1 / |C|
+                    const float a = kb_cabs<true>(c.x, c.y);
+                    const float sa = a > 0.0f ? s : 0.0f, r = a > 0.0f ? a : 1.0f;
+                    reinterpret_cast<float2*>(p.gx)[go] = make_float2(sa * (c.x / r), sa * (c.y / r));
                 } else if (p.in_mode == KB_CH_IN_SQUARE) {
                     const float a = reinterpret_cast<const float*>(p.x)[xo];
                     reinterpret_cast<float*>(p.gx)[go] = (2.0f * a) * s;

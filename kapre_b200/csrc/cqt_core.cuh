@@ -234,8 +234,8 @@ KB_CQ_FN void kb_cqt_fwd_block(const KbCqtParams& p, const KbCqtSeg& sg, const K
         const long long e = ob + (long long)(t0 + m) * p.o_st + (long long)(o.k0 + kk0) * p.o_sk;
         if (p.mag) {
             float* y = static_cast<float*>(p.out);
-            y[e] = sqrtf(fmaf(a0r[q], a0r[q], a0i[q] * a0i[q]));
-            if (two) y[e + p.o_sk] = sqrtf(fmaf(a1r[q], a1r[q], a1i[q] * a1i[q]));
+            y[e] = kb_cabs<true>(a0r[q], a0i[q]);
+            if (two) y[e + p.o_sk] = kb_cabs<true>(a1r[q], a1i[q]);
         } else {
             float2* y = static_cast<float2*>(p.out);
             y[e] = make_float2(a0r[q], a0i[q]);
@@ -349,7 +349,7 @@ KB_CQ_FN void kb_cqt_bwd_cta(const KbCqtParams& p, char* smem, long long cta, lo
                             ++jj;
                             if (++ph == o.h) { ph = 0; jj += o.pad; }
                         }
-                        const float m = sqrtf(fmaf(cr, cr, ci * ci));
+                        const float m = kb_cabs<true>(cr, ci);
                         const float sc = m > 0.0f ? gc[e].x / m : 0.0f;
                         gc[e] = make_float2(sc * cr, sc * ci);
                     }

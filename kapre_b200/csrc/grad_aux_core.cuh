@@ -21,13 +21,15 @@ KB_FN long long kb_pad_index(long long t, long long T, int mode) {
 }
 
 // ------------------------------------------------------------------------------------------ Phase
-// d angle(X) / dX: gX = g i X / |X|^2 (torch.angle's rule), 0 where |X| = 0.
+// d angle(X) / dX: gX = g i X / |X|^2 (torch.angle's rule), 0 where |X| = 0.  Formed as (g i (X / |X|)) / |X|:
+// every factor stays finite for a tiny or huge X, a part of X that is 0 gives 0 (not inf 0), and only a gradient
+// that really overflows becomes inf.
 KB_FN void kb_phase_bwd_elem(const float2* __restrict__ X, const float* __restrict__ g, float2* __restrict__ gX,
                              long long i) {
     const float2 v = X[i];
-    const float m = kb_sqrt(v.x * v.x + v.y * v.y);
-    const float s = m > 0.0f ? (g[i] / m) / m : 0.0f;
-    gX[i] = make_float2(-s * v.y, s * v.x);
+    const float m = kb_cabs(v.x, v.y);
+    const float s = m > 0.0f ? g[i] : 0.0f, r = m > 0.0f ? m : 1.0f;
+    gX[i] = make_float2(-(s * (v.y / r)) / r, (s * (v.x / r)) / r);
 }
 
 // ------------------------------------------------------------------------------------------ magnitude + phase
@@ -51,10 +53,12 @@ KB_FN void kb_mag_phase_bwd_elem(const KbMagPhaseBwdParams& p, long long i) {
     const float2 v = p.X[b * p.x_sb + c * p.x_sc + t * p.x_st + f * p.x_sf];
     const float gm = p.gm ? p.gm[b * p.m_sb + c * p.m_sc + t * p.m_st + f * p.m_sf] : 0.0f;
     const float gp = p.gp ? p.gp[b * p.p_sb + c * p.p_sc + t * p.p_st + f * p.p_sf] : 0.0f;
-    const float m = kb_sqrt(v.x * v.x + v.y * v.y);
-    float a = 0.0f, q = 0.0f;           // gX = a X + q i X
-    if (m > 0.0f) { a = gm / m; q = (gp / m) / m; }
-    p.gX[b * p.o_sb + c * p.o_sc + t * p.o_st + f * p.o_sf] = make_float2(a * v.x - q * v.y, a * v.y + q * v.x);
+    const float m = kb_cabs(v.x, v.y);
+    const bool ok = m > 0.0f;
+    const float a = ok ? gm : 0.0f, q = ok ? gp : 0.0f, r = ok ? m : 1.0f;   // gX = a U + i (q U) / |X|, U = X / |X|
+    const float ux = v.x / r, uy = v.y / r;
+    p.gX[b * p.o_sb + c * p.o_sc + t * p.o_st + f * p.o_sf] =
+        make_float2(a * ux - (q * uy) / r, a * uy + (q * ux) / r);
 }
 
 // ------------------------------------------------------------------------------------------ Delta

@@ -102,13 +102,14 @@ KB_FN void kb_istft_adj_elem(const KbIstftAdjParams& p, long long i) {
 
 // ------------------------------------------------------------------------------------------ Magnitude
 // d|X| / dX in PyTorch's convention for complex inputs: g X / |X|, 0 where |X| = 0 (tf.math.divide_no_nan,
-// torch.sgn).  |X| is formed exactly as the forward kernels form it.
+// torch.sgn).  |X| is formed exactly as the forward kernels form it.  X / |X| is formed first, so that a tiny or
+// huge X gives its unit vector; a NaN in X still reaches gX.
 KB_FN void kb_mag_bwd_elem(const float2* __restrict__ X, const float* __restrict__ g, float2* __restrict__ gX,
                            long long i) {
     const float2 v = X[i];
-    const float m = kb_sqrt(v.x * v.x + v.y * v.y);
-    const float s = m > 0.0f ? g[i] / m : 0.0f;
-    gX[i] = make_float2(s * v.x, s * v.y);
+    const float m = kb_cabs(v.x, v.y);
+    const float s = m > 0.0f ? g[i] : 0.0f, r = m > 0.0f ? m : 1.0f;
+    gX[i] = make_float2(s * (v.x / r), s * (v.y / r));
 }
 
 // ------------------------------------------------------------------------------------------ MagnitudeToDecibel

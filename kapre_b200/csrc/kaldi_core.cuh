@@ -426,8 +426,8 @@ KB_KALDI_FN void kb_kaldi_pair(const KbKaldiParams& p, const cpx* ex, float* pw,
                     X2 = X1;
                 }
                 const float n1 = cnorm(X1), n2 = cnorm(X2);
-                pg[k] = p.use_power ? n1 : sqrtf(n1);
-                if (kk >= 0) pg[kk] = p.use_power ? n2 : sqrtf(n2);
+                pg[k] = p.use_power ? n1 : kb_cabs<true>(X1.re, X1.im);
+                if (kk >= 0) pg[kk] = p.use_power ? n2 : kb_cabs<true>(X2.re, X2.im);
                 if (xsp) {
                     xsp[g * (P + 1) + k] = X1;
                     if (kk >= 0) xsp[g * (P + 1) + kk] = X2;

@@ -301,7 +301,7 @@ __global__ void kb_magnitude_kernel(const float2* __restrict__ x, float* __restr
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
          i += (long long)gridDim.x * blockDim.x) {
         const float2 v = x[i];
-        y[i] = kb_sqrt(v.x * v.x + v.y * v.y);
+        y[i] = kb_cabs(v.x, v.y);
     }
 }
 

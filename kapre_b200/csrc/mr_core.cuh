@@ -470,11 +470,11 @@ __device__ __forceinline__ void kb_mr_cta_t(const KbMrParams& q, char* smem, int
                         if (q.sk1) bins([&](int k, cpx X) { oc[k] = make_float2(X.re, X.im); });
                         else bins([&](int k, cpx X) { oc[k * sk] = make_float2(X.re, X.im); });
                     } else if (p.mode == KB_OUT_MAG_DB) {
-                        if (q.sk1) bins([&](int k, cpx X) { orl[k] = db(kb_sqrt(cnorm(X))); });
-                        else bins([&](int k, cpx X) { orl[k * sk] = db(kb_sqrt(cnorm(X))); });
+                        if (q.sk1) bins([&](int k, cpx X) { orl[k] = db(kb_cabs(X)); });
+                        else bins([&](int k, cpx X) { orl[k * sk] = db(kb_cabs(X)); });
                     } else {
-                        if (q.sk1) bins([&](int k, cpx X) { orl[k] = kb_sqrt(cnorm(X)); });
-                        else bins([&](int k, cpx X) { orl[k * sk] = kb_sqrt(cnorm(X)); });
+                        if (q.sk1) bins([&](int k, cpx X) { orl[k] = kb_cabs(X); });
+                        else bins([&](int k, cpx X) { orl[k * sk] = kb_cabs(X); });
                     }
                     R.runmax = rmax;
                 }

@@ -207,6 +207,64 @@ KB_D void kb_bar_wait(KbBar* bar, unsigned parity) {
 }
 #endif
 
+// |re + i im| over the whole float range.  The squared norm underflows below |X| ~ 2^-63 (sqrt.approx.ftz flushes it
+// to 0) and overflows above 2^64, so outside n in [2^-64, 2^64] both parts are first scaled by a power of two that
+// brings max(|re|, |im|) to [1, 4).  The scale is exact and even in the squared norm, so the rescaled form gives the
+// bits the plain form would give on the scaled input, and |2^k X| = 2^k |X| bit for bit while the result is normal.
+// Inside the range both squares are normal floats unless one part is below 2^-31 of the other.  RN selects the form
+// of the sites that round correctly, sqrtf(fmaf(re, re, im im)); otherwise kb_sqrt(cnorm(X)).  Zero, inf and NaN take
+// the plain form.  The scales are built from their exponent bits (ldexpf is a library routine with branches).
+KB_HD float kb_pow2(int e) {   // 2^e, -126 <= e <= 127
+#if defined(__CUDA_ARCH__)
+    return __uint_as_float((unsigned)(e + 127) << 23);
+#else
+    const uint32_t u = (uint32_t)(e + 127) << 23;
+    float r;
+    std::memcpy(&r, &u, 4);
+    return r;
+#endif
+}
+// The rescaled branch is rare; the STFT family's form keeps it out of line (__noinline__), so that the unrolled
+// epilogues carry one compare per bin.  The correctly rounded form stays inline: its kernels use no stack.
+template <bool RN>
+#if defined(KB_HOST_EMU)
+static inline float kb_cabs_rescaled(float re, float im)
+#else
+__device__ __forceinline__ float kb_cabs_rescaled(float re, float im)
+#endif
+{
+    auto plain = [](float x, float y) { return RN ? sqrtf(fmaf(x, x, y * y)) : kb_sqrt(cnorm(cmake(x, y))); };
+    const float a = fmaxf(fabsf(re), fabsf(im));
+    if (!(a > 0.0f) || a > 3.40282347e38f) return plain(re, im);
+    const int f = (int)(kb_f2u(a) >> 23);                          // biased exponent of a
+    const int e = (f < 1 ? 1 : f > 253 ? 253 : f) - 127;           // a in [2^e, 2^(e+1)) unless subnormal / top
+    const float down = kb_pow2(-e);
+    return plain(re * down, im * down) * kb_pow2(e);
+}
+#if !defined(KB_HOST_EMU)
+__device__ __noinline__ float kb_cabs_rescaled_approx(float re, float im) { return kb_cabs_rescaled<false>(re, im); }
+#endif
+template <bool RN = false>
+#if defined(KB_HOST_EMU)
+static inline float kb_cabs(float re, float im)
+#else
+KB_D float kb_cabs(float re, float im)
+#endif
+{
+    const float n = RN ? fmaf(re, re, im * im) : cnorm(cmake(re, im));
+    if (kb_f2u(n) - 0x1f800000u <= 0x40000000u) return RN ? sqrtf(n) : kb_sqrt(n);   // n in [2^-64, 2^64]
+#if defined(KB_HOST_EMU)
+    return kb_cabs_rescaled<RN>(re, im);
+#else
+    return RN ? kb_cabs_rescaled<true>(re, im) : kb_cabs_rescaled_approx(re, im);
+#endif
+}
+#if defined(KB_HOST_EMU)
+static inline float kb_cabs(cpx X) { return kb_cabs<false>(X.re, X.im); }
+#else
+KB_D float kb_cabs(cpx X) { return kb_cabs<false>(X.re, X.im); }
+#endif
+
 // atan2 for the Phase outputs (tf.math.angle, kapre/time_frequency.py:402): octant reduction to t = min / max in [0, 1],
 // atan(t) = t + t s q(s), s = t^2, q a degree-7 minimax fit (weighted least squares on Chebyshev nodes): max error 2.8e-7 rad
 // over random float32 arguments, the same as a correctly rounded float32 atan2 within 1 ulp of pi -- and ~20 instructions
@@ -220,7 +278,11 @@ KB_D float kb_atan2(float y, float x)
 {
     const float ax = fabsf(x), ay = fabsf(y);
     const float mx = fmaxf(ax, ay), mn = fminf(ax, ay);
-    const float t = mx == 0.0f ? 0.0f : kb_fdividef(mn, mx);
+    // __fdividef (mn times an approximate 1 / mx) returns 0 for 2^126 < mx < 2^128, and 1 / mx overflows for a
+    // subnormal mx: scale both operands by a power of two first (exact, and 1 in between, where the quotient keeps
+    // the bits of the unscaled division)
+    const float sc = mx > 0x1p126f ? 0x1p-4f : mx < 0x1p-100f ? 0x1p24f : 1.0f;
+    const float t = mx == 0.0f ? 0.0f : kb_fdividef(mn * sc, mx * sc);
     const float s = t * t;
     float r = 0.0026222908826366536f;
     r = fmaf(r, s, -0.015132737140170525f);
@@ -914,7 +976,7 @@ __device__ __forceinline__ void kb_stft_cta(const KbStftParams& p, char* smem, i
                                     const float2 v = make_float2(X.re, cj ? -X.im : X.im);
                                     if (sk == 1) oc[k] = v; else oc[k * sk] = v;
                                 } else {
-                                    float m = kb_sqrt(cnorm(X));
+                                    float m = kb_cabs(X);
                                     if (MODE == KB_OUT_MAG_PHASE)   // tf.math.angle, kapre/time_frequency.py:402
                                         orl[(long long)k * sk + p.ph_off] = kb_atan2(cj ? -X.im : X.im, X.re);
                                     if (dbany) {
@@ -998,8 +1060,8 @@ __device__ __forceinline__ void kb_stft_cta(const KbStftParams& p, char* smem, i
                                 }
                             }
                         } else {
-                            float m1 = kb_sqrt(cnorm(X1));
-                            float m2 = kb_sqrt(cnorm(X2));
+                            float m1 = fbmode ? kb_sqrt(cnorm(X1)) : kb_cabs(X1);
+                            float m2 = fbmode ? kb_sqrt(cnorm(X2)) : kb_cabs(X2);
                             if (fbmode) {
                                 magr[(gg * (Q / 2 + 1) + i) * 2 + 0] = m1;
                                 magr[(gg * (Q / 2 + 1) + i) * 2 + 1] = m2;

@@ -161,8 +161,8 @@ __device__ __forceinline__ void kb_mc_emit(const KbStftParams& p, bool dbany, vo
         if (kk >= 0) oc[kk * sk] = make_float2(X2.re, -X2.im);
     } else {
         float* orl = reinterpret_cast<float*>(o) + off;
-        float m1 = kb_sqrt(cnorm(X1));
-        float m2 = kb_sqrt(cnorm(X2));
+        float m1 = kb_cabs(X1);
+        float m2 = kb_cabs(X2);
         if (MODE == KB_OUT_MAG_PHASE) {   // tf.math.angle, kapre/time_frequency.py:402
             orl[k * sk + p.ph_off] = kb_atan2(X1.im, X1.re);
             if (kk >= 0) orl[kk * sk + p.ph_off] = kb_atan2(-X2.im, X2.re);

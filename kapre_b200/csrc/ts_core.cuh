@@ -106,7 +106,7 @@ KB_FN unsigned kb_ts_q(float2 z) {
     return (unsigned)(long long)rint((double)a * 683565275.5764316);     // 2^31 / pi
 }
 
-KB_FN float kb_ts_abs(float2 z) { return sqrtf(fmaf(z.x, z.x, z.y * z.y)); }
+KB_FN float kb_ts_abs(float2 z) { return kb_cabs<true>(z.x, z.y); }
 
 // (cos, sin) of pi s.  The device computes sincospif; the emulation rounds the float64 values.
 #if defined(KB_HOST_EMU)

@@ -503,6 +503,11 @@ int kb_emu_async_selftest() {
     return flagged;
 }
 
+// kb_cabs (|X| over the whole float range) on arrays: rn = 1 the correctly rounded form, 0 the kb_sqrt(cnorm) form
+void kb_emu_cabs(const float* re, const float* im, float* out, long long n, int rn) {
+    for (long long i = 0; i < n; ++i) out[i] = rn ? kb_cabs<true>(re[i], im[i]) : kb_cabs<false>(re[i], im[i]);
+}
+
 // kb_atan2 (the Phase outputs' polynomial atan2) on arrays, for the accuracy test
 void kb_emu_atan2(const float* y, const float* x, float* out, long long n) {
     for (long long i = 0; i < n; ++i) out[i] = kb_atan2(y[i], x[i]);

@@ -309,3 +309,13 @@ def emu_atan2(y, x):
     out = np.empty_like(y)
     lib.kb_emu_atan2(_fp(y), _fp(x), _fp(out), ctypes.c_longlong(y.size))
     return out
+
+
+def emu_cabs(re, im, rn):
+    """kb_cabs<rn> of kapre_b200/csrc/stft_core.cuh (host build of the same source) on float32 arrays."""
+    lib = load()
+    re = np.ascontiguousarray(re, np.float32)
+    im = np.ascontiguousarray(im, np.float32)
+    out = np.empty_like(re)
+    lib.kb_emu_cabs(_fp(re), _fp(im), _fp(out), ctypes.c_longlong(re.size), ctypes.c_int(int(rn)))
+    return out
