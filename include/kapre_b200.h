@@ -658,6 +658,42 @@ int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float*
                         int batch, int channels, int frames, double* tuning_dev, int* table_dev, void* workspace_dev,
                         void* stream);
 
+/* ---- harmonic/percussive separation (modelled on librosa.decompose.hpss) ------------------------------------------
+ * S (batch x channels x frames x bins, any element strides) is float32 magnitudes, used as given, or complex64, whose
+ * magnitude |X| is formed as kapre_magnitude forms it; S must be non-negative (not checked).  Per (item, channel) row:
+ *   H = median over kernel_h frames, P = median over kernel_p bins, each the element of rank k/2 of its window with
+ *   indices reflected with period 2n, edge included (scipy.ndimage.median_filter(mode='reflect')); a window holding NaN
+ *   gives NaN;
+ *   M_H = softmask(H, margin_h P), M_P = softmask(P, margin_p H) (librosa.util.softmask: a > b as 1/0 for power inf;
+ *   else 0.5 when both margins are 1 and max(a, b) < FLT_MIN, 0 otherwise, else (a/Z)^p / ((a/Z)^p + (b/Z)^p) with
+ *   Z = max(a, b));
+ *   outputs S M_H and S M_P (float S), M_H X and M_P X (complex64 S), or the masks themselves (float32).
+ * Every output's bits depend only on its row's data and its (frame, bin). */
+#define KAPRE_HPSS_MAX_KERNEL 64
+typedef struct {
+    int kernel_h, kernel_p;       /* 1 .. KAPRE_HPSS_MAX_KERNEL */
+    float power;                  /* > 0, may be +inf */
+    float margin_h, margin_p;     /* finite, >= 1 */
+    int mask;                     /* 1: write the masks instead of the components */
+} kapre_hpss_config;
+/* Either output may be NULL (not written).  Outputs must not overlap S.  One launch. */
+int kapre_hpss(const kapre_hpss_config* cfg, const void* S_dev, int is_complex, const kapre_spec_desc* S_desc, int batch,
+               int channels, int frames, int bins, void* h_dev, const kapre_spec_desc* h_desc, void* p_dev,
+               const kapre_spec_desc* p_desc, void* stream);
+/* Device scratch of kapre_hpss_backward: 16 bytes per element of S (a gradient and the index of the element it goes to,
+ * for each median). */
+int64_t kapre_hpss_workspace_bytes(int batch, int channels, int frames, int bins);
+/* Gradient of kapre_hpss to S (float32, or complex64 in torch's convention) at gS_desc's strides, given the gradients
+ * of its outputs (same dtype as the outputs: float32 masks, or the components in S's dtype); either may be NULL (zero).
+ * The direct term M_H g_H + M_P g_P plus the mask term through each median, which goes to the one element the median
+ * selected (rank k/2 under (value, position in the reflected window)); complex S then through |X| (g X / |X|, 0 at
+ * X = 0).  Infinite or undefined mask derivatives (max(a, b) < FLT_MIN, power inf, a zero median with power < 1)
+ * contribute 0.  Two launches; gS must not overlap the other buffers. */
+int kapre_hpss_backward(const kapre_hpss_config* cfg, const void* S_dev, int is_complex, const kapre_spec_desc* S_desc,
+                        int batch, int channels, int frames, int bins, const void* gh_dev, const kapre_spec_desc* gh_desc,
+                        const void* gp_dev, const kapre_spec_desc* gp_desc, void* gS_dev,
+                        const kapre_spec_desc* gS_desc, void* workspace_dev, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

@@ -100,6 +100,14 @@ class FramesDesc(Structure):
     _fields_ = [('stride_b', c_int64), ('stride_c', c_int64), ('stride_t', c_int64)]
 
 
+class HpssCfg(Structure):
+    _fields_ = [('kernel_h', c_int), ('kernel_p', c_int), ('power', c_float), ('margin_h', c_float),
+                ('margin_p', c_float), ('mask', c_int)]
+
+
+HPSS_MAX_KERNEL = 64
+
+
 class ChromaPlanDesc(Structure):
     _fields_ = [('n_chroma', c_int), ('n_bins', c_int), ('n_tables', c_int), ('tables', c_void_p),
                 ('n_smooth', c_int), ('smooth', c_void_p), ('n_tuning_bins', c_int), ('tuning_edges', c_void_p),
@@ -240,6 +248,12 @@ SYMBOLS = [
     ('kapre_chroma_tuning_workspace_bytes', c_int64, [c_void_p, c_int, c_int, c_int]),
     ('kapre_chroma_tuning', c_int, [c_void_p, c_int, c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),
+    ('kapre_hpss', c_int, [POINTER(HpssCfg), c_void_p, c_int, POINTER(SpecDesc), c_int, c_int, c_int, c_int, c_void_p,
+                           POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p]),
+    ('kapre_hpss_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int]),
+    ('kapre_hpss_backward', c_int, [POINTER(HpssCfg), c_void_p, c_int, POINTER(SpecDesc), c_int, c_int, c_int, c_int,
+                                    c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p,
+                                    POINTER(SpecDesc), c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

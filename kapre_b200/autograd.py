@@ -37,6 +37,9 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * chroma_stft, chroma_cqt, ChromaSTFT, ChromaCQT -> ``kapre_chroma_backward`` (y = W s recomputed, the gradient
   taken back through the normalisation and the threshold, then W^T and the input's square or modulus), then the STFT
   magnitude or CQT magnitude backward; the tuning estimate is a constant
+* hpss, harmonic, percussive, HPSS -> ``kapre_hpss_backward`` (the medians recomputed with the element each one
+  selected, the mask gradients written beside those indices, then a gather per element), then the STFT magnitude's
+  or the STFT and inverse STFT's backward
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
@@ -472,6 +475,28 @@ class _Chroma(torch.autograd.Function):
         return ops.chroma_backward(g, x, plan, cfg, data_format, table), None, None, None, None
 
 
+class _Hpss(torch.autograd.Function):
+    """Outputs the components ``want`` names, (harmonic, percussive) or one of them."""
+
+    @staticmethod
+    def forward(ctx, S, cfg, data_format, want_h, want_p):
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(S)
+        ctx.cfg = (cfg, data_format, want_h, want_p)
+        h, p = ops.hpss_forward(S, cfg, data_format, want_h, want_p)
+        return tuple(t for t in (h, p) if t is not None)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *gs):
+        S, = ctx.saved_tensors
+        cfg, data_format, want_h, want_p = ctx.cfg
+        gs = list(gs)
+        gh = gs.pop(0) if want_h else None
+        gp = gs.pop(0) if want_p else None
+        return ops.hpss_backward(gh, gp, S, cfg, data_format), None, None, None, None
+
+
 class _TimeStretch(torch.autograd.Function):
     """The forward is the plain time-stretch launch; autograd saves its output, from which the backward takes the
     magnitude and phase gradients, so the forward writes nothing extra."""
@@ -605,3 +630,10 @@ def cqt(x, plan, input_data_format, output_data_format, magnitude):
 
 def chroma(x, plan, cfg, data_format, table):
     return _Chroma.apply(x, plan, cfg, data_format, table)
+
+
+def hpss(S, cfg, data_format, want_h, want_p):
+    out = _Hpss.apply(S, cfg, data_format, want_h, want_p)
+    out = out if isinstance(out, tuple) else (out,)
+    it = iter(out)
+    return (next(it) if want_h else None), (next(it) if want_p else None)

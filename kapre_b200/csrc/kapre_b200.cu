@@ -39,6 +39,7 @@
 #include "cqt_core.cuh"
 #include "pitch_core.cuh"
 #include "chroma_core.cuh"
+#include "hpss_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -4307,6 +4308,108 @@ int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float*
         return rc;
     return kb_launch(kb_tune_argmax_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = 2 * KB_CH_THREADS * 4,
                                              .st = st}, p);
+}
+
+}  // extern "C"
+
+// ---- harmonic/percussive separation (hpss_core.cuh) ---------------------------------------------------------------
+template <int NSH, int NSP, int BWD>
+__global__ void __launch_bounds__(KB_HS_THREADS) kb_hpss_kernel(const __grid_constant__ KbHpssParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_hpss_cta<NSH, NSP, BWD>(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_HS_THREADS) kb_hpss_gather_kernel(const __grid_constant__ KbHpssParams p) {
+    kb_hpss_gather_cta(p, nullptr, blockIdx.x, gridDim.x);
+}
+
+template <int BWD>
+static int kb_hpss_tiles_launch(const KbHpssParams& p, cudaStream_t st) {
+    const int sh = kb_hs_slots(p.kh), sp = kb_hs_slots(p.kp);
+    void (*k)(const KbHpssParams) = sh == 32 ? (sp == 32 ? kb_hpss_kernel<32, 32, BWD> : kb_hpss_kernel<32, 64, BWD>)
+                                             : (sp == 32 ? kb_hpss_kernel<64, 32, BWD> : kb_hpss_kernel<64, 64, BWD>);
+    DevInfo dev;
+    int rc, grid;
+    if ((rc = kb_dev_info(&dev))) return rc;
+    const int smem = kb_hpss_smem(p.kh, p.kp, BWD);
+    if ((rc = kb_resident_grid(k, BWD ? "hpss_bwd" : "hpss", KB_HS_THREADS, smem, p.jobs, dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(k, {.grid = grid, .block = KB_HS_THREADS, .smem = smem, .st = st, .timed = !BWD}, p);
+}
+
+static int kb_hpss_params(const kapre_hpss_config* cfg, const void* S, int is_complex, const kapre_spec_desc* sd,
+                          int B, int C, int T, int K, KbHpssParams* out) {
+    if (!cfg || !sd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (B < 0 || C < 0 || T < 0 || K < 0) return kb_fail(KAPRE_E_INVALID, "hpss: negative size (%d, %d, %d, %d)", B, C, T, K);
+    if (cfg->kernel_h < 1 || cfg->kernel_h > KAPRE_HPSS_MAX_KERNEL || cfg->kernel_p < 1 ||
+        cfg->kernel_p > KAPRE_HPSS_MAX_KERNEL)
+        return kb_fail(KAPRE_E_INVALID, "hpss: kernel sizes (%d, %d) outside [1, %d]", cfg->kernel_h, cfg->kernel_p,
+                       KAPRE_HPSS_MAX_KERNEL);
+    if (!(cfg->margin_h >= 1.0f) || !(cfg->margin_p >= 1.0f) || !isfinite(cfg->margin_h) || !isfinite(cfg->margin_p))
+        return kb_fail(KAPRE_E_INVALID, "hpss: margins must be finite and >= 1");
+    if (!(cfg->power > 0.0f)) return kb_fail(KAPRE_E_INVALID, "hpss: power must be > 0");
+    KbHpssParams p{};
+    p.B = B; p.C = C; p.T = T; p.K = K;
+    p.kh = cfg->kernel_h; p.kp = cfg->kernel_p; p.mh = cfg->margin_h; p.mp = cfg->margin_p; p.power = cfg->power;
+    p.pmode = isinf(cfg->power) ? KB_HS_POW_INF : cfg->power == 1.0f ? KB_HS_POW_1
+                                : cfg->power == 2.0f ? KB_HS_POW_2 : KB_HS_POW_GENERIC;
+    p.split = cfg->margin_h == 1.0f && cfg->margin_p == 1.0f;
+    p.cplx = is_complex != 0; p.mask = cfg->mask != 0;
+    p.x = S; p.x_sb = sd->stride_b; p.x_sc = sd->stride_c; p.x_st = sd->stride_t; p.x_sk = sd->stride_f;
+    if (!kb_hpss_setup(p)) return kb_fail(KAPRE_E_INVALID, "hpss: too many tiles");
+    if (p.jobs && !S) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    *out = p;
+    return 0;
+}
+
+extern "C" {
+
+int kapre_hpss(const kapre_hpss_config* cfg, const void* S_dev, int is_complex, const kapre_spec_desc* S_desc, int batch,
+               int channels, int frames, int bins, void* h_dev, const kapre_spec_desc* h_desc, void* p_dev,
+               const kapre_spec_desc* p_desc, void* stream) {
+    KbHpssParams p;
+    int rc = kb_hpss_params(cfg, S_dev, is_complex, S_desc, batch, channels, frames, bins, &p);
+    if (rc) return rc;
+    if ((h_dev && !h_desc) || (p_dev && !p_desc)) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (!p.jobs || (!h_dev && !p_dev)) return 0;
+    p.oh = h_dev;
+    if (h_dev) { p.oh_sb = h_desc->stride_b; p.oh_sc = h_desc->stride_c; p.oh_st = h_desc->stride_t; p.oh_sk = h_desc->stride_f; }
+    p.op = p_dev;
+    if (p_dev) { p.op_sb = p_desc->stride_b; p.op_sc = p_desc->stride_c; p.op_st = p_desc->stride_t; p.op_sk = p_desc->stride_f; }
+    return kb_hpss_tiles_launch<0>(p, (cudaStream_t)stream);
+}
+
+int64_t kapre_hpss_workspace_bytes(int batch, int channels, int frames, int bins) {
+    if (batch < 0 || channels < 0 || frames < 0 || bins < 0) return kb_fail(KAPRE_E_INVALID, "hpss: negative size");
+    return (int64_t)batch * channels * frames * bins * 2 * (int64_t)sizeof(kb_hs_w);
+}
+
+int kapre_hpss_backward(const kapre_hpss_config* cfg, const void* S_dev, int is_complex, const kapre_spec_desc* S_desc,
+                        int batch, int channels, int frames, int bins, const void* gh_dev, const kapre_spec_desc* gh_desc,
+                        const void* gp_dev, const kapre_spec_desc* gp_desc, void* gS_dev,
+                        const kapre_spec_desc* gS_desc, void* workspace_dev, void* stream) {
+    KbHpssParams p;
+    int rc = kb_hpss_params(cfg, S_dev, is_complex, S_desc, batch, channels, frames, bins, &p);
+    if (rc) return rc;
+    if (!gS_desc || (gh_dev && !gh_desc) || (gp_dev && !gp_desc)) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (!p.jobs) return 0;
+    if (!gS_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.gh = gh_dev;
+    if (gh_dev) { p.gh_sb = gh_desc->stride_b; p.gh_sc = gh_desc->stride_c; p.gh_st = gh_desc->stride_t; p.gh_sk = gh_desc->stride_f; }
+    p.gp = gp_dev;
+    if (gp_dev) { p.gp_sb = gp_desc->stride_b; p.gp_sc = gp_desc->stride_c; p.gp_st = gp_desc->stride_t; p.gp_sk = gp_desc->stride_f; }
+    p.gx = gS_dev; p.gx_sb = gS_desc->stride_b; p.gx_sc = gS_desc->stride_c; p.gx_st = gS_desc->stride_t;
+    p.gx_sk = gS_desc->stride_f;
+    const long long n = (long long)batch * channels * frames * bins;
+    p.wh = (kb_hs_w*)workspace_dev; p.wp = p.wh + n;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = kb_hpss_tiles_launch<1>(p, st))) return rc;
+    DevInfo dev;
+    if ((rc = kb_dev_info(&dev))) return rc;
+    int grid;
+    if ((rc = kb_resident_grid(kb_hpss_gather_kernel, "hpss_gather", KB_HS_THREADS, 0,
+                               (n + KB_HS_THREADS - 1) / KB_HS_THREADS, dev.sm_count, &grid)))
+        return rc;
+    return kb_launch(kb_hpss_gather_kernel, {.grid = grid, .block = KB_HS_THREADS, .st = st}, p);
 }
 
 }  // extern "C"

@@ -2097,3 +2097,97 @@ def chroma_tuning(x, plan: ChromaPlan, in_mode, data_format=_CH_LAST_STR):
         N.check(N.lib().kapre_chroma_tuning(plan.handle(), int(in_mode), _ptr(x), ctypes.byref(xd), B, C, M,
                                             _ptr(tuning), _ptr(table), _ptr(ws), _stream_ptr()))
     return tuning, table
+
+
+# ------------------------------------------------------------------------------- harmonic/percussive separation
+def _hpss_pair(v, name):
+    if isinstance(v, (tuple, list)):
+        if len(v) != 2:
+            raise ValueError('%s must be a number or a pair, got %r' % (name, v))
+        return v[0], v[1]
+    return v, v
+
+
+def hpss_config(kernel_size=31, power=2.0, mask=False, margin=1.0):
+    """The ``kapre_hpss_config`` of ``hpss``'s arguments; a bad argument raises ``ValueError`` here, before any launch.
+    ``kernel_size`` and ``margin``: a number or a pair (harmonic, percussive)."""
+    kh, kp = _hpss_pair(kernel_size, 'kernel_size')
+    for k in (kh, kp):
+        if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 1 <= k <= N.HPSS_MAX_KERNEL:
+            raise ValueError('kernel_size must be integers in [1, %d], got %r' % (N.HPSS_MAX_KERNEL, kernel_size))
+    mh, mp = _hpss_pair(margin, 'margin')
+    for m in (mh, mp):
+        if isinstance(m, (bool, np.bool_)) or not isinstance(m, (int, float, np.integer, np.floating)) \
+                or not np.isfinite(float(m)) or not float(m) >= 1.0:
+            raise ValueError('margin must be finite and >= 1, got %r' % (margin,))
+    if isinstance(power, (bool, np.bool_)) or not isinstance(power, (int, float, np.integer, np.floating)) \
+            or not float(power) > 0.0:
+        raise ValueError('power must be > 0 (inf allowed), got %r' % (power,))
+    return N.HpssCfg(int(kh), int(kp), float(power), float(mh), float(mp), int(bool(mask)))
+
+
+def _hpss_input(S, data_format):
+    if not isinstance(S, torch.Tensor):
+        raise ValueError('hpss expects a torch tensor, got %s' % (type(S).__name__,))
+    if S.dim() != 4:
+        raise ValueError('hpss expects a 4-D spectrogram batch, got shape %s' % (tuple(S.shape),))
+    if S.dtype not in (torch.float32, torch.complex64):
+        raise ValueError('hpss expects float32 or complex64 input, got %s' % (S.dtype,))
+    if not S.is_cuda:
+        raise ValueError('hpss needs a CUDA spectrogram')
+    S = _raw(S)
+    sd, dims = _spec_desc(S, data_format)
+    return S, sd, dims
+
+
+def hpss_forward(S, cfg, data_format, want_h=True, want_p=True):
+    """(harmonic, percussive) of ``kapre_hpss`` (None for a component not wanted).  One launch."""
+    S, sd, (B, C, T, K) = _hpss_input(S, data_format)
+    dt = torch.float32 if cfg.mask else S.dtype
+    outs, descs = [None, None], [None, None]
+    for i, want in enumerate((want_h, want_p)):
+        if want:
+            outs[i], descs[i] = _spec_alloc(B, C, T, K, data_format, dt, S.device)
+    if S.numel():
+        N.check(N.lib().kapre_hpss(ctypes.byref(cfg), _ptr(S), int(S.is_complex()), ctypes.byref(sd), B, C, T, K,
+                                   _ptr(outs[0]) if want_h else None, ctypes.byref(descs[0]) if want_h else None,
+                                   _ptr(outs[1]) if want_p else None, ctypes.byref(descs[1]) if want_p else None,
+                                   _stream_ptr()))
+    return outs[0], outs[1]
+
+
+def hpss_backward(gh, gp, S, cfg, data_format):
+    """Gradient of ``hpss_forward`` with respect to S given its outputs' gradients (either may be None).  Two
+    launches over a workspace of ``kapre_hpss_workspace_bytes``."""
+    S, sd, (B, C, T, K) = _hpss_input(S, data_format)
+    gdt = torch.float32 if cfg.mask else S.dtype
+    gs = [None, None]
+    ds = [None, None]
+    for i, g in enumerate((gh, gp)):
+        if g is not None:
+            gs[i] = _raw(g.to(gdt))
+            ds[i], _ = _spec_desc(gs[i], data_format)
+    gS, gSd = _spec_alloc(B, C, T, K, data_format, S.dtype, S.device)
+    if gS.numel():
+        n = int(N.lib().kapre_hpss_workspace_bytes(B, C, T, K))
+        if n < 0:
+            N.check(n)
+        ws = torch.empty(max(n // 4, 1), dtype=torch.float32, device=S.device)
+        N.check(N.lib().kapre_hpss_backward(ctypes.byref(cfg), _ptr(S), int(S.is_complex()), ctypes.byref(sd), B, C, T,
+                                            K, _ptr(gs[0]) if gs[0] is not None else None,
+                                            ctypes.byref(ds[0]) if gs[0] is not None else None,
+                                            _ptr(gs[1]) if gs[1] is not None else None,
+                                            ctypes.byref(ds[1]) if gs[1] is not None else None,
+                                            _ptr(gS), ctypes.byref(gSd), _ptr(ws), _stream_ptr()))
+    return gS
+
+
+@_device_of_first_arg
+def hpss(S, cfg, data_format=_CH_LAST_STR, want_h=True, want_p=True):
+    """Harmonic/percussive separation of a CUDA spectrogram batch ``(B, T, K, C)`` / ``(B, C, T, K)`` (float32
+    magnitudes or complex64) under ``cfg`` (``hpss_config``): ``(harmonic, percussive)``, None for a component not
+    wanted.  One launch.  Differentiable with respect to S."""
+    if _wants_grad(S):
+        from . import autograd
+        return autograd.hpss(S, cfg, data_format, want_h, want_p)
+    return hpss_forward(S, cfg, data_format, want_h, want_p)

@@ -8,7 +8,7 @@ filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, o
 ``add_noise`` (torchaudio's, with deterministic float64 energies), or ``loudness`` and ``Loudness`` (torchaudio's
 BS.1770 gated loudness, with per-item lengths), or the pitch trackers ``yin``, ``pyin``, ``YIN`` and ``PYIN``
 (librosa's), or the chroma features ``chroma_stft``, ``chroma_cqt``, ``chroma_cens`` and ``estimate_tuning``
-(librosa's)."""
+(librosa's), or the harmonic/percussive separation ``hpss``, ``harmonic`` and ``percussive`` (librosa's)."""
 from __future__ import annotations
 
 import math
@@ -22,7 +22,8 @@ from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
            'Biquad', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
-           'YIN', 'PYIN', 'chroma_stft', 'chroma_cqt', 'chroma_cens', 'estimate_tuning']
+           'YIN', 'PYIN', 'chroma_stft', 'chroma_cqt', 'chroma_cens', 'estimate_tuning', 'hpss', 'harmonic',
+           'percussive']
 
 
 def _resolve(fmt):
@@ -880,3 +881,76 @@ def chroma_cens(waveform=None, sample_rate=22050, C=None, hop_length=512, f_min=
         X, mode = _cq_magnitude(None if waveform is None else waveform.detach(),
                                 None if C is None else C.detach(), cqt, fmt)
         return ops.chroma_cens(X, plan, mode, fmt)
+
+
+# ---- harmonic/percussive separation ------------------------------------------------------------------------------------
+def hpss(S, kernel_size=31, power=2.0, mask=False, margin=1.0, data_format='default'):
+    """Harmonic/percussive separation by median filtering (``librosa.decompose.hpss``, Fitzgerald 2010) of a CUDA
+    spectrogram batch ``(batch, frames, bins, ch)`` / ``(batch, ch, frames, bins)``: float32 magnitudes (or power),
+    used as given, or complex64 (``STFT``'s output), whose magnitude is formed as ``Magnitude`` forms it.  S must be
+    non-negative; this is not checked.
+
+    ``H`` and ``P`` are the medians of ``kernel_size`` values along frames and along bins, exactly as
+    ``scipy.ndimage.median_filter(mode='reflect')`` computes them (an even size takes the upper median); a window
+    holding NaN gives NaN.  The masks are ``softmask(H, margin_h P)`` and ``softmask(P, margin_p H)`` with librosa's
+    ``util.softmask``.  Returns ``(harmonic, percussive)``: ``S M`` for float input, ``M X`` for complex input, or the
+    masks with ``mask=True``; each shaped like S.  ``kernel_size`` (1 .. 64) and ``margin`` (finite, >= 1) are a
+    number or a pair (harmonic, percussive); ``power > 0`` may be ``inf``.  One launch; differentiable with respect
+    to S."""
+    backend.validate_data_format_str(data_format)
+    cfg = ops.hpss_config(kernel_size, power, mask, margin)
+    return ops.hpss(S, cfg, _resolve(_unwrap_format(data_format)))
+
+
+_hpss_transforms = {}
+
+
+def _hpss_component(waveform, component, kernel_size, power, margin, n_fft, win_length, hop_length, window_name,
+                    data_format):
+    from .time_frequency import STFT, InverseSTFT
+    backend.validate_data_format_str(data_format)
+    fmt = _resolve(_unwrap_format(data_format))
+    cfg = ops.hpss_config(kernel_size, power, False, margin)
+    win = n_fft if win_length is None else win_length
+    hop = win // 4 if hop_length is None else hop_length
+    if hop > win:
+        raise ValueError('hop_length (%r) must not exceed win_length (%r)' % (hop, win))
+    if not isinstance(waveform, torch.Tensor) or waveform.dim() != 3:
+        raise ValueError('%s expects a 3-D waveform batch' % (component,))
+    key = (n_fft, win_length, hop_length, window_name, fmt)
+    pair = _hpss_transforms.get(key)
+    if pair is None:
+        pair = (STFT(n_fft=n_fft, win_length=win_length, hop_length=hop_length, window_name=window_name,
+                     pad_begin=True, pad_end=True, input_data_format=fmt, output_data_format=_CH_LAST_STR),
+                InverseSTFT(n_fft=n_fft, win_length=win_length, hop_length=hop_length, forward_window_name=window_name,
+                            input_data_format=_CH_LAST_STR, output_data_format=fmt))
+        _hpss_transforms[key] = pair
+    stft, istft = pair
+    length = waveform.shape[2] if fmt == _CH_FIRST_STR else waveform.shape[1]
+    h, p = ops.hpss(stft.call(waveform), cfg, _CH_LAST_STR, want_h=component == 'harmonic',
+                    want_p=component == 'percussive')
+    y = istft.call(h if component == 'harmonic' else p)
+    start = stft.n_fft - stft.hop_length
+    return y[:, :, start:start + length] if fmt == _CH_FIRST_STR else y[:, start:start + length, :]
+
+
+def harmonic(waveform, kernel_size=31, power=2.0, margin=1.0, n_fft=2048, win_length=None, hop_length=None,
+             window_name=None, data_format='default'):
+    """The harmonic part of a CUDA waveform batch ``(batch, time, ch)`` / ``(batch, ch, time)``, the same shape out
+    (``librosa.effects.harmonic``): ``STFT`` with ``pad_begin`` and ``pad_end``, ``hpss`` writing the harmonic
+    component alone, ``InverseSTFT`` with the dual window, then ``time`` samples from ``n_fft - hop_length`` on, which
+    is where input sample 0 lands, so the output is time-aligned with the input.  With margins of 1 and a finite power
+    the masks sum to 1 and ``harmonic(y) + percussive(y)`` reproduces ``y`` to rounding.
+
+    Departure from librosa: the framing is kapre's (``pad_begin``/``pad_end`` and the dual window), not librosa's
+    centred frames and envelope-normalised ``istft``, so samples near the ends differ.  ``hop_length > win_length``
+    raises ``ValueError``.  Three launches; differentiable with respect to the waveform."""
+    return _hpss_component(waveform, 'harmonic', kernel_size, power, margin, n_fft, win_length, hop_length,
+                           window_name, data_format)
+
+
+def percussive(waveform, kernel_size=31, power=2.0, margin=1.0, n_fft=2048, win_length=None, hop_length=None,
+               window_name=None, data_format='default'):
+    """The percussive part of a CUDA waveform batch (``librosa.effects.percussive``); see ``harmonic``."""
+    return _hpss_component(waveform, 'percussive', kernel_size, power, margin, n_fft, win_length, hop_length,
+                           window_name, data_format)

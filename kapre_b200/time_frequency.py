@@ -24,7 +24,7 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
 __all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
            'PCEN', 'GriffinLim', 'InverseFilterbank', 'KaldiFbank', 'KaldiMFCC', 'KaldiSpectrogram', 'CQT',
-           'ChromaSTFT', 'ChromaCQT', 'ChromaCENS']
+           'ChromaSTFT', 'ChromaCQT', 'ChromaCENS', 'HPSS']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -856,4 +856,37 @@ class ChromaCENS(_ChromaLayer):
         ('n_chroma', 'n_chroma'), ('n_octaves', 'n_octaves'), ('bins_per_octave', 'bins_per_octave'),
         ('base_c', 'base_c'), ('norm', 'norm'), ('win_len_smooth', 'win_len_smooth'),
         ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class HPSS(Layer):
+    """One component of ``signal.hpss`` as a layer: a ``(batch, frames, bins, ch)`` / ``(batch, ch, frames, bins)``
+    magnitude (float32) or complex64 spectrogram in, the ``component`` (``'harmonic'`` or ``'percussive'``), or its
+    mask with ``mask=True``, out in the same shape.  Other arguments as ``signal.hpss``.  One launch; differentiable
+    with respect to the input."""
+
+    def __init__(self, component='harmonic', kernel_size=31, power=2.0, mask=False, margin=1.0, data_format='default',
+                 **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        if component not in ('harmonic', 'percussive'):
+            raise ValueError("component must be 'harmonic' or 'percussive', got %r" % (component,))
+        self.cfg = ops.hpss_config(kernel_size, power, mask, margin)
+        self.component = component
+        self.kernel_size = list(kernel_size) if isinstance(kernel_size, (tuple, list)) else kernel_size
+        self.power, self.mask = power, mask
+        self.margin = list(margin) if isinstance(margin, (tuple, list)) else margin
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+
+    def call(self, x):
+        h, p = ops.hpss(x, self.cfg, self.data_format, want_h=self.component == 'harmonic',
+                        want_p=self.component == 'percussive')
+        return h if self.component == 'harmonic' else p
+
+    _config_fields = (
+        ('component', 'component'), ('kernel_size', 'kernel_size'), ('power', 'power'), ('mask', 'mask'),
+        ('margin', 'margin'), ('data_format', 'data_format_str'),
     )
