@@ -694,6 +694,84 @@ int kapre_hpss_backward(const kapre_hpss_config* cfg, const void* S_dev, int is_
                         const void* gp_dev, const kapre_spec_desc* gp_desc, void* gS_dev,
                         const kapre_spec_desc* gS_desc, void* workspace_dev, void* stream);
 
+/* ---- onset strength, tempogram, tempo, onset detection, beat tracking (modelled on librosa 0.10) ------------------
+ * A row is one (item, channel) pair; every output's bits depend only on its row's data.  Per-frame signals (envelopes,
+ * masks) use kapre_frames_desc; masks are uint8 0 / 1.
+ *
+ * Onset strength of S (batch x channels x frames x bins, float32, any strides), per row with m = max_size and P =
+ * lag + pad_frames:  R[t][b] = max S[t][b - m/2 .. b - m/2 + m - 1] (bins outside [0, K) skipped),
+ * D[t][b] = max(0, S[t][b] - R[t - lag][b]) (NaN kept), A[t] = mean over b (float64 sum in ascending b, / K, rounded
+ * once) or median (numpy's; NaN in the frame gives NaN), out[t] = 0 for t < P, A[t - P + lag] otherwise. */
+#define KAPRE_ONSET_MAX_BINS 4097
+#define KAPRE_TEMPOGRAM_MAX_WIN 4096
+#define KAPRE_BEAT_MAX_PERIOD 4096
+enum { KAPRE_ONSET_MEAN = 0, KAPRE_ONSET_MEDIAN = 1 };
+typedef struct {
+    int lag;                      /* >= 1, < frames */
+    int max_size;                 /* 1 .. bins */
+    int aggregate;                /* KAPRE_ONSET_MEAN or KAPRE_ONSET_MEDIAN */
+    int pad_frames;               /* n_fft / (2 hop_length) for a centred S, else 0 */
+} kapre_onset_config;
+/* bins <= KAPRE_ONSET_MAX_BINS.  One launch. */
+int kapre_onset_strength(const kapre_onset_config* cfg, const float* S_dev, const kapre_spec_desc* S_desc, int batch,
+                         int channels, int frames, int bins, float* out_dev, const kapre_frames_desc* out_desc,
+                         void* stream);
+/* Device scratch of kapre_onset_strength_backward: 8 bytes per element of S. */
+int64_t kapre_onset_strength_workspace_bytes(int batch, int channels, int frames, int bins);
+/* Gradient of kapre_onset_strength to S given g, the envelope's gradient: relu'(0) = 0, each window maximum's
+ * gradient to the lowest of its tied bins, the median's to the element(s) it selected under (value, bin) (0.5 each
+ * for even bins).  Two launches, no floating-point atomics; gS must not overlap the other buffers. */
+int kapre_onset_strength_backward(const kapre_onset_config* cfg, const float* S_dev, const kapre_spec_desc* S_desc,
+                                  int batch, int channels, int frames, int bins, const float* g_dev,
+                                  const kapre_frames_desc* g_desc, float* gS_dev, const kapre_spec_desc* gS_desc,
+                                  void* workspace_dev, void* stream);
+/* Autocorrelation tempogram of envelopes e (batch x channels x frames): frame t is y = w * padded[t .. t + W) with w
+ * the periodic Hann window of W = win_length (2 .. KAPRE_TEMPOGRAM_MAX_WIN) and, with center, e padded by W/2 linear
+ * ramps to zero on each side (np.pad(mode='linear_ramp')), frames 0 .. frames - 1; without center frames
+ * 0 .. frames - W.  out[t][l] = sum_{j <= W-1-l} y[j] y[j + l] (float32 fma chain in ascending j), divided by
+ * max_l |out[t][l]| when norm_inf and that maximum is >= FLT_MIN.  out_desc: strides (b, c, t, lag).  One launch. */
+int kapre_tempogram(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
+                    int win_length, int center, int norm_inf, float* out_dev, const kapre_spec_desc* out_desc,
+                    void* stream);
+/* Tempo from a tempogram tg (batch x channels x frames x W, strides (b, c, t, lag)).  per_frame = 0: g is the
+ * float64 mean of tg over the frames (sums of 64-frame chunks added in ascending order, / frames), out holds
+ * batch x channels floats (contiguous), two launches over the workspace of kapre_tempo_workspace_bytes.
+ * per_frame = 1: g is tg per frame, out at out_desc's strides, one launch, no workspace.  The tempo is
+ * bpm_scale / argmax_l (log1p(1e6 g[l]) + logprior[l]) (first maximum, float64; a NaN score is skipped), with
+ * logprior a device array of W doubles.  A non-finite g, or no lag with a score, gives NaN. */
+int64_t kapre_tempo_workspace_bytes(int batch, int channels, int frames, int win_length);
+int kapre_tempo(const float* tg_dev, const kapre_spec_desc* tg_desc, int batch, int channels, int frames, int win_length,
+                const double* logprior_dev, double bpm_scale, int per_frame, float* out_dev,
+                const kapre_frames_desc* out_desc, void* workspace_dev, void* stream);
+#define KAPRE_PEAK_MAX_WINDOW (1 << 30)
+typedef struct {
+    int pre_max, post_max, pre_avg, post_avg, wait;   /* 0 .. KAPRE_PEAK_MAX_WINDOW; post_max, post_avg >= 1 */
+    int normalize;
+    double delta;
+} kapre_onset_detect_config;
+/* librosa's peak picking per row of e: x = e - min e, x / (max x + FLT_MIN) with normalize (float32); n is a
+ * candidate iff x[n] == max x[n - pre_max .. n + post_max), x[n] != 0 and x[n] >= mean x[n - pre_avg .. n + post_avg)
+ * + delta (float64; windows clipped to the row); candidates closer than wait + 1 to the last accepted one are dropped.
+ * A row whose x has no nonzero or a non-finite value has no onsets.  One launch. */
+int kapre_onset_detect(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
+                       const kapre_onset_detect_config* cfg, uint8_t* mask_dev, const kapre_frames_desc* mask_desc,
+                       void* stream);
+typedef struct {
+    double fps;                   /* sample_rate / hop_length, > 0 */
+    double tightness;             /* > 0 */
+    int trim;
+} kapre_beat_config;
+/* Device scratch of kapre_beat_track: the local score, cumulative score, backlinks and beats of every row
+ * (24 bytes per frame). */
+int64_t kapre_beat_track_workspace_bytes(int batch, int channels, int frames);
+/* librosa's dynamic-programming beat tracker per row of e.  bpm_dev: batch x channels floats (contiguous), or NULL to
+ * use bpm for every row; period p = rint(60 fps / bpm) (half to even).  tempo_dev (batch x channels, contiguous)
+ * receives the bpm used, 0 for an all-zero row and NaN for a non-finite one; mask_dev the beats.  A row with no
+ * beats, an all-zero or non-finite row, or a p outside [1, KAPRE_BEAT_MAX_PERIOD] has an empty mask.  One launch. */
+int kapre_beat_track(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
+                     const kapre_beat_config* cfg, const float* bpm_dev, float bpm, float* tempo_dev, uint8_t* mask_dev,
+                     const kapre_frames_desc* mask_desc, void* workspace_dev, void* stream);
+
 /* ---- per-channel energy normalisation (PCEN) ---------------------------------------------------
  * Each column (b, c, f) of a non-negative spectrogram E (batch x channels x frames x bands, any strides) is
  * processed along time:

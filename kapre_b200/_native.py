@@ -108,6 +108,26 @@ class HpssCfg(Structure):
 HPSS_MAX_KERNEL = 64
 
 
+class OnsetCfg(Structure):
+    _fields_ = [('lag', c_int), ('max_size', c_int), ('aggregate', c_int), ('pad_frames', c_int)]
+
+
+class OnsetDetectCfg(Structure):
+    _fields_ = [('pre_max', c_int), ('post_max', c_int), ('pre_avg', c_int), ('post_avg', c_int), ('wait', c_int),
+                ('normalize', c_int), ('delta', ctypes.c_double)]
+
+
+class BeatCfg(Structure):
+    _fields_ = [('fps', ctypes.c_double), ('tightness', ctypes.c_double), ('trim', c_int)]
+
+
+ONSET_MEAN, ONSET_MEDIAN = 0, 1
+ONSET_MAX_BINS = 4097
+TEMPOGRAM_MAX_WIN = 4096
+BEAT_MAX_PERIOD = 4096
+PEAK_MAX_WINDOW = 1 << 30
+
+
 class ChromaPlanDesc(Structure):
     _fields_ = [('n_chroma', c_int), ('n_bins', c_int), ('n_tables', c_int), ('tables', c_void_p),
                 ('n_smooth', c_int), ('smooth', c_void_p), ('n_tuning_bins', c_int), ('tuning_edges', c_void_p),
@@ -254,6 +274,22 @@ SYMBOLS = [
     ('kapre_hpss_backward', c_int, [POINTER(HpssCfg), c_void_p, c_int, POINTER(SpecDesc), c_int, c_int, c_int, c_int,
                                     c_void_p, POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p,
                                     POINTER(SpecDesc), c_void_p, c_void_p]),
+    ('kapre_onset_strength', c_int, [POINTER(OnsetCfg), c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int,
+                                     c_void_p, POINTER(FramesDesc), c_void_p]),
+    ('kapre_onset_strength_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int]),
+    ('kapre_onset_strength_backward', c_int, [POINTER(OnsetCfg), c_void_p, POINTER(SpecDesc), c_int, c_int, c_int,
+                                              c_int, c_void_p, POINTER(FramesDesc), c_void_p, POINTER(SpecDesc),
+                                              c_void_p, c_void_p]),
+    ('kapre_tempogram', c_int, [c_void_p, POINTER(FramesDesc), c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                POINTER(SpecDesc), c_void_p]),
+    ('kapre_tempo_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int]),
+    ('kapre_tempo', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, c_void_p, ctypes.c_double, c_int,
+                            c_void_p, POINTER(FramesDesc), c_void_p, c_void_p]),
+    ('kapre_onset_detect', c_int, [c_void_p, POINTER(FramesDesc), c_int, c_int, c_int, POINTER(OnsetDetectCfg),
+                                   c_void_p, POINTER(FramesDesc), c_void_p]),
+    ('kapre_beat_track_workspace_bytes', c_int64, [c_int, c_int, c_int]),
+    ('kapre_beat_track', c_int, [c_void_p, POINTER(FramesDesc), c_int, c_int, c_int, POINTER(BeatCfg), c_void_p,
+                                 c_float, c_void_p, c_void_p, POINTER(FramesDesc), c_void_p, c_void_p]),
     ('kapre_pcen_workspace', c_int, [c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
     ('kapre_pcen', c_int, [c_void_p, POINTER(SpecDesc), c_int, c_int, c_int, c_int, POINTER(PcenParams), c_void_p,
                            POINTER(SpecDesc), c_void_p, POINTER(SpecDesc), c_void_p, c_void_p]),

@@ -40,6 +40,9 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * hpss, harmonic, percussive, HPSS -> ``kapre_hpss_backward`` (the medians recomputed with the element each one
   selected, the mask gradients written beside those indices, then a gather per element), then the STFT magnitude's
   or the STFT and inverse STFT's backward
+* onset_strength, OnsetStrength -> ``kapre_onset_strength_backward`` (the tile recomputed with the bin each window
+  maximum came from and the median's selected bins, then a gather per element), then, from a waveform, the existing
+  backward passes of MagnitudeToDecibel, ApplyFilterbank and the STFT magnitude; ``detrend`` through lfilter's
 * TimeStretch     -> ``kapre_time_stretch_backward`` (reverse-time scan over the saved output and its gradient)
 
 The fused stack (``Sequential``'s STFT -> Magnitude [-> ApplyFilterbank] [-> MagnitudeToDecibel] launch) saves
@@ -637,3 +640,22 @@ def hpss(S, cfg, data_format, want_h, want_p):
     out = out if isinstance(out, tuple) else (out,)
     it = iter(out)
     return (next(it) if want_h else None), (next(it) if want_p else None)
+
+
+class _OnsetStrength(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, S, cfg, data_format):
+        ctx.save_for_backward(S)
+        ctx.cfg = (cfg, data_format)
+        return ops.onset_strength_forward(S, cfg, data_format)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        S, = ctx.saved_tensors
+        cfg, data_format = ctx.cfg
+        return ops.onset_strength_backward(g, S, cfg, data_format), None, None
+
+
+def onset_strength(S, cfg, data_format):
+    return _OnsetStrength.apply(S, cfg, data_format)

@@ -40,6 +40,7 @@
 #include "pitch_core.cuh"
 #include "chroma_core.cuh"
 #include "hpss_core.cuh"
+#include "rhythm_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -4410,6 +4411,241 @@ int kapre_hpss_backward(const kapre_hpss_config* cfg, const void* S_dev, int is_
                                (n + KB_HS_THREADS - 1) / KB_HS_THREADS, dev.sm_count, &grid)))
         return rc;
     return kb_launch(kb_hpss_gather_kernel, {.grid = grid, .block = KB_HS_THREADS, .st = st}, p);
+}
+
+}  // extern "C"
+
+// ---- onset strength, tempogram, tempo, peak picking, beat tracking (rhythm_core.cuh) --------------------------------
+template <int BWD>
+__global__ void __launch_bounds__(KB_RH_THREADS, 1) kb_onset_kernel(const __grid_constant__ KbOnsetParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_onset_cta<BWD>(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_RH_THREADS) kb_onset_gather_kernel(const __grid_constant__ KbOnsetParams p) {
+    kb_onset_gather_cta(p, nullptr, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_RH_THREADS) kb_tempogram_kernel(const __grid_constant__ KbTempogramParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_tempogram_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_RH_THREADS) kb_tempo_part_kernel(const __grid_constant__ KbTempoParams p) {
+    kb_tempo_part_cta(p, nullptr, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_RH_THREADS) kb_tempo_kernel(const __grid_constant__ KbTempoParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_tempo_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_RH_THREADS) kb_peak_kernel(const __grid_constant__ KbPeakParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_peak_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+__global__ void __launch_bounds__(KB_RH_THREADS, 1) kb_beat_kernel(const __grid_constant__ KbBeatParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_beat_cta(p, kb_smem, blockIdx.x, gridDim.x);
+}
+
+// A persistent launch of `kernel` over `jobs` jobs.
+template <typename K, typename P>
+static int kb_rh_launch(K kernel, const char* name, int smem, long long jobs, const P& p, cudaStream_t st, bool timed) {
+    DevInfo dev;
+    int rc, grid;
+    if ((rc = kb_dev_info(&dev))) return rc;
+    if ((rc = kb_resident_grid(kernel, name, KB_RH_THREADS, smem, jobs, dev.sm_count, &grid))) return rc;
+    return kb_launch(kernel, {.grid = grid, .block = KB_RH_THREADS, .smem = smem, .st = st, .timed = timed}, p);
+}
+
+static int kb_rh_rows(int B, int C, int T, const char* what) {
+    if (B < 0 || C < 0 || T < 0) return kb_fail(KAPRE_E_INVALID, "%s: negative size (%d, %d, %d)", what, B, C, T);
+    return 0;
+}
+
+static int kb_onset_params(const kapre_onset_config* cfg, const float* S, const kapre_spec_desc* sd, int B, int C,
+                           int T, int K, int bwd, KbOnsetParams* out) {
+    if (!cfg || !sd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_rh_rows(B, C, T, "onset_strength");
+    if (rc) return rc;
+    if (K < 1 || K > KAPRE_ONSET_MAX_BINS)
+        return kb_fail(KAPRE_E_INVALID, "onset_strength: bins %d outside [1, %d]", K, KAPRE_ONSET_MAX_BINS);
+    if (cfg->max_size < 1 || cfg->max_size > K)
+        return kb_fail(KAPRE_E_INVALID, "onset_strength: max_size %d outside [1, %d]", cfg->max_size, K);
+    if (cfg->lag < 1 || (T > 0 && cfg->lag >= T))
+        return kb_fail(KAPRE_E_INVALID, "onset_strength: lag %d outside [1, frames)", cfg->lag);
+    if (cfg->pad_frames < 0 || cfg->pad_frames > (1 << 28))
+        return kb_fail(KAPRE_E_INVALID, "onset_strength: pad_frames %d out of range", cfg->pad_frames);
+    if (cfg->aggregate != KAPRE_ONSET_MEAN && cfg->aggregate != KAPRE_ONSET_MEDIAN)
+        return kb_fail(KAPRE_E_INVALID, "onset_strength: unknown aggregate %d", cfg->aggregate);
+    KbOnsetParams p{};
+    p.B = B; p.C = C; p.T = T; p.K = K;
+    p.lag = cfg->lag; p.m = cfg->max_size; p.agg = cfg->aggregate; p.P = cfg->lag + cfg->pad_frames;
+    p.x = S; p.x_sb = sd->stride_b; p.x_sc = sd->stride_c; p.x_st = sd->stride_t; p.x_sk = sd->stride_f;
+    if (!kb_onset_setup(p, bwd)) return kb_fail(KAPRE_E_INVALID, "onset_strength: too many tiles");
+    if (p.jobs && !S) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    *out = p;
+    return 0;
+}
+
+static int kb_beat_ws_total(int B, int C, int T, int64_t* n) {
+    int rc = kb_rh_rows(B, C, T, "beat_track");
+    if (rc) return rc;
+    const long long rows = (long long)B * C;
+    if (rows && kb_beat_ws_bytes_row(T) > (1LL << 46) / rows) return kb_fail(KAPRE_E_INVALID, "beat_track: too large");
+    *n = rows * kb_beat_ws_bytes_row(T);
+    return 0;
+}
+
+extern "C" {
+
+int kapre_onset_strength(const kapre_onset_config* cfg, const float* S_dev, const kapre_spec_desc* S_desc, int batch,
+                         int channels, int frames, int bins, float* out_dev, const kapre_frames_desc* out_desc,
+                         void* stream) {
+    KbOnsetParams p;
+    int rc = kb_onset_params(cfg, S_dev, S_desc, batch, channels, frames, bins, 0, &p);
+    if (rc) return rc;
+    if (!out_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (!p.jobs) return 0;
+    if (!out_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.out = out_dev; p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t;
+    return kb_rh_launch(kb_onset_kernel<0>, "onset", kb_onset_smem(p.K, p.m, p.F, 0), p.jobs, p, (cudaStream_t)stream,
+                        true);
+}
+
+int64_t kapre_onset_strength_workspace_bytes(int batch, int channels, int frames, int bins) {
+    if (batch < 0 || channels < 0 || frames < 0 || bins < 0) return kb_fail(KAPRE_E_INVALID, "onset_strength: negative size");
+    return (int64_t)batch * channels * frames * bins * (int64_t)sizeof(kb_on_w);
+}
+
+int kapre_onset_strength_backward(const kapre_onset_config* cfg, const float* S_dev, const kapre_spec_desc* S_desc,
+                                  int batch, int channels, int frames, int bins, const float* g_dev,
+                                  const kapre_frames_desc* g_desc, float* gS_dev, const kapre_spec_desc* gS_desc,
+                                  void* workspace_dev, void* stream) {
+    KbOnsetParams p;
+    int rc = kb_onset_params(cfg, S_dev, S_desc, batch, channels, frames, bins, 1, &p);
+    if (rc) return rc;
+    if (!g_desc || !gS_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (!p.jobs) return 0;
+    if (!g_dev || !gS_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.g = g_dev; p.g_sb = g_desc->stride_b; p.g_sc = g_desc->stride_c; p.g_st = g_desc->stride_t;
+    p.gx = gS_dev; p.gx_sb = gS_desc->stride_b; p.gx_sc = gS_desc->stride_c; p.gx_st = gS_desc->stride_t;
+    p.gx_sk = gS_desc->stride_f;
+    p.ws = (kb_on_w*)workspace_dev;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = kb_rh_launch(kb_onset_kernel<1>, "onset_bwd", kb_onset_smem(p.K, p.m, p.F, 1), p.jobs, p, st, false)))
+        return rc;
+    const long long n = (long long)batch * channels * frames * bins;
+    return kb_rh_launch(kb_onset_gather_kernel, "onset_gather", 0, (n + KB_RH_THREADS - 1) / KB_RH_THREADS, p, st,
+                        false);
+}
+
+int kapre_tempogram(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
+                    int win_length, int center, int norm_inf, float* out_dev, const kapre_spec_desc* out_desc,
+                    void* stream) {
+    if (!e_desc || !out_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_rh_rows(batch, channels, frames, "tempogram");
+    if (rc) return rc;
+    if (win_length < 2 || win_length > KAPRE_TEMPOGRAM_MAX_WIN)
+        return kb_fail(KAPRE_E_INVALID, "tempogram: win_length %d outside [2, %d]", win_length, KAPRE_TEMPOGRAM_MAX_WIN);
+    if (!center && frames < win_length)
+        return kb_fail(KAPRE_E_INVALID, "tempogram: %d frames < win_length %d without center", frames, win_length);
+    KbTempogramParams p{};
+    p.B = batch; p.C = channels; p.T = frames; p.W = win_length; p.center = center != 0; p.norm = norm_inf != 0;
+    p.e = e_dev; p.e_sb = e_desc->stride_b; p.e_sc = e_desc->stride_c; p.e_st = e_desc->stride_t;
+    p.out = out_dev; p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t;
+    p.o_sk = out_desc->stride_f;
+    if (!kb_tempogram_setup(p)) return kb_fail(KAPRE_E_INVALID, "tempogram: too many tiles");
+    if (!p.jobs) return 0;
+    if (!e_dev || !out_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    return kb_rh_launch(kb_tempogram_kernel, "tempogram", kb_tg_words(p.W, p.F) * 4, p.jobs, p, (cudaStream_t)stream,
+                        true);
+}
+
+int64_t kapre_tempo_workspace_bytes(int batch, int channels, int frames, int win_length) {
+    int rc = kb_rh_rows(batch, channels, frames, "tempo");
+    if (rc) return rc;
+    if (win_length < 2 || win_length > KAPRE_TEMPOGRAM_MAX_WIN)
+        return kb_fail(KAPRE_E_INVALID, "tempo: win_length %d outside [2, %d]", win_length, KAPRE_TEMPOGRAM_MAX_WIN);
+    return kb_tempo_ws_bytes(batch, channels, frames, win_length);
+}
+
+int kapre_tempo(const float* tg_dev, const kapre_spec_desc* tg_desc, int batch, int channels, int frames, int win_length,
+                const double* logprior_dev, double bpm_scale, int per_frame, float* out_dev,
+                const kapre_frames_desc* out_desc, void* workspace_dev, void* stream) {
+    if (!tg_desc || (per_frame && !out_desc)) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_rh_rows(batch, channels, frames, "tempo");
+    if (rc) return rc;
+    if (win_length < 2 || win_length > KAPRE_TEMPOGRAM_MAX_WIN)
+        return kb_fail(KAPRE_E_INVALID, "tempo: win_length %d outside [2, %d]", win_length, KAPRE_TEMPOGRAM_MAX_WIN);
+    if (!per_frame && batch && channels && frames < 1) return kb_fail(KAPRE_E_INVALID, "tempo: no frames");
+    if (!(bpm_scale > 0.0) || !isfinite(bpm_scale)) return kb_fail(KAPRE_E_INVALID, "tempo: bpm_scale must be > 0");
+    KbTempoParams p{};
+    p.B = batch; p.C = channels; p.T = frames; p.W = win_length; p.per_frame = per_frame != 0;
+    p.tg = tg_dev; p.g_sb = tg_desc->stride_b; p.g_sc = tg_desc->stride_c; p.g_st = tg_desc->stride_t;
+    p.g_sk = tg_desc->stride_f;
+    p.logprior = logprior_dev; p.bpm_scale = bpm_scale; p.out = out_dev; p.part = (double*)workspace_dev;
+    if (per_frame) { p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t; }
+    kb_tempo_setup(p);
+    if (!p.jobs) return 0;
+    if (!tg_dev || !logprior_dev || !out_dev || (!per_frame && !workspace_dev))
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!per_frame &&
+        (rc = kb_rh_launch(kb_tempo_part_kernel, "tempo_part", 0, (long long)batch * channels * p.chunks, p, st, false)))
+        return rc;
+    return kb_rh_launch(kb_tempo_kernel, "tempo", kb_tempo_smem(p.W), p.jobs, p, st, false);
+}
+
+int kapre_onset_detect(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
+                       const kapre_onset_detect_config* cfg, uint8_t* mask_dev, const kapre_frames_desc* mask_desc,
+                       void* stream) {
+    if (!e_desc || !cfg || !mask_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_rh_rows(batch, channels, frames, "onset_detect");
+    if (rc) return rc;
+    if (cfg->pre_max < 0 || cfg->pre_avg < 0 || cfg->wait < 0 || cfg->post_max < 1 || cfg->post_avg < 1)
+        return kb_fail(KAPRE_E_INVALID, "onset_detect: pre_* and wait must be >= 0, post_* >= 1");
+    if (cfg->pre_max > KAPRE_PEAK_MAX_WINDOW || cfg->post_max > KAPRE_PEAK_MAX_WINDOW ||
+        cfg->pre_avg > KAPRE_PEAK_MAX_WINDOW || cfg->post_avg > KAPRE_PEAK_MAX_WINDOW || cfg->wait > KAPRE_PEAK_MAX_WINDOW)
+        return kb_fail(KAPRE_E_INVALID, "onset_detect: pre_*, post_* and wait must be <= %d", KAPRE_PEAK_MAX_WINDOW);
+    if (!isfinite(cfg->delta)) return kb_fail(KAPRE_E_INVALID, "onset_detect: delta must be finite");
+    KbPeakParams p{};
+    p.B = batch; p.C = channels; p.T = frames;
+    p.pre_max = cfg->pre_max; p.post_max = cfg->post_max; p.pre_avg = cfg->pre_avg; p.post_avg = cfg->post_avg;
+    p.wait = cfg->wait; p.normalize = cfg->normalize != 0; p.delta = cfg->delta;
+    p.e = e_dev; p.e_sb = e_desc->stride_b; p.e_sc = e_desc->stride_c; p.e_st = e_desc->stride_t;
+    p.mask = mask_dev; p.m_sb = mask_desc->stride_b; p.m_sc = mask_desc->stride_c; p.m_st = mask_desc->stride_t;
+    p.jobs = frames ? (long long)batch * channels : 0;
+    if (!p.jobs) return 0;
+    if (!e_dev || !mask_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    return kb_rh_launch(kb_peak_kernel, "onset_detect", kb_peak_smem(), p.jobs, p, (cudaStream_t)stream, false);
+}
+
+int64_t kapre_beat_track_workspace_bytes(int batch, int channels, int frames) {
+    int64_t n = 0;
+    int rc = kb_beat_ws_total(batch, channels, frames, &n);
+    return rc ? rc : n;
+}
+
+int kapre_beat_track(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
+                     const kapre_beat_config* cfg, const float* bpm_dev, float bpm, float* tempo_dev, uint8_t* mask_dev,
+                     const kapre_frames_desc* mask_desc, void* workspace_dev, void* stream) {
+    if (!e_desc || !cfg || !mask_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int64_t nws = 0;
+    int rc = kb_beat_ws_total(batch, channels, frames, &nws);
+    if (rc) return rc;
+    if (!(cfg->fps > 0.0) || !isfinite(cfg->fps)) return kb_fail(KAPRE_E_INVALID, "beat_track: fps must be > 0");
+    if (!(cfg->tightness > 0.0) || !isfinite(cfg->tightness))
+        return kb_fail(KAPRE_E_INVALID, "beat_track: tightness must be > 0");
+    if (!bpm_dev && !(bpm > 0.0f && isfinite(bpm))) return kb_fail(KAPRE_E_INVALID, "beat_track: bpm must be > 0");
+    KbBeatParams p{};
+    p.B = batch; p.C = channels; p.T = frames; p.trim = cfg->trim != 0; p.fps = cfg->fps; p.tightness = cfg->tightness;
+    p.bpm = bpm_dev; p.bpm_const = bpm;
+    p.e = e_dev; p.e_sb = e_desc->stride_b; p.e_sc = e_desc->stride_c; p.e_st = e_desc->stride_t;
+    p.tempo = tempo_dev; p.mask = mask_dev;
+    p.m_sb = mask_desc->stride_b; p.m_sc = mask_desc->stride_c; p.m_st = mask_desc->stride_t;
+    p.ws = workspace_dev;
+    p.jobs = (long long)batch * channels;
+    if (!p.jobs) return 0;
+    if (!frames) return kb_fail(KAPRE_E_INVALID, "beat_track: no frames");
+    if (!e_dev || !tempo_dev || !mask_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    return kb_rh_launch(kb_beat_kernel, "beat_track", kb_beat_smem(), p.jobs, p, (cudaStream_t)stream, false);
 }
 
 }  // extern "C"

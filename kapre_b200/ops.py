@@ -2191,3 +2191,246 @@ def hpss(S, cfg, data_format=_CH_LAST_STR, want_h=True, want_p=True):
         from . import autograd
         return autograd.hpss(S, cfg, data_format, want_h, want_p)
     return hpss_forward(S, cfg, data_format, want_h, want_p)
+
+
+# ------------------------------------------------------------------------------- onsets, tempo and beats
+def _check_int(name, v, lo, hi=None):
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v > hi):
+        raise ValueError('%s must be an integer in [%d, %s], got %r' % (name, lo, 'inf' if hi is None else hi, v))
+    return int(v)
+
+
+def _frames_desc(t: torch.Tensor, data_format: str):
+    """(B, T, C) channels_last or (B, C, T) channels_first -> kapre_frames_desc, (B, C, T)."""
+    if t.dim() != 3:
+        raise ValueError('expected a 3-D (batch, frames, ch) / (batch, ch, frames) tensor, got shape %s'
+                         % (tuple(t.shape),))
+    if data_format == _CH_LAST_STR:
+        B, T, C = t.shape
+        sb, st, sc = t.stride()
+    else:
+        B, C, T = t.shape
+        sb, sc, st = t.stride()
+    return N.FramesDesc(sb, sc, st), (B, C, T)
+
+
+def _envelope_input(e, name, data_format):
+    if not (isinstance(e, torch.Tensor) and e.is_cuda):
+        raise N.KapreNativeError('%s needs a CUDA tensor' % name)
+    if e.dtype != torch.float32:
+        raise ValueError('%s expects float32, got %s' % (name, e.dtype))
+    e = _raw(e.detach())
+    ed, dims = _frames_desc(e, data_format)
+    return e, ed, dims
+
+
+def onset_config(lag=1, max_size=1, aggregate='mean', pad_frames=0):
+    """The ``kapre_onset_config`` of ``onset_strength``'s arguments; a bad one raises ``ValueError`` here."""
+    lag = _check_int('lag', lag, 1)
+    max_size = _check_int('max_size', max_size, 1)
+    if aggregate not in ('mean', 'median'):
+        raise ValueError("aggregate must be 'mean' or 'median', got %r" % (aggregate,))
+    pad_frames = _check_int('pad_frames', pad_frames, 0, 1 << 28)
+    return N.OnsetCfg(lag, max_size, N.ONSET_MEAN if aggregate == 'mean' else N.ONSET_MEDIAN, pad_frames)
+
+
+def _onset_input(S, cfg, data_format):
+    if not (isinstance(S, torch.Tensor) and S.is_cuda):
+        raise N.KapreNativeError('onset_strength needs a CUDA spectrogram')
+    if S.dtype != torch.float32:
+        raise ValueError('onset_strength expects a float32 spectrogram, got %s' % (S.dtype,))
+    S = _raw(S.detach())
+    sd, (B, C, T, K) = _spec_desc(S, data_format)
+    onset_limits(cfg, K, T)
+    return S, sd, (B, C, T, K)
+
+
+def onset_limits(cfg, K, T):
+    """The limits of ``kapre_onset_strength`` for K bins and T frames; raises ``ValueError``."""
+    if not 1 <= K <= N.ONSET_MAX_BINS:
+        raise ValueError('onset_strength supports 1 to %d bins, got %d' % (N.ONSET_MAX_BINS, K))
+    if cfg.max_size > K:
+        raise ValueError('max_size (%d) must not exceed the %d bins' % (cfg.max_size, K))
+    if T and cfg.lag >= T:
+        raise ValueError('lag (%d) must be below the %d frames' % (cfg.lag, T))
+
+
+def onset_strength_forward(S, cfg, data_format):
+    """The envelope ``(B, T, C)`` / ``(B, C, T)`` of ``kapre_onset_strength``: one launch."""
+    S, sd, (B, C, T, K) = _onset_input(S, cfg, data_format)
+    out, od = _frames_alloc(B, C, T, data_format, torch.float32, S.device)
+    if out.numel():
+        N.check(N.lib().kapre_onset_strength(ctypes.byref(cfg), _ptr(S), ctypes.byref(sd), B, C, T, K, _ptr(out),
+                                             ctypes.byref(od), _stream_ptr()))
+    return out
+
+
+def onset_strength_backward(g, S, cfg, data_format):
+    """Gradient of ``onset_strength_forward`` with respect to S: two launches over a workspace of 8 bytes per
+    element."""
+    S, sd, (B, C, T, K) = _onset_input(S, cfg, data_format)
+    g = _raw(g.to(torch.float32))
+    gd, _ = _frames_desc(g, data_format)
+    gS, gSd = _spec_alloc(B, C, T, K, data_format, torch.float32, S.device)
+    if gS.numel():
+        n = int(N.lib().kapre_onset_strength_workspace_bytes(B, C, T, K))
+        if n < 0:
+            N.check(n)
+        ws = torch.empty(max(n // 4, 1), dtype=torch.float32, device=S.device)
+        N.check(N.lib().kapre_onset_strength_backward(ctypes.byref(cfg), _ptr(S), ctypes.byref(sd), B, C, T, K,
+                                                      _ptr(g), ctypes.byref(gd), _ptr(gS), ctypes.byref(gSd),
+                                                      _ptr(ws), _stream_ptr()))
+    return gS
+
+
+@_device_of_first_arg
+def onset_strength(S, cfg, data_format=_CH_LAST_STR):
+    """Onset strength envelope of a float32 CUDA spectrogram ``(B, T, K, C)`` / ``(B, C, T, K)`` under ``cfg``
+    (``onset_config``).  One launch; differentiable with respect to S."""
+    _onset_input(S, cfg, data_format)
+    if _wants_grad(S):
+        from . import autograd
+        return autograd.onset_strength(S, cfg, data_format)
+    return onset_strength_forward(S, cfg, data_format)
+
+
+def tempogram_check(win_length, frames=None, center=True):
+    win_length = _check_int('win_length', win_length, 2, N.TEMPOGRAM_MAX_WIN)
+    if not center and frames is not None and frames < win_length:
+        raise ValueError('without center the envelope needs at least win_length=%d frames, got %d'
+                         % (win_length, frames))
+    return win_length
+
+
+@_device_of_first_arg
+def tempogram(e, win_length=384, center=True, norm_inf=True, data_format=_CH_LAST_STR):
+    """Autocorrelation tempogram of a float32 CUDA envelope ``(B, T, C)`` / ``(B, C, T)``: ``(B, frames, W, C)`` /
+    ``(B, C, frames, W)`` float32.  One launch; no gradient (an input that requires grad under grad mode raises)."""
+    if _wants_grad(e):
+        raise ValueError('tempogram has no gradient: call it under torch.no_grad() or on a detached envelope')
+    e, ed, (B, C, T) = _envelope_input(e, 'tempogram', data_format)
+    W = tempogram_check(win_length, T, center)
+    n_out = T if center else T - W + 1
+    out, od = _spec_alloc(B, C, n_out, W, data_format, torch.float32, e.device)
+    if out.numel():
+        N.check(N.lib().kapre_tempogram(_ptr(e), ctypes.byref(ed), B, C, T, W, int(bool(center)), int(bool(norm_inf)),
+                                        _ptr(out), ctypes.byref(od), _stream_ptr()))
+    return out
+
+
+class TempoPlan:
+    """The float64 log-prior over the lags of one tempo configuration, built on the host and kept per device."""
+
+    def __init__(self, win_length, sample_rate, hop_length, start_bpm=120.0, std_bpm=1.0, max_tempo=320.0):
+        self.W = tempogram_check(win_length)
+        self.bpm_scale = 60.0 * float(sample_rate) / float(hop_length)
+        lags = np.arange(self.W, dtype=np.float64)
+        with np.errstate(divide='ignore'):
+            bpm = self.bpm_scale / lags
+            prior = -0.5 * ((np.log2(bpm) - np.log2(float(start_bpm))) / float(std_bpm)) ** 2
+        if max_tempo is not None:
+            prior[:int(np.argmax(bpm < float(max_tempo)))] = -np.inf
+        prior[0] = -np.inf
+        self.logprior = prior
+        self._per_device = {}
+
+    def table(self, device):
+        t = self._per_device.get(device)
+        if t is None:
+            t = torch.from_numpy(self.logprior).to(device)
+            self._per_device[device] = t
+        return t
+
+
+@_device_of_first_arg
+def tempo(tg, plan: TempoPlan, per_frame=False, data_format=_CH_LAST_STR):
+    """Tempo (bpm) from a float32 CUDA tempogram ``(B, frames, W, C)`` / ``(B, C, frames, W)``: ``(B, C)``, or per
+    frame ``(B, frames, C)`` / ``(B, C, frames)``.  Two launches (one per frame); no gradient."""
+    if not (isinstance(tg, torch.Tensor) and tg.is_cuda):
+        raise N.KapreNativeError('tempo needs a CUDA tempogram')
+    if tg.dtype != torch.float32:
+        raise ValueError('tempo expects a float32 tempogram, got %s' % (tg.dtype,))
+    tg = _raw(tg.detach())
+    gd, (B, C, T, W) = _spec_desc(tg, data_format)
+    if W != plan.W:
+        raise ValueError('the tempogram has %d lags, the plan %d' % (W, plan.W))
+    if not per_frame and B * C and T < 1:
+        raise ValueError('tempo needs at least one frame')
+    if per_frame:
+        out, od = _frames_alloc(B, C, T, data_format, torch.float32, tg.device)
+    else:
+        out, od = torch.empty((B, C), dtype=torch.float32, device=tg.device), None
+    if out.numel():
+        ws = None
+        if not per_frame:
+            n = int(N.lib().kapre_tempo_workspace_bytes(B, C, T, W))
+            if n < 0:
+                N.check(n)
+            ws = torch.empty(max(n // 8, 1), dtype=torch.float64, device=tg.device)
+        N.check(N.lib().kapre_tempo(_ptr(tg), ctypes.byref(gd), B, C, T, W, _ptr(plan.table(tg.device)),
+                                    ctypes.c_double(plan.bpm_scale), int(bool(per_frame)), _ptr(out),
+                                    ctypes.byref(od) if od is not None else None,
+                                    _ptr(ws) if ws is not None else None, _stream_ptr()))
+    return out
+
+
+def onset_detect_config(pre_max, post_max, pre_avg, post_avg, wait, delta, normalize):
+    args = (('pre_max', pre_max, 0), ('post_max', post_max, 1), ('pre_avg', pre_avg, 0), ('post_avg', post_avg, 1),
+            ('wait', wait, 0))
+    vals = [_check_int(n, v, lo, N.PEAK_MAX_WINDOW) for n, v, lo in args]
+    if isinstance(delta, (bool, np.bool_)) or not np.isfinite(float(delta)):
+        raise ValueError('delta must be a finite number, got %r' % (delta,))
+    return N.OnsetDetectCfg(*vals, int(bool(normalize)), float(delta))
+
+
+@_device_of_first_arg
+def onset_detect(e, cfg, data_format=_CH_LAST_STR):
+    """Onset mask (bool, the envelope's shape) of a float32 CUDA envelope under ``cfg`` (``onset_detect_config``).
+    One launch."""
+    e, ed, (B, C, T) = _envelope_input(e, 'onset_detect', data_format)
+    mask, md = _frames_alloc(B, C, T, data_format, torch.bool, e.device)
+    if mask.numel():
+        N.check(N.lib().kapre_onset_detect(_ptr(e), ctypes.byref(ed), B, C, T, ctypes.byref(cfg), _ptr(mask),
+                                           ctypes.byref(md), _stream_ptr()))
+    return mask
+
+
+def beat_config(sample_rate, hop_length, tightness, trim):
+    fps = float(sample_rate) / float(hop_length)
+    if not (np.isfinite(fps) and fps > 0):
+        raise ValueError('sample_rate / hop_length must be positive, got %r / %r' % (sample_rate, hop_length))
+    if isinstance(tightness, (bool, np.bool_)) or not (np.isfinite(float(tightness)) and float(tightness) > 0):
+        raise ValueError('tightness must be positive, got %r' % (tightness,))
+    return N.BeatCfg(fps, float(tightness), int(bool(trim)))
+
+
+@_device_of_first_arg
+def beat_track(e, cfg, bpm, data_format=_CH_LAST_STR):
+    """(tempo (B, C) float32, beat mask (bool, the envelope's shape)) of a float32 CUDA envelope under ``cfg``
+    (``beat_config``); ``bpm`` is a float for every row or a ``(B, C)`` float32 CUDA tensor.  One launch over a
+    workspace of 24 bytes per frame."""
+    e, ed, (B, C, T) = _envelope_input(e, 'beat_track', data_format)
+    bpm_t, bpm_v = None, 0.0
+    if isinstance(bpm, torch.Tensor):
+        if bpm.shape != (B, C) or bpm.dtype != torch.float32 or bpm.device != e.device:
+            raise ValueError('bpm must be a (%d, %d) float32 tensor on %s' % (B, C, e.device))
+        bpm_t = bpm.detach().contiguous()
+    else:
+        bpm_v = float(bpm)
+        p = np.rint(60.0 * cfg.fps / bpm_v) if bpm_v > 0 and np.isfinite(bpm_v) else 0
+        if not 1 <= p <= N.BEAT_MAX_PERIOD:
+            raise ValueError('bpm=%r gives a beat period of %r frames, outside [1, %d]'
+                             % (bpm, p, N.BEAT_MAX_PERIOD))
+    tempo_out = torch.empty((B, C), dtype=torch.float32, device=e.device)
+    mask, md = _frames_alloc(B, C, T, data_format, torch.bool, e.device)
+    if B * C and T < 1:
+        raise ValueError('beat_track needs at least one frame')
+    if tempo_out.numel():
+        n = int(N.lib().kapre_beat_track_workspace_bytes(B, C, T))
+        if n < 0:
+            N.check(n)
+        ws = torch.empty(max(n // 8, 1), dtype=torch.float64, device=e.device)
+        N.check(N.lib().kapre_beat_track(_ptr(e), ctypes.byref(ed), B, C, T, ctypes.byref(cfg),
+                                         _ptr(bpm_t) if bpm_t is not None else None, ctypes.c_float(bpm_v),
+                                         _ptr(tempo_out), _ptr(mask), ctypes.byref(md), _ptr(ws), _stream_ptr()))
+    return tempo_out, mask

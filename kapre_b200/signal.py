@@ -8,7 +8,8 @@ filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, o
 ``add_noise`` (torchaudio's, with deterministic float64 energies), or ``loudness`` and ``Loudness`` (torchaudio's
 BS.1770 gated loudness, with per-item lengths), or the pitch trackers ``yin``, ``pyin``, ``YIN`` and ``PYIN``
 (librosa's), or the chroma features ``chroma_stft``, ``chroma_cqt``, ``chroma_cens`` and ``estimate_tuning``
-(librosa's), or the harmonic/percussive separation ``hpss``, ``harmonic`` and ``percussive`` (librosa's)."""
+(librosa's), or the harmonic/percussive separation ``hpss``, ``harmonic`` and ``percussive`` (librosa's), or the
+rhythm features ``onset_strength``, ``onset_detect``, ``tempogram``, ``tempo`` and ``beat_track`` (librosa's)."""
 from __future__ import annotations
 
 import math
@@ -23,7 +24,7 @@ from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
            'Biquad', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
            'YIN', 'PYIN', 'chroma_stft', 'chroma_cqt', 'chroma_cens', 'estimate_tuning', 'hpss', 'harmonic',
-           'percussive']
+           'percussive', 'onset_strength', 'onset_detect', 'tempogram', 'tempo', 'beat_track']
 
 
 def _resolve(fmt):
@@ -954,3 +955,235 @@ def percussive(waveform, kernel_size=31, power=2.0, margin=1.0, n_fft=2048, win_
     """The percussive part of a CUDA waveform batch (``librosa.effects.percussive``); see ``harmonic``."""
     return _hpss_component(waveform, 'percussive', kernel_size, power, margin, n_fft, win_length, hop_length,
                            window_name, data_format)
+
+
+# ---- onsets, tempo and beats -------------------------------------------------------------------------------------------
+def _rhythm_frontend(sample_rate, n_fft, hop_length, n_mels, fmin, fmax):
+    """(StftPlan, Filterbank) of librosa's default onset feature: the periodic Hann STFT and the slaney mel bank."""
+    n_fft = backend._check_n_fft(n_fft)
+    if isinstance(hop_length, bool) or int(hop_length) != hop_length or int(hop_length) < 1:
+        raise ValueError('hop_length must be a positive integer, got %r' % (hop_length,))
+    sr = float(sample_rate)
+    if not (np.isfinite(sr) and sr > 0):
+        raise ValueError('sample_rate must be positive, got %r' % (sample_rate,))
+    n_mels = ops._check_int('n_mels', n_mels, 1)
+    stft = _cached(('stft', n_fft, int(hop_length), None),
+                   lambda: ops.StftPlan(n_fft, n_fft, int(hop_length), backend.get_window_fn(None)(n_fft)))
+    key = ('onset_mel', sr, n_fft, n_mels, float(fmin), None if fmax is None else float(fmax))
+    fb = _cached(key, lambda: ops.Filterbank(backend.filterbank_mel(sr, n_fft // 2 + 1, n_mels, fmin, fmax)))
+    return stft, fb
+
+
+def _onset_feature(waveform, sample_rate, n_fft, hop_length, n_mels, fmin, fmax, fmt):
+    """librosa's default onset feature of a waveform batch: the centred |STFT|^2, the mel bank and
+    ``MagnitudeToDecibel(1.0, 1e-10, 80)`` (the clamp reference is each item's maximum)."""
+    stft, fb = _rhythm_frontend(sample_rate, n_fft, hop_length, n_mels, fmin, fmax)
+    X = _centred_magnitude(waveform, stft, fmt, True)
+    return backend.magnitude_to_decibel(ops.apply_filterbank(X * X, fb, fmt), ref_value=1.0, amin=1e-10,
+                                        dynamic_range=80.0)
+
+
+def _one_source(a, b, names):
+    if (a is None) == (b is None):
+        raise ValueError('pass exactly one of %s and %s' % names)
+
+
+def onset_strength(waveform=None, sample_rate=22050, S=None, lag=1, max_size=1, detrend=False, center=True,
+                   aggregate='mean', n_fft=2048, hop_length=512, n_mels=128, fmin=0.0, fmax=None,
+                   data_format='default'):
+    """Spectral-flux onset strength (modelled on ``librosa.onset.onset_strength``): float32 ``(batch, frames, ch)`` /
+    ``(batch, ch, frames)``, one value per frame of S.
+
+    From ``waveform`` (``(batch, time, ch)`` / ``(batch, ch, time)`` float32 CUDA), S is librosa's default feature:
+    the centred periodic-Hann STFT (``n_fft // 2`` zeros on each side, ``1 + time // hop_length`` frames), squared,
+    ``backend.filterbank_mel(sample_rate, n_fft // 2 + 1, n_mels, fmin, fmax)`` and ``MagnitudeToDecibel(1.0,
+    1e-10, 80)``, whose clamp reference is each item's maximum (librosa: the whole array's).  ``S`` (instead): any
+    float32 spectrogram in this library's layout, 1 to 4097 bins, used as given.
+
+    With m = ``max_size`` and K bins: ``R[t][b]`` = max of S[t] over bins ``b - m//2 .. b - m//2 + m - 1`` inside
+    the row, ``D = max(0, S[t] - R[t - lag])`` (NaN kept), the mean (float64 sum / K, rounded once) or numpy's
+    median over bins, then ``lag + n_fft // (2 hop_length)`` (with ``center``, else ``lag``) zeros in front and the
+    row cut to its frames; ``detrend`` then runs ``lfilter(b=[1, -1], a=[1, -0.99])``.  Restated from librosa's
+    definitions, not checked against librosa.
+
+    One launch from S (plus four for ``detrend``), four more from a waveform.  Differentiable with respect to S and
+    the waveform: relu'(0) = 0, a window maximum's gradient to the lowest of its tied bins, the median's to the
+    element(s) it selected."""
+    fmt = _resolve(_unwrap_format(data_format))
+    _one_source(waveform, S, ('waveform', 'S'))
+    n_fft = backend._check_n_fft(n_fft)
+    hop_length = ops._check_int('hop_length', hop_length, 1)
+    cfg = ops.onset_config(lag, max_size, aggregate, n_fft // (2 * hop_length) if center else 0)
+    if S is None:
+        if not (isinstance(waveform, torch.Tensor) and waveform.dim() == 3):
+            raise ValueError('waveform must be a 3-D (batch, time, ch) / (batch, ch, time) tensor')
+        length = waveform.shape[1] if fmt == _CH_LAST_STR else waveform.shape[2]
+        ops.onset_limits(cfg, ops._check_int('n_mels', n_mels, 1), 1 + length // hop_length)
+        S = _onset_feature(waveform, sample_rate, n_fft, hop_length, n_mels, fmin, fmax, fmt)
+    elif not (isinstance(S, torch.Tensor) and S.is_cuda):
+        raise ops.N.KapreNativeError('S must be a CUDA tensor')
+    e = ops.onset_strength(S, cfg, fmt)
+    if detrend:
+        b = torch.tensor([[[1.0, -1.0]]], dtype=torch.float32, device=e.device)
+        a = torch.tensor([[[1.0, -0.99]]], dtype=torch.float32, device=e.device)
+        e = ops.lfilter(e, b, a, clamp=False, data_format=fmt)
+    return e
+
+
+def _envelope(waveform, onset_envelope, sample_rate, hop_length, fmt, aggregate='mean'):
+    _one_source(waveform, onset_envelope, ('waveform', 'onset_envelope'))
+    if onset_envelope is not None:
+        return onset_envelope
+    with torch.no_grad():
+        return onset_strength(waveform.detach(), sample_rate=sample_rate, hop_length=hop_length, aggregate=aggregate,
+                              data_format=fmt)
+
+
+def tempogram(waveform=None, sample_rate=22050, onset_envelope=None, hop_length=512, win_length=384, center=True,
+              norm=np.inf, data_format='default'):
+    """Autocorrelation tempogram (modelled on ``librosa.feature.tempogram``): float32 ``(batch, frames,
+    win_length, ch)`` / ``(batch, ch, frames, win_length)``.
+
+    With W = ``win_length`` (2 .. 4096) and ``center``, the envelope gets ``W // 2`` linear ramps to zero on each
+    side (``np.pad(mode='linear_ramp')``) and there is one frame per envelope frame; without it the frames are
+    0 .. T - W.  Each frame is windowed by the periodic Hann window of W, autocorrelated (``ac[l] = sum y[j]
+    y[j + l]``, a float32 fma chain in ascending j) and, with ``norm=np.inf``, divided by its largest ``|ac|`` unless
+    that is below FLT_MIN; ``norm=None`` leaves it.  From a waveform the envelope is ``onset_strength`` at its defaults
+    with this ``hop_length``.  Restated from librosa's definitions, not checked against librosa.
+
+    One launch from the envelope.  No gradient: under grad mode an input that requires grad raises."""
+    fmt = _resolve(_unwrap_format(data_format))
+    if norm is not None and norm != np.inf:
+        raise ValueError('norm must be np.inf or None, got %r' % (norm,))
+    for x in (waveform, onset_envelope):
+        if ops._wants_grad(x):
+            raise ValueError('tempogram has no gradient: call it under torch.no_grad() or on a detached input')
+    ops.tempogram_check(win_length)
+    e = _envelope(waveform, onset_envelope, sample_rate, hop_length, fmt)
+    return ops.tempogram(e, win_length, center, norm is not None, fmt)
+
+
+_tempo_plans = {}
+
+
+def _tempo_plan(sample_rate, hop_length, ac_size, start_bpm, std_bpm, max_tempo, win_length=None):
+    """The TempoPlan of one configuration: W lags from ``ac_size`` (librosa's ``time_to_frames``), or ``win_length``
+    (a given tempogram's own lag count) when that is not None."""
+    for name, v in (('start_bpm', start_bpm), ('std_bpm', std_bpm)):
+        if isinstance(v, bool) or not (np.isfinite(float(v)) and float(v) > 0):
+            raise ValueError('%s must be positive, got %r' % (name, v))
+    sr = float(sample_rate)
+    if not (np.isfinite(sr) and sr > 0):
+        raise ValueError('sample_rate must be positive, got %r' % (sample_rate,))
+    hop = ops._check_int('hop_length', hop_length, 1)
+    if win_length is None:
+        W = int(math.floor(math.floor(float(ac_size) * sr) / hop))
+        if not 2 <= W <= ops.N.TEMPOGRAM_MAX_WIN:
+            raise ValueError('ac_size=%r gives a window of %d frames, outside [2, %d]'
+                             % (ac_size, W, ops.N.TEMPOGRAM_MAX_WIN))
+    else:
+        W = ops.tempogram_check(win_length)
+    key = (sr, hop, W, float(start_bpm), float(std_bpm), None if max_tempo is None else float(max_tempo))
+    plan = _tempo_plans.get(key)
+    if plan is None:
+        plan = ops.TempoPlan(W, sr, hop, start_bpm, std_bpm, max_tempo)
+        _tempo_plans[key] = plan
+    return plan
+
+
+def tempo(waveform=None, sample_rate=22050, onset_envelope=None, tg=None, hop_length=512, start_bpm=120.0,
+          std_bpm=1.0, ac_size=8.0, max_tempo=320.0, aggregate='mean', data_format='default'):
+    """Tempo in bpm (modelled on ``librosa.feature.tempo``): float32 ``(batch, ch)``, or per frame ``(batch, frames,
+    ch)`` / ``(batch, ch, frames)`` with ``aggregate=None``.
+
+    From a waveform or an envelope, tg is the centred ``norm=inf`` tempogram of W = floor(floor(ac_size sr) / hop)
+    lags (2 .. 4096).  A given ``tg`` (``(batch, frames, W, ch)`` / ``(batch, ch, frames, W)`` float32) is used with
+    its own W, as librosa does, and ``ac_size`` is not used.  g is the float64 mean of tg over its frames (or each
+    frame with ``aggregate=None``).  With ``bpm[l] = 60 sr / (hop l)`` and a log-normal prior around ``start_bpm``
+    (``std_bpm`` octaves; lags below the first one under ``max_tempo`` excluded), the tempo is ``bpm[first argmax
+    (log1p(1e6 g) + logprior)]`` in float64.  Restated from librosa's definitions, not checked against librosa.
+
+    Departures: a row (or frame) holding a non-finite value gives NaN.  A lag whose score is NaN (g below -1e-6,
+    which a detrended or user-made envelope can give) is skipped, as ``np.nanargmax`` skips it, where numpy's argmax
+    would pick it; a row with no lag left gives NaN.
+
+    Launches: two from ``tg`` (one with ``aggregate=None``), one more from an envelope, five more from a waveform.
+    No gradient: an input that requires grad is accepted and the output carries no ``grad_fn``."""
+    fmt = _resolve(_unwrap_format(data_format))
+    if aggregate not in ('mean', None):
+        raise ValueError("aggregate must be 'mean' or None, got %r" % (aggregate,))
+    if sum(x is not None for x in (waveform, onset_envelope, tg)) != 1:
+        raise ValueError('pass exactly one of waveform, onset_envelope and tg')
+    W = None
+    if tg is not None:
+        if not isinstance(tg, torch.Tensor) or tg.dim() != 4:
+            raise ValueError('tg must be a 4-D tempogram tensor')
+        W = int(tg.shape[2] if fmt == _CH_LAST_STR else tg.shape[3])
+    plan = _tempo_plan(sample_rate, hop_length, ac_size, start_bpm, std_bpm, max_tempo, W)
+    with torch.no_grad():
+        if tg is None:
+            e = _envelope(waveform, onset_envelope, sample_rate, hop_length, fmt)
+            tg = ops.tempogram(e.detach(), plan.W, True, True, fmt)
+        return ops.tempo(tg, plan, aggregate is None, fmt)
+
+
+def onset_detect(waveform=None, sample_rate=22050, onset_envelope=None, hop_length=512, normalize=True, pre_max=None,
+                 post_max=None, pre_avg=None, post_avg=None, delta=0.07, wait=None, data_format='default'):
+    """Onsets by peak picking (modelled on ``librosa.onset.onset_detect`` with ``sparse=False``): a bool mask shaped
+    like the envelope.
+
+    Defaults: ``pre_max = wait = floor(0.03 sr / hop)``, ``post_max = 1``, ``pre_avg = floor(0.1 sr / hop)``,
+    ``post_avg = pre_avg + 1``.  With ``normalize`` x = (e - min e) / (max(e - min e) + FLT_MIN) in float32; frame n
+    is a candidate when x[n] is the maximum of x[n - pre_max .. n + post_max), is nonzero and is at least the
+    float64 mean of x[n - pre_avg .. n + post_avg) plus ``delta`` (windows clipped to the row); candidates within
+    ``wait`` frames of the last accepted one are dropped.  A row with no nonzero x or a non-finite value has no
+    onsets.  Restated from librosa's definitions, not checked against librosa.
+
+    One launch from the envelope (five more from a waveform).  No gradient."""
+    fmt = _resolve(_unwrap_format(data_format))
+    sr = float(sample_rate)
+    hop = ops._check_int('hop_length', hop_length, 1)
+    d_pre_max = int(0.03 * sr // hop)
+    d_pre_avg = int(0.10 * sr // hop)
+    cfg = ops.onset_detect_config(d_pre_max if pre_max is None else pre_max, 1 if post_max is None else post_max,
+                                  d_pre_avg if pre_avg is None else pre_avg,
+                                  d_pre_avg + 1 if post_avg is None else post_avg,
+                                  d_pre_max if wait is None else wait, delta, normalize)
+    with torch.no_grad():
+        e = _envelope(waveform, onset_envelope, sample_rate, hop, fmt)
+        return ops.onset_detect(e, cfg, fmt)
+
+
+def beat_track(waveform=None, sample_rate=22050, onset_envelope=None, hop_length=512, start_bpm=120.0,
+               tightness=100.0, trim=True, bpm=None, data_format='default'):
+    """Dynamic-programming beat tracking (modelled on ``librosa.beat.beat_track``): ``(tempo, beats)``, tempo float32
+    ``(batch, ch)`` and beats a bool mask shaped like the envelope.
+
+    From a waveform the envelope is ``onset_strength(aggregate='median')``.  ``bpm=None`` takes each row's
+    ``tempo(onset_envelope=e, start_bpm=start_bpm)`` on the device; a given ``bpm`` is used for every row.  The
+    period is p = rint(60 (sr / hop) / bpm), 1 .. 4096.  The local score is the envelope over its standard deviation
+    (ddof=1) convolved with exp(-0.5 (32 d / p)^2), d = -p .. p; the float64 dynamic programme scores each frame
+    from offsets -2p .. -rint(p / 2) with ``-tightness ln(-d / p)^2``, the last beat is the last frame whose doubled
+    cumulative score (at local maxima) exceeds their median, backlinks give the rest, and with ``trim`` the weak
+    beats at both ends are dropped (keeping librosa's slice, which drops the last strong one too).  An all-zero row
+    gives tempo 0 and no beats, a non-finite one tempo NaN and no beats.  Restated from librosa's definitions, not
+    checked against librosa.
+
+    Nothing is synchronised with the host, so the call can be captured in a CUDA graph.  Launches: one, plus three for
+    the tempo and five for a waveform's envelope.  No gradient."""
+    fmt = _resolve(_unwrap_format(data_format))
+    cfg = ops.beat_config(sample_rate, ops._check_int('hop_length', hop_length, 1), tightness, trim)
+    if bpm is None:
+        plan = _tempo_plan(sample_rate, hop_length, 8.0, start_bpm, 1.0, 320.0)
+    else:
+        if isinstance(bpm, bool) or not (np.isfinite(float(bpm)) and float(bpm) > 0):
+            raise ValueError('bpm must be positive, got %r' % (bpm,))
+        p = int(np.rint(60.0 * cfg.fps / float(bpm)))
+        if not 1 <= p <= ops.N.BEAT_MAX_PERIOD:
+            raise ValueError('bpm=%r gives a beat period of %d frames, outside [1, %d]'
+                             % (bpm, p, ops.N.BEAT_MAX_PERIOD))
+    with torch.no_grad():
+        e = _envelope(waveform, onset_envelope, sample_rate, hop_length, fmt, aggregate='median')
+        if bpm is None:
+            bpm = ops.tempo(ops.tempogram(e.detach(), plan.W, True, True, fmt), plan, False, fmt)
+        return ops.beat_track(e, cfg, bpm, fmt)

@@ -24,7 +24,7 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 
 __all__ = ['Layer', 'STFT', 'InverseSTFT', 'Magnitude', 'Phase', 'MagnitudeToDecibel', 'ApplyFilterbank', 'Delta',
            'PCEN', 'GriffinLim', 'InverseFilterbank', 'KaldiFbank', 'KaldiMFCC', 'KaldiSpectrogram', 'CQT',
-           'ChromaSTFT', 'ChromaCQT', 'ChromaCENS', 'HPSS']
+           'ChromaSTFT', 'ChromaCQT', 'ChromaCENS', 'HPSS', 'OnsetStrength', 'Tempogram']
 
 _name_counters = {}
 _REGISTRY = {}
@@ -889,4 +889,53 @@ class HPSS(Layer):
     _config_fields = (
         ('component', 'component'), ('kernel_size', 'kernel_size'), ('power', 'power'), ('mask', 'mask'),
         ('margin', 'margin'), ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class OnsetStrength(_ChromaLayer):
+    """``signal.onset_strength`` as a layer: ``(batch, time, ch)`` / ``(batch, ch, time)`` waveforms in, the ``(batch,
+    frames, ch)`` / ``(batch, ch, frames)`` envelope out.  Same arguments; differentiable with respect to the
+    input."""
+    _fn = 'onset_strength'
+
+    def __init__(self, sample_rate=22050, lag=1, max_size=1, detrend=False, center=True, aggregate='mean', n_fft=2048,
+                 hop_length=512, n_mels=128, fmin=0.0, fmax=None, data_format='default', **kwargs):
+        super().__init__(data_format, dict(sample_rate=sample_rate, lag=lag, max_size=max_size, detrend=detrend,
+                                           center=center, aggregate=aggregate, n_fft=n_fft, hop_length=hop_length,
+                                           n_mels=n_mels, fmin=fmin, fmax=fmax), **kwargs)
+
+    def _check(self):
+        from . import signal
+        ops.onset_limits(ops.onset_config(self.lag, self.max_size, self.aggregate), self.n_mels, 0)
+        signal._rhythm_frontend(self.sample_rate, self.n_fft, self.hop_length, self.n_mels, self.fmin, self.fmax)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'), ('lag', 'lag'), ('max_size', 'max_size'), ('detrend', 'detrend'),
+        ('center', 'center'), ('aggregate', 'aggregate'), ('n_fft', 'n_fft'), ('hop_length', 'hop_length'),
+        ('n_mels', 'n_mels'), ('fmin', 'fmin'), ('fmax', 'fmax'), ('data_format', 'data_format_str'),
+    )
+
+
+@register_keras_serializable(package='Kapre')
+class Tempogram(_ChromaLayer):
+    """``signal.tempogram`` as a layer: waveforms in, ``(batch, frames, win_length, ch)`` / ``(batch, ch, frames,
+    win_length)`` out.  Same arguments; no gradient."""
+    _fn = 'tempogram'
+
+    def __init__(self, sample_rate=22050, hop_length=512, win_length=384, center=True, norm=np.inf,
+                 data_format='default', **kwargs):
+        super().__init__(data_format, dict(sample_rate=sample_rate, hop_length=hop_length, win_length=win_length,
+                                           center=center, norm=norm), **kwargs)
+
+    def _check(self):
+        from . import signal
+        ops.tempogram_check(self.win_length)
+        if self.norm is not None and self.norm != np.inf:
+            raise ValueError('norm must be np.inf or None, got %r' % (self.norm,))
+        signal._rhythm_frontend(self.sample_rate, 2048, self.hop_length, 128, 0.0, None)
+
+    _config_fields = (
+        ('sample_rate', 'sample_rate'), ('hop_length', 'hop_length'), ('win_length', 'win_length'),
+        ('center', 'center'), ('norm', 'norm'), ('data_format', 'data_format_str'),
     )
