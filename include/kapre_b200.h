@@ -897,7 +897,10 @@ const char* kapre_last_error(void);
 int kapre_version(void);
 /* Number of kernels this library has launched in this process (for bench.py's gpu_launches). */
 uint64_t kapre_launch_count(void);
-/* Name of the last fused-forward launch configuration, e.g. "Q16 TF16 NW4 grid296 smem98304". */
+/* Name of the last fused-forward launch configuration, e.g. "Q16 TF16 NW4 grid296 smem98304", or of the last
+ * persistent launch, "<kernel> grid=G tiles=T".  A call that makes several persistent launches (the CQT, HPSS and
+ * onset-strength gradients, pYIN, CENS, the tuning estimate, tempo) reports all of them in launch order, joined
+ * with "; ". */
 const char* kapre_last_launch_info(void);
 /* Kernel timing for bench.py's roofline: enable = n > 0 brackets every n-th fused forward / inverse
  * kernel launch by CUDA events on its own stream (n = 1: every launch; a stride leaves the other

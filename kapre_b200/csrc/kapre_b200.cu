@@ -163,6 +163,17 @@ static int kb_resident_grid(K kernel, const char* name, int block, int smem, lon
     return 0;
 }
 
+// The launch report of a call that makes several persistent launches: add() after each launch keeps its report, and
+// at the end of the call the report is all of them in launch order, joined with "; ", so that the grid of every
+// launch can be read (kb_resident_grid alone would leave only the last).
+struct KbLaunchReports {
+    std::string all;
+    void add() { all += (all.empty() ? "" : "; ") + g_launch_info; }
+    ~KbLaunchReports() {
+        if (!all.empty()) g_launch_info = all;
+    }
+};
+
 // ------------------------------------------------------------------------------------------
 // __global__ wrappers
 // ------------------------------------------------------------------------------------------
@@ -3781,6 +3792,7 @@ int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kap
     float* ws = (float*)workspace_dev;
     const cudaStream_t st = (cudaStream_t)stream;
     const int smem = kb_cqt_bwd_smem();
+    KbLaunchReports reports;    // every octave's launch and the resampling launches between them
     // lowest octave first: g_i = adjoint_i(G) + R^T g_{i+1}
     for (int i = n_oct - 1; i >= 0; --i) {
         const KbCqtOct& o = p.oct[i];
@@ -3791,6 +3803,7 @@ int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kap
             const kapre_wave_desc gd = kb_cqt_level_desc(p.B, p.C, p.oct[i + 1].L);
             const kapre_wave_desc rd = kb_cqt_level_desc(p.B, p.C, o.L);
             if ((rc = kapre_resample_backward(plan->rs, ws + glvl[i + 1], &gd, ws + rlvl[i], &rd, stream))) return rc;
+            reports.add();
             p.add = ws + rlvl[i];
         }
         if (i == 0) { p.gy = gx_dev; p.gy_sb = gx_desc->stride_b; p.gy_sc = gx_desc->stride_c; p.gy_sl = gx_desc->stride_l; }
@@ -3802,6 +3815,7 @@ int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kap
             return rc;
         if ((rc = kb_launch(kb_cqt_bwd_kernel, {.grid = grid, .block = KB_CQT_BWD_THREADS, .smem = smem, .st = st}, p)))
             return rc;
+        reports.add();
     }
     return 0;
 }
@@ -4017,8 +4031,10 @@ int kapre_pyin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wav
     if (!x_dev || !f0_dev || !voiced_flag_dev || !voiced_prob_dev || !workspace_dev)
         return kb_fail(KAPRE_E_INVALID, "null data pointer");
     const cudaStream_t st = (cudaStream_t)stream;
+    KbLaunchReports reports;
     if ((rc = kb_pitch_launch(plan, x_dev, x_desc, voiced_prob_dev, out_desc, cmndf_dev, cmndf_desc, workspace_dev, st)))
         return rc;
+    reports.add();
     KbVitParams v = plan->vit;
     int64_t bp;
     kb_pitch_ws_layout(plan, rows, M, &bp);
@@ -4033,6 +4049,7 @@ int kapre_pyin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wav
     const int smem = kb_vit_smem(v.n, v.w);
     int grid;
     if ((rc = kb_resident_grid(kb_viterbi_kernel, "viterbi", v.nt, smem, rows, plan->dev.sm_count, &grid))) return rc;
+    reports.add();
     return kb_launch(kb_viterbi_kernel, {.grid = grid, .block = v.nt, .smem = smem, .st = st, .timed = true}, v);
 }
 
@@ -4231,7 +4248,9 @@ int kapre_chroma_cens(const kapre_chroma_plan* plan, int in_mode, const void* x_
     p.out = (float*)workspace_dev;
     p.o_sc = (long long)frames * NC; p.o_sb = channels * p.o_sc; p.o_st = NC; p.o_sk = 1;
     const cudaStream_t st = (cudaStream_t)stream;
+    KbLaunchReports reports;
     if ((rc = kb_chroma_fwd_launch(plan, p, st))) return rc;
+    reports.add();
     KbCensParams c{};
     c.NC = NC; c.N = plan->d.n_smooth; c.w = plan->smooth;
     c.B = batch; c.C = channels; c.M = frames;
@@ -4245,6 +4264,7 @@ int kapre_chroma_cens(const kapre_chroma_plan* plan, int in_mode, const void* x_
     int grid;
     if ((rc = kb_resident_grid(kb_cens_kernel, "cens", KB_CH_THREADS, smem, c.jobs, plan->dev.sm_count, &grid)))
         return rc;
+    reports.add();
     return kb_launch(kb_cens_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = smem, .st = st}, c);
 }
 
@@ -4285,6 +4305,7 @@ int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float*
     KB_CUDA(cudaMemsetAsync(w + off[2], 0xff, (size_t)batch * 4, st));
     const long long rows = (long long)batch * channels;
     int grid;
+    KbLaunchReports reports;
     if (frames > 0) {
         p.tiles = ((long long)frames + KB_CH_PEAK_TF - 1) / KB_CH_PEAK_TF;
         p.jobs = rows * p.tiles;
@@ -4294,6 +4315,7 @@ int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float*
         if ((rc = kb_launch(kb_tune_peak_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = kb_tune_peak_smem(),
                                                   .st = st}, p)))
             return rc;
+        reports.add();
         p.tiles = ((long long)frames + KB_CH_SEL_TF - 1) / KB_CH_SEL_TF;
         p.jobs = rows * p.tiles;
         if ((rc = kb_resident_grid(kb_tune_sel_kernel, "tune_select", KB_CH_THREADS, kb_tune_sel_smem(), p.jobs,
@@ -4303,10 +4325,12 @@ int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float*
             if ((rc = kb_launch(kb_tune_sel_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = kb_tune_sel_smem(),
                                                      .st = st}, p)))
                 return rc;
+        reports.add();
     }
     if ((rc = kb_resident_grid(kb_tune_argmax_kernel, "tune_argmax", KB_CH_THREADS, 2 * KB_CH_THREADS * 4, batch,
                                plan->dev.sm_count, &grid)))
         return rc;
+    reports.add();
     return kb_launch(kb_tune_argmax_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = 2 * KB_CH_THREADS * 4,
                                              .st = st}, p);
 }
@@ -4403,13 +4427,16 @@ int kapre_hpss_backward(const kapre_hpss_config* cfg, const void* S_dev, int is_
     const long long n = (long long)batch * channels * frames * bins;
     p.wh = (kb_hs_w*)workspace_dev; p.wp = p.wh + n;
     cudaStream_t st = (cudaStream_t)stream;
+    KbLaunchReports reports;
     if ((rc = kb_hpss_tiles_launch<1>(p, st))) return rc;
+    reports.add();
     DevInfo dev;
     if ((rc = kb_dev_info(&dev))) return rc;
     int grid;
     if ((rc = kb_resident_grid(kb_hpss_gather_kernel, "hpss_gather", KB_HS_THREADS, 0,
                                (n + KB_HS_THREADS - 1) / KB_HS_THREADS, dev.sm_count, &grid)))
         return rc;
+    reports.add();
     return kb_launch(kb_hpss_gather_kernel, {.grid = grid, .block = KB_HS_THREADS, .st = st}, p);
 }
 
@@ -4529,11 +4556,15 @@ int kapre_onset_strength_backward(const kapre_onset_config* cfg, const float* S_
     p.gx_sk = gS_desc->stride_f;
     p.ws = (kb_on_w*)workspace_dev;
     cudaStream_t st = (cudaStream_t)stream;
+    KbLaunchReports reports;
     if ((rc = kb_rh_launch(kb_onset_kernel<1>, "onset_bwd", kb_onset_smem(p.K, p.m, p.F, 1), p.jobs, p, st, false)))
         return rc;
+    reports.add();
     const long long n = (long long)batch * channels * frames * bins;
-    return kb_rh_launch(kb_onset_gather_kernel, "onset_gather", 0, (n + KB_RH_THREADS - 1) / KB_RH_THREADS, p, st,
-                        false);
+    rc = kb_rh_launch(kb_onset_gather_kernel, "onset_gather", 0, (n + KB_RH_THREADS - 1) / KB_RH_THREADS, p, st,
+                      false);
+    reports.add();
+    return rc;
 }
 
 int kapre_tempogram(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
@@ -4587,10 +4618,16 @@ int kapre_tempo(const float* tg_dev, const kapre_spec_desc* tg_desc, int batch, 
     if (!tg_dev || !logprior_dev || !out_dev || (!per_frame && !workspace_dev))
         return kb_fail(KAPRE_E_INVALID, "null data pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    if (!per_frame &&
-        (rc = kb_rh_launch(kb_tempo_part_kernel, "tempo_part", 0, (long long)batch * channels * p.chunks, p, st, false)))
-        return rc;
-    return kb_rh_launch(kb_tempo_kernel, "tempo", kb_tempo_smem(p.W), p.jobs, p, st, false);
+    KbLaunchReports reports;
+    if (!per_frame) {
+        if ((rc = kb_rh_launch(kb_tempo_part_kernel, "tempo_part", 0, (long long)batch * channels * p.chunks, p, st,
+                               false)))
+            return rc;
+        reports.add();
+    }
+    rc = kb_rh_launch(kb_tempo_kernel, "tempo", kb_tempo_smem(p.W), p.jobs, p, st, false);
+    reports.add();
+    return rc;
 }
 
 int kapre_onset_detect(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
