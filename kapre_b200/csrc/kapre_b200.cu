@@ -133,6 +133,33 @@ static int kb_launch(void (*kernel)(P...), const KbLaunch& l, A&&... args) {
     return 0;
 }
 
+// Regions of one scratch buffer, each starting on a 256-byte boundary; with a null base it only measures.  Each
+// operation's regions are described once, in a layout function that both its sizing function and the operation call,
+// so the size a caller allocates and the regions the kernels write cannot drift apart.  take<T>(d0, d1, ...) reserves
+// d0 d1 ... elements of T; a negative count, or a count or total beyond int64, sets `overflow` instead of wrapping.
+struct KbLayout {
+    char* base = nullptr;
+    int64_t end = 0;
+    bool overflow = false;
+    void pad() {
+        overflow |= __builtin_add_overflow(end, (int64_t)255, &end);
+        end &= ~(int64_t)255;
+    }
+    template <typename T, typename... N>
+    T* take(N... dims) {
+        pad();
+        const int64_t at = end;
+        int64_t bytes = sizeof(T);
+        for (const long long d : {(long long)dims...}) overflow |= d < 0 || __builtin_mul_overflow(bytes, (int64_t)d, &bytes);
+        overflow |= __builtin_add_overflow(end, bytes, &end);
+        return base && !overflow ? (T*)(base + at) : nullptr;
+    }
+    // what a sizing function returns: the total, or KAPRE_E_INVALID when it does not fit in int64
+    int64_t bytes(const char* what) const {
+        return overflow ? kb_fail(KAPRE_E_INVALID, "%s workspace overflows", what) : end;
+    }
+};
+
 // SMs x resident threads per SM of the current device: the thread count the time-scan kernels (PCEN, time stretch)
 // size their time chunks against.
 static int kb_resident_threads(long long* threads) {
@@ -1707,6 +1734,11 @@ static void kb_stft_adj_geom(const kapre_stft_plan* p, int length, int pad_begin
     *direct = !pad_begin && *ola_len <= length;
 }
 
+// the workspace of the STFT adjoint: the (B, C, ola_len) overlap-add, unless it goes straight into gx
+static float* kb_stft_adj_layout(KbLayout& L, int batch, int channels, int T, long long ola_len, bool direct) {
+    return direct || T <= 0 ? nullptr : L.take<float>(batch, channels, ola_len);
+}
+
 extern "C" {
 
 int64_t kapre_stft_backward_workspace_bytes(const kapre_stft_plan* plan, int batch, int channels, int length,
@@ -1716,8 +1748,9 @@ int64_t kapre_stft_backward_workspace_bytes(const kapre_stft_plan* plan, int bat
     long long ola_len;
     bool direct;
     kb_stft_adj_geom(plan, length, pad_begin, pad_end, &T, &ola_len, &direct);
-    if (direct || T <= 0) return 0;
-    return (int64_t)batch * channels * ola_len * (int64_t)sizeof(float);
+    KbLayout L;
+    kb_stft_adj_layout(L, batch, channels, T, ola_len, direct);
+    return L.bytes("stft_backward");
 }
 
 int kapre_stft_backward(const kapre_stft_plan* plan, const void* g_dev, const kapre_spec_desc* gd, int batch,
@@ -1759,7 +1792,8 @@ int kapre_stft_backward(const kapre_stft_plan* plan, const void* g_dev, const ka
             q.ola = gx_dev;
         } else {
             od.stride_b = (long long)channels * ola_len; od.stride_c = ola_len; od.stride_l = 1;
-            q.ola = (const float*)workspace_dev;
+            KbLayout L{(char*)workspace_dev};
+            q.ola = kb_stft_adj_layout(L, batch, channels, T, ola_len, direct);
         }
         q.a_sb = od.stride_b; q.a_sc = od.stride_c; q.a_sl = od.stride_l;
         if ((rc = kapre_istft_inverse(adj, g_dev, batch, channels, T, gd, (float*)q.ola, &od, stream))) return rc;
@@ -2238,8 +2272,22 @@ static int kb_conv_geom(const kapre_convolve_plan* plan, long long L, long long 
     return 0;
 }
 
-static long long kb_conv_spec_bytes(long long n_sig, long long frames, int B) {
-    return (n_sig * frames * (B + 1) * 8 + 255) / 256 * 256;
+// The forward workspace: the signal's spectra X, first because kapre_convolve_backward reads them at offset 0, then
+// the output's spectra Y.
+static void kb_conv_layout(KbLayout& L, int batch, int channels, int J, int T, int B, float2** X, float2** Y) {
+    *X = L.take<float2>(batch, channels, J, B + 1);
+    *Y = L.take<float2>(batch, channels, T, B + 1);
+    L.pad();
+}
+
+// The backward workspace: the output gradient's spectra G, the signal gradient's spectra gX, and the STFT adjoint's
+// overlap-add, which it needs only when the length is not a multiple of the block.
+static void kb_conv_backward_layout(KbLayout& L, int batch, int channels, int length, int J, int T, int B, float2** G,
+                                    float2** gX, float** ola) {
+    *G = L.take<float2>(batch, channels, T, B + 1);
+    *gX = L.take<float2>(batch, channels, J, B + 1);
+    *ola = length % B ? L.take<float>(batch, channels, J, B) : nullptr;
+    L.pad();
 }
 
 static kapre_spec_desc kb_conv_spec_desc(int C, int frames, int B) {
@@ -2318,8 +2366,10 @@ int64_t kapre_convolve_workspace_bytes(const kapre_convolve_plan* plan, int batc
     if (batch < 0 || channels < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
     int J, T, n, rc;
     if ((rc = kb_conv_geom(plan, length, P, &J, &T, &n))) return rc;
-    const long long sig = (long long)batch * channels;
-    return kb_conv_spec_bytes(sig, J, plan->B) + kb_conv_spec_bytes(sig, T, plan->B);
+    KbLayout L;
+    float2 *X, *Y;
+    kb_conv_layout(L, batch, channels, J, T, plan->B, &X, &Y);
+    return L.bytes("convolve");
 }
 
 int kapre_convolve(const kapre_convolve_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, const void* H_dev,
@@ -2337,8 +2387,9 @@ int kapre_convolve(const kapre_convolve_plan* plan, const float* x_dev, const ka
     const int Bn = x_desc->batch, C = x_desc->channels;
     if (Bn == 0 || C == 0) return 0;
     if (!x_dev || !H_dev || !y_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
-    void* X = workspace_dev;
-    void* Y = (char*)workspace_dev + kb_conv_spec_bytes((long long)Bn * C, J, plan->B);
+    KbLayout L{(char*)workspace_dev};
+    float2 *X, *Y;
+    kb_conv_layout(L, Bn, C, J, T, plan->B, &X, &Y);
     const kapre_spec_desc Xd = kb_conv_spec_desc(C, J, plan->B), Yd = kb_conv_spec_desc(C, T, plan->B);
     cudaStream_t st = (cudaStream_t)stream;
     if ((rc = kapre_stft_forward(plan->stft, x_dev, x_desc, 0, 1, KAPRE_OUT_COMPLEX, X, &Xd, nullptr, nullptr, nullptr,
@@ -2358,9 +2409,11 @@ int64_t kapre_convolve_backward_workspace_bytes(const kapre_convolve_plan* plan,
     if (batch < 0 || channels < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
     int J, T, n, rc;
     if ((rc = kb_conv_geom(plan, length, P, &J, &T, &n))) return rc;
-    const long long sig = (long long)batch * channels;
-    const long long ola = length % plan->B ? (sig * J * plan->B * 4 + 255) / 256 * 256 : 0;
-    return kb_conv_spec_bytes(sig, T, plan->B) + kb_conv_spec_bytes(sig, J, plan->B) + ola;
+    KbLayout L;
+    float2 *G, *gX;
+    float* ola;
+    kb_conv_backward_layout(L, batch, channels, length, J, T, plan->B, &G, &gX, &ola);
+    return L.bytes("convolve_backward");
 }
 
 int kapre_convolve_backward(const kapre_convolve_plan* plan, const float* gy_dev, const kapre_wave_desc* gy_desc,
@@ -2382,10 +2435,10 @@ int kapre_convolve_backward(const kapre_convolve_plan* plan, const float* gy_dev
     if (Bn == 0 || C == 0 || (!gx_dev && !gH_dev)) return 0;
     if (!gy_dev || !workspace_dev || (gx_dev && !H_dev) || (gH_dev && !X_dev))
         return kb_fail(KAPRE_E_INVALID, "null data pointer");
-    const long long sig = (long long)Bn * C;
-    void* G = workspace_dev;
-    void* gX = (char*)workspace_dev + kb_conv_spec_bytes(sig, T, plan->B);
-    void* ola = (char*)gX + kb_conv_spec_bytes(sig, J, plan->B);
+    KbLayout L{(char*)workspace_dev};
+    float2 *G, *gX;
+    float* ola;
+    kb_conv_backward_layout(L, Bn, C, gx_desc->length, J, T, plan->B, &G, &gX, &ola);
     const kapre_spec_desc Gd = kb_conv_spec_desc(C, T, plan->B), gXd = kb_conv_spec_desc(C, J, plan->B);
     cudaStream_t st = (cudaStream_t)stream;
     if ((rc = kapre_istft_backward(plan->istft, gy_dev, gy_desc, Bn, C, T, G, &Gd, stream))) return rc;
@@ -2469,6 +2522,9 @@ static int kb_pcen_setup(KbPcenParams& p, const kapre_spec_desc* E_desc, int bat
     return 0;
 }
 
+// the workspace of a chunked scan: the (K, n_cols) chunk end states
+static void kb_pcen_layout(KbLayout& L, KbPcenParams& p) { p.state = p.K > 1 ? L.take<float>(p.K, p.n_cols) : nullptr; }
+
 extern "C" {
 
 int kapre_pcen_workspace(int batch, int channels, int frames, int bands, int* chunks, int64_t* workspace_bytes) {
@@ -2476,12 +2532,14 @@ int kapre_pcen_workspace(int batch, int channels, int frames, int bands, int* ch
     if (batch < 0 || channels < 0 || frames < 0 || bands < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
     KbPcenParams p{};
     p.T = frames;
-    const long long n_cols = (long long)batch * channels * bands;
+    p.n_cols = (long long)batch * channels * bands;
     int K = 1, rc;
-    if (n_cols * frames > 0 && (rc = kb_pcen_pick_chunks(n_cols, frames, &K))) return rc;
+    if (p.n_cols * frames > 0 && (rc = kb_pcen_pick_chunks(p.n_cols, frames, &K))) return rc;
     kb_pcen_set_chunks(p, K);
+    KbLayout L;
+    kb_pcen_layout(L, p);
+    if ((*workspace_bytes = L.bytes("pcen")) < 0) return (int)*workspace_bytes;
     *chunks = p.K;
-    *workspace_bytes = p.K > 1 ? (int64_t)p.K * n_cols * 4 : 0;
     return 0;
 }
 
@@ -2501,7 +2559,8 @@ int kapre_pcen(const float* E_dev, const kapre_spec_desc* E_desc, int batch, int
     p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_st = y_desc->stride_t; p.y_sf = y_desc->stride_f;
     p.M = M_dev;
     if (M_dev) { p.m_sb = M_desc->stride_b; p.m_sc = M_desc->stride_c; p.m_st = M_desc->stride_t; p.m_sf = M_desc->stride_f; }
-    p.state = (float*)workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    kb_pcen_layout(L, p);
     // one thread per (chunk, column): the state pass covers chunks 0 .. K - 2, the output pass all K
     const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
     const long long grid = (n + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS;
@@ -2537,7 +2596,8 @@ int kapre_pcen_backward(const float* E_dev, const kapre_spec_desc* E_desc, const
     p.m_sb = M_desc->stride_b; p.m_sc = M_desc->stride_c; p.m_st = M_desc->stride_t; p.m_sf = M_desc->stride_f;
     p.gy = gy_dev; p.g_sb = gy_desc->stride_b; p.g_sc = gy_desc->stride_c; p.g_st = gy_desc->stride_t; p.g_sf = gy_desc->stride_f;
     p.gE = gE_dev; p.o_sb = gE_desc->stride_b; p.o_sc = gE_desc->stride_c; p.o_st = gE_desc->stride_t; p.o_sf = gE_desc->stride_f;
-    p.state = (float*)workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    kb_pcen_layout(L, p);
     p.part = param_partials_dev;
     const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
     const long long grid = (n + KB_PCEN_THREADS - 1) / KB_PCEN_THREADS;
@@ -2561,18 +2621,24 @@ __global__ void __launch_bounds__(KB_GL_THREADS) kb_gl_project_kernel(const __gr
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += step) kb_gl_project_elem(p, i);
 }
 
-// Workspace layout: spectrum buffers 0 and 1 (each n complex64, rounded up to 256 B), then the (B, C, L) waveform.
-static long long kb_gl_spec_bytes(long long n) { return (n * 8 + 255) / 256 * 256; }
+// Workspace: spectrum buffers 0 and 1 (each (B, C, frames, F) complex64), then the (B, C, len) waveform.
+static void kb_gl_layout(KbLayout& L, int batch, int channels, int frames, int F, long long len, float2** X, float** wave) {
+    X[0] = L.take<float2>(batch, channels, frames, F);
+    X[1] = L.take<float2>(batch, channels, frames, F);
+    *wave = L.take<float>(batch, channels, len);
+}
 
 extern "C" {
 
 int64_t kapre_griffin_lim_workspace_bytes(const kapre_stft_plan* plan, int batch, int channels, int frames) {
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null argument");
     if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
-    if (batch == 0 || channels == 0 || frames == 0) return 0;
-    const long long n = (long long)batch * channels * frames * (plan->n_fft / 2 + 1);
-    const long long L = (long long)(frames - 1) * plan->hop + plan->win_length;
-    return 2 * kb_gl_spec_bytes(n) + (long long)batch * channels * L * 4;
+    const long long len = frames > 0 ? (long long)(frames - 1) * plan->hop + plan->win_length : 0;
+    KbLayout L;
+    float2* X[2];
+    float* wave;
+    kb_gl_layout(L, batch, channels, frames, plan->n_fft / 2 + 1, len, X, &wave);
+    return L.bytes("griffin_lim");
 }
 
 int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft, const float* S_dev,
@@ -2610,8 +2676,10 @@ int kapre_griffin_lim(const kapre_stft_plan* stft, const kapre_istft_plan* istft
     p.beta = cfg->momentum / (1.0f + cfg->momentum);
     p.init = cfg->init;
     p.seed = (unsigned long long)cfg->seed;
-    float2* X[2] = {(float2*)workspace_dev, (float2*)((char*)workspace_dev + kb_gl_spec_bytes(p.n))};
-    float* wave = (float*)((char*)workspace_dev + 2 * kb_gl_spec_bytes(p.n));
+    KbLayout ws{(char*)workspace_dev};
+    float2* X[2];
+    float* wave;
+    kb_gl_layout(ws, batch, channels, frames, F, L, X, &wave);
     const kapre_spec_desc sd = {(int64_t)channels * frames * F, (int64_t)frames * F, F, 1};
     const kapre_wave_desc wd = {batch, channels, (int32_t)L, (int64_t)channels * L, L, 1};
     int grid;
@@ -2709,6 +2777,9 @@ static bool kb_ts_overlap(const void* p, const kapre_spec_desc* pd, int pt, cons
     return a0 < b1 && b0 < a1;
 }
 
+// the workspace of a chunked scan: the (K, n_cols) chunk sums
+static void kb_ts_layout(KbLayout& L, KbTsParams& p) { p.state = p.K > 1 ? L.take<float>(p.K, p.n_cols) : nullptr; }
+
 extern "C" {
 
 int kapre_time_stretch_workspace(int batch, int channels, int frames, int bins, double rate, int* chunks,
@@ -2718,8 +2789,10 @@ int kapre_time_stretch_workspace(int batch, int channels, int frames, int bins, 
     KbTsParams p{};
     int rc = kb_ts_setup(p, &d, batch, channels, frames, bins, rate);
     if (rc) return rc;
+    KbLayout L;
+    kb_ts_layout(L, p);
+    if ((*workspace_bytes = L.bytes("time_stretch")) < 0) return (int)*workspace_bytes;
     *chunks = p.K;
-    *workspace_bytes = p.K > 1 ? (int64_t)p.K * p.n_cols * 4 : 0;
     return 0;
 }
 
@@ -2737,7 +2810,8 @@ int kapre_time_stretch(const void* X_dev, const kapre_spec_desc* X_desc, int bat
         return kb_fail(KAPRE_E_INVALID, "a time stretch over %d time chunks needs a workspace", p.K);
     p.X = (const float2*)X_dev;
     p.Y = (float2*)Y_dev; p.y_sb = Y_desc->stride_b; p.y_sc = Y_desc->stride_c; p.y_st = Y_desc->stride_t; p.y_sf = Y_desc->stride_f;
-    p.state = workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    kb_ts_layout(L, p);
     // one thread per (chunk, column): the state pass covers chunks 0 .. K - 2, the output pass all K
     const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
     if (n > 0xffffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many time-stretch columns");
@@ -2772,7 +2846,8 @@ int kapre_time_stretch_backward(const void* X_dev, const kapre_spec_desc* X_desc
     p.g_sb = G_desc->stride_b; p.g_sc = G_desc->stride_c; p.g_st = G_desc->stride_t; p.g_sf = G_desc->stride_f;
     p.gX = (float2*)gX_dev;
     p.o_sb = gX_desc->stride_b; p.o_sc = gX_desc->stride_c; p.o_st = gX_desc->stride_t; p.o_sf = gX_desc->stride_f;
-    p.state = workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    kb_ts_layout(L, p);
     const long long ns = (long long)(p.K - 1) * p.n_cols, n = ns + p.n_cols;
     if (n > 0xffffffffLL) return kb_fail(KAPRE_E_UNSUPPORTED, "too many time-stretch columns");
     const cudaStream_t st = (cudaStream_t)stream;
@@ -2889,17 +2964,15 @@ __global__ void __launch_bounds__(32) kb_iir_out_kernel(const __grid_constant__ 
     kb_iir_out_cta(p, kb_smem, (long long)blockIdx.x);
 }
 
-static int64_t kb_iir_align(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
-// Workspace sections: powers (one set per column at most), chunk end states, block carries.  -1: overflow.
-static int64_t kb_iir_ws(long long n_cols, int K, int nblk, int64_t* off_e, int64_t* off_blk) {
-    const double total = (double)n_cols * (KB_IIR_NPOW * 64 * 8 + (double)K * KB_IIR_N * 4 + (double)nblk * KB_IIR_N * 8);
-    if (total > 4.0e18) return -1;
-    const int64_t pw = kb_iir_align((int64_t)n_cols * KB_IIR_NPOW * 64 * 8);
-    const int64_t e = kb_iir_align((int64_t)n_cols * K * KB_IIR_N * 4);
-    *off_e = pw;
-    *off_blk = pw + e;
-    return pw + e + kb_iir_align((int64_t)n_cols * nblk * KB_IIR_N * 8);
+// Workspace sections: powers (one set per column at most), chunk end states, block carries.  More than 4e18 bytes
+// counts as an overflow.
+static void kb_iir_layout(KbLayout& L, KbIirParams& p) {
+    const double total = (double)p.n_cols * (KB_IIR_NPOW * 64 * 8 + (double)p.K * KB_IIR_N * 4 + (double)p.nblk * KB_IIR_N * 8);
+    L.overflow |= total > 4.0e18;
+    p.pw = L.take<double>(p.n_cols, KB_IIR_NPOW * 64);
+    p.e = L.take<float>(p.n_cols, p.K, KB_IIR_N);
+    p.blk = L.take<double>(p.n_cols, p.nblk, KB_IIR_N);
+    L.pad();
 }
 
 static int kb_iir_check_sizes(int batch, int channels, int length, int order) {
@@ -2935,12 +3008,9 @@ static int kb_iir_prepare(KbIirParams& p, const kapre_wave_desc* xd, const kapre
     if (p.n_cols == 0 || p.L == 0) return 1;
     if (!cf->b || !cf->a) return kb_fail(KAPRE_E_INVALID, "null coefficient pointer");
     if (!workspace_dev) return kb_fail(KAPRE_E_INVALID, "null workspace");
-    int64_t off_e, off_blk;
-    if (kb_iir_ws(p.n_cols, p.K, p.nblk, &off_e, &off_blk) < 0) return kb_fail(KAPRE_E_INVALID, "IIR workspace overflows");
-    p.pw = (double*)workspace_dev;
-    p.e = (float*)((char*)workspace_dev + off_e);
-    p.blk = (double*)((char*)workspace_dev + off_blk);
-    return 0;
+    KbLayout L{(char*)workspace_dev};
+    kb_iir_layout(L, p);
+    return L.overflow ? kb_fail(KAPRE_E_INVALID, "IIR workspace overflows") : 0;
 }
 
 // The largest element offset + 1 of a wave descriptor (the bulk copies' bound), strides assumed >= 0 where they matter.
@@ -2974,11 +3044,12 @@ extern "C" {
 int64_t kapre_lfilter_workspace_bytes(int batch, int channels, int length, int order) {
     int rc = kb_iir_check_sizes(batch, channels, length, order);
     if (rc) return rc;
-    const int K = (int)(((long long)length + KB_IIR_TC - 1) / KB_IIR_TC);
-    int64_t off_e, off_blk;
-    const int64_t n = kb_iir_ws((long long)batch * channels, K, (K + KB_IIR_W - 1) / KB_IIR_W, &off_e, &off_blk);
-    if (n < 0) return kb_fail(KAPRE_E_INVALID, "IIR workspace overflows");
-    return n;
+    KbIirParams p{};
+    p.B = batch; p.C = channels; p.L = length;
+    kb_iir_setup(p);
+    KbLayout L;
+    kb_iir_layout(L, p);
+    return L.bytes("IIR");
 }
 
 int kapre_lfilter(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_iir_coeffs* coeffs, int flags,
@@ -3048,14 +3119,16 @@ __global__ void __launch_bounds__(KB_NOISE_WARPS * 32, 4) kb_noise_out_kernel(co
     if (tile < p.tiles) kb_noise_out_tile(p, kb_smem + w * kb_noise_smem(kb_noise_cg_max(p)).total, tile);
 }
 
-// Workspace bytes (the segment sums) of a shape; -1: a negative size or an overflow.
-static int64_t kb_noise_ws(int batch, int channels, int length) {
+// The workspace of a shape: the (B C, nseg, 2) segment sums.  -1: a negative size or an overflow.
+static int kb_noise_layout(KbLayout& L, int batch, int channels, int length, double** part) {
     if (batch < 0 || channels < 0 || length < 0) return -1;
     const long long nseg = ((long long)length + KB_NOISE_SEG - 1) / KB_NOISE_SEG;
     const long long groups = ((long long)channels + KB_NOISE_G - 1) / KB_NOISE_G;
     const double total = (double)batch * channels * nseg * 16.0;
     if (total > 4.0e18 || (double)batch * groups * nseg / KB_NOISE_WARPS > 2147483647.0) return -1;
-    return ((int64_t)batch * channels * nseg * 16 + 255) & ~(int64_t)255;
+    *part = L.take<double>(batch, channels, nseg, 2);
+    L.pad();
+    return L.overflow ? -1 : 0;
 }
 
 static bool kb_noise_same_shape(const kapre_wave_desc* a, const kapre_wave_desc* b) {
@@ -3075,7 +3148,8 @@ static KbNoiseWave kb_noise_wave(const float* p, const kapre_wave_desc* d) {
 static int kb_noise_prepare(KbNoiseParams& p, const kapre_wave_desc* xd, const kapre_noise_source* ns,
                             const kapre_snr_desc* sd, void* workspace_dev) {
     if (!xd || !ns || !sd) return kb_fail(KAPRE_E_INVALID, "null argument");
-    if (kb_noise_ws(xd->batch, xd->channels, xd->length) < 0)
+    KbLayout L{(char*)workspace_dev};
+    if (kb_noise_layout(L, xd->batch, xd->channels, xd->length, &p.part) < 0)
         return kb_fail(KAPRE_E_INVALID, "add_noise: negative size or too many samples (%d, %d, %d)", xd->batch,
                        xd->channels, xd->length);
     if (ns->mode == KAPRE_NOISE_TENSOR) {
@@ -3106,7 +3180,6 @@ static int kb_noise_prepare(KbNoiseParams& p, const kapre_wave_desc* xd, const k
     }
     p.snr = sd->snr; p.snr_sb = sd->snr_stride_b; p.snr_sc = sd->snr_stride_c;
     p.len = sd->lengths; p.len_sb = sd->lengths_stride_b; p.len_sc = sd->lengths_stride_c;
-    p.part = (double*)workspace_dev;
     return 0;
 }
 
@@ -3124,9 +3197,11 @@ static int kb_noise_launch(const KbNoiseParams& p, cudaStream_t st) {
 extern "C" {
 
 int64_t kapre_add_noise_workspace_bytes(int batch, int channels, int length) {
-    const int64_t n = kb_noise_ws(batch, channels, length);
-    if (n < 0) return kb_fail(KAPRE_E_INVALID, "add_noise: negative size or too many samples");
-    return n;
+    KbLayout L;
+    double* part;
+    if (kb_noise_layout(L, batch, channels, length, &part) < 0)
+        return kb_fail(KAPRE_E_INVALID, "add_noise: negative size or too many samples");
+    return L.end;
 }
 
 int kapre_add_noise(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_noise_source* noise,
@@ -3225,6 +3300,25 @@ struct kapre_kaldi_plan {
     const int* klo; const int* klen; const int* kidx; const float* kw;
     const float* dct;
 };
+
+// The plan's tables in its one device block.  With a null base only measures.
+static void kb_kaldi_table_layout(KbLayout& L, const KbKaldiTables& t, kapre_kaldi_plan* pl) {
+    pl->wh = L.take<float>(t.wh.size()); pl->half = L.take<float>(t.half.size());
+    pl->twp = L.take<float2>(t.twp.size()); pl->twn = L.take<float2>(t.twn.size());
+    pl->mlo = L.take<int>(t.mlo.size()); pl->mlen = L.take<int>(t.mlen.size()); pl->moff = L.take<int>(t.moff.size());
+    pl->mw = L.take<float>(t.mw.size());
+    pl->klo = L.take<int>(t.klo.size()); pl->klen = L.take<int>(t.klen.size()); pl->kidx = L.take<int>(t.kidx.size());
+    pl->kw = L.take<float>(t.kw.size());
+    pl->dct = L.take<float>(t.dct.size());
+}
+
+// The backward workspace: the per-frame gradients gf, then the mean-subtracted output gradient gc (empty without mean
+// subtraction).
+static void kb_kaldi_layout(KbLayout& L, const kapre_kaldi_plan* plan, int batch, int channels, int frames, float** gf,
+                            float** gc) {
+    *gf = L.take<float>(batch, channels, frames, plan->cfg.window_size);
+    *gc = L.take<float>(batch, channels, frames, plan->cfg.subtract_mean ? plan->K : 0);
+}
 
 static bool kb_finite(float v) { return kb_kaldi_finite(v); }
 
@@ -3354,45 +3448,30 @@ int kapre_kaldi_plan_create(const kapre_kaldi_config* cfg, const float* window_h
     const int bad = kb_kaldi_tables(W, N, M, cfg->kind == KAPRE_KALDI_MFCC ? M * cfg->num_ceps : 0, window_host,
                                     banks_host, dct_host, t);
     if (bad) return kb_fail(KAPRE_E_INVALID, "kaldi: non-finite %s", bad == 1 ? "window" : bad == 2 ? "mel weight" : "DCT");
-    std::vector<float> &wh = t.wh, &half = t.half, &mw = t.mw, &kw = t.kw, &dct = t.dct;
-    std::vector<float2> &twp = t.twp, &twn = t.twn;
-    std::vector<int> &mlo = t.mlo, &mlen = t.mlen, &moff = t.moff, &klo = t.klo, &klen = t.klen, &kidx = t.kidx;
-    // one device block
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const size_t o_wh = take(wh.size() * 4), o_half = take(half.size() * 4), o_twp = take(twp.size() * 8),
-                 o_twn = take(twn.size() * 8), o_mlo = take(mlo.size() * 4), o_mlen = take(mlen.size() * 4),
-                 o_moff = take(moff.size() * 4), o_mw = take(mw.size() * 4), o_klo = take(klo.size() * 4),
-                 o_klen = take(klen.size() * 4), o_kidx = take(kidx.size() * 4), o_kw = take(kw.size() * 4),
-                 o_dct = take(dct.size() * 4);
-    std::vector<char> host(off, 0);
-    auto put = [&](size_t o, const void* src, size_t bytes) { memcpy(host.data() + o, src, bytes); };
-    put(o_wh, wh.data(), wh.size() * 4); put(o_half, half.data(), half.size() * 4);
-    put(o_twp, twp.data(), twp.size() * 8); put(o_twn, twn.data(), twn.size() * 8);
-    put(o_mlo, mlo.data(), mlo.size() * 4); put(o_mlen, mlen.data(), mlen.size() * 4);
-    put(o_moff, moff.data(), moff.size() * 4); put(o_mw, mw.data(), mw.size() * 4);
-    put(o_klo, klo.data(), klo.size() * 4); put(o_klen, klen.data(), klen.size() * 4);
-    put(o_kidx, kidx.data(), kidx.size() * 4); put(o_kw, kw.data(), kw.size() * 4);
-    put(o_dct, dct.data(), dct.size() * 4);
     kapre_kaldi_plan* pl = new kapre_kaldi_plan();
     pl->cfg = *cfg;
     pl->Q = Q; pl->P = P;
     pl->K = cfg->kind == KAPRE_KALDI_FBANK ? M + cfg->use_energy
           : cfg->kind == KAPRE_KALDI_MFCC ? cfg->num_ceps : P + 1;
     if ((rc = kb_dev_info(&pl->dev))) { delete pl; return rc; }
-    if (cudaMalloc(&pl->block, off) != cudaSuccess) { delete pl; return kb_fail(KAPRE_E_NOMEM, "kaldi: plan allocation"); }
-    if (cudaMemcpy(pl->block, host.data(), off, cudaMemcpyHostToDevice) != cudaSuccess) {
+    KbLayout size;
+    kb_kaldi_table_layout(size, t, pl);
+    if (cudaMalloc(&pl->block, size.end) != cudaSuccess) { delete pl; return kb_fail(KAPRE_E_NOMEM, "kaldi: plan allocation"); }
+    KbLayout L{(char*)pl->block};
+    kb_kaldi_table_layout(L, t, pl);
+    // staged on the host at the same offsets, then one upload
+    std::vector<char> host(size.end, 0);
+    auto put = [&](const void* dev, const auto& v) {
+        memcpy(host.data() + ((const char*)dev - L.base), v.data(), v.size() * sizeof(v[0]));
+    };
+    put(pl->wh, t.wh); put(pl->half, t.half); put(pl->twp, t.twp); put(pl->twn, t.twn);
+    put(pl->mlo, t.mlo); put(pl->mlen, t.mlen); put(pl->moff, t.moff); put(pl->mw, t.mw);
+    put(pl->klo, t.klo); put(pl->klen, t.klen); put(pl->kidx, t.kidx); put(pl->kw, t.kw);
+    put(pl->dct, t.dct);
+    if (cudaMemcpy(pl->block, host.data(), size.end, cudaMemcpyHostToDevice) != cudaSuccess) {
         cudaFree(pl->block); delete pl;
         return kb_fail(KAPRE_E_CUDA, "kaldi: plan upload");
     }
-    char* d = (char*)pl->block;
-    pl->wh = (const float*)(d + o_wh); pl->half = (const float*)(d + o_half);
-    pl->twp = (const float2*)(d + o_twp); pl->twn = (const float2*)(d + o_twn);
-    pl->mlo = (const int*)(d + o_mlo); pl->mlen = (const int*)(d + o_mlen); pl->moff = (const int*)(d + o_moff);
-    pl->mw = (const float*)(d + o_mw);
-    pl->klo = (const int*)(d + o_klo); pl->klen = (const int*)(d + o_klen); pl->kidx = (const int*)(d + o_kidx);
-    pl->kw = (const float*)(d + o_kw);
-    pl->dct = (const float*)(d + o_dct);
     *out = pl;
     return 0;
 }
@@ -3424,9 +3503,10 @@ int64_t kapre_kaldi_workspace_bytes(const kapre_kaldi_plan* plan, int batch, int
     const double cols = (double)batch * channels * frames;
     const double bytes = cols * plan->cfg.window_size * 4.0 + (plan->cfg.subtract_mean ? cols * plan->K * 4.0 : 0.0);
     if (bytes > 4.0e18) return kb_fail(KAPRE_E_INVALID, "kaldi: workspace overflow");
-    const int64_t gf = ((int64_t)batch * channels * frames * plan->cfg.window_size * 4 + 255) & ~(int64_t)255;
-    const int64_t gc = plan->cfg.subtract_mean ? (int64_t)batch * channels * frames * plan->K * 4 : 0;
-    return gf + gc;
+    KbLayout L;
+    float *gf, *gc;
+    kb_kaldi_layout(L, plan, batch, channels, frames, &gf, &gc);
+    return L.bytes("kaldi");
 }
 
 int kapre_kaldi_features(const kapre_kaldi_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc,
@@ -3466,15 +3546,15 @@ int kapre_kaldi_features_backward(const kapre_kaldi_plan* plan, const float* gy_
         return kb_fail(KAPRE_E_INVALID, "null data pointer");
     p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_sl = x_desc->stride_l;
     p.gx = gx_dev; p.gx_sb = gx_desc->stride_b; p.gx_sc = gx_desc->stride_c; p.gx_sl = gx_desc->stride_l;
-    p.gf = (float*)workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    float* gc;
+    kb_kaldi_layout(L, plan, p.B, p.C, p.T, &p.gf, &gc);
     p.bwd = 1;
     const cudaStream_t st = (cudaStream_t)stream;
     if (p.jobs > 0) {
         p.g = gy_dev; p.g_sb = gy_desc->stride_b; p.g_sc = gy_desc->stride_c; p.g_st = gy_desc->stride_t;
         p.g_sk = gy_desc->stride_f;
         if (plan->cfg.subtract_mean) {
-            float* gc = (float*)((char*)workspace_dev +
-                                 (((int64_t)p.B * p.C * p.T * p.W * 4 + 255) & ~(int64_t)255));
             kapre_spec_desc cd;
             cd.stride_f = 1; cd.stride_t = p.K; cd.stride_c = (int64_t)p.T * p.K; cd.stride_b = cd.stride_c * p.C;
             if ((rc = kb_kaldi_cmn(p, gy_dev, *gy_desc, gc, cd, st))) return rc;
@@ -3511,10 +3591,11 @@ __global__ void __launch_bounds__(KB_LOUD_WARPS * 32) kb_loud_bwd_kernel(const _
     if (tile < p.tiles) kb_loud_bwd_tile(p, kb_smem + w * kb_loud_smem().total, tile);
 }
 
-// Checks a shape and fills the geometry; the workspace (piece sums) and stats ((E2, |J2|) per item, then one decision
-// byte per block) sizes, or -1 on a bad argument or an overflow.
-static int kb_loud_geometry(KbLoudParams& p, int batch, int channels, int length, int gate, int step, int64_t* ws,
-                            int64_t* stats) {
+// Checks a shape, fills the geometry and lays out the two buffers: the workspace (the (B, K, 2C) piece sums) and the
+// stats record ((E2, |J2|) per item, then one decision byte per block, in one region).  -1 on a bad argument or an
+// overflow.
+static int kb_loud_geometry(KbLoudParams& p, int batch, int channels, int length, int gate, int step, KbLayout& ws,
+                            KbLayout& rec) {
     if (batch < 0 || channels < 1 || channels > KB_LOUD_MAXC || length < 0 || gate < 1 || step < 1 || step > gate)
         return -1;
     p.B = batch; p.C = channels; p.L = length; p.G = gate; p.S = step;
@@ -3522,9 +3603,13 @@ static int kb_loud_geometry(KbLoudParams& p, int batch, int channels, int length
     const double w = (double)batch * p.K * 2 * channels * 8.0, s = (double)batch * (16.0 + p.Jmax);
     const double tiles = (double)batch * (p.Kb > p.K ? p.Kb : p.K);
     if (w > 4.0e18 || s > 4.0e18 || tiles / KB_LOUD_WARPS > 2147483647.0) return -1;
-    *ws = ((int64_t)batch * p.K * 2 * channels * 8 + 255) & ~(int64_t)255;
-    *stats = ((int64_t)batch * 16 + (int64_t)batch * p.Jmax + 255) & ~(int64_t)255;
-    return 0;
+    p.part = ws.take<double>(batch, p.K, 2 * channels);
+    ws.pad();
+    unsigned char* r = rec.take<unsigned char>(batch, 16 + p.Jmax);
+    rec.pad();
+    p.stats = (double*)r;
+    p.mask = r ? r + (int64_t)batch * 16 : nullptr;
+    return ws.overflow || rec.overflow ? -1 : 0;
 }
 
 static int kb_loud_launch(void (*kernel)(KbLoudParams), long long work, const KbLoudParams& p, cudaStream_t st) {
@@ -3536,20 +3621,20 @@ extern "C" {
 
 int64_t kapre_loudness_workspace_bytes(int batch, int channels, int length, int gate, int step, int64_t* stats_bytes) {
     KbLoudParams p{};
-    int64_t ws = 0, stats = 0;
-    if (kb_loud_geometry(p, batch, channels, length, gate, step, &ws, &stats) < 0)
+    KbLayout ws, rec;
+    if (kb_loud_geometry(p, batch, channels, length, gate, step, ws, rec) < 0)
         return kb_fail(KAPRE_E_INVALID, "loudness: bad size (%d, %d, %d), gate %d or step %d, or an overflow", batch,
                        channels, length, gate, step);
-    if (stats_bytes) *stats_bytes = stats;
-    return ws;
+    if (stats_bytes) *stats_bytes = rec.end;
+    return ws.end;
 }
 
 int kapre_loudness(const float* y_dev, const kapre_wave_desc* y_desc, const int32_t* lengths_dev, int gate, int step,
                    float* out_dev, void* stats_dev, void* workspace_dev, void* stream) {
     if (!y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
     KbLoudParams p{};
-    int64_t ws = 0, stats = 0;
-    if (kb_loud_geometry(p, y_desc->batch, y_desc->channels, y_desc->length, gate, step, &ws, &stats) < 0)
+    KbLayout ws{(char*)workspace_dev}, rec{(char*)stats_dev};
+    if (kb_loud_geometry(p, y_desc->batch, y_desc->channels, y_desc->length, gate, step, ws, rec) < 0)
         return kb_fail(KAPRE_E_INVALID, "loudness: bad size (%d, %d, %d), gate %d or step %d, or an overflow",
                        y_desc->batch, y_desc->channels, y_desc->length, gate, step);
     if (p.B == 0) return 0;
@@ -3558,9 +3643,6 @@ int kapre_loudness(const float* y_dev, const kapre_wave_desc* y_desc, const int3
     p.y = y_dev; p.y_sb = y_desc->stride_b; p.y_sc = y_desc->stride_c; p.y_sl = y_desc->stride_l;
     p.len = lengths_dev;
     p.out = out_dev;
-    p.part = (double*)workspace_dev;
-    p.stats = (double*)stats_dev;
-    p.mask = (unsigned char*)stats_dev + (int64_t)p.B * 16;
     p.tiles = (long long)p.B * p.K;
     const cudaStream_t st = (cudaStream_t)stream;
     int rc;
@@ -3573,8 +3655,8 @@ int kapre_loudness_backward(const float* gl_dev, const float* y_dev, const kapre
                             const kapre_wave_desc* gy_desc, void* stream) {
     if (!y_desc || !gy_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
     KbLoudParams p{};
-    int64_t ws = 0, stats = 0;
-    if (kb_loud_geometry(p, y_desc->batch, y_desc->channels, y_desc->length, gate, step, &ws, &stats) < 0)
+    KbLayout ws, rec{(char*)const_cast<void*>(stats_dev)};
+    if (kb_loud_geometry(p, y_desc->batch, y_desc->channels, y_desc->length, gate, step, ws, rec) < 0)
         return kb_fail(KAPRE_E_INVALID, "loudness: bad size (%d, %d, %d), gate %d or step %d, or an overflow",
                        y_desc->batch, y_desc->channels, y_desc->length, gate, step);
     if (gy_desc->batch != p.B || gy_desc->channels != p.C || gy_desc->length != p.L)
@@ -3587,8 +3669,6 @@ int kapre_loudness_backward(const float* gl_dev, const float* y_dev, const kapre
     p.len = lengths_dev;
     p.gl = gl_dev;
     p.gy = gy_dev; p.g_sb = gy_desc->stride_b; p.g_sc = gy_desc->stride_c; p.g_sl = gy_desc->stride_l;
-    p.stats = (double*)const_cast<void*>(stats_dev);
-    p.mask = (unsigned char*)const_cast<void*>(stats_dev) + (int64_t)p.B * 16;
     return kb_loud_launch(kb_loud_bwd_kernel, p.tiles, p, (cudaStream_t)stream);
 }
 
@@ -3621,19 +3701,18 @@ static long long kb_cqt_level_len(long long L, int i) {
     return L;
 }
 
-// Float offsets, 256 B aligned, of the pyramid levels 1 .. n_oct-1 (forward workspace), or (backward workspace) of the
-// adjoint's levels 1 .. n_oct-1 and its resampling adjoints at levels 0 .. n_oct-2.  Returns the total in bytes.
-static int64_t kb_cqt_layout(int n_oct, long long bc, long long L, int backward, int64_t* lvl, int64_t* glvl,
-                             int64_t* rlvl) {
-    int64_t off = 0;
-    auto take = [&](long long n) { const int64_t o = off; off += (n * 4 + 255) / 256 * 64; return o; };
-    if (!backward)
-        for (int i = 1; i < n_oct; ++i) lvl[i] = take(bc * kb_cqt_level_len(L, i));
-    else {
-        for (int i = 1; i < n_oct; ++i) glvl[i] = take(bc * kb_cqt_level_len(L, i));
-        for (int i = 0; i + 1 < n_oct; ++i) rlvl[i] = take(bc * kb_cqt_level_len(L, i));
-    }
-    return off * 4;
+// The forward workspace: the (B, C, L_i) pyramid levels 1 .. n_oct-1, which the backward reads too.
+static void kb_cqt_layout(KbLayout& L, int n_oct, int batch, int channels, int length, float** lvl) {
+    for (int i = 1; i < n_oct; ++i) lvl[i] = L.take<float>(batch, channels, kb_cqt_level_len(length, i));
+    L.pad();
+}
+
+// The backward workspace: the adjoint's levels 1 .. n_oct-1, then its resampling adjoints at levels 0 .. n_oct-2.
+static void kb_cqt_backward_layout(KbLayout& L, int n_oct, int batch, int channels, int length, float** glvl,
+                                   float** rlvl) {
+    for (int i = 1; i < n_oct; ++i) glvl[i] = L.take<float>(batch, channels, kb_cqt_level_len(length, i));
+    for (int i = 0; i + 1 < n_oct; ++i) rlvl[i] = L.take<float>(batch, channels, kb_cqt_level_len(length, i));
+    L.pad();
 }
 
 static int kb_cqt_check_shape(const kapre_cqt_plan* plan, const kapre_wave_desc* xd) {
@@ -3650,18 +3729,19 @@ static int kb_cqt_check_shape(const kapre_cqt_plan* plan, const kapre_wave_desc*
 }
 
 // Common fields: levels (level 0 = x, the others contiguous (B, C, L_i) in the workspace) and sizes.
-static KbCqtParams kb_cqt_params(const kapre_cqt_plan* plan, const float* x, const kapre_wave_desc* xd, float* ws) {
+static KbCqtParams kb_cqt_params(const kapre_cqt_plan* plan, const float* x, const kapre_wave_desc* xd, const void* ws) {
     KbCqtParams p = plan->geo;
     p.B = xd->batch; p.C = xd->channels;
     p.M = 1 + xd->length / plan->cfg.hop_length;
     p.tab = plan->tab; p.btab = plan->btab;
-    int64_t lvl[KB_CQT_MAX_OCT], g[KB_CQT_MAX_OCT], r[KB_CQT_MAX_OCT];
-    kb_cqt_layout(p.n_oct, (long long)p.B * p.C, xd->length, 0, lvl, g, r);
+    KbLayout L{(char*)const_cast<void*>(ws)};
+    float* lvl[KB_CQT_MAX_OCT];
+    kb_cqt_layout(L, p.n_oct, p.B, p.C, xd->length, lvl);
     for (int i = 0; i < p.n_oct; ++i) {
         KbCqtOct& o = p.oct[i];
         o.L = (int)kb_cqt_level_len(xd->length, i);
         if (i == 0) { o.y = x; o.y_sb = xd->stride_b; o.y_sc = xd->stride_c; o.y_sl = xd->stride_l; }
-        else { o.y = ws + lvl[i]; o.y_sb = (long long)p.C * o.L; o.y_sc = o.L; o.y_sl = 1; }
+        else { o.y = lvl[i]; o.y_sb = (long long)p.C * o.L; o.y_sc = o.L; o.y_sl = 1; }
     }
     return p;
 }
@@ -3734,8 +3814,11 @@ int64_t kapre_cqt_workspace_bytes(const kapre_cqt_plan* plan, int batch, int cha
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
     if (batch < 0 || channels < 0 || length < 0) return kb_fail(KAPRE_E_INVALID, "cqt: negative size");
     if ((double)batch * channels * (length + 1.0) * 3.0 > 4.0e18) return kb_fail(KAPRE_E_INVALID, "cqt: size overflow");
-    int64_t a[KB_CQT_MAX_OCT], b[KB_CQT_MAX_OCT], c[KB_CQT_MAX_OCT];
-    return kb_cqt_layout(plan->geo.n_oct, (long long)batch * channels, length, backward ? 1 : 0, a, b, c);
+    KbLayout L;
+    float *a[KB_CQT_MAX_OCT], *b[KB_CQT_MAX_OCT];
+    if (backward) kb_cqt_backward_layout(L, plan->geo.n_oct, batch, channels, length, a, b);
+    else kb_cqt_layout(L, plan->geo.n_oct, batch, channels, length, a);
+    return L.bytes("cqt");
 }
 
 int kapre_cqt(const kapre_cqt_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, int magnitude,
@@ -3746,7 +3829,7 @@ int kapre_cqt(const kapre_cqt_plan* plan, const float* x_dev, const kapre_wave_d
     if (magnitude != 0 && magnitude != 1) return kb_fail(KAPRE_E_INVALID, "cqt: magnitude must be 0 or 1");
     if ((long long)x_desc->batch * x_desc->channels == 0) return 0;
     if (!x_dev || !out_dev || (plan->geo.n_oct > 1 && !workspace_dev)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
-    KbCqtParams p = kb_cqt_params(plan, x_dev, x_desc, (float*)workspace_dev);
+    KbCqtParams p = kb_cqt_params(plan, x_dev, x_desc, workspace_dev);
     p.n_threads = KB_CQT_THREADS;
     p.mag = magnitude;
     p.out = out_dev; p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t;
@@ -3782,14 +3865,14 @@ int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kap
     const int n_oct = plan->geo.n_oct;
     if (!g_dev || !gx_dev || (n_oct > 1 && !workspace_dev) || (magnitude && (!x_dev || (n_oct > 1 && !fwd_workspace_dev))))
         return kb_fail(KAPRE_E_INVALID, "null data pointer");
-    KbCqtParams p = kb_cqt_params(plan, x_dev, x_desc, (float*)const_cast<void*>(fwd_workspace_dev));
+    KbCqtParams p = kb_cqt_params(plan, x_dev, x_desc, fwd_workspace_dev);
     p.n_threads = KB_CQT_BWD_THREADS;
     p.mag = magnitude;
     p.g = g_dev; p.g_sb = g_desc->stride_b; p.g_sc = g_desc->stride_c; p.g_st = g_desc->stride_t;
     p.g_sk = g_desc->stride_f;
-    int64_t lvl[KB_CQT_MAX_OCT], glvl[KB_CQT_MAX_OCT], rlvl[KB_CQT_MAX_OCT];
-    kb_cqt_layout(n_oct, bc, x_desc->length, 1, lvl, glvl, rlvl);
-    float* ws = (float*)workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    float *glvl[KB_CQT_MAX_OCT], *rlvl[KB_CQT_MAX_OCT];
+    kb_cqt_backward_layout(L, n_oct, p.B, p.C, x_desc->length, glvl, rlvl);
     const cudaStream_t st = (cudaStream_t)stream;
     const int smem = kb_cqt_bwd_smem();
     KbLaunchReports reports;    // every octave's launch and the resampling launches between them
@@ -3802,12 +3885,12 @@ int kapre_cqt_backward(const kapre_cqt_plan* plan, const float* x_dev, const kap
         if (i + 1 < n_oct && p.oct[i + 1].L > 0) {
             const kapre_wave_desc gd = kb_cqt_level_desc(p.B, p.C, p.oct[i + 1].L);
             const kapre_wave_desc rd = kb_cqt_level_desc(p.B, p.C, o.L);
-            if ((rc = kapre_resample_backward(plan->rs, ws + glvl[i + 1], &gd, ws + rlvl[i], &rd, stream))) return rc;
+            if ((rc = kapre_resample_backward(plan->rs, glvl[i + 1], &gd, rlvl[i], &rd, stream))) return rc;
             reports.add();
-            p.add = ws + rlvl[i];
+            p.add = rlvl[i];
         }
         if (i == 0) { p.gy = gx_dev; p.gy_sb = gx_desc->stride_b; p.gy_sc = gx_desc->stride_c; p.gy_sl = gx_desc->stride_l; }
-        else { p.gy = ws + glvl[i]; p.gy_sb = (long long)p.C * o.L; p.gy_sc = o.L; p.gy_sl = 1; }
+        else { p.gy = glvl[i]; p.gy_sb = (long long)p.C * o.L; p.gy_sc = o.L; p.gy_sl = 1; }
         const long long tiles = bc * ((o.L + o.TS - 1) / o.TS);
         int grid;
         if ((rc = kb_resident_grid(kb_cqt_bwd_kernel, "cqt_bwd", KB_CQT_BWD_THREADS, smem, tiles, plan->dev.sm_count,
@@ -3870,6 +3953,22 @@ static int kb_pitch_check_shape(const kapre_pitch_plan* plan, const kapre_wave_d
     return 0;
 }
 
+// The pYIN workspace: per frame the candidate count, probabilities and pitch bins, then the Viterbi back-pointers.
+struct KbPyinWs {
+    int* cand_n;
+    float* cand_p;
+    unsigned short *cand_bin, *bp;
+};
+
+static KbPyinWs kb_pyin_layout(KbLayout& L, const kapre_pitch_plan* plan, int batch, int channels, int M) {
+    KbPyinWs w;
+    w.cand_n = L.take<int>(batch, channels, M);
+    w.cand_p = L.take<float>(batch, channels, M, plan->geo.cmax);
+    w.cand_bin = L.take<unsigned short>(batch, channels, M, plan->geo.cmax);
+    w.bp = L.take<unsigned short>(batch, channels, M, 2 * plan->cfg.n_pitch);
+    return w;
+}
+
 // The difference-function launch of kapre_yin (pyin = 0) and kapre_pyin.
 static int kb_pitch_launch(const kapre_pitch_plan* plan, const float* x, const kapre_wave_desc* xd, float* out,
                            const kapre_frames_desc* od, float* cm, const kapre_spec_desc* cd, void* ws, cudaStream_t st) {
@@ -3881,11 +3980,9 @@ static int kb_pitch_launch(const kapre_pitch_plan* plan, const float* x, const k
     p.cm = cm;
     if (cm) { p.c_sb = cd->stride_b; p.c_sc = cd->stride_c; p.c_st = cd->stride_t; p.c_sk = cd->stride_f; }
     if (p.pyin) {
-        const long long fr = (long long)p.B * p.C * p.M;
-        char* w = (char*)ws;
-        p.cand_n = (int*)w;
-        p.cand_p = (float*)(w + (fr * 4 + 255) / 256 * 256);
-        p.cand_bin = (unsigned short*)((char*)p.cand_p + (fr * p.cmax * 4 + 255) / 256 * 256);
+        KbLayout L{(char*)ws};
+        const KbPyinWs w = kb_pyin_layout(L, plan, p.B, p.C, p.M);
+        p.cand_n = w.cand_n; p.cand_p = w.cand_p; p.cand_bin = w.cand_bin;
     }
     if (!kb_pitch_setup(p)) return kb_fail(KAPRE_E_INVALID, "pitch: too many tiles");
     int grid, rc;
@@ -3893,15 +3990,6 @@ static int kb_pitch_launch(const kapre_pitch_plan* plan, const float* x, const k
         return rc;
     return kb_launch(kb_pitch_kernel, {.grid = grid, .block = KB_PITCH_THREADS, .smem = p.smem, .st = st,
                                        .timed = true}, p);
-}
-
-static int64_t kb_pitch_ws_layout(const kapre_pitch_plan* plan, long long rows, int M, int64_t* bp_off) {
-    const long long fr = rows * M;
-    int64_t off = (fr * 4 + 255) / 256 * 256;
-    off += (fr * plan->geo.cmax * 4 + 255) / 256 * 256;
-    off += (fr * plan->geo.cmax * 2 + 255) / 256 * 256;
-    *bp_off = off;
-    return off + fr * 2LL * plan->cfg.n_pitch * 2;
 }
 
 extern "C" {
@@ -3994,8 +4082,9 @@ int64_t kapre_pitch_workspace_bytes(const kapre_pitch_plan* plan, int batch, int
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
     if (batch < 0 || channels < 0 || length < 0) return kb_fail(KAPRE_E_INVALID, "pitch: negative size");
     if (!plan->geo.pyin) return 0;
-    int64_t bp;
-    return kb_pitch_ws_layout(plan, (long long)batch * channels, kb_pitch_frames(plan->cfg, length), &bp);
+    KbLayout L;
+    kb_pyin_layout(L, plan, batch, channels, kb_pitch_frames(plan->cfg, length));
+    return L.bytes("pyin");
 }
 
 int kapre_yin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* f0_dev,
@@ -4036,14 +4125,10 @@ int kapre_pyin(const kapre_pitch_plan* plan, const float* x_dev, const kapre_wav
         return rc;
     reports.add();
     KbVitParams v = plan->vit;
-    int64_t bp;
-    kb_pitch_ws_layout(plan, rows, M, &bp);
-    char* w = (char*)workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    const KbPyinWs w = kb_pyin_layout(L, plan, x_desc->batch, x_desc->channels, M);
     v.M = M; v.C = x_desc->channels; v.rows = rows;
-    v.cand_n = (const int*)w;
-    v.cand_p = (const float*)(w + (rows * M * 4 + 255) / 256 * 256);
-    v.cand_bin = (const unsigned short*)((const char*)v.cand_p + (rows * M * plan->geo.cmax * 4 + 255) / 256 * 256);
-    v.bp = (unsigned short*)(w + bp);
+    v.cand_n = w.cand_n; v.cand_p = w.cand_p; v.cand_bin = w.cand_bin; v.bp = w.bp;
     v.vp = voiced_prob_dev; v.f0 = f0_dev; v.flag = voiced_flag_dev;
     v.o_sb = out_desc->stride_b; v.o_sc = out_desc->stride_c; v.o_st = out_desc->stride_t;
     const int smem = kb_vit_smem(v.n, v.w);
@@ -4127,15 +4212,22 @@ static int kb_chroma_fwd_launch(const kapre_chroma_plan* plan, const KbChromaPar
     return kb_launch(kb_chroma_kernel, {.grid = grid, .block = KB_CH_THREADS, .smem = smem, .st = st, .timed = true}, p);
 }
 
-static int64_t kb_tune_ws(const kapre_chroma_plan* plan, long long B, long long rows, long long M, int64_t* off) {
-    const long long cap = (plan->d.peak_hi - plan->d.peak_lo + 1) / 2;
-    int64_t o = 0;
-    off[0] = o; o += (B * 1024 * 4 + 255) / 256 * 256;                         // radix histograms
-    off[1] = o; o += (B * plan->d.n_tuning_bins * 4 + 255) / 256 * 256;         // residual histograms
-    off[2] = o; o += (B * 4 + 255) / 256 * 256;                                 // smallest mag above the lower rank
-    off[3] = o; o += (rows * M * cap * 4 + 255) / 256 * 256;                    // peak mags
-    off[4] = o; o += (rows * M * cap * 4 + 255) / 256 * 256;                    // peak pitches
-    return o;
+// The chroma_cens workspace: the (B, C, frames, n_chroma) chroma that the smoothing pass reads.
+static float* kb_cens_layout(KbLayout& L, const kapre_chroma_plan* plan, int batch, int channels, int frames) {
+    return L.take<float>(batch, channels, frames, plan->d.n_chroma);
+}
+
+// The tuning workspace: per item the radix and residual histograms and the smallest magnitude above the lower rank,
+// then per frame the peak magnitudes and pitches.
+static void kb_tune_layout(KbLayout& L, const kapre_chroma_plan* plan, int batch, int channels, int frames,
+                           KbTuneParams& p) {
+    const int cap = (plan->d.peak_hi - plan->d.peak_lo + 1) / 2;
+    p.hist = L.take<unsigned>(batch, 1024);
+    p.res = L.take<unsigned>(batch, plan->d.n_tuning_bins);
+    p.above = L.take<unsigned>(batch);
+    p.mag = L.take<float>(batch, channels, frames, cap);
+    p.pitch = L.take<float>(batch, channels, frames, cap);
+    L.pad();
 }
 
 extern "C" {
@@ -4229,7 +4321,9 @@ int kapre_chroma_backward(const kapre_chroma_plan* plan, const kapre_chroma_conf
 int64_t kapre_chroma_cens_workspace_bytes(const kapre_chroma_plan* plan, int batch, int channels, int frames) {
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
     if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "chroma: negative size");
-    return (int64_t)batch * channels * frames * plan->d.n_chroma * 4;
+    KbLayout L;
+    kb_cens_layout(L, plan, batch, channels, frames);
+    return L.bytes("chroma_cens");
 }
 
 int kapre_chroma_cens(const kapre_chroma_plan* plan, int in_mode, const void* x_dev, const kapre_spec_desc* x_desc,
@@ -4244,8 +4338,10 @@ int kapre_chroma_cens(const kapre_chroma_plan* plan, int in_mode, const void* x_
     if (!p.jobs) return 0;
     if (!workspace_dev) return kb_fail(KAPRE_E_INVALID, "null workspace");
     const int NC = plan->d.n_chroma;
+    KbLayout L{(char*)workspace_dev};
+    float* q = kb_cens_layout(L, plan, batch, channels, frames);
     p.cens = 1;
-    p.out = (float*)workspace_dev;
+    p.out = q;
     p.o_sc = (long long)frames * NC; p.o_sb = channels * p.o_sc; p.o_st = NC; p.o_sk = 1;
     const cudaStream_t st = (cudaStream_t)stream;
     KbLaunchReports reports;
@@ -4256,7 +4352,7 @@ int kapre_chroma_cens(const kapre_chroma_plan* plan, int in_mode, const void* x_
     c.B = batch; c.C = channels; c.M = frames;
     c.tiles = ((long long)frames + KB_CH_SMOOTH_TF - 1) / KB_CH_SMOOTH_TF;
     c.jobs = (long long)batch * channels * c.tiles;
-    c.q = (const float*)workspace_dev;
+    c.q = q;
     c.out = out_dev; c.o_sb = out_desc->stride_b; c.o_sc = out_desc->stride_c; c.o_st = out_desc->stride_t;
     c.o_sk = out_desc->stride_f;
     const int smem = kb_cens_smem(NC, c.N);
@@ -4272,8 +4368,10 @@ int64_t kapre_chroma_tuning_workspace_bytes(const kapre_chroma_plan* plan, int b
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
     if (batch < 0 || channels < 0 || frames < 0) return kb_fail(KAPRE_E_INVALID, "chroma: negative size");
     if (!plan->d.n_tuning_bins) return kb_fail(KAPRE_E_INVALID, "chroma: the plan has no tuning estimate");
-    int64_t off[5];
-    return kb_tune_ws(plan, batch, (long long)batch * channels, frames, off);
+    KbLayout L;
+    KbTuneParams p{};
+    kb_tune_layout(L, plan, batch, channels, frames, p);
+    return L.bytes("chroma_tuning");
 }
 
 int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float* x_dev, const kapre_spec_desc* x_desc,
@@ -4295,14 +4393,12 @@ int kapre_chroma_tuning(const kapre_chroma_plan* plan, int in_mode, const float*
     p.B = batch; p.C = channels; p.M = frames;
     p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_st = x_desc->stride_t;
     p.x_sk = x_desc->stride_f;
-    int64_t off[5];
-    kb_tune_ws(plan, batch, (long long)batch * channels, frames, off);
-    char* w = (char*)workspace_dev;
-    p.hist = (unsigned*)(w + off[0]); p.res = (unsigned*)(w + off[1]); p.above = (unsigned*)(w + off[2]);
-    p.mag = (float*)(w + off[3]); p.pitch = (float*)(w + off[4]);
+    KbLayout L{(char*)workspace_dev};
+    kb_tune_layout(L, plan, batch, channels, frames, p);
     p.tuning = tuning_dev; p.tab = table_dev;
-    KB_CUDA(cudaMemsetAsync(w, 0, (size_t)off[2], st));
-    KB_CUDA(cudaMemsetAsync(w + off[2], 0xff, (size_t)batch * 4, st));
+    // both histograms, which the layout puts next to each other, start at zero; the minima start at the largest value
+    KB_CUDA(cudaMemsetAsync(p.hist, 0, (size_t)((char*)p.above - (char*)p.hist), st));
+    KB_CUDA(cudaMemsetAsync(p.above, 0xff, (size_t)batch * 4, st));
     const long long rows = (long long)batch * channels;
     int grid;
     KbLaunchReports reports;
@@ -4361,6 +4457,12 @@ static int kb_hpss_tiles_launch(const KbHpssParams& p, cudaStream_t st) {
     return kb_launch(k, {.grid = grid, .block = KB_HS_THREADS, .smem = smem, .st = st, .timed = !BWD}, p);
 }
 
+// The backward workspace: one region of 2n weights, the harmonic median's n and then the percussive median's n.
+static void kb_hpss_layout(KbLayout& L, int batch, int channels, int frames, int bins, KbHpssParams& p) {
+    p.wh = L.take<kb_hs_w>(batch, channels, frames, bins, 2);
+    p.wp = p.wh ? p.wh + (long long)batch * channels * frames * bins : nullptr;
+}
+
 static int kb_hpss_params(const kapre_hpss_config* cfg, const void* S, int is_complex, const kapre_spec_desc* sd,
                           int B, int C, int T, int K, KbHpssParams* out) {
     if (!cfg || !sd) return kb_fail(KAPRE_E_INVALID, "null argument");
@@ -4405,7 +4507,10 @@ int kapre_hpss(const kapre_hpss_config* cfg, const void* S_dev, int is_complex, 
 
 int64_t kapre_hpss_workspace_bytes(int batch, int channels, int frames, int bins) {
     if (batch < 0 || channels < 0 || frames < 0 || bins < 0) return kb_fail(KAPRE_E_INVALID, "hpss: negative size");
-    return (int64_t)batch * channels * frames * bins * 2 * (int64_t)sizeof(kb_hs_w);
+    KbLayout L;
+    KbHpssParams p{};
+    kb_hpss_layout(L, batch, channels, frames, bins, p);
+    return L.bytes("hpss");
 }
 
 int kapre_hpss_backward(const kapre_hpss_config* cfg, const void* S_dev, int is_complex, const kapre_spec_desc* S_desc,
@@ -4424,8 +4529,9 @@ int kapre_hpss_backward(const kapre_hpss_config* cfg, const void* S_dev, int is_
     if (gp_dev) { p.gp_sb = gp_desc->stride_b; p.gp_sc = gp_desc->stride_c; p.gp_st = gp_desc->stride_t; p.gp_sk = gp_desc->stride_f; }
     p.gx = gS_dev; p.gx_sb = gS_desc->stride_b; p.gx_sc = gS_desc->stride_c; p.gx_st = gS_desc->stride_t;
     p.gx_sk = gS_desc->stride_f;
+    KbLayout L{(char*)workspace_dev};
+    kb_hpss_layout(L, batch, channels, frames, bins, p);
     const long long n = (long long)batch * channels * frames * bins;
-    p.wh = (kb_hs_w*)workspace_dev; p.wp = p.wh + n;
     cudaStream_t st = (cudaStream_t)stream;
     KbLaunchReports reports;
     if ((rc = kb_hpss_tiles_launch<1>(p, st))) return rc;
@@ -4511,12 +4617,21 @@ static int kb_onset_params(const kapre_onset_config* cfg, const float* S, const 
     return 0;
 }
 
-static int kb_beat_ws_total(int B, int C, int T, int64_t* n) {
+// The onset strength backward's workspace: the (B, C, frames, bins) weights the gather pass reads.
+static kb_on_w* kb_onset_layout(KbLayout& L, int B, int C, int T, int K) { return L.take<kb_on_w>(B, C, T, K); }
+
+// The tempo workspace: the mean's float64 partial sums per row, chunk and lag.
+static double* kb_tempo_layout(KbLayout& L, int B, int C, int T, int W) {
+    return (double*)L.take<char>(kb_tempo_ws_bytes(B, C, T, W));
+}
+
+// Checks a shape and lays out the beat tracker's workspace: per row ls, cs (double T), back and beats (int T).
+static int kb_beat_layout(KbLayout& L, int B, int C, int T, void** ws) {
     int rc = kb_rh_rows(B, C, T, "beat_track");
     if (rc) return rc;
     const long long rows = (long long)B * C;
     if (rows && kb_beat_ws_bytes_row(T) > (1LL << 46) / rows) return kb_fail(KAPRE_E_INVALID, "beat_track: too large");
-    *n = rows * kb_beat_ws_bytes_row(T);
+    *ws = L.take<char>(B, C, kb_beat_ws_bytes_row(T));
     return 0;
 }
 
@@ -4538,7 +4653,9 @@ int kapre_onset_strength(const kapre_onset_config* cfg, const float* S_dev, cons
 
 int64_t kapre_onset_strength_workspace_bytes(int batch, int channels, int frames, int bins) {
     if (batch < 0 || channels < 0 || frames < 0 || bins < 0) return kb_fail(KAPRE_E_INVALID, "onset_strength: negative size");
-    return (int64_t)batch * channels * frames * bins * (int64_t)sizeof(kb_on_w);
+    KbLayout L;
+    kb_onset_layout(L, batch, channels, frames, bins);
+    return L.bytes("onset_strength");
 }
 
 int kapre_onset_strength_backward(const kapre_onset_config* cfg, const float* S_dev, const kapre_spec_desc* S_desc,
@@ -4554,7 +4671,8 @@ int kapre_onset_strength_backward(const kapre_onset_config* cfg, const float* S_
     p.g = g_dev; p.g_sb = g_desc->stride_b; p.g_sc = g_desc->stride_c; p.g_st = g_desc->stride_t;
     p.gx = gS_dev; p.gx_sb = gS_desc->stride_b; p.gx_sc = gS_desc->stride_c; p.gx_st = gS_desc->stride_t;
     p.gx_sk = gS_desc->stride_f;
-    p.ws = (kb_on_w*)workspace_dev;
+    KbLayout L{(char*)workspace_dev};
+    p.ws = kb_onset_layout(L, batch, channels, frames, bins);
     cudaStream_t st = (cudaStream_t)stream;
     KbLaunchReports reports;
     if ((rc = kb_rh_launch(kb_onset_kernel<1>, "onset_bwd", kb_onset_smem(p.K, p.m, p.F, 1), p.jobs, p, st, false)))
@@ -4594,7 +4712,9 @@ int64_t kapre_tempo_workspace_bytes(int batch, int channels, int frames, int win
     if (rc) return rc;
     if (win_length < 2 || win_length > KAPRE_TEMPOGRAM_MAX_WIN)
         return kb_fail(KAPRE_E_INVALID, "tempo: win_length %d outside [2, %d]", win_length, KAPRE_TEMPOGRAM_MAX_WIN);
-    return kb_tempo_ws_bytes(batch, channels, frames, win_length);
+    KbLayout L;
+    kb_tempo_layout(L, batch, channels, frames, win_length);
+    return L.bytes("tempo");
 }
 
 int kapre_tempo(const float* tg_dev, const kapre_spec_desc* tg_desc, int batch, int channels, int frames, int win_length,
@@ -4611,7 +4731,9 @@ int kapre_tempo(const float* tg_dev, const kapre_spec_desc* tg_desc, int batch, 
     p.B = batch; p.C = channels; p.T = frames; p.W = win_length; p.per_frame = per_frame != 0;
     p.tg = tg_dev; p.g_sb = tg_desc->stride_b; p.g_sc = tg_desc->stride_c; p.g_st = tg_desc->stride_t;
     p.g_sk = tg_desc->stride_f;
-    p.logprior = logprior_dev; p.bpm_scale = bpm_scale; p.out = out_dev; p.part = (double*)workspace_dev;
+    p.logprior = logprior_dev; p.bpm_scale = bpm_scale; p.out = out_dev;
+    KbLayout L{(char*)workspace_dev};
+    p.part = kb_tempo_layout(L, batch, channels, frames, win_length);
     if (per_frame) { p.o_sb = out_desc->stride_b; p.o_sc = out_desc->stride_c; p.o_st = out_desc->stride_t; }
     kb_tempo_setup(p);
     if (!p.jobs) return 0;
@@ -4655,29 +4777,29 @@ int kapre_onset_detect(const float* e_dev, const kapre_frames_desc* e_desc, int 
 }
 
 int64_t kapre_beat_track_workspace_bytes(int batch, int channels, int frames) {
-    int64_t n = 0;
-    int rc = kb_beat_ws_total(batch, channels, frames, &n);
-    return rc ? rc : n;
+    KbLayout L;
+    void* ws;
+    int rc = kb_beat_layout(L, batch, channels, frames, &ws);
+    return rc ? rc : L.bytes("beat_track");
 }
 
 int kapre_beat_track(const float* e_dev, const kapre_frames_desc* e_desc, int batch, int channels, int frames,
                      const kapre_beat_config* cfg, const float* bpm_dev, float bpm, float* tempo_dev, uint8_t* mask_dev,
                      const kapre_frames_desc* mask_desc, void* workspace_dev, void* stream) {
     if (!e_desc || !cfg || !mask_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
-    int64_t nws = 0;
-    int rc = kb_beat_ws_total(batch, channels, frames, &nws);
+    KbBeatParams p{};
+    KbLayout L{(char*)workspace_dev};
+    int rc = kb_beat_layout(L, batch, channels, frames, &p.ws);
     if (rc) return rc;
     if (!(cfg->fps > 0.0) || !isfinite(cfg->fps)) return kb_fail(KAPRE_E_INVALID, "beat_track: fps must be > 0");
     if (!(cfg->tightness > 0.0) || !isfinite(cfg->tightness))
         return kb_fail(KAPRE_E_INVALID, "beat_track: tightness must be > 0");
     if (!bpm_dev && !(bpm > 0.0f && isfinite(bpm))) return kb_fail(KAPRE_E_INVALID, "beat_track: bpm must be > 0");
-    KbBeatParams p{};
     p.B = batch; p.C = channels; p.T = frames; p.trim = cfg->trim != 0; p.fps = cfg->fps; p.tightness = cfg->tightness;
     p.bpm = bpm_dev; p.bpm_const = bpm;
     p.e = e_dev; p.e_sb = e_desc->stride_b; p.e_sc = e_desc->stride_c; p.e_st = e_desc->stride_t;
     p.tempo = tempo_dev; p.mask = mask_dev;
     p.m_sb = mask_desc->stride_b; p.m_sc = mask_desc->stride_c; p.m_st = mask_desc->stride_t;
-    p.ws = workspace_dev;
     p.jobs = (long long)batch * channels;
     if (!p.jobs) return 0;
     if (!frames) return kb_fail(KAPRE_E_INVALID, "beat_track: no frames");

@@ -85,6 +85,14 @@ def _workspace(n_items: int, device) -> torch.Tensor:
     return ws
 
 
+def _scratch(n: int, device) -> torch.Tensor:
+    """Device scratch of the ``n`` bytes a ``kapre_*_workspace_bytes`` function returned; raises on its error code."""
+    n = int(n)
+    if n < 0:
+        N.check(n)
+    return torch.empty(max(n, 1), dtype=torch.uint8, device=device)
+
+
 def _wants_grad(t) -> bool:
     """True when a CUDA tensor input should be recorded for autograd (see ``autograd.py``)."""
     return isinstance(t, torch.Tensor) and t.is_cuda and t.requires_grad and torch.is_grad_enabled()
@@ -453,9 +461,7 @@ def stft_backward(g: torch.Tensor, plan: StftPlan, input_data_format, output_dat
         return gx
     lib = N.lib()
     nbytes = int(lib.kapre_stft_backward_workspace_bytes(plan.handle(), B, C, L, int(bool(pad_begin)), int(bool(pad_end))))
-    if nbytes < 0:
-        N.check(nbytes)
-    ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=g.device) if nbytes else None
+    ws = _scratch(nbytes, g.device) if nbytes else None
     N.check(lib.kapre_stft_backward(plan.handle(), _ptr(g), ctypes.byref(gd), B, C, T, int(bool(pad_begin)),
                                     int(bool(pad_end)), _ptr(gx), ctypes.byref(xd), _ptr(ws) if ws is not None else None,
                                     _stream_ptr()))
@@ -927,7 +933,7 @@ def convolve_full(x, H, plan: ConvolvePlan, data_format):
     nbytes = _conv_workspace_bytes(plan, B, C, L, P)
     T = -(-L // blk) + P - 1
     y, yd = _wave_alloc(B, C, (T + 1) * blk, data_format, x.device)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    ws = _scratch(nbytes, x.device)
     if y.numel():
         Hd = _spec_contiguous_desc(H, H.shape[0] == 1, H.shape[1] == 1)
         N.check(N.lib().kapre_convolve(plan.handle(), _ptr(x), ctypes.byref(xd), _ptr(H), ctypes.byref(Hd), P, _ptr(y),
@@ -943,8 +949,7 @@ def convolve_backward(g_full, H, X, plan: ConvolvePlan, data_format, length, wan
     P, blk = H.shape[2], plan.block
     gx, xd = _wave_alloc(B, C, int(length), data_format, g_full.device)
     gH = torch.empty((B, C, P, blk + 1), dtype=torch.complex64, device=g_full.device) if want_h else None
-    ws = torch.empty(_conv_workspace_bytes(plan, B, C, int(length), P, backward=True), dtype=torch.uint8,
-                     device=g_full.device)
+    ws = _scratch(_conv_workspace_bytes(plan, B, C, int(length), P, backward=True), g_full.device)
     Hd = _spec_contiguous_desc(H, H.shape[0] == 1, H.shape[1] == 1)
     Xd = N.SpecDesc(*X.stride()) if want_h else None
     gHd = N.SpecDesc(*gH.stride()) if want_h else None
@@ -1054,10 +1059,7 @@ def _iir_coeffs(b, a):
 
 
 def lfilter_workspace(B, C, L, order, device):
-    n = int(N.lib().kapre_lfilter_workspace_bytes(B, C, L, order))
-    if n < 0:
-        N.check(n)
-    return torch.empty(max(n, 1), dtype=torch.uint8, device=device)
+    return _scratch(N.lib().kapre_lfilter_workspace_bytes(B, C, L, order), device)
 
 
 def lfilter_forward(x, b, a, flags, data_format):
@@ -1140,7 +1142,7 @@ def add_noise_workspace_bytes(B, C, L):
 
 
 def add_noise_workspace(B, C, L, device):
-    return torch.empty(max(add_noise_workspace_bytes(B, C, L), 1), dtype=torch.uint8, device=device)
+    return _scratch(add_noise_workspace_bytes(B, C, L), device)
 
 
 def _noise_source(noise, bank, data_format):
@@ -1306,9 +1308,9 @@ def loudness_forward(y, lengths, G, S, data_format):
     yd, (B, C, L) = _wave_desc(y, data_format)
     nw, ns = loudness_sizes(B, C, L, G, S)
     out = torch.empty(B, dtype=torch.float32, device=y.device)
-    stats = torch.empty(max(ns, 1), dtype=torch.uint8, device=y.device)
+    stats = _scratch(ns, y.device)
     if B:
-        ws = torch.empty(max(nw, 1), dtype=torch.uint8, device=y.device)
+        ws = _scratch(nw, y.device)
         N.check(N.lib().kapre_loudness(_ptr(y), ctypes.byref(yd), _ptr(lengths) if lengths is not None else None, G, S,
                                        _ptr(out), _ptr(stats), _ptr(ws), _stream_ptr()))
     return out, stats
@@ -1385,8 +1387,7 @@ def _pcen_workspace(B, C, T, F, device):
     """(chunks, scratch tensor or None) the library uses for this shape on the current device."""
     k, nbytes = ctypes.c_int(1), ctypes.c_int64(0)
     N.check(N.lib().kapre_pcen_workspace(B, C, T, F, ctypes.byref(k), ctypes.byref(nbytes)))
-    ws = torch.empty(nbytes.value // 4, dtype=torch.float32, device=device) if nbytes.value else None
-    return k.value, ws
+    return k.value, _scratch(nbytes.value, device) if nbytes.value else None
 
 
 @_device_of_first_arg
@@ -1463,10 +1464,7 @@ def griffin_lim(S: torch.Tensor, stft_plan: StftPlan, istft_plan: IstftPlan, n_i
     if y.numel() == 0:
         return y
     lib = N.lib()
-    nbytes = lib.kapre_griffin_lim_workspace_bytes(stft_plan.handle(), B, C, T)
-    if nbytes < 0:
-        N.check(nbytes)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=S.device)
+    ws = _scratch(lib.kapre_griffin_lim_workspace_bytes(stft_plan.handle(), B, C, T), S.device)
     cfg = N.GlCfg(int(n_iter), float(momentum), int(init), int(seed))
     N.check(lib.kapre_griffin_lim(stft_plan.handle(), istft_plan.handle(), _ptr(S), ctypes.byref(sd), B, C, T,
                                   ctypes.byref(cfg), _ptr(y), ctypes.byref(yd), _ptr(ws), _stream_ptr()))
@@ -1489,8 +1487,7 @@ def _time_stretch_workspace(B, C, T, F, rate, device):
     """(chunks, scratch tensor or None) the library uses for this shape on the current device."""
     k, nbytes = ctypes.c_int(1), ctypes.c_int64(0)
     N.check(N.lib().kapre_time_stretch_workspace(B, C, T, F, rate, ctypes.byref(k), ctypes.byref(nbytes)))
-    ws = torch.empty(nbytes.value // 4, dtype=torch.int32, device=device) if nbytes.value else None
-    return k.value, ws
+    return k.value, _scratch(nbytes.value, device) if nbytes.value else None
 
 
 @_device_of_first_arg
@@ -1742,10 +1739,7 @@ def kaldi_backward(gy, x, plan: KaldiPlan, lengths_h, lengths_d, data_format, di
     gx, od = _wave_alloc(B, C, L, data_format, x.device)
     if gx.numel():
         h = plan.handle()
-        n = int(N.lib().kapre_kaldi_workspace_bytes(h, B, C, T, 1))
-        if n < 0:
-            N.check(n)
-        ws = torch.empty(max(n, 1), dtype=torch.uint8, device=x.device)
+        ws = _scratch(N.lib().kapre_kaldi_workspace_bytes(h, B, C, T, 1), x.device)
         lp = lengths_h.ctypes.data_as(ctypes.c_void_p) if lengths_h is not None else None
         N.check(N.lib().kapre_kaldi_features_backward(
             h, _ptr(gy), ctypes.byref(gd), _ptr(x), ctypes.byref(xd), lp,
@@ -1807,10 +1801,7 @@ class CqtPlan(_PerDevice):
         return 1 + int(length) // self.hop_length
 
     def workspace(self, B, C, L, backward, device):
-        n = int(N.lib().kapre_cqt_workspace_bytes(self.handle(), B, C, L, int(backward)))
-        if n < 0:
-            N.check(n)
-        return torch.empty(max((n + 3) // 4, 1), dtype=torch.float32, device=device)
+        return _scratch(N.lib().kapre_cqt_workspace_bytes(self.handle(), B, C, L, int(backward)), device)
 
 
 def cqt_forward(x, plan: CqtPlan, input_data_format, output_data_format, magnitude):
@@ -1900,10 +1891,7 @@ class PitchPlan(_PerDevice):
         return 0 if lp < g['frame_length'] else 1 + (lp - g['frame_length']) // g['hop_length']
 
     def workspace(self, B, C, L, device):
-        n = int(N.lib().kapre_pitch_workspace_bytes(self.handle(), B, C, L))
-        if n < 0:
-            N.check(n)
-        return torch.empty(max((n + 3) // 4, 1), dtype=torch.float32, device=device)
+        return _scratch(N.lib().kapre_pitch_workspace_bytes(self.handle(), B, C, L), device)
 
 
 def _frames_alloc(B, C, M, data_format, dtype, device):
@@ -2072,10 +2060,7 @@ def chroma_cens(x, plan: ChromaPlan, in_mode, data_format=_CH_LAST_STR):
     x, xd, (B, C, M) = _chroma_input(x.detach(), plan, data_format, True)
     out, od = _spec_alloc(B, C, M, plan.n_chroma, data_format, torch.float32, x.device)
     if out.numel():
-        n = int(N.lib().kapre_chroma_cens_workspace_bytes(plan.handle(), B, C, M))
-        if n < 0:
-            N.check(n)
-        ws = torch.empty(max(n // 4, 1), dtype=torch.float32, device=x.device)
+        ws = _scratch(N.lib().kapre_chroma_cens_workspace_bytes(plan.handle(), B, C, M), x.device)
         N.check(N.lib().kapre_chroma_cens(plan.handle(), int(in_mode), _ptr(x), ctypes.byref(xd), B, C, M, _ptr(out),
                                           ctypes.byref(od), _ptr(ws), _stream_ptr()))
     return out
@@ -2090,10 +2075,7 @@ def chroma_tuning(x, plan: ChromaPlan, in_mode, data_format=_CH_LAST_STR):
     tuning = torch.empty(B, dtype=torch.float64, device=x.device)
     table = torch.empty(B, dtype=torch.int32, device=x.device)
     if B:
-        n = int(N.lib().kapre_chroma_tuning_workspace_bytes(plan.handle(), B, C, M))
-        if n < 0:
-            N.check(n)
-        ws = torch.empty(max((n + 3) // 4, 1), dtype=torch.float32, device=x.device)
+        ws = _scratch(N.lib().kapre_chroma_tuning_workspace_bytes(plan.handle(), B, C, M), x.device)
         N.check(N.lib().kapre_chroma_tuning(plan.handle(), int(in_mode), _ptr(x), ctypes.byref(xd), B, C, M,
                                             _ptr(tuning), _ptr(table), _ptr(ws), _stream_ptr()))
     return tuning, table
@@ -2169,10 +2151,7 @@ def hpss_backward(gh, gp, S, cfg, data_format):
             ds[i], _ = _spec_desc(gs[i], data_format)
     gS, gSd = _spec_alloc(B, C, T, K, data_format, S.dtype, S.device)
     if gS.numel():
-        n = int(N.lib().kapre_hpss_workspace_bytes(B, C, T, K))
-        if n < 0:
-            N.check(n)
-        ws = torch.empty(max(n // 4, 1), dtype=torch.float32, device=S.device)
+        ws = _scratch(N.lib().kapre_hpss_workspace_bytes(B, C, T, K), S.device)
         N.check(N.lib().kapre_hpss_backward(ctypes.byref(cfg), _ptr(S), int(S.is_complex()), ctypes.byref(sd), B, C, T,
                                             K, _ptr(gs[0]) if gs[0] is not None else None,
                                             ctypes.byref(ds[0]) if gs[0] is not None else None,
@@ -2273,10 +2252,7 @@ def onset_strength_backward(g, S, cfg, data_format):
     gd, _ = _frames_desc(g, data_format)
     gS, gSd = _spec_alloc(B, C, T, K, data_format, torch.float32, S.device)
     if gS.numel():
-        n = int(N.lib().kapre_onset_strength_workspace_bytes(B, C, T, K))
-        if n < 0:
-            N.check(n)
-        ws = torch.empty(max(n // 4, 1), dtype=torch.float32, device=S.device)
+        ws = _scratch(N.lib().kapre_onset_strength_workspace_bytes(B, C, T, K), S.device)
         N.check(N.lib().kapre_onset_strength_backward(ctypes.byref(cfg), _ptr(S), ctypes.byref(sd), B, C, T, K,
                                                       _ptr(g), ctypes.byref(gd), _ptr(gS), ctypes.byref(gSd),
                                                       _ptr(ws), _stream_ptr()))
@@ -2363,10 +2339,7 @@ def tempo(tg, plan: TempoPlan, per_frame=False, data_format=_CH_LAST_STR):
     if out.numel():
         ws = None
         if not per_frame:
-            n = int(N.lib().kapre_tempo_workspace_bytes(B, C, T, W))
-            if n < 0:
-                N.check(n)
-            ws = torch.empty(max(n // 8, 1), dtype=torch.float64, device=tg.device)
+            ws = _scratch(N.lib().kapre_tempo_workspace_bytes(B, C, T, W), tg.device)
         N.check(N.lib().kapre_tempo(_ptr(tg), ctypes.byref(gd), B, C, T, W, _ptr(plan.table(tg.device)),
                                     ctypes.c_double(plan.bpm_scale), int(bool(per_frame)), _ptr(out),
                                     ctypes.byref(od) if od is not None else None,
@@ -2426,10 +2399,7 @@ def beat_track(e, cfg, bpm, data_format=_CH_LAST_STR):
     if B * C and T < 1:
         raise ValueError('beat_track needs at least one frame')
     if tempo_out.numel():
-        n = int(N.lib().kapre_beat_track_workspace_bytes(B, C, T))
-        if n < 0:
-            N.check(n)
-        ws = torch.empty(max(n // 8, 1), dtype=torch.float64, device=e.device)
+        ws = _scratch(N.lib().kapre_beat_track_workspace_bytes(B, C, T), e.device)
         N.check(N.lib().kapre_beat_track(_ptr(e), ctypes.byref(ed), B, C, T, ctypes.byref(cfg),
                                          _ptr(bpm_t) if bpm_t is not None else None, ctypes.c_float(bpm_v),
                                          _ptr(tempo_out), _ptr(mask), ctypes.byref(md), _ptr(ws), _stream_ptr()))
