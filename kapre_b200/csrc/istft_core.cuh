@@ -170,7 +170,7 @@ __device__ __forceinline__ void kb_istft_cta(const KbIstftParams& p, char* smem,
                     const int fi = cl + R_ * idx;
                     const int t = tf0 + fi;
                     if (fi < TFc && t >= 0 && t < p.T) {
-                        kb_fft_dif<32>(R.v);
+                        kb_fft<32>(R.v);
                         cpx* ex = ex_s + warp * EXW + (g * Q + q) * 33;
                         const cpx* tw = twp_s + q * 33;
                         ex[0] = R.v[0];
@@ -198,7 +198,7 @@ __device__ __forceinline__ void kb_istft_cta(const KbIstftParams& p, char* smem,
                         const bool pair_ok = ((fi * H) & 1) == 0;
 #pragma unroll
                         for (int i = 0; i < FPW; ++i) {
-                            kb_fft_dif<Q>(R.v + i * Q);
+                            kb_fft<Q>(R.v + i * Q);
                             const int k1 = q + Q * i;
 #pragma unroll
                             for (int k2 = 0; k2 < Q; ++k2) {
@@ -440,7 +440,7 @@ __device__ __forceinline__ void kb_istft2_cta(const KbIstftParams& p, char* smem
                 const int fl = warp * FPW + g;
                 const int t = tfr + fl;
                 if (f_base + fl < n_need && t >= 0 && t < p.T) {
-                    kb_fft_dif<32>(R.v);
+                    kb_fft<32>(R.v);
                     cpx* ex = ex_s + warp * EXW + (g * Q + q) * 33;
                     const cpx* tw = twp_s + q * 33;
                     ex[0] = R.v[0];
@@ -477,7 +477,7 @@ __device__ __forceinline__ void kb_istft2_cta(const KbIstftParams& p, char* smem
                     const cpx* d2 = reinterpret_cast<const cpx*>(dual_s);
 #pragma unroll
                     for (int i = 0; i < FPW; ++i) {
-                        kb_fft_dif<Q>(R.v + i * Q);
+                        kb_fft<Q>(R.v + i * Q);
                         const int k1 = q + Q * i;
 #pragma unroll
                         for (int k2 = 0; k2 < Q; ++k2) {

@@ -132,6 +132,30 @@ struct KbIstftParams {
     int seg;                             // streaming kernel (kb_istft2_cta): output hops per tile
 };
 
+// Scalar steps with their rounding spelled out: on the device __fadd_rn / __fsub_rn / __fmaf_rn are never contracted
+// or reassociated by the compiler, and the host build computes the same fused multiply-add with std::fmaf.
+KB_HD float kb_add(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+KB_HD float kb_sub(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+KB_HD float kb_fma(float a, float b, float c) {
+#if defined(__CUDA_ARCH__)
+    return __fmaf_rn(a, b, c);
+#else
+    return std::fmaf(a, b, c);
+#endif
+}
+
 // Complex number = one aligned register pair.  The device forms spell out every rounding step
 // (__fmul_rn / __fadd_rn / __fmaf_rn are never contracted or reassociated by the compiler), so a complex
 // product is exactly one rounded product followed by one fused multiply-add per component.
@@ -199,14 +223,8 @@ KB_HD cpx cfma_s(cpx a, float s, cpx c) {
     return cmake(std::fmaf(a.re, s, c.re), std::fmaf(a.im, s, c.im));   // one rounding, as on the device
 #endif
 }
-// d * (c - i sn): twiddle with separately given cosine / sine (compile-time constants at the call sites)
-KB_HD cpx cmul_tw(cpx d, float c, float sn) {
-#if defined(__CUDA_ARCH__)
-    return cmake(__fmaf_rn(d.im, sn, __fmul_rn(d.re, c)), __fmaf_rn(d.re, -sn, __fmul_rn(d.im, c)));
-#else
-    return cmake(d.re * c + d.im * sn, d.im * c - d.re * sn);
-#endif
-}
+// a (.) b + c element-wise: window multiply of two packed samples folded into the addition that consumes it
+KB_HD cpx cfma_elem(cpx a, cpx b, cpx c) { return cmake(kb_fma(a.re, b.re, c.re), kb_fma(a.im, b.im, c.im)); }
 // |a|^2
 KB_HD float cnorm(cpx a) {
 #if defined(__CUDA_ARCH__)

@@ -485,42 +485,58 @@ KB_HD void kb_store_vec(float* dst, const float* src) {
 // Step 1: window the frame at `fr`, 32-point DFTs over z[q + Q j], twiddle, store transposed (32 x 33).
 //   wmode 2: cosine-sum window evaluated in registers (KbStftParams::cwq), samples read as aligned pairs
 //   wmode 1: window table, aligned pairs;  wmode 0: window table, scalar loads (odd sample offset)
-template <int Q, bool TW0 = false>
-KB_FN void kb_col_window_dft32(KbThreadRegs& R, const float* fr, const float* __restrict__ wh_s,
-                               const kb_f4* __restrict__ cwq_s, float cw_a0, const cpx* __restrict__ twp_s,
-                               cpx* region, int g, int q, int wmode) {
+// The window multiply fused into the first radix-2 pass of the FFT (kb_fft<32>, pairs j and j + 16):
+// v[j] = x[j] w[j] + x[j + 16] w[j + 16] and v[j + 16] = x[j] w[j] - x[j + 16] w[j + 16], one rounded product each.
+// Shared with the all-channel kernels (stft_mc_core.cuh), so that both compute the same bits up to the pair step.
+template <int Q>
+KB_FN void kb_col_window_pass1(KbThreadRegs& R, const float* fr, const float* __restrict__ wh_s,
+                               const kb_f4* __restrict__ cwq_s, float cw_a0, int q, int wmode) {
+    auto first_pass = [&](int j, cpx xa, cpx wa, cpx xb, cpx wb) {
+        const cpx pb = cmul_elem(xb, wb);
+        R.v[j] = cfma_elem(xa, wa, pb);
+        R.v[j + 16] = cfma_elem(xa, wa, cmake(-pb.re, -pb.im));
+    };
     if (wmode == 2) {
         // 0.5 w[2(q + Q j) + {0,1}] = a0 - cc * cos(2 pi j / 32) + ss * sin(2 pi j / 32)
         const kb_f4 cq = cwq_s[q];
         const cpx cc = cmake(cq.x, cq.y), ss = cmake(cq.z, cq.w);
         const cpx a0 = cmake(cw_a0, cw_a0);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            const int n2 = 2 * (q + Q * j);
-            const cpx xv = *reinterpret_cast<const cpx*>(fr + n2);
+        auto win = [&](int j) {
             const float cj = j <= 16 ? kb_cos32(j) : kb_cos32(32 - j);
             const float sj = j <= 16 ? kb_sin32(j) : -kb_sin32(32 - j);
             cpx wv = a0;
             if (cj != 0.0f) wv = cfma_s(cc, -cj, wv);
             if (sj != 0.0f) wv = cfma_s(ss, sj, wv);
-            R.v[j] = cmul_elem(xv, wv);
+            return wv;
+        };
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int n2 = 2 * (q + Q * j), m2 = n2 + 32 * Q;
+            first_pass(j, *reinterpret_cast<const cpx*>(fr + n2), win(j), *reinterpret_cast<const cpx*>(fr + m2), win(j + 16));
         }
     } else if (wmode == 1) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            const int n2 = 2 * (q + Q * j);
-            const cpx xv = *reinterpret_cast<const cpx*>(fr + n2);
-            const cpx wv = *reinterpret_cast<const cpx*>(wh_s + n2);
-            R.v[j] = cmul_elem(xv, wv);
+        for (int j = 0; j < 16; ++j) {
+            const int n2 = 2 * (q + Q * j), m2 = n2 + 32 * Q;
+            first_pass(j, *reinterpret_cast<const cpx*>(fr + n2), *reinterpret_cast<const cpx*>(wh_s + n2),
+                       *reinterpret_cast<const cpx*>(fr + m2), *reinterpret_cast<const cpx*>(wh_s + m2));
         }
     } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            const int n2 = 2 * (q + Q * j);
-            R.v[j] = cmake(fr[n2] * wh_s[n2], fr[n2 + 1] * wh_s[n2 + 1]);
+        for (int j = 0; j < 16; ++j) {
+            const int n2 = 2 * (q + Q * j), m2 = n2 + 32 * Q;
+            first_pass(j, cmake(fr[n2], fr[n2 + 1]), cmake(wh_s[n2], wh_s[n2 + 1]),
+                       cmake(fr[m2], fr[m2 + 1]), cmake(wh_s[m2], wh_s[m2 + 1]));
         }
     }
-    kb_fft_dif<32>(R.v);
+}
+
+template <int Q, bool TW0 = false>
+KB_FN void kb_col_window_dft32(KbThreadRegs& R, const float* fr, const float* __restrict__ wh_s,
+                               const kb_f4* __restrict__ cwq_s, float cw_a0, const cpx* __restrict__ twp_s,
+                               cpx* region, int g, int q, int wmode) {
+    kb_col_window_pass1<Q>(R, fr, wh_s, cwq_s, cw_a0, q, wmode);
+    kb_fft<32, 2>(R.v);
     cpx* ex = region + (g * Q + q) * 33;
     const cpx* tw = twp_s + q * 33;
     ex[0] = TW0 ? cmul(R.v[0], tw[0]) : R.v[0];   // TW0: spectrum shift of column 0 for the paired-column form (kb_make_twp)
@@ -548,7 +564,7 @@ KB_FN void kb_col_dftq_store(KbThreadRegs& R, cpx* region, int g, int q, int zst
     cpx* zs = region + g * zstr;
 #pragma unroll
     for (int i = 0; i < FPW; ++i) {
-        kb_fft_dif<Q>(R.v + i * Q);
+        kb_fft<Q>(R.v + i * Q);
         const int k1 = q + Q * i;
 #pragma unroll
         for (int k2 = 0; k2 < Q; ++k2) zs[k1 + 32 * k2] = R.v[i * Q + kb_brev<Q>(k2)];
@@ -595,8 +611,8 @@ KB_FN void kb_col_dftq_pair(KbThreadRegs& R, const cpx* __restrict__ twn2_s, int
     for (int u = 0; u < CP; ++u) {
         cpx* a = R.v + (2 * u) * Q;
         cpx* b = R.v + (2 * u + 1) * Q;
-        kb_fft_dif<Q>(a);
-        kb_fft_dif<Q>(b);
+        kb_fft<Q>(a);
+        kb_fft<Q>(b);
         const int r = q + Q * u;
         const bool sp = (u == 0) && (q == 0);      // the self-paired columns
         const int kLo = sp ? 16 : r;               // slot i < H:  bin kLo + 32 i
@@ -1193,13 +1209,27 @@ __device__ __forceinline__ void kb_stft_cta(const KbStftParams& p, char* smem, i
 #pragma unroll
                 for (int g = 0; g < FPW; ++g) { a0[g] = 0.0f; a1[g] = 0.0f; }
                 const int ce = cg_s[grp + 1];
-                for (int i = cg_s[grp]; i < ce; ++i) {
-                    const kb_f4 wv = cw_s[i];                             // 16 B, uniform within the group
-                    const kb_i2 mt = cm_s[i];                             // byte offsets (see the table prologue)
-                    const float* mp = reinterpret_cast<const float*>(reinterpret_cast<const char*>(mw) + mt.x);
-                    float m01[2 * FPW], m23[2 * FPW];          // bins (k, k+1) and (k+2, k+3), k even
-                    kb_load_vec<2 * FPW>(m01, mp);
-                    kb_load_vec<2 * FPW>(m23, mp + 2 * FPW);
+                // Software-pipelined one chunk ahead: the next chunk's descriptor, weights and magnitudes are loaded
+                // before this chunk's products and flush, so the loads do not wait behind the out_s stores (which the
+                // compiler may not reorder them across) and the descriptor -> address -> magnitude chain overlaps
+                // the arithmetic.  The last iteration re-reads its own chunk instead of one past the list.
+                int i = cg_s[grp];
+                kb_f4 wv;
+                kb_i2 mt;
+                float m01[2 * FPW], m23[2 * FPW];              // bins (k, k+1) and (k+2, k+3), k even
+                auto load_chunk = [&](int c, kb_f4& w4, kb_i2& d, float* v01, float* v23) {
+                    w4 = cw_s[c];                                          // 16 B, uniform within the group
+                    d = cm_s[c];                                           // byte offsets (see the table prologue)
+                    const float* mp = reinterpret_cast<const float*>(reinterpret_cast<const char*>(mw) + d.x);
+                    kb_load_vec<2 * FPW>(v01, mp);
+                    kb_load_vec<2 * FPW>(v23, mp + 2 * FPW);
+                };
+                if (i < ce) load_chunk(i, wv, mt, m01, m23);
+                for (; i < ce; ++i) {
+                    kb_f4 wn;
+                    kb_i2 mn;
+                    float n01[2 * FPW], n23[2 * FPW];
+                    load_chunk(i + 1 < ce ? i + 1 : i, wn, mn, n01, n23);
 #pragma unroll
                     for (int g = 0; g < FPW; ++g) {
                         a0[g] += wv.x * m01[g];
@@ -1216,6 +1246,10 @@ __device__ __forceinline__ void kb_stft_cta(const KbStftParams& p, char* smem, i
                             a1[g] = 0.0f;
                         }
                     }
+                    wv = wn;
+                    mt = mn;
+#pragma unroll
+                    for (int j = 0; j < 2 * FPW; ++j) { m01[j] = n01[j]; m23[j] = n23[j]; }
                 }
             KB_PHASE_END
             }

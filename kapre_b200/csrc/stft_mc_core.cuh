@@ -181,7 +181,8 @@ __device__ __forceinline__ void kb_mc_emit(const KbStftParams& p, bool dbany, vo
 }
 
 // (The three FFT steps are written out in this body rather than calling the kb_col_* helpers of
-// stft_core.cuh: with the helpers ptxas schedules the Q = 32 instantiations 11 % slower -- measured on cfg3.)
+// stft_core.cuh: with the helpers ptxas schedules the Q = 32 instantiations 11 % slower -- measured on cfg3.
+// Only the windowed first FFT pass is shared, kb_col_window_pass1, so that both kernels compute the same bits.)
 template <int Q, int MODE>
 #if defined(KB_HOST_EMU)
 inline void kb_stft_mc_cta(const KbStftParams& p, char* smem, int cta, int n_cta)
@@ -269,37 +270,8 @@ __device__ __forceinline__ void kb_stft_mc_cta(const KbStftParams& p, char* smem
                 if (col < NCOL) {
                     const int fl = kb_fdiv(col, C, p.mc_magic_c), ch = col - fl * C;
                     const float* fr = smp + ch * spanp + fl * H;
-                    if (use_cosw) {
-                        const kb_f4 cq = cwq_s[q];
-                        const cpx cc = cmake(cq.x, cq.y), ss = cmake(cq.z, cq.w);
-                        const cpx a0 = cmake(p.cw_a0, p.cw_a0);
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int n2 = 2 * (q + Q * j);
-                            const cpx xv = *reinterpret_cast<const cpx*>(fr + n2);
-                            const float cj = j <= 16 ? kb_cos32(j) : kb_cos32(32 - j);
-                            const float sj = j <= 16 ? kb_sin32(j) : -kb_sin32(32 - j);
-                            cpx wv = a0;
-                            if (cj != 0.0f) wv = cfma_s(cc, -cj, wv);
-                            if (sj != 0.0f) wv = cfma_s(ss, sj, wv);
-                            R.v[j] = cmul_elem(xv, wv);
-                        }
-                    } else if (even_base) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int n2 = 2 * (q + Q * j);
-                            const cpx xv = *reinterpret_cast<const cpx*>(fr + n2);
-                            const cpx wv = *reinterpret_cast<const cpx*>(wh_s + n2);
-                            R.v[j] = cmul_elem(xv, wv);
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int n2 = 2 * (q + Q * j);
-                            R.v[j] = cmake(fr[n2] * wh_s[n2], fr[n2 + 1] * wh_s[n2 + 1]);
-                        }
-                    }
-                    kb_fft_dif<32>(R.v);
+                    kb_col_window_pass1<Q>(R, fr, wh_s, cwq_s, p.cw_a0, q, use_cosw ? 2 : (even_base ? 1 : 0));
+                    kb_fft<32, 2>(R.v);
                     cpx* ex = ex_s + warp * EXS + (g * Q + q) * 33;
                     const cpx* tw = twp_s + q * 33;
                     ex[0] = R.v[0];
@@ -344,7 +316,7 @@ __device__ __forceinline__ void kb_stft_mc_cta(const KbStftParams& p, char* smem
                     cpx* zs = ex_s + warp * EXS + g * ZSTR;
 #pragma unroll
                     for (int i = 0; i < FPW; ++i) {
-                        kb_fft_dif<Q>(R.v + i * Q);
+                        kb_fft<Q>(R.v + i * Q);
                         const int k1 = q + Q * i;
 #pragma unroll
                         for (int k2 = 0; k2 < Q; ++k2) zs[k1 + 32 * k2] = R.v[i * Q + kb_brev<Q>(k2)];
