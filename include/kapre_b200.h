@@ -371,6 +371,36 @@ int kapre_lfilter_backward(const float* gy_dev, const kapre_wave_desc* gy_desc, 
                            const kapre_iir_coeffs* coeffs, int flags, float* gx_dev, const kapre_wave_desc* gx_desc,
                            float* partials_dev, void* workspace_dev, void* stream);
 
+/* ---- second-order-section cascades (scipy.signal.sosfilt) -------------------------------------------------------
+ * Along the time axis of every (item, channel) column, S sections in row order, each row [b0, b1, b2, a0, a1, a2]
+ * in direct form II transposed with state (z1, z2) (a0 is taken to be 1 and not read):
+ *   y_s[t] = b0 x_s[t] + z1,   z1 <- b1 x_s[t] - a1 y_s[t] + z2,   z2 <- b2 x_s[t] - a2 y_s[t],
+ * x_0 = x, x_(s+1) = y_s, y = y_(S-1).  1 <= S <= 8 (KAPRE_E_UNSUPPORTED otherwise).  Coefficients: S rows of 6
+ * consecutive floats per filter at sos + i stride_b + c stride_c; a stride of 0 shares one filter over the batch or
+ * the channels.  KAPRE_IIR_REVERSE runs the cascade in reverse time (sample t is read and written at L-1-t).
+ * The kernel is lfilter's chunked scan over the cascade's 2S-dimensional state (DESIGN.md §SOS): y[t] depends on
+ * x[0..t], the coefficients and zi alone, not on the length, the batch, the strides or broadcasting.  Four launches. */
+typedef struct {
+    const float* sos;
+    int64_t stride_b, stride_c;
+    int n_sections;
+} kapre_sos_coeffs;
+/* A (batch, channels, S, 2) float32 state in scipy's convention: (z1, z2) of section s of column (i, c) are the two
+ * consecutive floats at i stride_b + c stride_c + s stride_s.  Strides of 0 broadcast an initial state. */
+typedef struct {
+    int64_t stride_b, stride_c, stride_s;
+} kapre_sos_state_desc;
+/* Scratch of kapre_sosfilt.  < 0 on error: a negative size, n_sections outside [1, 8], or a workspace or chunk count
+ * beyond int64 / int32. */
+int64_t kapre_sosfilt_workspace_bytes(int batch, int channels, int length, int n_sections);
+/* y = sosfilt(x) from the initial state zi (NULL: zero), writing the final state to zf when zf_dev is not NULL (the
+ * state after the last sample processed, which is sample 0 with KAPRE_IIR_REVERSE; not written when length is 0).
+ * flags: 0 or KAPRE_IIR_REVERSE.  x_desc and y_desc: same batch, channels and length, any strides; y must not alias
+ * x. */
+int kapre_sosfilt(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_sos_coeffs* sos, const float* zi_dev,
+                  const kapre_sos_state_desc* zi_desc, int flags, float* y_dev, const kapre_wave_desc* y_desc,
+                  float* zf_dev, const kapre_sos_state_desc* zf_desc, void* workspace_dev, void* stream);
+
 /* ---- additive noise at a target SNR (torchaudio.functional.add_noise) -------------------------------------------
  * For every (item, channel) column of x (L samples), noise n, snr in dB and valid length len:
  *   Ex = sum_{t < len} x[t]^2,  En = sum_{t < len} n[t]^2,  s = sqrt(Ex / En) 10^(-snr / 20),  y[t] = x[t] + s n[t]

@@ -54,6 +54,14 @@ class IirCoeffs(Structure):
 IIR_CLAMP, IIR_REVERSE = 1, 2
 
 
+class SosCoeffs(Structure):
+    _fields_ = [('sos', c_void_p), ('stride_b', c_int64), ('stride_c', c_int64), ('n_sections', c_int)]
+
+
+class SosStateDesc(Structure):
+    _fields_ = [('stride_b', c_int64), ('stride_c', c_int64), ('stride_s', c_int64)]
+
+
 class NoiseSource(Structure):
     _fields_ = [('mode', c_int), ('noise', c_void_p), ('noise_desc', WaveDesc), ('bank', c_void_p),
                 ('bank_length', c_int64), ('start', c_void_p), ('clip_len', c_void_p), ('offset', c_void_p)]
@@ -220,6 +228,9 @@ SYMBOLS = [
     ('kapre_lfilter_backward', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, POINTER(WaveDesc), c_void_p,
                                        POINTER(WaveDesc), POINTER(IirCoeffs), c_int, c_void_p, POINTER(WaveDesc),
                                        c_void_p, c_void_p, c_void_p]),
+    ('kapre_sosfilt_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int]),
+    ('kapre_sosfilt', c_int, [c_void_p, POINTER(WaveDesc), POINTER(SosCoeffs), c_void_p, POINTER(SosStateDesc), c_int,
+                              c_void_p, POINTER(WaveDesc), c_void_p, POINTER(SosStateDesc), c_void_p, c_void_p]),
     ('kapre_add_noise_workspace_bytes', c_int64, [c_int, c_int, c_int]),
     ('kapre_add_noise', c_int, [c_void_p, POINTER(WaveDesc), POINTER(NoiseSource), POINTER(SnrDesc), c_void_p,
                                 POINTER(WaveDesc), c_void_p, c_void_p, c_void_p]),

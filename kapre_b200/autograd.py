@@ -24,6 +24,8 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
 * lfilter, filtfilt, IIRFilter, Biquad, RandomBiquad -> ``kapre_lfilter_backward`` (the all-pole recursion run the
   other way on the output gradient; input and normalised-coefficient gradients, the rest through torch's division
   by a0)
+* sosfilt, sosfiltfilt, SOSFilter -> ``kapre_sosfilt`` in the other time direction from a zero state (the input
+  gradient; sosfiltfilt's data-dependent initial states through the DC gain, no coefficient or zi gradient)
 * add_noise, BackgroundNoise -> ``kapre_add_noise_backward`` (a segment-sum pass over g n, then the input, noise and
   snr gradients from the saved energies)
 * loudness, Loudness, LoudnessNormalization -> ``kapre_loudness_backward`` (gL (20 / ln 10) g_c y n(t) / (E2 |J2| G)
@@ -385,6 +387,36 @@ class _Lfilter(torch.autograd.Function):
                 ga if ctx.needs_input_grad[2] else None, None, None)
 
 
+class _Sosfilt(torch.autograd.Function):
+    """A causal LTI filter's transpose is the same filter run in reverse time, so the backward is one more forward
+    launch with the reverse flag flipped, from a zero state: gx = F^T gy.  With ``scale`` the initial state is
+    ``scale * z`` for the unit-step steady state z, whose zero-input response is ``scale (H(1) 1 - F 1)``; its adjoint
+    is ``H(1) sum(gy) - sum(F^T gy)``, which needs nothing beyond gx.  zf is not differentiable."""
+
+    @staticmethod
+    def forward(ctx, x, scale, sos, zi, dc_gain, reverse, data_format, want_zf):
+        zi_eff = zi if scale is None else zi * scale.to(zi.dtype).reshape(scale.shape + (1, 1))
+        y, zf = ops.sosfilt_forward(x, sos, zi_eff, reverse, data_format, want_zf)
+        ctx.save_for_backward(sos, dc_gain)
+        ctx.cfg = (reverse, data_format)
+        if zf is None:
+            zf = y.new_empty(0)
+        ctx.mark_non_differentiable(zf)
+        return y, zf
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy, _gzf):
+        sos, dc_gain = ctx.saved_tensors
+        reverse, data_format = ctx.cfg
+        gx, _ = ops.sosfilt_forward(gy, sos, None, not reverse, data_format, False)
+        gscale = None
+        if ctx.needs_input_grad[1]:
+            t = 1 if data_format == ops._CH_LAST_STR else 2
+            gscale = (dc_gain * gy.double().sum(t) - gx.double().sum(t)).float()
+        return (gx if ctx.needs_input_grad[0] else None, gscale, None, None, None, None, None, None)
+
+
 class _AddNoise(torch.autograd.Function):
     """The forward is the plain two-launch mix, which also writes the per-column energies (Ex, En) for the backward;
     the noise is a tensor (differentiable) or a bank (a constant).  snr and the noise arrive as (B, C) / full-shape
@@ -593,6 +625,11 @@ def pcen(E, params, eps, data_format):
 
 def lfilter(x, b, a, flags, data_format):
     return _Lfilter.apply(x.float(), b, a, flags, data_format)
+
+
+def sosfilt(x, scale, sos, zi, dc_gain, reverse, data_format, want_zf):
+    y, zf = _Sosfilt.apply(x.float(), scale, sos, zi, dc_gain, reverse, data_format, want_zf)
+    return y, (zf if want_zf else None)
 
 
 def time_stretch(X, rate, data_format):

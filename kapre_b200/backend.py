@@ -263,6 +263,36 @@ def biquad_coefficients(kind: str, sample_rate, freq, Q=0.707, gain=0.0):
     return np.stack(b, -1), np.stack(a, -1)
 
 
+def sos_steady_state(sos):
+    """(zi, gain) of a second-order-section cascade ``sos`` (..., S, 6): zi (..., S, 2) is ``scipy.signal.sosfilt_zi``
+    (each section's ``lfilter_zi``, the steady state of a unit step, scaled by the DC gain of the sections before it)
+    and gain (...) the cascade's DC gain.  Float64 NumPy for host coefficients (normalised by a0, as scipy does);
+    float64 torch on the tensor's device for a tensor, with a0 taken to be 1 and no synchronisation.  Closed form per
+    biquad: with B1 = b1 - a1 b0, B2 = b2 - a2 b0, z1 = (B1 + B2) / (1 + a1 + a2) and z2 = B2 - a2 z1."""
+    import torch
+    if isinstance(sos, torch.Tensor):
+        s = sos.detach().to(torch.float64)
+        lib, stack, cat = torch, torch.stack, torch.cat
+    else:
+        s = np.asarray(sos, np.float64)
+        s = s / s[..., 3:4]
+        lib, stack, cat = np, np.stack, np.concatenate
+    b0, b1, b2, a1, a2 = (s[..., k] for k in (0, 1, 2, 4, 5))
+    den = 1.0 + a1 + a2
+    z1 = (b1 - a1 * b0 + b2 - a2 * b0) / den
+    z2 = b2 - a2 * b0 - a2 * z1
+    g = (b0 + b1 + b2) / den
+    before = lib.cumprod(cat([lib.ones_like(g[..., :1]), g[..., :-1]], -1), -1)     # DC gain ahead of each section
+    return stack([z1 * before, z2 * before], -1), lib.prod(g, -1)
+
+
+def sosfilt_zi(sos):
+    """``scipy.signal.sosfilt_zi`` restated: the (..., S, 2) initial state of ``sosfilt`` that is the steady state of a
+    unit step (``backend.sos_steady_state``).  Float64 NumPy for host coefficients, float64 torch on the device for a
+    tensor (a0 is not read; nothing synchronises)."""
+    return sos_steady_state(sos)[0]
+
+
 def k_weighting_coefficients(sample_rate):
     """The two filters of ITU-R BS.1770's K-weighting as ``torchaudio.functional.loudness`` designs them: ((b, a) of
     ``treble_biquad(sample_rate, 4.0, 1500.0, 1 / sqrt(2))``, (b, a) of ``highpass_biquad(sample_rate, 38.0, 0.5)``),

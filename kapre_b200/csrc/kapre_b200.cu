@@ -33,6 +33,7 @@
 #include "ts_core.cuh"
 #include "fbinv_core.cuh"
 #include "iir_core.cuh"
+#include "sos_core.cuh"
 #include "noise_core.cuh"
 #include "kaldi_core.cuh"
 #include "loudness_core.cuh"
@@ -3097,6 +3098,132 @@ int kapre_lfilter_backward(const float* gy_dev, const kapre_wave_desc* gy_desc, 
         p.yr = y_dev; p.yr_sb = y_desc->stride_b; p.yr_sc = y_desc->stride_c; p.yr_sl = y_desc->stride_l;
     }
     return kb_iir_launch(p, gy_dev, gy_desc, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+// ---- second-order sections (sos_core.cuh) ---------------------------------------------------------------------------
+template <int S>
+__global__ void __launch_bounds__(32) kb_sos_powers_kernel(const __grid_constant__ KbSosParams p) {
+    __shared__ double m[3 * 4 * S * S];
+    kb_sos_powers_cta<S>(p, m, (long long)blockIdx.x);
+}
+template <int S>
+__global__ void __launch_bounds__(32) kb_sos_state_kernel(const __grid_constant__ KbSosParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_sos_state_cta<S>(p, kb_smem, (long long)blockIdx.x);
+}
+template <int S>
+__global__ void __launch_bounds__(128) kb_sos_carry_kernel(const __grid_constant__ KbSosParams p) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.g.n_cols) kb_sos_carry_col<S>(p, i);
+}
+template <int S>
+__global__ void __launch_bounds__(32) kb_sos_out_kernel(const __grid_constant__ KbSosParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    kb_sos_out_cta<S>(p, kb_smem, (long long)blockIdx.x);
+}
+
+// Workspace sections: powers (one set per column at most), chunk end states, block carries, each 2S wide.
+static void kb_sos_layout(KbLayout& L, KbSosParams& p) {
+    const int D = 2 * p.S;
+    p.g.pw = L.take<double>(p.g.n_cols, KB_IIR_NPOW * D * D);
+    p.g.e = L.take<float>(p.g.n_cols, p.g.K, D);
+    p.g.blk = L.take<double>(p.g.n_cols, p.g.nblk, D);
+    L.pad();
+}
+
+static int kb_sos_check_sizes(int batch, int channels, int length, int n_sections) {
+    if (batch < 0 || channels < 0 || length < 0) return kb_fail(KAPRE_E_INVALID, "negative size");
+    if (n_sections < 1 || n_sections > KB_SOS_MAX)
+        return kb_fail(KAPRE_E_UNSUPPORTED, "%d sections: 1 to %d are supported", n_sections, KB_SOS_MAX);
+    return kb_iir_check_sizes(batch, channels, length, 0);
+}
+
+// Fills the geometry and the workspace pointers; 1: nothing to do.
+static int kb_sos_prepare(KbSosParams& p, const kapre_wave_desc* xd, const kapre_sos_coeffs* cf, void* workspace_dev) {
+    if (!xd || !cf) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_sos_check_sizes(xd->batch, xd->channels, xd->length, cf->n_sections);
+    if (rc) return rc;
+    if (cf->stride_b < 0 || cf->stride_c < 0) return kb_fail(KAPRE_E_INVALID, "coefficient strides must be >= 0");
+    p.g.B = xd->batch; p.g.C = xd->channels; p.g.L = xd->length;
+    p.g.x_sb = xd->stride_b; p.g.x_sc = xd->stride_c; p.g.x_sl = xd->stride_l;
+    p.g.ac = cf->sos; p.g.a_sb = cf->stride_b; p.g.a_sc = cf->stride_c;
+    p.S = cf->n_sections;
+    kb_iir_setup(p.g);
+    if (p.g.n_cols == 0 || p.g.L == 0) return 1;
+    if (!cf->sos) return kb_fail(KAPRE_E_INVALID, "null coefficient pointer");
+    if (!workspace_dev) return kb_fail(KAPRE_E_INVALID, "null workspace");
+    KbLayout L{(char*)workspace_dev};
+    kb_sos_layout(L, p);
+    return L.overflow ? kb_fail(KAPRE_E_INVALID, "SOS workspace overflows") : 0;
+}
+
+template <int S>
+static int kb_sos_launch_s(const KbSosParams& p, cudaStream_t st) {
+    const long long n_f = (long long)p.g.n_fb * p.g.n_fc, tiles = p.g.n_cols * p.g.nblk;
+    const int smem = kb_sos_smem(S).total;
+    int rc;
+    if ((rc = kb_launch(kb_sos_powers_kernel<S>, {.grid = (int)n_f, .block = 32, .st = st}, p))) return rc;
+    if ((rc = kb_launch(kb_sos_state_kernel<S>, {.grid = (int)tiles, .block = 32, .smem = smem, .st = st, .timed = true},
+                        p)))
+        return rc;
+    if ((rc = kb_launch(kb_sos_carry_kernel<S>, {.grid = (int)((p.g.n_cols + 127) / 128), .block = 128, .st = st}, p)))
+        return rc;
+    return kb_launch(kb_sos_out_kernel<S>, {.grid = (int)tiles, .block = 32, .smem = smem, .st = st, .timed = true}, p);
+}
+
+static int kb_sos_launch(const KbSosParams& p, cudaStream_t st) {
+    switch (p.S) {
+    case 1: return kb_sos_launch_s<1>(p, st);
+    case 2: return kb_sos_launch_s<2>(p, st);
+    case 3: return kb_sos_launch_s<3>(p, st);
+    case 4: return kb_sos_launch_s<4>(p, st);
+    case 5: return kb_sos_launch_s<5>(p, st);
+    case 6: return kb_sos_launch_s<6>(p, st);
+    case 7: return kb_sos_launch_s<7>(p, st);
+    case 8: return kb_sos_launch_s<8>(p, st);
+    }
+    return kb_fail(KAPRE_E_UNSUPPORTED, "%d sections", p.S);
+}
+
+extern "C" {
+
+int64_t kapre_sosfilt_workspace_bytes(int batch, int channels, int length, int n_sections) {
+    int rc = kb_sos_check_sizes(batch, channels, length, n_sections);
+    if (rc) return rc;
+    KbSosParams p{};
+    p.g.B = batch; p.g.C = channels; p.g.L = length;
+    p.S = n_sections;
+    kb_iir_setup(p.g);
+    KbLayout L;
+    kb_sos_layout(L, p);
+    return L.bytes("SOS");
+}
+
+int kapre_sosfilt(const float* x_dev, const kapre_wave_desc* x_desc, const kapre_sos_coeffs* sos, const float* zi_dev,
+                  const kapre_sos_state_desc* zi_desc, int flags, float* y_dev, const kapre_wave_desc* y_desc,
+                  float* zf_dev, const kapre_sos_state_desc* zf_desc, void* workspace_dev, void* stream) {
+    if (!y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    if (flags & ~KAPRE_IIR_REVERSE) return kb_fail(KAPRE_E_INVALID, "unknown flags 0x%x", flags);
+    if ((zi_dev && !zi_desc) || (zf_dev && !zf_desc)) return kb_fail(KAPRE_E_INVALID, "a state needs its descriptor");
+    if (zi_dev && (zi_desc->stride_b < 0 || zi_desc->stride_c < 0 || zi_desc->stride_s < 0))
+        return kb_fail(KAPRE_E_INVALID, "zi strides must be >= 0");
+    KbSosParams p{};
+    int rc = kb_sos_prepare(p, x_desc, sos, workspace_dev);
+    if (rc < 0) return rc;
+    if (!kb_iir_same_shape(x_desc, y_desc)) return kb_fail(KAPRE_E_INVALID, "input and output shapes differ");
+    if (rc == 1) return 0;
+    if (!x_dev || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    if ((const void*)x_dev == (const void*)y_dev) return kb_fail(KAPRE_E_INVALID, "sosfilt cannot run in place");
+    p.g.x = x_dev;
+    p.g.x_numel = kb_iir_numel(x_desc);
+    p.g.x_align = (unsigned)(((uintptr_t)x_dev >> 2) & 3u);
+    p.g.y = y_dev; p.g.y_sb = y_desc->stride_b; p.g.y_sc = y_desc->stride_c; p.g.y_sl = y_desc->stride_l;
+    p.g.reverse = (flags & KAPRE_IIR_REVERSE) ? 1 : 0;
+    if (zi_dev) { p.zi = zi_dev; p.zi_sb = zi_desc->stride_b; p.zi_sc = zi_desc->stride_c; p.zi_ss = zi_desc->stride_s; }
+    if (zf_dev) { p.zf = zf_dev; p.zf_sb = zf_desc->stride_b; p.zf_sc = zf_desc->stride_c; p.zf_ss = zf_desc->stride_s; }
+    return kb_sos_launch(p, (cudaStream_t)stream);
 }
 
 }  // extern "C"

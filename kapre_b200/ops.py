@@ -1133,6 +1133,107 @@ def lfilter(x, b, a, clamp=True, reverse=False, data_format=_CH_LAST_STR):
     return lfilter_forward(x, b, a, flags | (N.IIR_CLAMP if clamp else 0), data_format)
 
 
+SOS_MAX_SECTIONS = 8
+
+
+def _shared_axes(shape, B, C, what):
+    """(Bc, Cc) of a per-filter tensor whose leading axes are () , (ch,) or (batch, ch), each 1 (shared) or the
+    waveform's."""
+    if len(shape) == 0:
+        return 1, 1
+    Bc, Cc = (1, shape[0]) if len(shape) == 1 else shape
+    if Bc not in (1, B) or Cc not in (1, C):
+        raise ValueError('%s: batch %d and channels %d must be 1 or the waveform\'s (%d, %d)' % (what, Bc, Cc, B, C))
+    return Bc, Cc
+
+
+def sos_check(x, sos, data_format):
+    """Shapes of ``sosfilt``'s operands: x (B, L, C) / (B, C, L); sos (S, 6), (C, S, 6) or (B, C, S, 6) with axes of 1
+    shared and 1 <= S <= 8.  Returns (B, C, L), (Bc, Cc, S)."""
+    if x.dim() != 3:
+        raise ValueError('sosfilt expects a 3-D waveform batch, got shape %s' % (tuple(x.shape),))
+    B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == _CH_LAST_STR else tuple(x.shape)
+    if sos.dim() not in (2, 3, 4) or sos.shape[-1] != 6:
+        raise ValueError('sos must be (S, 6), (ch, S, 6) or (batch, ch, S, 6), got shape %s' % (tuple(sos.shape),))
+    S = sos.shape[-2]
+    if not 1 <= S <= SOS_MAX_SECTIONS:
+        raise ValueError('%d sections: 1 to %d are supported' % (S, SOS_MAX_SECTIONS))
+    Bc, Cc = _shared_axes(tuple(sos.shape[:-2]), B, C, 'sos')
+    return (B, C, L), (Bc, Cc, S)
+
+
+def sos_state_check(z, B, C, S, name):
+    """A state tensor of ``sosfilt``: (S, 2), (C, S, 2) or (B, C, S, 2) with axes of 1 shared.  Returns (Bz, Cz)."""
+    if z.dim() not in (2, 3, 4) or tuple(z.shape[-2:]) != (S, 2):
+        raise ValueError('%s must be (%d, 2), (ch, %d, 2) or (batch, ch, %d, 2), got shape %s'
+                         % (name, S, S, S, tuple(z.shape)))
+    return _shared_axes(tuple(z.shape[:-2]), B, C, name)
+
+
+def sosfilt_workspace(B, C, L, S, device):
+    return _scratch(N.lib().kapre_sosfilt_workspace_bytes(B, C, L, S), device)
+
+
+def _sos_state_desc(z):
+    """kapre_sos_state_desc of a (Bz, Cz, S, 2) tensor whose last axis is contiguous; axes of 1 get stride 0."""
+    return N.SosStateDesc(0 if z.shape[0] == 1 else z.stride(0), 0 if z.shape[1] == 1 else z.stride(1), z.stride(2))
+
+
+def sosfilt_forward(x, sos, zi, reverse, data_format, want_zf):
+    """(y, zf) = ``kapre_sosfilt`` of x with float32 coefficients sos (Bc, Cc, S, 6) and initial state zi
+    (Bz, Cz, S, 2) or None, on x's device: four launches.  zf (B, C, S, 2) is None unless ``want_zf``."""
+    x = _raw(x.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    y, yd = _wave_alloc(B, C, L, data_format, x.device)
+    S = sos.shape[2]
+    zf = torch.empty((B, C, S, 2), dtype=torch.float32, device=x.device) if want_zf else None
+    if zi is not None:
+        zi = zi.detach().to(torch.float32).contiguous()
+    if y.numel() == 0:
+        if zf is not None:
+            zf.copy_(zi.expand(B, C, S, 2) if zi is not None else torch.zeros_like(zf))
+        return y, zf
+    sos = sos.detach().to(torch.float32).contiguous()
+    cf = N.SosCoeffs(sos.data_ptr(), 0 if sos.shape[0] == 1 else sos.stride(0), 0 if sos.shape[1] == 1 else sos.stride(1),
+                     S)
+    zd = _sos_state_desc(zi) if zi is not None else None
+    fd = _sos_state_desc(zf) if zf is not None else None
+    ws = sosfilt_workspace(B, C, L, S, x.device)
+    N.check(N.lib().kapre_sosfilt(_ptr(x), ctypes.byref(xd), ctypes.byref(cf), _ptr(zi) if zi is not None else None,
+                                  ctypes.byref(zd) if zd is not None else None, N.IIR_REVERSE if reverse else 0, _ptr(y),
+                                  ctypes.byref(yd), _ptr(zf) if zf is not None else None,
+                                  ctypes.byref(fd) if fd is not None else None, _ptr(ws), _stream_ptr()))
+    return y, zf
+
+
+@_device_of_first_arg
+def sosfilt(x, sos, zi=None, scale=None, dc_gain=None, reverse=False, data_format=_CH_LAST_STR, want_zf=False):
+    """Second-order-section cascade along the time axis of x (B, L, C) / (B, C, L) with float32 coefficients sos
+    (Bc, Cc, S, 6) on x's device (a0 is not read), from the initial state zi (Bz, Cz, S, 2) or zero.  With ``scale``
+    ((B, C)) the initial state is ``zi * scale``, where zi must be the unit-step steady state of the cascade and
+    ``dc_gain`` ((Bc, Cc)) its DC gain: that is how ``sosfiltfilt`` starts, and the gradient reaches ``scale``.
+    ``reverse`` runs it in reverse time.  Returns (y, zf), zf None unless ``want_zf``; zf carries no gradient.
+    Everything is validated before any launch.  Differentiable with respect to x (and ``scale``)."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and sos.is_cuda):
+        raise N.KapreNativeError('sosfilt needs CUDA tensors')
+    if sos.device != x.device or (zi is not None and zi.device != x.device):
+        raise ValueError('waveform on %s, coefficients or state elsewhere' % (x.device,))
+    if sos.dim() != 4:
+        raise ValueError('coefficients must be 4-D (batch, channels, sections, 6)')
+    (B, C, L), (_, _, S) = sos_check(x, sos, data_format)
+    if zi is not None:
+        sos_state_check(zi, B, C, S, 'zi')
+    if torch.is_grad_enabled() and (sos.requires_grad or (zi is not None and zi.requires_grad)):
+        raise ValueError('sosfilt has no gradient with respect to sos or zi; detach them')
+    sosfilt_workspace(B, C, L, S, x.device)                 # size checks before anything is launched
+    if _wants_grad(x) or _wants_grad(scale):
+        from . import autograd
+        return autograd.sosfilt(x, scale, sos, zi, dc_gain, reverse, data_format, want_zf)
+    if scale is not None:
+        zi = zi * scale.to(zi.dtype).reshape(B, C, 1, 1)
+    return sosfilt_forward(x, sos, zi, reverse, data_format, want_zf)
+
+
 def add_noise_workspace_bytes(B, C, L):
     """``kapre_add_noise_workspace_bytes``; raises on a negative size or an overflow."""
     n = int(N.lib().kapre_add_noise_workspace_bytes(B, C, L))

@@ -5,6 +5,7 @@ kernels through the C ABI.  ``Resample`` (polyphase sample-rate conversion) has 
 reference, which expects audio to be resampled before it reaches the model; neither has ``Speed`` (speed perturbation by any
 real factor, band-limited interpolation), ``Convolve`` (convolution with long filters, partitioned FFT) or the IIR
 filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan), or
+the second-order-section cascades ``sosfilt``, ``sosfiltfilt`` and ``SOSFilter`` (scipy's, on the same scan), or
 ``add_noise`` (torchaudio's, with deterministic float64 energies), or ``loudness`` and ``Loudness`` (torchaudio's
 BS.1770 gated loudness, with per-item lengths), or the pitch trackers ``yin``, ``pyin``, ``YIN`` and ``PYIN``
 (librosa's), or the chroma features ``chroma_stft``, ``chroma_cqt``, ``chroma_cens`` and ``estimate_tuning``
@@ -22,7 +23,7 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
-           'Biquad', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
+           'Biquad', 'sosfilt', 'sosfiltfilt', 'SOSFilter', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
            'YIN', 'PYIN', 'chroma_stft', 'chroma_cqt', 'chroma_cens', 'estimate_tuning', 'hpss', 'harmonic',
            'percussive', 'onset_strength', 'onset_detect', 'tempogram', 'tempo', 'beat_track']
 
@@ -465,6 +466,166 @@ class Biquad(Layer):
         ('clamp', 'clamp'),
         ('data_format', 'data_format_str'),
     )
+
+
+def _host_sos(sos):
+    """Validated float64 host copy of second-order sections: (S, 6), (ch, S, 6) or (batch, ch, S, 6), 1 <= S <= 8,
+    finite, every a0 == 1 (as ``scipy.signal.sosfilt`` requires)."""
+    sos = np.asarray(sos, np.float64)
+    if sos.ndim not in (2, 3, 4) or sos.shape[-1] != 6:
+        raise ValueError('sos must be (S, 6), (ch, S, 6) or (batch, ch, S, 6), got shape %s' % (sos.shape,))
+    if not 1 <= sos.shape[-2] <= ops.SOS_MAX_SECTIONS:
+        raise ValueError('%d sections: 1 to %d are supported' % (sos.shape[-2], ops.SOS_MAX_SECTIONS))
+    if not np.all(np.isfinite(sos)):
+        raise ValueError('sos must be finite')
+    if np.any(sos[..., 3] != 1):
+        raise ValueError('every section must have a0 == 1 (sos[..., 3])')
+    return sos
+
+
+def _sos_tensor(x, sos, data_format):
+    """sos as a (Bc, Cc, S, 6) float32 tensor on x's device after every check (``ops.sos_check``; a0 == 1 and finite
+    values for host coefficients).  The coefficients are rounded to float32 once."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise ops.N.KapreNativeError('sosfilt needs a CUDA waveform')
+    if isinstance(sos, torch.Tensor) and sos.requires_grad and torch.is_grad_enabled():
+        raise ValueError('sosfilt has no gradient with respect to sos; detach it')
+    if isinstance(sos, torch.Tensor) and sos.is_cuda:
+        if sos.device != x.device:
+            raise ValueError('sos on %s, the waveform on %s' % (sos.device, x.device))
+        t = sos
+    else:
+        t = torch.from_numpy(_host_sos(sos.detach().cpu().numpy() if isinstance(sos, torch.Tensor) else sos))
+    _, (Bc, Cc, S) = ops.sos_check(x, t, data_format)
+    return t.to(device=x.device, dtype=torch.float32).reshape(Bc, Cc, S, 6)
+
+
+def sosfilt(waveform, sos, zi=None, data_format='default'):
+    """``scipy.signal.sosfilt`` along the time axis of ``waveform`` ``(batch, time, ch)`` / ``(batch, ch, time)`` (a CUDA
+    tensor): S second-order sections in row order, each row ``[b0, b1, b2, a0, a1, a2]`` run in direct form II
+    transposed,
+
+        y = b0 x + z1,   z1 <- b1 x - a1 y + z2,   z2 <- b2 x - a2 y,
+
+    the output of one section the input of the next.  ``sos``: ``(S, 6)`` (one filter), ``(ch, S, 6)`` or
+    ``(batch, ch, S, 6)`` with axes of 1 shared, 1 <= S <= 8 (order 16); scipy's ``output='sos'`` designs.  a0 must be
+    1: host coefficients with another a0 raise, and a0 of a CUDA tensor is not read (a check would synchronise).  The
+    coefficients are rounded to float32 once.
+
+    ``zi``: the initial state, ``(S, 2)``, ``(ch, S, 2)`` or ``(batch, ch, S, 2)`` in scipy's convention (for example
+    ``backend.sosfilt_zi(sos) * x0``); with it the call returns ``(y, zf)``, zf the ``(batch, ch, S, 2)`` float32 final
+    state, which continues the filter when passed as the next piece's ``zi``.  Without it the state starts at zero and
+    only y is returned.
+
+    Four launches (``kapre_sosfilt``): the chunked scan of ``lfilter`` over the cascade's 2S-dimensional state, so
+    sharp filters that direct form cannot hold in float32 (``butter(8, 0.05)``) stay stable, and an output depends
+    only on the input up to it, the coefficients and zi.  Differentiable with respect to the waveform (the backward is
+    the same four launches in reverse time); zf carries no gradient, and a ``sos`` or ``zi`` that requires grad
+    raises under grad mode."""
+    fmt = _resolve(_unwrap_format(data_format))
+    s = _sos_tensor(waveform, sos, fmt)
+    z = None
+    if zi is not None:
+        z = zi if isinstance(zi, torch.Tensor) else torch.from_numpy(np.asarray(zi, np.float32))
+        if torch.is_grad_enabled() and z.requires_grad:
+            raise ValueError('sosfilt has no gradient with respect to zi; detach it')
+        if z.is_cuda and z.device != waveform.device:
+            raise ValueError('zi on %s, the waveform on %s' % (z.device, waveform.device))
+        B, C = waveform.shape[0], waveform.shape[2 if fmt == _CH_LAST_STR else 1]
+        Bz, Cz = ops.sos_state_check(z, B, C, s.shape[2], 'zi')
+        z = z.to(device=waveform.device, dtype=torch.float32).reshape(Bz, Cz, s.shape[2], 2)
+    y, zf = ops.sosfilt(waveform, s, z, reverse=False, data_format=fmt, want_zf=zi is not None)
+    return (y, zf) if zi is not None else y
+
+
+SOS_PADTYPES = ('odd', 'even', 'constant', None)
+
+
+def _extend(x, n, padtype, t):
+    """scipy's odd / even / constant extension of axis t by n samples on either side, with torch ops."""
+    L = x.shape[t]
+    first, last = x.narrow(t, 0, 1), x.narrow(t, L - 1, 1)
+    left, right = x.narrow(t, 1, n).flip(t), x.narrow(t, L - 1 - n, n).flip(t)
+    if padtype == 'odd':
+        left, right = 2 * first - left, 2 * last - right
+    elif padtype == 'constant':
+        left, right = first.expand_as(left), last.expand_as(right)
+    return torch.cat([left, x, right], t)
+
+
+def sosfiltfilt(waveform, sos, padtype='odd', padlen=None, data_format='default'):
+    """``scipy.signal.sosfiltfilt``: zero-phase filtering by ``sosfilt`` forward and then in reverse time, on the
+    waveform extended at both ends.  ``padtype``: 'odd', 'even', 'constant' or None (no extension); ``padlen``
+    defaults to ``3 (2 S + 1 - min(#(b2 == 0), #(a2 == 0)))`` (for per-item or per-channel coefficients, the largest
+    over the filters; for CUDA coefficients counting reads them back, so pass ``padlen`` to avoid the
+    synchronisation).  The forward pass starts from ``sosfilt_zi(sos) * x_ext[0]``, the reverse pass from
+    ``sosfilt_zi(sos) * y[-1]``, and the extension is trimmed.  ``time <= padlen`` raises.  Arguments otherwise as
+    ``sosfilt``.
+
+    Eight launches; the reverse pass runs the kernel backwards in time, so nothing is flipped.  Differentiable with
+    respect to the waveform, through both data-dependent initial states."""
+    fmt = _resolve(_unwrap_format(data_format))
+    s = _sos_tensor(waveform, sos, fmt)
+    if padtype not in SOS_PADTYPES:
+        raise ValueError('padtype must be one of %s, got: %r' % (SOS_PADTYPES, padtype))
+    t = 1 if fmt == _CH_LAST_STR else 2
+    L = waveform.shape[t]
+    if padtype is None:
+        edge = 0
+    elif padlen is None:
+        h = s.detach().cpu() if isinstance(sos, torch.Tensor) and sos.is_cuda else np.asarray(_host_sos(
+            sos.detach().numpy() if isinstance(sos, torch.Tensor) else sos), np.float32)
+        h = np.asarray(h).reshape(-1, s.shape[2], 6)
+        taps = 2 * s.shape[2] + 1 - np.minimum((h[..., 2] == 0).sum(-1), (h[..., 5] == 0).sum(-1))
+        edge = 3 * int(taps.max())
+    else:
+        if isinstance(padlen, bool) or not isinstance(padlen, (int, np.integer)) or padlen < 0:
+            raise ValueError('padlen must be a non-negative integer, got: %r' % (padlen,))
+        edge = int(padlen)
+    if L <= edge:
+        raise ValueError('the waveform\'s length %d must be greater than padlen, which is %d' % (L, edge))
+    B, C = waveform.shape[0], waveform.shape[3 - t]
+    ops.sosfilt_workspace(B, C, L + 2 * edge, s.shape[2], waveform.device)     # size checks before any launch
+    ext = _extend(waveform, edge, padtype, t) if edge else waveform
+    zi, gain = backend.sos_steady_state(s)
+    y, _ = ops.sosfilt(ext, s, zi, scale=ext.select(t, 0), dc_gain=gain, reverse=False, data_format=fmt)
+    y, _ = ops.sosfilt(y, s, zi, scale=y.select(t, y.shape[t] - 1), dc_gain=gain, reverse=True, data_format=fmt)
+    return y.narrow(t, edge, L) if edge else y
+
+
+@register_keras_serializable(package='Kapre')
+class SOSFilter(Layer):
+    """A fixed second-order-section cascade (``sosfilt`` from a zero state): ``(batch, time, ch)`` /
+    ``(batch, ch, time)`` in, the same shape out.  ``sos``: ``(S, 6)``, ``(ch, S, 6)`` or ``(batch, ch, S, 6)`` as for
+    ``sosfilt``, 1 <= S <= 8, a0 == 1 (scipy's ``output='sos'`` designs).  The coefficients are uploaded once per
+    device as float32, so a call can be captured in a CUDA graph.  Differentiable with respect to the input."""
+
+    def __init__(self, sos, data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        self.sos = _host_sos(sos)
+        self.data_format_str = data_format
+        self.data_format = _resolve(data_format)
+        self._coeffs = {}
+
+    def coefficients(self, device):
+        """sos as a float32 tensor on ``device``, made on first use there."""
+        key = device.index if device.index is not None else torch.cuda.current_device()
+        c = self._coeffs.get(key)
+        if c is None:
+            c = self._coeffs[key] = torch.tensor(self.sos, dtype=torch.float32, device=device)
+        return c
+
+    def call(self, x):
+        if not (isinstance(x, torch.Tensor) and x.is_cuda):
+            raise ops.N.KapreNativeError('SOSFilter needs a CUDA waveform')
+        return sosfilt(x, self.coefficients(x.device), data_format=self.data_format)
+
+    def get_config(self):
+        config = super().get_config()
+        config.update({'sos': self.sos.tolist(), 'data_format': self.data_format_str})
+        return config
 
 
 def dct2_htk_matrix(n_mels: int, n_mfccs: int) -> np.ndarray:
