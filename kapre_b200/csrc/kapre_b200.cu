@@ -10,7 +10,9 @@
 #include <stdlib.h>
 #include <string.h>
 #include <atomic>
+#include <functional>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -472,16 +474,55 @@ static int kb_dev_info(DevInfo* d) {
     return 0;
 }
 
-template <typename T>
-static int kb_upload(const std::vector<T>& h, T** d) {
-    KB_CUDA(cudaMalloc((void**)d, h.size() * sizeof(T)));
-    KB_CUDA(cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return 0;
-}
+// A plan's constant device tables: one allocation, freed when the plan is deleted.
+struct KbTables {
+    void* block = nullptr;
+    KbTables() = default;
+    KbTables(const KbTables&) = delete;
+    KbTables& operator=(const KbTables&) = delete;
+    ~KbTables() { cudaFree(block); }
+};
+
+// Builds a plan's KbTables.  add() copies a host array into a staging buffer, at the offset KbLayout gives it (each
+// region on a 256-byte boundary), and keeps the plan field that is to point at it; the field of an empty array is set
+// null.  upload() pads the end to 256 bytes, so that a bulk copy which rounds a table's size up stays inside the
+// block, makes one allocation and one copy, and sets the fields.  A failed upload leaves `t` and the fields unset.
+class KbTableUpload {
+    KbLayout L;
+    std::vector<char> host;
+    std::vector<std::function<void(char*)>> fields;
+
+  public:
+    template <typename T, typename P>   // P: T or const T
+    void add(const std::vector<T>& v, P** field) {
+        static_assert(std::is_same<std::remove_const_t<P>, T>::value, "a table field points at the table's type");
+        *field = nullptr;
+        if (v.empty()) return;
+        L.pad();
+        const int64_t at = L.end;
+        L.take<T>(v.size());
+        host.resize(L.end);
+        memcpy(host.data() + at, v.data(), v.size() * sizeof(T));
+        fields.push_back([field, at](char* base) { *field = (P*)(base + at); });
+    }
+    int upload(KbTables& t, const char* what) {
+        if (host.empty()) return 0;
+        L.pad();
+        host.resize(L.end);
+        KbTables made;
+        if (cudaMalloc(&made.block, L.end) != cudaSuccess) return kb_fail(KAPRE_E_NOMEM, "%s: plan allocation", what);
+        if (cudaMemcpy(made.block, host.data(), L.end, cudaMemcpyHostToDevice) != cudaSuccess)
+            return kb_fail(KAPRE_E_CUDA, "%s: plan upload", what);
+        std::swap(t.block, made.block);
+        for (auto& set : fields) set((char*)t.block);
+        return 0;
+    }
+};
 
 struct kapre_stft_plan {
     int n_fft, win_length, hop, Q;
     DevInfo dev;
+    KbTables tables;
     float* wh = nullptr;      // fused path: 0.5 * window padded to n_fft
     kb_f4* cwq = nullptr;     // cosine-sum window factors (cosw), see KbStftParams
     int cosw = 0;
@@ -515,7 +556,7 @@ static void kb_tc_pack_b(const double* M, float* hi, float* lo) {
             }
 }
 
-static int kb_tc_tables(kapre_stft_plan* p) {
+static void kb_tc_tables(kapre_stft_plan* p, KbTableUpload& tb) {
     std::vector<double> M(1024);
     std::vector<float> f1(2048), cs(4096);
     for (int n1 = 0; n1 < 32; ++n1)
@@ -541,16 +582,13 @@ static int kb_tc_tables(kapre_stft_plan* p) {
         const double a = -2.0 * M_PI * (double)j / 32.0;
         w32[j] = make_float2((float)cos(a), (float)sin(a));
     }
-    int rc;
-    if ((rc = kb_upload(f1, &p->tc_f1)) || (rc = kb_upload(cs, &p->tc_cs)) || (rc = kb_upload(tw, &p->tc_tw)) ||
-        (rc = kb_upload(w32, &p->tc_w32)))
-        return rc;
-    return 0;
+    tb.add(f1, &p->tc_f1); tb.add(cs, &p->tc_cs); tb.add(tw, &p->tc_tw); tb.add(w32, &p->tc_w32);
 }
 
 struct kapre_istft_plan {
     int n_fft, win_length, hop, Q, win;
     DevInfo dev;
+    KbTables tables;
     float* dual = nullptr;    // fused path (kb_make_dual)
     float2* twp = nullptr;
     float2* twn = nullptr;
@@ -565,6 +603,7 @@ struct kapre_istft_plan {
 struct kapre_filterbank {
     int n_freq, n_bands, n_w;
     DevInfo dev;
+    KbTables tables;
     KbBand* bands = nullptr;   // band-major form (stand-alone ApplyFilterbank kernel)
     float* w = nullptr;
     int Q = 0;                 // chunk-list form for the fused kernel (n_freq == 32*Q + 1), else 0
@@ -878,13 +917,14 @@ int kapre_stft_plan_create(int n_fft, int win_length, int hop_length, const floa
     p->window_host.assign(window_host, window_host + win_length);
     int rc = kb_dev_info(&p->dev);
     if (rc) { delete p; return rc; }
+    KbTableUpload tb;
     if (p->Q) {
         std::vector<float> wh; std::vector<float2> twp, twn, twn2;
         double ca = 0.0, cb = 0.0;
         if (kb_fit_cosine_window(window_host, win_length, n_fft, &ca, &cb) && kb_env_int("KAPRE_B200_NOCOSW", 0) == 0) {
             std::vector<kb_f4> cwq;
             kb_make_cwq(p->Q, n_fft, cb, cwq);
-            if ((rc = kb_upload(cwq, &p->cwq))) { kapre_stft_plan_destroy(p); return rc; }
+            tb.add(cwq, &p->cwq);
             p->cosw = 1;
             p->cw_a0 = (float)(0.5 * ca);
             kb_make_wh_cosw(p->Q, p->cw_a0, cwq, wh);   // the table frames read when not windowed in registers
@@ -894,13 +934,10 @@ int kapre_stft_plan_create(int n_fft, int win_length, int hop_length, const floa
         kb_make_twp(p->Q, twp);
         kb_make_twn(n_fft, twn);
         kb_make_twn2(n_fft, twn2);
-        if ((rc = kb_upload(wh, &p->wh)) || (rc = kb_upload(twp, &p->twp)) || (rc = kb_upload(twn, &p->twn)) ||
-            (rc = kb_upload(twn2, &p->twn2))) {
-            kapre_stft_plan_destroy(p); return rc;
-        }
+        tb.add(wh, &p->wh); tb.add(twp, &p->twp); tb.add(twn, &p->twn); tb.add(twn2, &p->twn2);
         if (n_fft == 1024 && win_length == 1024 && kb_fit_cosine_window(window_host, win_length, n_fft, &ca, &cb) && ca > 0.0) {
             p->win_a = ca; p->win_b = cb;
-            if ((rc = kb_tc_tables(p))) { kapre_stft_plan_destroy(p); return rc; }
+            kb_tc_tables(p, tb);
         }
     }
     {   // generic tables are always built: they also serve sizes the fused kernel cannot take
@@ -910,16 +947,15 @@ int kapre_stft_plan_create(int n_fft, int win_length, int hop_length, const floa
             const double a = -2.0 * M_PI * (double)r / (double)n_fft;
             tw[r] = make_float2((float)cos(a), (float)sin(a));
         }
-        if ((rc = kb_upload(w, &p->w)) || (rc = kb_upload(tw, &p->tw))) { kapre_stft_plan_destroy(p); return rc; }
+        tb.add(w, &p->w); tb.add(tw, &p->tw);
     }
+    if ((rc = tb.upload(p->tables, "stft"))) { delete p; return rc; }
     *out = p;
     return 0;
 }
 
 void kapre_stft_plan_destroy(kapre_stft_plan* p) {
     if (!p) return;
-    cudaFree(p->wh); cudaFree(p->cwq); cudaFree(p->twp); cudaFree(p->twn); cudaFree(p->twn2); cudaFree(p->w); cudaFree(p->tw);
-    cudaFree(p->tc_f1); cudaFree(p->tc_cs); cudaFree(p->tc_tw); cudaFree(p->tc_w32);
     kapre_istft_plan_destroy(p->adj);
     delete p;
 }
@@ -1232,14 +1268,13 @@ int kapre_istft_plan_create(int n_fft, int win_length, int hop_length, const flo
     p->dual_host.assign(dual_window_host, dual_window_host + win_length);
     int rc = kb_dev_info(&p->dev);
     if (rc) { delete p; return rc; }
+    KbTableUpload tb;
     if (p->Q) {
         std::vector<float> dual; std::vector<float2> twp, twn;
         kb_make_dual(dual_window_host, p->win, n_fft, dual);
         kb_make_twp(p->Q, twp);
         kb_make_twn(n_fft, twn);
-        if ((rc = kb_upload(dual, &p->dual)) || (rc = kb_upload(twp, &p->twp)) || (rc = kb_upload(twn, &p->twn))) {
-            kapre_istft_plan_destroy(p); return rc;
-        }
+        tb.add(dual, &p->dual); tb.add(twp, &p->twp); tb.add(twn, &p->twn);
     }
     {
         std::vector<float> dn(p->win);
@@ -1249,15 +1284,15 @@ int kapre_istft_plan_create(int n_fft, int win_length, int hop_length, const flo
             const double a = 2.0 * M_PI * (double)r / (double)n_fft;
             tw[r] = make_float2((float)cos(a), (float)sin(a));
         }
-        if ((rc = kb_upload(dn, &p->dualn)) || (rc = kb_upload(tw, &p->tw))) { kapre_istft_plan_destroy(p); return rc; }
+        tb.add(dn, &p->dualn); tb.add(tw, &p->tw);
     }
+    if ((rc = tb.upload(p->tables, "istft"))) { delete p; return rc; }
     *out = p;
     return 0;
 }
 
 void kapre_istft_plan_destroy(kapre_istft_plan* p) {
     if (!p) return;
-    cudaFree(p->dual); cudaFree(p->twp); cudaFree(p->twn); cudaFree(p->dualn); cudaFree(p->tw);
     kapre_stft_plan_destroy(p->adj);
     delete p;
 }
@@ -1392,36 +1427,29 @@ int kapre_filterbank_create(const float* fb_host, int n_freq, int n_bands, kapre
     std::vector<KbBand> bands; std::vector<float> w;
     kb_make_bands(fb_host, n_freq, n_bands, bands, w);
     f->n_w = (int)w.size();
-    if ((rc = kb_upload(bands, &f->bands)) || (rc = kb_upload(w, &f->w))) { kapre_filterbank_destroy(f); return rc; }
+    KbTableUpload tb;
+    tb.add(bands, &f->bands); tb.add(w, &f->w);
     f->Q = kb_q_for_nfft((n_freq - 1) * 2);
     if (f->Q) {
         std::vector<kb_f4> cw; std::vector<kb_i2> cm; std::vector<int> cg;
         kb_make_fb_chunks(fb_host, n_freq, n_bands, 32, cw, cm, cg);
         f->n_chunks = (int)cw.size();
-        if ((rc = kb_upload(cw, &f->cw)) || (rc = kb_upload(cm, &f->cm)) || (rc = kb_upload(cg, &f->cg))) {
-            kapre_filterbank_destroy(f); return rc;
-        }
+        tb.add(cw, &f->cw); tb.add(cm, &f->cm); tb.add(cg, &f->cg);
         std::vector<kb_i2> bd; std::vector<int> bg;
         kb_make_fb_band_desc(cm, cg, 32, bd, bg);
         f->n_bd = (int)bd.size();
-        if ((rc = kb_upload(bd, &f->bd)) || (rc = kb_upload(bg, &f->bg))) { kapre_filterbank_destroy(f); return rc; }
+        tb.add(bd, &f->bd); tb.add(bg, &f->bg);
         std::vector<kb_f4> mw; std::vector<kb_i2> ms; std::vector<int> mg;
         kb_make_fb_mma(fb_host, n_freq, n_bands, mw, ms, mg);
         f->n_msteps = (int)ms.size();
-        if ((rc = kb_upload(mw, &f->mw)) || (rc = kb_upload(ms, &f->ms)) || (rc = kb_upload(mg, &f->mg))) {
-            kapre_filterbank_destroy(f); return rc;
-        }
+        tb.add(mw, &f->mw); tb.add(ms, &f->ms); tb.add(mg, &f->mg);
     }
+    if ((rc = tb.upload(f->tables, "filterbank"))) { delete f; return rc; }
     *out = f;
     return 0;
 }
 
-void kapre_filterbank_destroy(kapre_filterbank* f) {
-    if (!f) return;
-    cudaFree(f->bands); cudaFree(f->w); cudaFree(f->cw); cudaFree(f->cm); cudaFree(f->cg);
-    cudaFree(f->mw); cudaFree(f->ms); cudaFree(f->mg); cudaFree(f->bd); cudaFree(f->bg);
-    delete f;
-}
+void kapre_filterbank_destroy(kapre_filterbank* f) { delete f; }
 
 int kapre_apply_filterbank(const kapre_filterbank* fb, const float* x_dev, int batch, int channels, int frames,
                            const kapre_spec_desc* xd, float* out_dev, const kapre_spec_desc* od, void* stream) {
@@ -1599,9 +1627,12 @@ int kapre_tc_dft_stage1(const float* x_dev, int n_items, long long item_stride, 
     DevInfo dev;
     int rc = kb_dev_info(&dev);
     if (rc) return rc;
-    static float* d_fmat[64] = {nullptr};
+    // one matrix per device, kept for the life of the process (never freed: a static KbTables would call cudaFree
+    // at exit, when the CUDA runtime may already be gone)
+    static KbTables* const fmat = new KbTables[64];
     if (dev.device < 0 || dev.device >= 64) return kb_fail(KAPRE_E_UNSUPPORTED, "device index");
-    if (!d_fmat[dev.device]) {
+    KbTables& t = fmat[dev.device];
+    if (!t.block) {
         std::vector<float> f(2048);
         for (int kc = 0; kc < 8; ++kc)
             for (int c = 0; c < 32; ++c)
@@ -1617,13 +1648,16 @@ int kapre_tc_dft_stage1(const float* x_dev, int n_items, long long item_stride, 
                     f[(size_t)(kc * 32 + c) * 4 + e] = hi;
                     f[1024 + (size_t)(kc * 32 + c) * 4 + e] = w - hi;
                 }
-        if ((rc = kb_upload(f, &d_fmat[dev.device]))) return rc;
+        KbTableUpload tb;
+        const float* m;   // the block's one table, at its start
+        tb.add(f, &m);
+        if ((rc = tb.upload(t, "tc_dft"))) return rc;
     }
     KbTcParams p{};
     p.x = x_dev; p.item_stride = item_stride; p.n_items = n_items; p.length = length;
     p.T = 1 + (length - KB_TC_NFFT) / KB_TC_HOP;
     p.out = out_dev; p.store = store;
-    p.fmat = fmat_override_dev ? fmat_override_dev : d_fmat[dev.device];   // override: layout debugging (2048 floats)
+    p.fmat = fmat_override_dev ? fmat_override_dev : (const float*)t.block;   // override: layout debugging (2048 floats)
     p.n_tiles_t = (p.T + KB_TC_TILE_F - 1) / KB_TC_TILE_F;
     const long long tiles = (long long)n_items * p.n_tiles_t;
     const long long gmax = (long long)dev.sm_count * 2;
@@ -2001,6 +2035,7 @@ struct kapre_resample_plan {
     int up, down, n_taps, hl, f, Kp;
     int symmetric;
     DevInfo dev;
+    KbTables tables;
     float* tab = nullptr;       // up rows of Kp taps, gain folded in (resample_core.cuh)
     std::vector<float> taps_host;
     // adjoint (kapre_resample_backward): up and down exchanged, gain up; made on first use
@@ -2027,13 +2062,15 @@ static int kb_resample_plan_build(int up, int down, const float* taps, int n_tap
     if (rc) { delete p; return rc; }
     if (kb_resample_smem(up, p->Kp, 1, down, 1) > p->dev.smem_optin) {
         const int need = up * p->Kp * 4;
-        kapre_resample_plan_destroy(p);
+        delete p;
         return kb_fail(KAPRE_E_UNSUPPORTED, "resampling table of %d x %d taps (%d B) does not fit in shared memory", up,
                        need / 4 / up, need);
     }
     std::vector<float> tab;
     kb_resample_table(up, down, taps, n_taps, gain, tab);
-    if ((rc = kb_upload(tab, &p->tab))) { kapre_resample_plan_destroy(p); return rc; }
+    KbTableUpload tb;
+    tb.add(tab, &p->tab);
+    if ((rc = tb.upload(p->tables, "resample"))) { delete p; return rc; }
     *out = p;
     return 0;
 }
@@ -2056,10 +2093,8 @@ static int kb_resample_launch(const kapre_resample_plan* plan, const float* x_de
     if ((long long)yd->batch * yd->channels * yd->length == 0) return 0;
     if (!x_dev || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     if ((const void*)x_dev == (const void*)y_dev) return kb_fail(KAPRE_E_INVALID, "resampling cannot run in place");
-    int cur = -1;
-    KB_CUDA(cudaGetDevice(&cur));
-    if (cur != plan->dev.device)
-        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
     KbResampleParams p{};
     const int B = xd->batch, C = xd->channels;
     p.x = x_dev; p.x_sb = xd->stride_b; p.x_sc = xd->stride_c; p.x_sl = xd->stride_l;
@@ -2081,7 +2116,7 @@ static int kb_resample_launch(const kapre_resample_plan* plan, const float* x_de
         return kb_fail(KAPRE_E_UNSUPPORTED, "%d channels of a %d:%d resampler do not fit in shared memory", p.G, plan->up, plan->down);
     if (!kb_resample_setup(p, KB_RESAMPLE_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
     const int smem = kb_resample_smem(p.up, p.Kp, p.NT, p.down, p.G);
-    int grid, rc;
+    int grid;
     if ((rc = kb_resident_grid(kb_resample_kernel, "resample", KB_RESAMPLE_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
         return rc;
     return kb_launch(kb_resample_kernel, {.grid = grid, .block = KB_RESAMPLE_THREADS, .smem = smem,
@@ -2105,7 +2140,6 @@ int kapre_resample_plan_create(int up, int down, const float* taps_host, int n_t
 
 void kapre_resample_plan_destroy(kapre_resample_plan* p) {
     if (!p) return;
-    cudaFree(p->tab);
     kapre_resample_plan_destroy(p->adj);
     delete p;
 }
@@ -2123,6 +2157,9 @@ int kapre_resample(const kapre_resample_plan* plan, const float* x_dev, const ka
 int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev, const kapre_wave_desc* g_desc,
                             float* gx_dev, const kapre_wave_desc* gx_desc, void* stream) {
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null argument");
+    // before the adjoint is made: it is made on the current device
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
     if (!plan->symmetric) return kb_fail(KAPRE_E_UNSUPPORTED, "the resampling backward pass needs a symmetric filter");
     kapre_resample_plan* p = const_cast<kapre_resample_plan*>(plan);
     kapre_resample_plan* adj;
@@ -2130,7 +2167,7 @@ int kapre_resample_backward(const kapre_resample_plan* plan, const float* g_dev,
         std::lock_guard<std::mutex> lk(p->adj_mu);
         if (!p->adj) {
             // A^T g = (up / down) resample(g; down, up): gain down of the exchanged plan times up / down
-            int rc = kb_resample_plan_build(p->down, p->up, p->taps_host.data(), p->n_taps, (double)p->up, &p->adj);
+            rc = kb_resample_plan_build(p->down, p->up, p->taps_host.data(), p->n_taps, (double)p->up, &p->adj);
             if (rc) { p->adj = nullptr; return rc; }
         }
         adj = p->adj;
@@ -2148,6 +2185,7 @@ __global__ void __launch_bounds__(KB_SINC_THREADS, 2) kb_sinc_resample_kernel(co
 
 struct kapre_sinc_plan {
     DevInfo dev;
+    KbTables tables;
     float2* tab = nullptr;      // KB_SINC_NTAB pairs (h, forward difference)
     double integral = 1.0;      // I
 };
@@ -2176,10 +2214,8 @@ static int kb_sinc_launch(const kapre_sinc_plan* plan, const float* x_dev, const
     if ((long long)yd->batch * yd->channels * yd->length == 0) return 0;
     if ((!x_dev && xd->length > 0) || !y_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     if ((const void*)x_dev == (const void*)y_dev) return kb_fail(KAPRE_E_INVALID, "interpolation cannot run in place");
-    int cur = -1;
-    KB_CUDA(cudaGetDevice(&cur));
-    if (cur != plan->dev.device)
-        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
     double step, off, s, gain;
     kb_sinc_args(ratio, offset, adjoint, &step, &off, &s, &gain);
     KbSincParams p{};
@@ -2204,7 +2240,7 @@ static int kb_sinc_launch(const kapre_sinc_plan* plan, const float* x_dev, const
         return kb_fail(KAPRE_E_UNSUPPORTED, "%d interleaved channels at ratio %g do not fit in shared memory", p.G, ratio);
     if (!kb_sinc_setup(p, step, off, s, gain, plan->integral, KB_SINC_THREADS)) return kb_fail(KAPRE_E_UNSUPPORTED, "too many tiles");
     const int smem = kb_sinc_smem(p.NT, step, p.nw, p.G);
-    int grid, rc;
+    int grid;
     if ((rc = kb_resident_grid(kb_sinc_resample_kernel, "sinc", KB_SINC_THREADS, smem, p.n_tiles, plan->dev.sm_count, &grid)))
         return rc;
     return kb_launch(kb_sinc_resample_kernel, {.grid = grid, .block = KB_SINC_THREADS, .smem = smem,
@@ -2225,16 +2261,14 @@ int kapre_sinc_plan_create(kapre_sinc_plan** out) {
     std::vector<float2> tab;
     kb_sinc_table(tab);
     p->integral = kb_sinc_integral();
-    if ((rc = kb_upload(tab, &p->tab))) { kapre_sinc_plan_destroy(p); return rc; }
+    KbTableUpload tb;
+    tb.add(tab, &p->tab);
+    if ((rc = tb.upload(p->tables, "sinc"))) { delete p; return rc; }
     *out = p;
     return 0;
 }
 
-void kapre_sinc_plan_destroy(kapre_sinc_plan* p) {
-    if (!p) return;
-    cudaFree(p->tab);
-    delete p;
-}
+void kapre_sinc_plan_destroy(kapre_sinc_plan* p) { delete p; }
 
 int kapre_sinc_resample(const kapre_sinc_plan* plan, const float* x_dev, const kapre_wave_desc* x_desc, float* y_dev,
                         const kapre_wave_desc* y_desc, double ratio, double offset, void* stream) {
@@ -2870,6 +2904,7 @@ __global__ void __launch_bounds__(KB_FBI_WARPS * 32, 1) kb_fbi_kernel(const __gr
 struct kapre_fb_inverse_plan {
     int n_freq, n_bands;
     DevInfo dev;
+    KbTables tables;
     float step = 0.0f;
     KbBand* bands = nullptr;
     float* w = nullptr;
@@ -2890,20 +2925,15 @@ int kapre_fb_inverse_plan_create(const float* fb_host, int n_freq, int n_bands, 
     KbFbiTables t;
     kb_fbi_make_tables(fb_host, n_freq, n_bands, t);
     f->step = t.step;
-    if ((rc = kb_upload(t.bands, &f->bands)) || (rc = kb_upload(t.w, &f->w)) || (rc = kb_upload(t.cptr, &f->cptr)) ||
-        (rc = kb_upload(t.cols, &f->cols)) || (rc = kb_upload(t.inv_d, &f->inv_d))) {
-        kapre_fb_inverse_plan_destroy(f);
-        return rc;
-    }
+    KbTableUpload tb;
+    tb.add(t.bands, &f->bands); tb.add(t.w, &f->w); tb.add(t.cptr, &f->cptr); tb.add(t.cols, &f->cols);
+    tb.add(t.inv_d, &f->inv_d);
+    if ((rc = tb.upload(f->tables, "fb_inverse"))) { delete f; return rc; }
     *out = f;
     return 0;
 }
 
-void kapre_fb_inverse_plan_destroy(kapre_fb_inverse_plan* f) {
-    if (!f) return;
-    cudaFree(f->bands); cudaFree(f->w); cudaFree(f->cptr); cudaFree(f->cols); cudaFree(f->inv_d);
-    delete f;
-}
+void kapre_fb_inverse_plan_destroy(kapre_fb_inverse_plan* f) { delete f; }
 
 int kapre_filterbank_invert(const kapre_fb_inverse_plan* plan, const kapre_fb_inverse_cfg* cfg, const float* x_dev,
                             int batch, int channels, int frames, const kapre_spec_desc* x_desc, float* out_dev,
@@ -3421,23 +3451,12 @@ struct kapre_kaldi_plan {
     kapre_kaldi_config cfg;
     int Q, K, P;
     DevInfo dev;
-    void* block = nullptr;                          // every table in one allocation
+    KbTables tables;
     const float* wh; const float* half; const float2* twp; const float2* twn;
     const int* mlo; const int* mlen; const int* moff; const float* mw;
     const int* klo; const int* klen; const int* kidx; const float* kw;
     const float* dct;
 };
-
-// The plan's tables in its one device block.  With a null base only measures.
-static void kb_kaldi_table_layout(KbLayout& L, const KbKaldiTables& t, kapre_kaldi_plan* pl) {
-    pl->wh = L.take<float>(t.wh.size()); pl->half = L.take<float>(t.half.size());
-    pl->twp = L.take<float2>(t.twp.size()); pl->twn = L.take<float2>(t.twn.size());
-    pl->mlo = L.take<int>(t.mlo.size()); pl->mlen = L.take<int>(t.mlen.size()); pl->moff = L.take<int>(t.moff.size());
-    pl->mw = L.take<float>(t.mw.size());
-    pl->klo = L.take<int>(t.klo.size()); pl->klen = L.take<int>(t.klen.size()); pl->kidx = L.take<int>(t.kidx.size());
-    pl->kw = L.take<float>(t.kw.size());
-    pl->dct = L.take<float>(t.dct.size());
-}
 
 // The backward workspace: the per-frame gradients gf, then the mean-subtracted output gradient gc (empty without mean
 // subtraction).
@@ -3503,6 +3522,8 @@ static KbKaldiParams kb_kaldi_params(const kapre_kaldi_plan* pl) {
 static int kb_kaldi_prepare(KbKaldiParams& p, const kapre_kaldi_plan* pl, const kapre_wave_desc* xd,
                             const int32_t* len_h, const int32_t* len_d, int frames, float dither, uint64_t seed) {
     if (!pl || !xd) return kb_fail(KAPRE_E_INVALID, "null argument");
+    int rc = kb_check_device(pl->dev);
+    if (rc) return rc;
     if (xd->batch < 0 || xd->channels < 0 || xd->length < 0)
         return kb_fail(KAPRE_E_INVALID, "kaldi: negative size (%d, %d, %d)", xd->batch, xd->channels, xd->length);
     if (!kb_finite(dither) || dither < 0.0f) return kb_fail(KAPRE_E_INVALID, "kaldi: dither must be finite and >= 0");
@@ -3581,33 +3602,17 @@ int kapre_kaldi_plan_create(const kapre_kaldi_config* cfg, const float* window_h
     pl->K = cfg->kind == KAPRE_KALDI_FBANK ? M + cfg->use_energy
           : cfg->kind == KAPRE_KALDI_MFCC ? cfg->num_ceps : P + 1;
     if ((rc = kb_dev_info(&pl->dev))) { delete pl; return rc; }
-    KbLayout size;
-    kb_kaldi_table_layout(size, t, pl);
-    if (cudaMalloc(&pl->block, size.end) != cudaSuccess) { delete pl; return kb_fail(KAPRE_E_NOMEM, "kaldi: plan allocation"); }
-    KbLayout L{(char*)pl->block};
-    kb_kaldi_table_layout(L, t, pl);
-    // staged on the host at the same offsets, then one upload
-    std::vector<char> host(size.end, 0);
-    auto put = [&](const void* dev, const auto& v) {
-        memcpy(host.data() + ((const char*)dev - L.base), v.data(), v.size() * sizeof(v[0]));
-    };
-    put(pl->wh, t.wh); put(pl->half, t.half); put(pl->twp, t.twp); put(pl->twn, t.twn);
-    put(pl->mlo, t.mlo); put(pl->mlen, t.mlen); put(pl->moff, t.moff); put(pl->mw, t.mw);
-    put(pl->klo, t.klo); put(pl->klen, t.klen); put(pl->kidx, t.kidx); put(pl->kw, t.kw);
-    put(pl->dct, t.dct);
-    if (cudaMemcpy(pl->block, host.data(), size.end, cudaMemcpyHostToDevice) != cudaSuccess) {
-        cudaFree(pl->block); delete pl;
-        return kb_fail(KAPRE_E_CUDA, "kaldi: plan upload");
-    }
+    KbTableUpload tb;
+    tb.add(t.wh, &pl->wh); tb.add(t.half, &pl->half); tb.add(t.twp, &pl->twp); tb.add(t.twn, &pl->twn);
+    tb.add(t.mlo, &pl->mlo); tb.add(t.mlen, &pl->mlen); tb.add(t.moff, &pl->moff); tb.add(t.mw, &pl->mw);
+    tb.add(t.klo, &pl->klo); tb.add(t.klen, &pl->klen); tb.add(t.kidx, &pl->kidx); tb.add(t.kw, &pl->kw);
+    tb.add(t.dct, &pl->dct);
+    if ((rc = tb.upload(pl->tables, "kaldi"))) { delete pl; return rc; }
     *out = pl;
     return 0;
 }
 
-void kapre_kaldi_plan_destroy(kapre_kaldi_plan* plan) {
-    if (!plan) return;
-    cudaFree(plan->block);
-    delete plan;
-}
+void kapre_kaldi_plan_destroy(kapre_kaldi_plan* plan) { delete plan; }
 
 int kapre_kaldi_num_frames(const kapre_kaldi_plan* plan, int length) {
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
@@ -3815,6 +3820,7 @@ struct kapre_cqt_plan {
     kapre_cqt_config cfg;
     KbCqtParams geo;                        // octaves and segments (per-call fields unset)
     DevInfo dev;
+    KbTables tables;
     float2* tab = nullptr;
     float2* btab = nullptr;
     kapre_resample_plan* rs = nullptr;      // the 2:1 decimator
@@ -3848,11 +3854,7 @@ static int kb_cqt_check_shape(const kapre_cqt_plan* plan, const kapre_wave_desc*
         return kb_fail(KAPRE_E_INVALID, "cqt: negative size (%d, %d, %d)", xd->batch, xd->channels, xd->length);
     if ((double)xd->batch * xd->channels * (xd->length + 1.0) * 3.0 > 4.0e18)
         return kb_fail(KAPRE_E_INVALID, "cqt: size overflow");
-    int cur = -1;
-    KB_CUDA(cudaGetDevice(&cur));
-    if (cur != plan->dev.device)
-        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
-    return 0;
+    return kb_check_device(plan->dev);
 }
 
 // Common fields: levels (level 0 = x, the others contiguous (B, C, L_i) in the workspace) and sizes.
@@ -3914,9 +3916,11 @@ int kapre_cqt_plan_create(const kapre_cqt_config* cfg, const float* taps_host, c
     }
     for (const float2& v : tab)
         if (!std::isfinite(v.x) || !std::isfinite(v.y)) { delete pl; return kb_fail(KAPRE_E_INVALID, "cqt: non-finite tap"); }
-    if ((rc = kb_dev_info(&pl->dev)) || (rc = kb_upload(tab, &pl->tab)) || (rc = kb_upload(btab, &pl->btab)) ||
+    KbTableUpload tb;
+    tb.add(tab, &pl->tab); tb.add(btab, &pl->btab);
+    if ((rc = kb_dev_info(&pl->dev)) || (rc = tb.upload(pl->tables, "cqt")) ||
         (rc = kapre_resample_plan_create(1, 2, decim_taps_host, n_decim_taps, &pl->rs))) {
-        kapre_cqt_plan_destroy(pl);
+        delete pl;
         return rc;
     }
     *out = pl;
@@ -3925,8 +3929,6 @@ int kapre_cqt_plan_create(const kapre_cqt_config* cfg, const float* taps_host, c
 
 void kapre_cqt_plan_destroy(kapre_cqt_plan* plan) {
     if (!plan) return;
-    cudaFree(plan->tab);
-    cudaFree(plan->btab);
     kapre_resample_plan_destroy(plan->rs);
     delete plan;
 }
@@ -4047,21 +4049,19 @@ struct kapre_pitch_plan {
     KbPitchParams geo;                      // tiling and tables (per-call fields unset)
     KbVitParams vit;
     DevInfo dev;
-    std::vector<void*> bufs;                // device tables
+    KbTables tables;
 };
 
+// One pYIN table, converted to T and checked finite after the conversion.
 template <typename T>
-static int kb_pitch_upload(kapre_pitch_plan* pl, const double* src, size_t n, const T** dst) {
+static int kb_pitch_table(KbTableUpload& tb, const double* src, size_t n, const T** dst) {
     std::vector<T> h(n);
     for (size_t i = 0; i < n; ++i) {
         h[i] = (T)src[i];
         if (!std::isfinite((double)h[i])) return kb_fail(KAPRE_E_INVALID, "pitch: non-finite table entry");
     }
-    T* d = nullptr;
-    int rc = kb_upload(h, &d);
-    if (d) pl->bufs.push_back(d);
-    *dst = d;
-    return rc;
+    tb.add(h, dst);
+    return 0;
 }
 
 static int kb_pitch_frames(const kapre_pitch_config& c, long long length) {
@@ -4073,11 +4073,7 @@ static int kb_pitch_check_shape(const kapre_pitch_plan* plan, const kapre_wave_d
     if (!plan || !xd) return kb_fail(KAPRE_E_INVALID, "null argument");
     if (xd->batch < 0 || xd->channels < 0 || xd->length < 0)
         return kb_fail(KAPRE_E_INVALID, "pitch: negative size (%d, %d, %d)", xd->batch, xd->channels, xd->length);
-    int cur = -1;
-    KB_CUDA(cudaGetDevice(&cur));
-    if (cur != plan->dev.device)
-        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
-    return 0;
+    return kb_check_device(plan->dev);
 }
 
 // The pYIN workspace: per frame the candidate count, probabilities and pitch bins, then the Viterbi back-pointers.
@@ -4159,6 +4155,7 @@ int kapre_pitch_plan_create(const kapre_pitch_config* cfg, const kapre_pitch_tab
         delete pl;
         return kb_fail(KAPRE_E_UNSUPPORTED, "pitch: one frame does not fit the kernel's shared memory");
     }
+    KbTableUpload tb;
     int rc = kb_dev_info(&pl->dev);
     if (!rc && g.smem > pl->dev.smem_optin) rc = kb_fail(KAPRE_E_UNSUPPORTED, "pitch: %d B of shared memory", g.smem);
     if (!rc && tab) {
@@ -4176,28 +4173,25 @@ int kapre_pitch_plan_create(const kapre_pitch_config* cfg, const kapre_pitch_tab
         const double* edges = tab->period_edges;
         std::vector<double> one(1, 0.0);
         if (c.n_pitch == 1) edges = one.data();
-        if (!rc) rc = kb_pitch_upload<float>(pl, tab->beta_probs, c.n_thresholds, &g.beta);
-        if (!rc) rc = kb_pitch_upload<float>(pl, tab->boltzmann_pow, g.cmax + 1, &g.bpow);
-        if (!rc) rc = kb_pitch_upload<float>(pl, tab->boltzmann_norm, g.cmax + 1, &g.bnorm);
-        if (!rc) rc = kb_pitch_upload<float>(pl, tab->no_trough_bonus, c.n_thresholds + 1, &g.bonus);
-        if (!rc) rc = kb_pitch_upload<double>(pl, edges, c.n_pitch > 1 ? c.n_pitch - 1 : 1, &g.edges);
-        if (!rc) rc = kb_pitch_upload<float>(pl, tab->freqs, c.n_pitch, &v.freq);
-        if (!rc) rc = kb_pitch_upload<float>(pl, tab->log_triangle, c.band_width, &v.ltri);
-        if (!rc) rc = kb_pitch_upload<float>(pl, tab->log_row_norm, c.n_pitch, &v.lnorm);
+        if (!rc) rc = kb_pitch_table<float>(tb, tab->beta_probs, c.n_thresholds, &g.beta);
+        if (!rc) rc = kb_pitch_table<float>(tb, tab->boltzmann_pow, g.cmax + 1, &g.bpow);
+        if (!rc) rc = kb_pitch_table<float>(tb, tab->boltzmann_norm, g.cmax + 1, &g.bnorm);
+        if (!rc) rc = kb_pitch_table<float>(tb, tab->no_trough_bonus, c.n_thresholds + 1, &g.bonus);
+        if (!rc) rc = kb_pitch_table<double>(tb, edges, c.n_pitch > 1 ? c.n_pitch - 1 : 1, &g.edges);
+        if (!rc) rc = kb_pitch_table<float>(tb, tab->freqs, c.n_pitch, &v.freq);
+        if (!rc) rc = kb_pitch_table<float>(tb, tab->log_triangle, c.band_width, &v.ltri);
+        if (!rc) rc = kb_pitch_table<float>(tb, tab->log_row_norm, c.n_pitch, &v.lnorm);
     }
+    if (!rc) rc = tb.upload(pl->tables, "pitch");
     if (rc) {
-        kapre_pitch_plan_destroy(pl);
+        delete pl;
         return rc;
     }
     *out = pl;
     return 0;
 }
 
-void kapre_pitch_plan_destroy(kapre_pitch_plan* plan) {
-    if (!plan) return;
-    for (void* b : plan->bufs) cudaFree(b);
-    delete plan;
-}
+void kapre_pitch_plan_destroy(kapre_pitch_plan* plan) { delete plan; }
 
 int kapre_pitch_num_frames(const kapre_pitch_plan* plan, int length) {
     if (!plan) return kb_fail(KAPRE_E_INVALID, "null plan");
@@ -4296,6 +4290,7 @@ __global__ void __launch_bounds__(KB_CH_THREADS) kb_cens_kernel(const __grid_con
 struct kapre_chroma_plan {
     kapre_chroma_plan_desc d;
     DevInfo dev;
+    KbTables tables;
     float* W = nullptr;                   // n_tables x n_chroma x n_bins
     float* smooth = nullptr;
     double* edges = nullptr;
@@ -4305,10 +4300,8 @@ static int kb_chroma_check(const kapre_chroma_plan* plan, const void* x, const k
                            const void* out, const kapre_spec_desc* od) {
     if (!plan || !xd || !od) return kb_fail(KAPRE_E_INVALID, "null argument");
     if (B < 0 || C < 0 || M < 0) return kb_fail(KAPRE_E_INVALID, "chroma: negative size (%d, %d, %d)", B, C, M);
-    int cur = -1;
-    KB_CUDA(cudaGetDevice(&cur));
-    if (cur != plan->dev.device)
-        return kb_fail(KAPRE_E_INVALID, "plan was created on device %d but device %d is current", plan->dev.device, cur);
+    const int rc = kb_check_device(plan->dev);
+    if (rc) return rc;
     if ((long long)B * C * M && (!x || !out)) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     return 0;
 }
@@ -4377,36 +4370,25 @@ int kapre_chroma_plan_create(const kapre_chroma_plan_desc* desc, kapre_chroma_pl
     kapre_chroma_plan* pl = new kapre_chroma_plan();
     pl->d = d;
     pl->d.tables = nullptr; pl->d.smooth = nullptr; pl->d.tuning_edges = nullptr;
-    int rc = kb_dev_info(&pl->dev);
-    if (!rc && d.n_tables) {
+    KbTableUpload tb;
+    if (d.n_tables) {
         const size_t n = (size_t)d.n_tables * d.n_chroma * d.n_bins;
         std::vector<float> h(n);
         for (size_t i = 0; i < n; ++i) h[i] = (float)d.tables[i];
-        rc = kb_upload(h, &pl->W);
+        tb.add(h, &pl->W);
     }
-    if (!rc && d.n_smooth) {
-        std::vector<float> h(d.smooth, d.smooth + d.n_smooth);
-        rc = kb_upload(h, &pl->smooth);
-    }
-    if (!rc && d.n_tuning_bins) {
-        std::vector<double> h(d.tuning_edges, d.tuning_edges + d.n_tuning_bins + 1);
-        rc = kb_upload(h, &pl->edges);
-    }
-    if (rc) {
-        kapre_chroma_plan_destroy(pl);
+    if (d.n_smooth) tb.add(std::vector<float>(d.smooth, d.smooth + d.n_smooth), &pl->smooth);
+    if (d.n_tuning_bins) tb.add(std::vector<double>(d.tuning_edges, d.tuning_edges + d.n_tuning_bins + 1), &pl->edges);
+    int rc;
+    if ((rc = kb_dev_info(&pl->dev)) || (rc = tb.upload(pl->tables, "chroma"))) {
+        delete pl;
         return rc;
     }
     *out = pl;
     return 0;
 }
 
-void kapre_chroma_plan_destroy(kapre_chroma_plan* plan) {
-    if (!plan) return;
-    cudaFree(plan->W);
-    cudaFree(plan->smooth);
-    cudaFree(plan->edges);
-    delete plan;
-}
+void kapre_chroma_plan_destroy(kapre_chroma_plan* plan) { delete plan; }
 
 int kapre_chroma(const kapre_chroma_plan* plan, const kapre_chroma_config* cfg, const void* x_dev,
                  const kapre_spec_desc* x_desc, int batch, int channels, int frames, const int* table_dev, float* out_dev,
