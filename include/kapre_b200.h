@@ -479,6 +479,36 @@ int kapre_loudness_backward(const float* gl_dev, const float* y_dev, const kapre
                             const int32_t* lengths_dev, int gate, int step, const void* stats_dev, float* gy_dev,
                             const kapre_wave_desc* gy_desc, void* stream);
 
+/* ---- loudness meter: series, loudness range and true peak (EBU R128, EBU Tech 3341 / 3342, ITU-R BS.1770-4) -----
+ * kapre_loudness_stats runs on the K-weighted signal y as kapre_loudness does (same lengths rule, channels <= 5), and
+ * writes per item: the integrated loudness (kapre_loudness's two passes, so bit for bit its result); the momentary
+ * series (batch, Jm) with Jm = (length - gate) / step + 1 (0 when length < gate) and the short-term series
+ * (batch, Js) with gate3 in place of gate, both row-major: entry j is -0.691 + 10 log10(E_j) over the window
+ * [j step, j step + window), E_j the channel-weighted mean square, and -inf for j at or past the item's own window
+ * count; and the loudness range (EBU Tech 3342) of the short-term windows: J1 = {s_j > -70}, Gamma = -0.691 +
+ * 10 log10(mean_J1 E_j) - 20, J2 = {j in J1 : s_j > Gamma}, n = |J2|, v the ascending s of J2,
+ * LRA = v[((n-1) 95 + 50) / 100] - v[((n-1) 10 + 50) / 100] (0 when n = 0), float64 and rounded once.  A non-finite
+ * window energy makes that item's entries and LRA NaN.  Six launches (two when length < gate). */
+/* Scratch of kapre_loudness_stats; < 0 on a bad size (as kapre_loudness, and gate3 < gate) or an overflow. */
+int64_t kapre_loudness_stats_workspace_bytes(int batch, int channels, int length, int gate, int step, int gate3);
+int kapre_loudness_stats(const float* y_dev, const kapre_wave_desc* y_desc, const int32_t* lengths_dev, int gate,
+                         int step, int gate3, float* integrated_dev, float* momentary_dev, float* short_term_dev,
+                         float* lra_dev, void* workspace_dev, void* stream);
+/* True peak per (item, channel) column of a waveform x (any channel count, lengths as kapre_loudness, length <= 2^30):
+ * TP = 20 log10 max_t |z[t]|, z = scipy.signal.resample_poly(x[:len], 4, 1) with taps_host the 81 float32 taps of its
+ * filter (kapre_b200.signal.resample_filter(4, 1)); z is formed as kapre_resample forms it, in registers, and never
+ * written.  -inf for a silent column, NaN when a NaN reaches z.  out_dev: (batch, channels) float32 row-major;
+ * stats_dev (its size in *stats_bytes): z[t*] and the first argmax t*, which kapre_true_peak_backward reads. */
+int64_t kapre_true_peak_workspace_bytes(int batch, int channels, int length, int64_t* stats_bytes);
+/* Two launches. */
+int kapre_true_peak(const float* x_dev, const kapre_wave_desc* x_desc, const int32_t* lengths_dev,
+                    const float* taps_host, float* out_dev, void* stats_dev, void* workspace_dev, void* stream);
+/* gx = the gradient of kapre_true_peak at output gradient g_dev ((batch, channels) float32 row-major):
+ * gx[n] = g (20 / ln 10) 4 h[t* - 4n + 40] / z[t*] inside h's support and n < len, else exactly 0 (also for -inf
+ * columns).  gx_desc: x's shape, any strides.  One launch. */
+int kapre_true_peak_backward(const float* g_dev, const int32_t* lengths_dev, const float* taps_host,
+                             const void* stats_dev, float* gx_dev, const kapre_wave_desc* gx_desc, void* stream);
+
 /* ---- Kaldi-compatible features (torchaudio.compliance.kaldi.fbank / mfcc / spectrogram) -------------------
  * Every (item, channel) column of a float32 waveform is framed, dithered, DC-removed, pre-emphasised, windowed,
  * zero-padded to padded_window_size and transformed as torchaudio 2.11's functions do (one frame set per channel

@@ -242,6 +242,14 @@ SYMBOLS = [
                                c_void_p]),
     ('kapre_loudness_backward', c_int, [c_void_p, c_void_p, POINTER(WaveDesc), c_void_p, c_int, c_int, c_void_p,
                                         c_void_p, POINTER(WaveDesc), c_void_p]),
+    ('kapre_loudness_stats_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    ('kapre_loudness_stats', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_void_p]),
+    ('kapre_true_peak_workspace_bytes', c_int64, [c_int, c_int, c_int, POINTER(c_int64)]),
+    ('kapre_true_peak', c_int, [c_void_p, POINTER(WaveDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p]),
+    ('kapre_true_peak_backward', c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(WaveDesc),
+                                         c_void_p]),
     ('kapre_kaldi_plan_create', c_int, [POINTER(KaldiCfg), c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
     ('kapre_kaldi_plan_destroy', None, [c_void_p]),
     ('kapre_kaldi_num_frames', c_int, [c_void_p, c_int]),

@@ -526,7 +526,15 @@ class LoudnessNormalization(Layer):
     """Loudness normalisation to a target per item (EBU R128's -23 LUFS, streaming's -14, or a random target per
     example): ``(batch, time, ch)`` / ``(batch, ch, time)`` in (ch <= 5), the same shape out, each item scaled by
     ``10^((target - L) / 20)`` with L its BS.1770 loudness (``signal.loudness``).  Items whose L is not finite
-    (silent, shorter than one 400 ms block, or with a non-finite sample) come back unchanged.  Nothing limits peaks.
+    (silent, shorter than one 400 ms block, or with a non-finite sample) come back unchanged.
+
+    ``true_peak_limit`` (dBTP, default None) caps the gain so that the output's true peak stays at or below it, as EBU
+    R128 pairs a loudness target with a true-peak ceiling (for example -1 dBTP): the gain is then
+    ``min(10^((target - L) / 20), 10^((limit - TP) / 20))`` with TP the item's largest ``signal.true_peak`` over its
+    channels.  The true peak is linear in the waveform, so the output's is at most the limit up to float32 rounding;
+    an item the limit binds lands below its loudness target.  Only the gain scales: the waveform's shape is kept.  The
+    gradient follows whichever term is smaller, as ``torch.minimum``'s does.  With None the layer runs as if the
+    argument did not exist.
 
     ``call(x, lufs=None, lengths=None)`` draws the targets uniformly from ``lufs_range`` with
     ``np.random.default_rng(seed)``; ``lufs`` (a number or ``batch`` values) replaces the draw, which is then not made.
@@ -534,7 +542,8 @@ class LoudnessNormalization(Layer):
     no sync; a captured graph (``Sequential.capture``) replays the draw made when it was captured.  The gradient
     reaches ``x``, through the gain as well."""
 
-    def __init__(self, sample_rate, lufs_range=(-23.0, -23.0), seed=None, data_format='default', **kwargs):
+    def __init__(self, sample_rate, lufs_range=(-23.0, -23.0), seed=None, data_format='default', true_peak_limit=None,
+                 **kwargs):
         super().__init__(**kwargs)
         backend.validate_data_format_str(data_format)
         data_format = _unwrap_format(data_format)
@@ -542,6 +551,12 @@ class LoudnessNormalization(Layer):
         r = tuple(float(v) for v in lufs_range)
         if len(r) != 2 or not (np.isfinite(r[0]) and np.isfinite(r[1])) or r[0] > r[1]:
             raise ValueError('lufs_range must be a (low, high) pair of finite numbers, got: %r' % (lufs_range,))
+        if true_peak_limit is not None:
+            if isinstance(true_peak_limit, bool) or not isinstance(true_peak_limit, (int, float, np.integer, np.floating)) \
+                    or not np.isfinite(true_peak_limit):
+                raise ValueError('true_peak_limit must be a finite number of dBTP or None, got: %r' % (true_peak_limit,))
+            true_peak_limit = float(true_peak_limit)
+        self.true_peak_limit = true_peak_limit
         self.sample_rate = sample_rate
         self.lufs_range = r
         self.seed = seed
@@ -576,12 +591,19 @@ class LoudnessNormalization(Layer):
         t = host.to(x.device, non_blocking=True)
         L = ops.loudness(x, self.sample_rate, lengths, self.data_format)
         # a non-finite L gives the exponent 0 (gain 1), and no gradient flows into it
-        L = torch.where(torch.isfinite(L), L, t)
-        gain = torch.pow(10.0, (t - L) / 20.0)
+        finite = torch.isfinite(L)
+        L = torch.where(finite, L, t)
+        if self.true_peak_limit is None:
+            gain = torch.pow(10.0, (t - L) / 20.0)
+        else:
+            # the item's largest channel true peak; items left unchanged get the limit itself (exponent 0, no gradient)
+            tp = ops.true_peak(x, lengths, self.data_format).amax(dim=1)
+            tp = torch.where(finite, tp, torch.full_like(tp, self.true_peak_limit))
+            gain = torch.pow(10.0, torch.minimum(t - L, self.true_peak_limit - tp) / 20.0)
         return x * gain.view(B, 1, 1)
 
     def get_config(self):
         config = super().get_config()
         config.update({'sample_rate': self.sample_rate, 'lufs_range': list(self.lufs_range), 'seed': self.seed,
-                       'data_format': self.data_format_original})
+                       'data_format': self.data_format_original, 'true_peak_limit': self.true_peak_limit})
         return config

@@ -28,6 +28,8 @@ of their own (see ``include/kapre_b200.h``, "backward passes"):
   gradient; sosfiltfilt's data-dependent initial states through the DC gain, no coefficient or zi gradient)
 * add_noise, BackgroundNoise -> ``kapre_add_noise_backward`` (a segment-sum pass over g n, then the input, noise and
   snr gradients from the saved energies)
+* true_peak, LoudnessNormalization(true_peak_limit=...) -> ``kapre_true_peak_backward`` ((20 / ln 10) 4 h[t* - 4n + 40]
+  / z[t*] at the saved first argmax t*)
 * loudness, Loudness, LoudnessNormalization -> ``kapre_loudness_backward`` (gL (20 / ln 10) g_c y n(t) / (E2 |J2| G)
   from the saved gate decisions), then the two lfilter gradients of the K-weighting
 * kaldi_fbank, kaldi_mfcc, kaldi_spectrogram, KaldiFbank, KaldiMFCC, KaldiSpectrogram -> ``kapre_kaldi_features_backward``
@@ -459,6 +461,25 @@ class _Loudness(torch.autograd.Function):
         return ops.loudness_backward(g, y, lengths, G, S, stats, data_format), None, None, None, None
 
 
+class _TruePeak(torch.autograd.Function):
+    """The forward is the plain two-launch measurement; its stats (z[t*], t*) are all the one-launch backward reads."""
+
+    @staticmethod
+    def forward(ctx, x, lengths, data_format):
+        out, stats = ops.true_peak_forward(x, lengths, data_format)
+        ctx.save_for_backward(lengths, stats)
+        B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == ops._CH_LAST_STR else tuple(x.shape)
+        ctx.cfg = ((B, C, L), data_format, x.device)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        lengths, stats = ctx.saved_tensors
+        shape, data_format, device = ctx.cfg
+        return ops.true_peak_backward(g, lengths, stats, shape, data_format, device), None, None
+
+
 class _KaldiFeatures(torch.autograd.Function):
     """The forward is the plain feature launch; only the waveform is saved, and the backward regenerates the dither
     from (seed, item, channel, frame, sample)."""
@@ -658,6 +679,10 @@ def add_noise(x, noise, snr, lengths, bank, data_format):
 
 def loudness(y, lengths, G, S, data_format):
     return _Loudness.apply(y, lengths, G, S, data_format)
+
+
+def true_peak(x, lengths, data_format):
+    return _TruePeak.apply(x, lengths, data_format)
 
 
 def kaldi_features(x, plan, lengths_h, lengths_d, data_format, dither, seed):

@@ -39,6 +39,7 @@
 #include "noise_core.cuh"
 #include "kaldi_core.cuh"
 #include "loudness_core.cuh"
+#include "meter_core.cuh"
 #include "cqt_core.cuh"
 #include "pitch_core.cuh"
 #include "chroma_core.cuh"
@@ -3802,6 +3803,178 @@ int kapre_loudness_backward(const float* gl_dev, const float* y_dev, const kapre
     p.gl = gl_dev;
     p.gy = gy_dev; p.g_sb = gy_desc->stride_b; p.g_sc = gy_desc->stride_c; p.g_sl = gy_desc->stride_l;
     return kb_loud_launch(kb_loud_bwd_kernel, p.tiles, p, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+// ---- loudness meter: true peak, loudness series and range (meter_core.cuh) ------------------------------------------
+// Every kernel waits for the previous kernel in the stream before touching data, so all may be launched with PDL.
+__global__ void __launch_bounds__(KB_TP_WARPS * 32) kb_tp_peak_kernel(const __grid_constant__ KbTpParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long tile = (long long)blockIdx.x * KB_TP_WARPS + w;
+    if (tile < p.tiles) kb_tp_peak_tile(p, kb_smem + w * kb_tp_smem().total, tile);
+}
+__global__ void __launch_bounds__(KB_TP_WARPS * 32) kb_tp_fold_kernel(const __grid_constant__ KbTpParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long col = (long long)blockIdx.x * KB_TP_WARPS + w;
+    if (col < (long long)p.B * p.C) kb_tp_fold_tile(p, kb_smem + w * kb_tp_smem().total, col);
+}
+__global__ void __launch_bounds__(256) kb_tp_bwd_kernel(const __grid_constant__ KbTpParams p) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i < (long long)p.B * p.C * p.L) kb_tp_bwd(p, i);
+}
+__global__ void __launch_bounds__(256) kb_meter_series_kernel(const __grid_constant__ KbLoudParams p, float* out,
+                                                              double* e) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i < (long long)p.B * p.Jmax) kb_meter_series(p, out, e, i);
+}
+__global__ void __launch_bounds__(KB_LOUD_WARPS * 32) kb_meter_lra_kernel(const __grid_constant__ KbLoudParams p,
+                                                                          double* e, float* out) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int w = (int)(threadIdx.x >> 5);
+    const long long b = (long long)blockIdx.x * KB_LOUD_WARPS + w;
+    if (b < p.B) kb_meter_lra_tile(p, e, out, kb_smem + w * kb_lra_smem().total, b);
+}
+
+// Checks a shape, fills the geometry (taps may be null when only sizing) and lays out the workspace (the (B, C, nseg)
+// tile keys) and the stats record ((B, C) z[t*], then (B, C) t*).  -1 on a bad argument or an overflow.
+static int kb_tp_geometry(KbTpParams& p, int batch, int channels, int length, const float* taps, KbLayout& ws,
+                          KbLayout& rec) {
+    if (batch < 0 || channels < 1 || length < 0 || length > KB_TP_MAX_LEN) return -1;
+    p.B = batch; p.C = channels; p.L = length;
+    float zero[KB_TP_TAPS] = {};
+    kb_tp_setup(p, taps ? taps : zero);
+    const double cols = (double)batch * channels;
+    if (cols * p.nseg / KB_TP_WARPS > 2147483647.0 || cols * length / 256.0 > 2147483647.0) return -1;
+    p.tiles = (long long)batch * channels * p.nseg;
+    p.key = ws.take<unsigned long long>(batch, channels, p.nseg);
+    ws.pad();
+    p.zs = rec.take<float>(batch, channels);
+    p.ts = rec.take<unsigned>(batch, channels);
+    rec.pad();
+    return ws.overflow || rec.overflow ? -1 : 0;
+}
+
+static int kb_tp_launch(void (*kernel)(KbTpParams), long long work, const KbTpParams& p, cudaStream_t st) {
+    return kb_launch(kernel, {.grid = (int)((work + KB_TP_WARPS - 1) / KB_TP_WARPS), .block = KB_TP_WARPS * 32,
+                              .smem = KB_TP_WARPS * kb_tp_smem().total, .st = st, .pdl = true}, p);
+}
+
+// The loudness-stats workspace: kapre_loudness's piece sums and stats record for the 400 ms blocks, the same for the
+// 3 s windows, and the (B, J_S) float64 window energies the range pass reads.
+static int kb_meter_geometry(KbLoudParams& pm, KbLoudParams& ps, int batch, int channels, int length, int gate,
+                             int step, int gate3, KbLayout& ws, double** e) {
+    if (gate3 < gate) return -1;
+    if (kb_loud_geometry(pm, batch, channels, length, gate, step, ws, ws) < 0) return -1;
+    if (kb_loud_geometry(ps, batch, channels, length, gate3, step, ws, ws) < 0) return -1;
+    *e = ws.take<double>(batch, ps.Jmax);
+    ws.pad();
+    if ((double)batch * (pm.Jmax > ps.Jmax ? pm.Jmax : ps.Jmax) / 256.0 > 2147483647.0) return -1;
+    return ws.overflow ? -1 : 0;
+}
+
+extern "C" {
+
+int64_t kapre_true_peak_workspace_bytes(int batch, int channels, int length, int64_t* stats_bytes) {
+    KbTpParams p{};
+    KbLayout ws, rec;
+    if (kb_tp_geometry(p, batch, channels, length, nullptr, ws, rec) < 0)
+        return kb_fail(KAPRE_E_INVALID, "true_peak: bad size (%d, %d, %d) or an overflow", batch, channels, length);
+    if (stats_bytes) *stats_bytes = rec.end;
+    return ws.end;
+}
+
+int kapre_true_peak(const float* x_dev, const kapre_wave_desc* x_desc, const int32_t* lengths_dev,
+                    const float* taps_host, float* out_dev, void* stats_dev, void* workspace_dev, void* stream) {
+    if (!x_desc || !taps_host) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbTpParams p{};
+    KbLayout ws{(char*)workspace_dev}, rec{(char*)stats_dev};
+    if (kb_tp_geometry(p, x_desc->batch, x_desc->channels, x_desc->length, taps_host, ws, rec) < 0)
+        return kb_fail(KAPRE_E_INVALID, "true_peak: bad size (%d, %d, %d) or an overflow", x_desc->batch,
+                       x_desc->channels, x_desc->length);
+    if (p.B == 0) return 0;
+    if (!out_dev || !stats_dev || (p.tiles && (!x_dev || !workspace_dev)))
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.x = x_dev; p.x_sb = x_desc->stride_b; p.x_sc = x_desc->stride_c; p.x_sl = x_desc->stride_l;
+    p.len = lengths_dev;
+    p.out = out_dev;
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if (p.tiles && (rc = kb_tp_launch(kb_tp_peak_kernel, p.tiles, p, st))) return rc;
+    return kb_tp_launch(kb_tp_fold_kernel, (long long)p.B * p.C, p, st);
+}
+
+int kapre_true_peak_backward(const float* g_dev, const int32_t* lengths_dev, const float* taps_host,
+                             const void* stats_dev, float* gx_dev, const kapre_wave_desc* gx_desc, void* stream) {
+    if (!gx_desc || !taps_host) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbTpParams p{};
+    KbLayout ws, rec{(char*)const_cast<void*>(stats_dev)};
+    if (kb_tp_geometry(p, gx_desc->batch, gx_desc->channels, gx_desc->length, taps_host, ws, rec) < 0)
+        return kb_fail(KAPRE_E_INVALID, "true_peak: bad size (%d, %d, %d) or an overflow", gx_desc->batch,
+                       gx_desc->channels, gx_desc->length);
+    const long long n = (long long)p.B * p.C * p.L;
+    if (n == 0) return 0;
+    if (!g_dev || !stats_dev || !gx_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    p.len = lengths_dev;
+    p.g = g_dev;
+    p.gx = gx_dev; p.g_sb = gx_desc->stride_b; p.g_sc = gx_desc->stride_c; p.g_sl = gx_desc->stride_l;
+    return kb_launch(kb_tp_bwd_kernel, {.grid = (int)((n + 255) / 256), .block = 256, .st = (cudaStream_t)stream,
+                                        .pdl = true}, p);
+}
+
+int64_t kapre_loudness_stats_workspace_bytes(int batch, int channels, int length, int gate, int step, int gate3) {
+    KbLoudParams pm{}, ps{};
+    KbLayout ws;
+    double* e;
+    if (kb_meter_geometry(pm, ps, batch, channels, length, gate, step, gate3, ws, &e) < 0)
+        return kb_fail(KAPRE_E_INVALID, "loudness_stats: bad size (%d, %d, %d), gate %d, step %d or gate3 %d, or an "
+                       "overflow", batch, channels, length, gate, step, gate3);
+    return ws.end;
+}
+
+int kapre_loudness_stats(const float* y_dev, const kapre_wave_desc* y_desc, const int32_t* lengths_dev, int gate,
+                         int step, int gate3, float* integrated_dev, float* momentary_dev, float* short_term_dev,
+                         float* lra_dev, void* workspace_dev, void* stream) {
+    if (!y_desc) return kb_fail(KAPRE_E_INVALID, "null argument");
+    KbLoudParams pm{}, ps{};
+    KbLayout ws{(char*)workspace_dev};
+    double* e;
+    if (kb_meter_geometry(pm, ps, y_desc->batch, y_desc->channels, y_desc->length, gate, step, gate3, ws, &e) < 0)
+        return kb_fail(KAPRE_E_INVALID, "loudness_stats: bad size (%d, %d, %d), gate %d, step %d or gate3 %d, or an "
+                       "overflow", y_desc->batch, y_desc->channels, y_desc->length, gate, step, gate3);
+    if (pm.B == 0) return 0;
+    if (!integrated_dev || !lra_dev || !workspace_dev || (pm.Jmax && !momentary_dev) || (ps.Jmax && !short_term_dev) ||
+        (pm.K && !y_dev))
+        return kb_fail(KAPRE_E_INVALID, "null data pointer");
+    for (KbLoudParams* p : {&pm, &ps}) {
+        p->y = y_dev; p->y_sb = y_desc->stride_b; p->y_sc = y_desc->stride_c; p->y_sl = y_desc->stride_l;
+        p->len = lengths_dev;
+        p->tiles = (long long)p->B * p->K;
+    }
+    pm.out = integrated_dev;
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    // integrated loudness: kapre_loudness's two passes as they are
+    if (pm.tiles && (rc = kb_loud_launch(kb_loud_energy_kernel, pm.tiles, pm, st))) return rc;
+    if ((rc = kb_loud_launch(kb_loud_gate_kernel, pm.B, pm, st))) return rc;
+    const long long nm = (long long)pm.B * pm.Jmax, ns = (long long)ps.B * ps.Jmax;
+    if (nm && (rc = kb_launch(kb_meter_series_kernel, {.grid = (int)((nm + 255) / 256), .block = 256, .st = st,
+                                                       .pdl = true}, pm, momentary_dev, (double*)nullptr)))
+        return rc;
+    if (ps.tiles && (rc = kb_loud_launch(kb_loud_energy_kernel, ps.tiles, ps, st))) return rc;
+    if (ns && (rc = kb_launch(kb_meter_series_kernel, {.grid = (int)((ns + 255) / 256), .block = 256, .st = st,
+                                                       .pdl = true}, ps, short_term_dev, e)))
+        return rc;
+    return kb_launch(kb_meter_lra_kernel, {.grid = (int)((ps.B + KB_LOUD_WARPS - 1) / KB_LOUD_WARPS),
+                                           .block = KB_LOUD_WARPS * 32, .smem = KB_LOUD_WARPS * kb_lra_smem().total,
+                                           .st = st, .pdl = true}, ps, e, lra_dev);
 }
 
 }  // extern "C"

@@ -6,6 +6,7 @@ a missing library, a CPU-only process or a non-CUDA tensor raises.
 """
 from __future__ import annotations
 
+import collections
 import ctypes
 import math
 import threading
@@ -1470,6 +1471,126 @@ def loudness(x, sample_rate, lengths=None, data_format=_CH_LAST_STR):
         from . import autograd
         return autograd.loudness(y, lengths, G, S, data_format)
     return loudness_forward(y, lengths, G, S, data_format)[0]
+
+
+LoudnessStats = collections.namedtuple('LoudnessStats',
+                                       ['integrated', 'momentary', 'short_term', 'loudness_range', 'true_peak'])
+_true_peak_taps = None
+
+
+def true_peak_taps():
+    """The 81 float32 taps of ``signal.resample_filter(4, 1)``, made once on the host."""
+    global _true_peak_taps
+    if _true_peak_taps is None:
+        from .signal import resample_filter
+        _true_peak_taps = np.ascontiguousarray(resample_filter(4, 1), np.float32)
+    return _true_peak_taps
+
+
+def _taps_ptr():
+    return true_peak_taps().ctypes.data_as(ctypes.c_void_p)
+
+
+def true_peak_sizes(B, C, L):
+    """(workspace bytes, stats bytes) of ``kapre_true_peak``; raises on a bad size or an overflow."""
+    stats = ctypes.c_int64(0)
+    n = int(N.lib().kapre_true_peak_workspace_bytes(B, C, L, ctypes.byref(stats)))
+    if n < 0:
+        N.check(n)
+    return n, int(stats.value)
+
+
+def true_peak_forward(x, lengths, data_format):
+    """(dBTP (B, C) float32, stats) of x: ``kapre_true_peak``, two launches."""
+    x = _raw(x.to(torch.float32))
+    xd, (B, C, L) = _wave_desc(x, data_format)
+    nw, ns = true_peak_sizes(B, C, L)
+    out = torch.empty((B, C), dtype=torch.float32, device=x.device)
+    stats = _scratch(ns, x.device)
+    if B:
+        ws = _scratch(nw, x.device)
+        N.check(N.lib().kapre_true_peak(_ptr(x), ctypes.byref(xd), _ptr(lengths) if lengths is not None else None,
+                                        _taps_ptr(), _ptr(out), _ptr(stats), _ptr(ws), _stream_ptr()))
+    return out, stats
+
+
+def true_peak_backward(g, lengths, stats, shape, data_format, device):
+    """The gradient of ``true_peak_forward`` with respect to x of (B, C, L) = ``shape`` at output gradient g (B, C):
+    one launch."""
+    B, C, L = shape
+    g = g.to(torch.float32).contiguous()
+    gx, gd = _wave_alloc(B, C, L, data_format, device)
+    if gx.numel():
+        N.check(N.lib().kapre_true_peak_backward(_ptr(g), _ptr(lengths) if lengths is not None else None, _taps_ptr(),
+                                                 _ptr(stats), _ptr(gx), ctypes.byref(gd), _stream_ptr()))
+    return gx
+
+
+def _meter_input(x, name, data_format, max_channels):
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise N.KapreNativeError('%s needs a CUDA waveform' % name)
+    if x.dim() != 3:
+        raise ValueError('%s expects a 3-D waveform batch, got shape %s' % (name, tuple(x.shape)))
+    B, C, L = (x.shape[0], x.shape[2], x.shape[1]) if data_format == _CH_LAST_STR else tuple(x.shape)
+    if not 1 <= C <= max_channels:
+        raise ValueError('%s supports 1 to %d channels, got %d' % (name, max_channels, C))
+    return B, C, L
+
+
+@_device_of_first_arg
+def true_peak(x, lengths=None, data_format=_CH_LAST_STR):
+    """True peak (dBTP) per (item, channel) of x (B, L, C) / (B, C, L): ``kapre_true_peak`` (two launches).  Checked
+    before any launch; differentiable with respect to x (one backward launch)."""
+    B, C, L = _meter_input(x, 'true_peak', data_format, 2 ** 31 - 1)
+    if lengths is not None:
+        lengths = _item_lengths(lengths, B, L, x.device)
+    true_peak_sizes(B, C, L)
+    if _wants_grad(x):
+        from . import autograd
+        return autograd.true_peak(x, lengths, data_format)
+    return true_peak_forward(x, lengths, data_format)[0]
+
+
+def loudness_stats_sizes(B, C, L, G, S, G3):
+    """Workspace bytes of ``kapre_loudness_stats``; raises on a bad size or an overflow."""
+    n = int(N.lib().kapre_loudness_stats_workspace_bytes(B, C, L, G, S, G3))
+    if n < 0:
+        N.check(n)
+    return n
+
+
+@_device_of_first_arg
+def loudness_stats(x, sample_rate, lengths=None, data_format=_CH_LAST_STR):
+    """``LoudnessStats`` of x (B, L, C) / (B, C, L), C <= 5: the K-weighting as in ``loudness`` (eight launches), then
+    ``kapre_loudness_stats`` (six) and ``kapre_true_peak`` on x (two).  Everything is checked before any launch; no
+    gradient (an input that requires grad under grad mode raises)."""
+    if _wants_grad(x):
+        raise ValueError('loudness_stats has no gradient: use loudness and true_peak, which are differentiable, or call '
+                         'it under torch.no_grad() or on a detached waveform')
+    B, C, L = _meter_input(x, 'loudness_stats', data_format, LOUDNESS_MAX_CHANNELS)
+    (b1, a1), (b2, a2) = k_weighting(sample_rate, x.device)
+    G, S = loudness_geometry(sample_rate)
+    G3 = int(round(3 * sample_rate))
+    if lengths is not None:
+        lengths = _item_lengths(lengths, B, L, x.device)
+    nw = loudness_stats_sizes(B, C, L, G, S, G3)            # size checks before anything is launched
+    true_peak_sizes(B, C, L)
+    lfilter_workspace(B, C, L, 2, x.device)
+    y = lfilter(x, b1, a1, clamp=True, data_format=data_format)
+    y = _raw(lfilter(y, b2, a2, clamp=True, data_format=data_format))
+    yd, _ = _wave_desc(y, data_format)
+    Jm, Js = ((L - g) // S + 1 if L >= g else 0 for g in (G, G3))
+    dev = x.device
+    integrated = torch.empty(B, dtype=torch.float32, device=dev)
+    momentary = torch.empty((B, Jm), dtype=torch.float32, device=dev)
+    short_term = torch.empty((B, Js), dtype=torch.float32, device=dev)
+    lra = torch.empty(B, dtype=torch.float32, device=dev)
+    if B:
+        ws = _scratch(nw, dev)
+        N.check(N.lib().kapre_loudness_stats(_ptr(y), ctypes.byref(yd), _ptr(lengths) if lengths is not None else None,
+                                             G, S, G3, _ptr(integrated), _ptr(momentary), _ptr(short_term), _ptr(lra),
+                                             _ptr(ws), _stream_ptr()))
+    return LoudnessStats(integrated, momentary, short_term, lra, true_peak_forward(x, lengths, data_format)[0])
 
 
 def _pcen_params(params, eps, device):

@@ -7,7 +7,8 @@ real factor, band-limited interpolation), ``Convolve`` (convolution with long fi
 filters ``lfilter``, ``filtfilt``, ``IIRFilter`` and ``Biquad`` (torchaudio's, on a chunked linear-recurrence scan), or
 the second-order-section cascades ``sosfilt``, ``sosfiltfilt`` and ``SOSFilter`` (scipy's, on the same scan), or
 ``add_noise`` (torchaudio's, with deterministic float64 energies), or ``loudness`` and ``Loudness`` (torchaudio's
-BS.1770 gated loudness, with per-item lengths), or the pitch trackers ``yin``, ``pyin``, ``YIN`` and ``PYIN``
+BS.1770 gated loudness, with per-item lengths), or the loudness meter ``loudness_stats`` and ``true_peak`` (EBU R128's
+momentary and short-term loudness, loudness range and true peak), or the pitch trackers ``yin``, ``pyin``, ``YIN`` and ``PYIN``
 (librosa's), or the chroma features ``chroma_stft``, ``chroma_cqt``, ``chroma_cens`` and ``estimate_tuning``
 (librosa's), or the harmonic/percussive separation ``hpss``, ``harmonic`` and ``percussive`` (librosa's), or the
 rhythm features ``onset_strength``, ``onset_detect``, ``tempogram``, ``tempo`` and ``beat_track`` (librosa's)."""
@@ -23,7 +24,8 @@ from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
 from .time_frequency import Layer, _unwrap_format, register_keras_serializable
 
 __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', 'lfilter', 'filtfilt', 'IIRFilter',
-           'Biquad', 'sosfilt', 'sosfiltfilt', 'SOSFilter', 'add_noise', 'loudness', 'Loudness', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
+           'Biquad', 'sosfilt', 'sosfiltfilt', 'SOSFilter', 'add_noise', 'loudness', 'Loudness', 'loudness_stats', 'true_peak',
+           'LoudnessStats', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
            'YIN', 'PYIN', 'chroma_stft', 'chroma_cqt', 'chroma_cens', 'estimate_tuning', 'hpss', 'harmonic',
            'percussive', 'onset_strength', 'onset_detect', 'tempogram', 'tempo', 'beat_track']
 
@@ -330,6 +332,52 @@ def loudness(waveform, sample_rate, lengths=None, data_format='default'):
     coefficients are uploaded once per device and rate, so a call can be captured in a CUDA graph.  Differentiable
     with respect to ``waveform``."""
     return ops.loudness(waveform, sample_rate, lengths, _resolve(_unwrap_format(data_format)))
+
+
+LoudnessStats = ops.LoudnessStats
+LoudnessStats.__doc__ = """What ``loudness_stats`` returns: ``integrated`` (batch,) LKFS, ``momentary`` (batch, J_M) and
+``short_term`` (batch, J_S) LUFS series, ``loudness_range`` (batch,) LU and ``true_peak`` (batch, ch) dBTP."""
+
+
+def loudness_stats(waveform, sample_rate, lengths=None, data_format='default'):
+    """The EBU R128 loudness meter per item of ``waveform`` ``(batch, time, ch)`` / ``(batch, ch, time)`` (a CUDA
+    tensor, ch <= 5), as a ``LoudnessStats`` of float32 tensors.  ``lengths`` as in ``loudness``.
+
+    With ``G = round(0.4 sample_rate)``, ``S = round(G / 4)`` and ``G3 = round(3 sample_rate)``:
+
+    - ``integrated`` ``(batch,)``: ``loudness`` of the same input, bit for bit (the same passes run).
+    - ``momentary`` ``(batch, J_M)``, ``J_M = (time - G) // S + 1`` (0 when ``time < G``): entry j is
+      ``-0.691 + 10 log10(sum_c g_c e_cj)``, e_cj the mean square of channel c of the K-weighted signal over
+      ``[jS, jS + G)``, ungated.  Entries at or past the item's own count ``(len - G) // S + 1`` are ``-inf``, as is a
+      silent window, so ``amax`` over a row is the item's maximum momentary loudness.
+    - ``short_term`` ``(batch, J_S)``: the same with the 3 s window ``G3`` and the same step.
+    - ``loudness_range`` ``(batch,)`` LU, EBU Tech 3342 on the short-term windows: the absolute gate at -70 LUFS, the
+      relative gate 20 LU below the mean energy of the windows above it (strict comparisons), then the 95th minus the
+      10th percentile of the remaining loudnesses by the nearest-rank rule ``v[((n - 1) p + 50) // 100]``; 0 when no
+      window remains.  Float64 throughout, rounded once; selected on the device without a sort or a length limit.
+    - ``true_peak`` ``(batch, ch)``: ``true_peak`` of the waveform.
+
+    A non-finite sample makes that item's results NaN (true peak: that channel's) and no other item's.  The
+    K-weighting runs once and feeds every output.  Sixteen launches: two ``kapre_lfilter`` calls of four,
+    ``kapre_loudness_stats``'s six passes and ``kapre_true_peak``'s two.  No host sync and output sizes from ``time``
+    alone, so a call can be captured in a CUDA graph.  No gradient: called under grad mode on an input that requires
+    grad it raises; ``loudness`` and ``true_peak`` are differentiable."""
+    return ops.loudness_stats(waveform, sample_rate, lengths, _resolve(_unwrap_format(data_format)))
+
+
+def true_peak(waveform, lengths=None, data_format='default'):
+    """True peak in dBTP per (item, channel) of ``waveform`` ``(batch, time, ch)`` / ``(batch, ch, time)`` (a CUDA
+    tensor, any channel count, time <= 2^30), as a ``(batch, ch)`` float32 tensor:
+    ``20 log10 max_t |z_c[t]|`` with ``z_c = scipy.signal.resample_poly(x_c[:len], 4, 1)``, 4x oversampling with
+    ``resample_filter(4, 1)``, scipy's default Kaiser design.  ITU-R BS.1770-4 Annex 2 gives a 48-tap filter as an
+    example that any compliant filter may replace; using scipy's makes ``resample_poly`` in float64 an exact oracle.
+    No K-weighting and no sample rate.  ``lengths`` as in ``loudness``.
+
+    z is formed in registers exactly as ``Resample`` forms it and never written; the maximum and its first argmax are
+    exact and do not depend on the batch, the strides or the data format.  A silent channel gives ``-inf``; a NaN that
+    reaches z gives NaN.  Two launches; differentiable with respect to ``waveform`` (one launch): the gradient is
+    ``torch.amax``'s through the fixed linear map x -> z at the first argmax, and exactly 0 for ``-inf`` channels."""
+    return ops.true_peak(waveform, lengths, _resolve(_unwrap_format(data_format)))
 
 
 @register_keras_serializable(package='Kapre')
