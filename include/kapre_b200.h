@@ -401,6 +401,29 @@ int kapre_sosfilt(const float* x_dev, const kapre_wave_desc* x_desc, const kapre
                   const kapre_sos_state_desc* zi_desc, int flags, float* y_dev, const kapre_wave_desc* y_desc,
                   float* zf_dev, const kapre_sos_state_desc* zf_desc, void* workspace_dev, void* stream);
 
+/* ---- image-source room impulse responses (DESIGN.md §RIR) -----------------------------------------------------------
+ * Shoebox room [0, Lx] x [0, Ly] x [0, Lz], walls (x=0, x=Lx, y=0, y=Ly, z=0, z=Lz) with pressure reflection
+ * coefficients beta_w.  Image (n, p), n in Z^3, p in {0,1}^3: i_d = 2 n_d L_d + (1 - 2 p_d) s_d, r = |i - m|,
+ * tau = r fs / c, g = prod_d beta_(d,lo)^|n_d - p_d| beta_(d,hi)^|n_d| / (4 pi r), and
+ *   h[floor(tau) + k] += g w[k] sinc(k - half - frac(tau)),  k < W,  w = np.hanning(W),
+ * over the images of order <= max_order (all, when it is -1).  Output samples [start, start + output_length) of every
+ * (item, mic) response, float32 at element strides (stride_b, stride_m, stride_t).  A sample's bits depend only on
+ * its item's record, its mic and its index, not on the batch, the strides or start.  One launch.
+ * records: batch records of 14 float64 (room[3], source[3], beta[6], max_order, start), then (batch, n_mics, 3)
+ * float64 mic positions; records_host is validated before anything is launched and records_dev (the same values on
+ * the device) is what the kernel reads.  KAPRE_E_INVALID for a side that is not finite and positive, a source or mic
+ * not strictly inside its room, a mic within 1 mm of the source, beta outside [0, 1], a max_order that is not -1 or a
+ * non-negative integer, a start that is not a non-negative integer or with start + output_length >= 2^31, an even
+ * filter_length or one outside [1, 255], output_length < 1, and a response whose image bound (lattice boxes meeting
+ * the arrival ball of radius (start + output_length) c / fs, times 8) exceeds 2^24, whatever its max_order: the
+ * kernel's enumeration walks the whole ball.
+ * With records_dev and out_dev both NULL the call only validates records_host.
+ * KAPRE_RIR_UNIT_NORM: a second launch scales each response to unit L2 norm (a float64 sum in a fixed order). */
+#define KAPRE_RIR_UNIT_NORM 1
+int kapre_rir_ism(const double* records_host, const double* records_dev, int batch, int n_mics, int output_length,
+                  int filter_length, double sample_rate, double sound_speed, int flags, float* out_dev,
+                  int64_t stride_b, int64_t stride_m, int64_t stride_t, void* stream);
+
 /* ---- additive noise at a target SNR (torchaudio.functional.add_noise) -------------------------------------------
  * For every (item, channel) column of x (L samples), noise n, snr in dB and valid length len:
  *   Ex = sum_{t < len} x[t]^2,  En = sum_{t < len} n[t]^2,  s = sqrt(Ex / En) 10^(-snr / 20),  y[t] = x[t] + s n[t]

@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, '_lib', 'libkapre_b200.so')
@@ -52,6 +52,7 @@ class IirCoeffs(Structure):
 
 
 IIR_CLAMP, IIR_REVERSE = 1, 2
+RIR_UNIT_NORM = 1
 
 
 class SosCoeffs(Structure):
@@ -231,6 +232,8 @@ SYMBOLS = [
     ('kapre_sosfilt_workspace_bytes', c_int64, [c_int, c_int, c_int, c_int]),
     ('kapre_sosfilt', c_int, [c_void_p, POINTER(WaveDesc), POINTER(SosCoeffs), c_void_p, POINTER(SosStateDesc), c_int,
                               c_void_p, POINTER(WaveDesc), c_void_p, POINTER(SosStateDesc), c_void_p, c_void_p]),
+    ('kapre_rir_ism', c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_int, c_void_p,
+                              c_int64, c_int64, c_int64, c_void_p]),
     ('kapre_add_noise_workspace_bytes', c_int64, [c_int, c_int, c_int]),
     ('kapre_add_noise', c_int, [c_void_p, POINTER(WaveDesc), POINTER(NoiseSource), POINTER(SnrDesc), c_void_p,
                                 POINTER(WaveDesc), c_void_p, c_void_p, c_void_p]),

@@ -4,8 +4,11 @@ masking is one CUDA pass (``kapre_spec_augment``).  ``TimeStretch``: a phase voc
 interpolation (``kapre_sinc_resample``) back to the input length.  ``Reverb``: convolution with a room impulse response
 drawn from a bank (``kapre_convolve``).  ``RandomBiquad``: a biquad drawn per item (``kapre_lfilter``).
 ``BackgroundNoise``: a noise excerpt from a bank added at a drawn SNR (``kapre_add_noise``).  ``LoudnessNormalization``:
-a gain to a drawn loudness target (``kapre_lfilter`` and ``kapre_loudness``)."""
+a gain to a drawn loudness target (``kapre_lfilter`` and ``kapre_loudness``).  ``RoomReverb``: convolution with a room
+impulse response simulated per item (``kapre_rir_ism`` and ``kapre_convolve``)."""
 from __future__ import annotations
+
+import math
 
 import numpy as np
 import torch
@@ -380,6 +383,154 @@ class RandomBiquad(Layer):
         config.update({'kind': self.kind, 'sample_rate': self.sample_rate, 'freq_range': list(self.freq_range),
                        'Q_range': list(self.Q_range), 'gain_range': list(self.gain_range), 'seed': self.seed,
                        'data_format': self.data_format_original})
+        return config
+
+
+def _range_pair(name, r, positive=True):
+    r = tuple(float(v) for v in r)
+    if len(r) != 2 or not (np.isfinite(r[0]) and np.isfinite(r[1])) or r[0] > r[1] or (positive and not r[0] > 0):
+        raise ValueError('%s must be a (low, high) pair of finite%s numbers, got: %r'
+                         % (name, ' positive' if positive else '', r))
+    return r
+
+
+@register_keras_serializable(package='Kapre')
+class RoomReverb(Layer):
+    """Reverberation by a room simulated per item with the image-source method: ``(batch, time, ch)`` /
+    ``(batch, ch, time)`` in, the same shape out, ``y[t] = sum_k h[k] x[t - k]`` for ``t < time``, every channel of an
+    item convolved with the item's response (``Reverb``'s contract, with the response simulated instead of drawn).
+
+    Each call draws, per item in turn, with ``np.random.default_rng(seed)``: the three room sides, each uniform in
+    its ``room_range``; the RT60, uniform in ``rt60_range``; the source and then the mic, uniform in the room shrunk by
+    ``wall_margin`` on every side, the mic drawn again from the same generator while it is closer than
+    ``min_distance`` to the source.  ``last_choice = (room, rt60, source, mic)`` records the draw.  All six walls
+    absorb ``backend.inverse_sabine(rt60, room)``.
+
+    The response is ``rir_length`` samples (default ``ceil(rt60_range[1] * sample_rate)``) of
+    ``signal.simulate_rir_ism`` (``max_order``, ``delay_filter_length``) starting at ``round(tau) + half``, the sample
+    nearest the direct path's peak (``tau = |source - mic| sample_rate / 343``, ``half = (delay_filter_length - 1) /
+    2``), scaled to unit L2 norm by a float64 sum in a fixed order.  A call is ``kapre_rir_ism`` with that scaling (two
+    launches), the response's block spectra and ``kapre_convolve`` (four).  The gradient reaches ``x`` through the
+    convolution's; a captured graph (``Sequential.capture``) replays the draw made when it was captured.
+
+    Construction raises ValueError when a corner of the ranges needs an absorption above 1, when ``min_distance`` is
+    more than half the diagonal of the smallest room inside the margins, or when the longest response in the smallest
+    room could exceed ``simulate_rir_ism``'s image cap."""
+
+    def __init__(self, sample_rate, room_range=((3, 10), (3, 10), (2.5, 4)), rt60_range=(0.2, 0.8), wall_margin=0.5,
+                 min_distance=0.5, max_order=None, rir_length=None, delay_filter_length=81, seed=None,
+                 data_format='default', **kwargs):
+        super().__init__(**kwargs)
+        backend.validate_data_format_str(data_format)
+        data_format = _unwrap_format(data_format)
+        if not (np.isfinite(float(sample_rate)) and float(sample_rate) > 0):
+            raise ValueError('sample_rate must be finite and positive, got: %r' % (sample_rate,))
+        if len(room_range) != 3:
+            raise ValueError('room_range must hold three (low, high) pairs, got: %r' % (room_range,))
+        self.room_range = tuple(_range_pair('room_range', r) for r in room_range)
+        self.rt60_range = _range_pair('rt60_range', rt60_range)
+        self.wall_margin, self.min_distance = float(wall_margin), float(min_distance)
+        if not (self.wall_margin > 0 and self.min_distance > 0):
+            raise ValueError('wall_margin and min_distance must be positive, got %r and %r' % (wall_margin, min_distance))
+        inner = np.array([r[0] for r in self.room_range]) - 2 * self.wall_margin
+        # two uniform points of a box lie at least half its diagonal apart with a probability of about 0.2 or more
+        # (1/4 on a segment), so the mic's redraw ends quickly
+        if not (np.all(inner > 0) and self.min_distance <= 0.5 * np.sqrt(np.sum(inner ** 2))):
+            raise ValueError('the smallest room %s cannot hold a wall margin of %g m and a source-mic distance of %g m '
+                             '(at most half the diagonal inside the margins)'
+                             % ([r[0] for r in self.room_range], self.wall_margin, self.min_distance))
+        for corner in np.ndindex(2, 2, 2):
+            backend.inverse_sabine(self.rt60_range[0], [self.room_range[d][corner[d]] for d in range(3)])
+        if max_order is not None and (isinstance(max_order, bool) or not isinstance(max_order, (int, np.integer))
+                                      or max_order < 0):
+            raise ValueError('max_order must be None or a non-negative int, got: %r' % (max_order,))
+        self.sample_rate = float(sample_rate)
+        self.max_order = max_order
+        self.delay_filter_length = int(delay_filter_length)
+        if not (1 <= self.delay_filter_length <= 255 and self.delay_filter_length % 2 == 1):
+            raise ValueError('delay_filter_length must be an odd int from 1 to 255, got: %r' % (delay_filter_length,))
+        self.rir_length = int(math.ceil(self.rt60_range[1] * self.sample_rate)) if rir_length is None else int(rir_length)
+        if self.rir_length < 1:
+            raise ValueError('rir_length must be >= 1, got: %r' % (rir_length,))
+        self._rir_length_arg = rir_length
+        # the image cap of kapre_rir_ism, for the longest arrival time in the smallest room: the response ends at most
+        # (largest room's inner diagonal + c rir_length / fs) plus the filter's half away from the direct path, and
+        # per axis at most R / L + 2 lattice boxes meet a ball of radius R
+        far = np.sqrt(np.sum((np.array([r[1] for r in self.room_range]) - 2 * self.wall_margin) ** 2))
+        t_end = math.floor(far * self.sample_rate / 343.0 + 0.5) + (self.delay_filter_length - 1) // 2 + self.rir_length
+        R = t_end * 343.0 / self.sample_rate
+        bound = 8.0 * np.prod([R / r[0] + 2.0 for r in self.room_range])
+        if bound > ops.RIR_MAX_IMAGES:
+            raise ValueError('rir_length %d in the smallest room %s may need up to %.3g images, above the cap of %d'
+                             % (self.rir_length, [r[0] for r in self.room_range], bound, ops.RIR_MAX_IMAGES))
+        self.seed = seed
+        self.rng = np.random.default_rng(seed)
+        self.last_choice = None
+        self.data_format_original = data_format
+        self.data_format = _resolve(data_format)
+        self.plan = ops.convolve_plan(ops.convolve_block_size(self.rir_length))
+        self._captured = []
+
+    MAX_REDRAWS = 1000
+
+    def draw(self, batch):
+        """(room, rt60, source, mic) arrays of ``batch`` draws, in the documented order.  A mic that is still too
+        close after ``MAX_REDRAWS`` redraws raises ValueError (construction keeps that far less likely than 1e-90)."""
+        lo = np.array([r[0] for r in self.room_range])
+        hi = np.array([r[1] for r in self.room_range])
+        room, rt60 = np.zeros((batch, 3)), np.zeros(batch)
+        source, mic = np.zeros((batch, 3)), np.zeros((batch, 3))
+        m = self.wall_margin
+        for b in range(batch):
+            room[b] = self.rng.uniform(lo, hi)
+            rt60[b] = self.rng.uniform(self.rt60_range[0], self.rt60_range[1])
+            source[b] = self.rng.uniform(m, room[b] - m)
+            mic[b] = self.rng.uniform(m, room[b] - m)
+            redraws = 0
+            while np.sqrt(np.sum((mic[b] - source[b]) ** 2)) < self.min_distance:
+                if redraws == self.MAX_REDRAWS:
+                    raise ValueError('no mic at least %g m from the source after %d redraws in room %s'
+                                     % (self.min_distance, redraws, room[b]))
+                mic[b] = self.rng.uniform(m, room[b] - m)
+                redraws += 1
+        return room, rt60, source, mic
+
+    def records(self, room, rt60, source, mic, sound_speed=343.0):
+        """The ``kapre_rir_ism`` records of a draw: (B, 14) items, each starting at its direct path's peak."""
+        B = room.shape[0]
+        rec = np.zeros((B, ops.RIR_RECORD), np.float64)
+        rec[:, 0:3], rec[:, 3:6] = room, source
+        for b in range(B):
+            rec[b, 6:12] = np.sqrt(1.0 - backend.inverse_sabine(rt60[b], room[b], sound_speed))
+        rec[:, 12] = -1.0 if self.max_order is None else float(self.max_order)
+        tau = np.sqrt(np.sum((source - mic) ** 2, axis=1)) * self.sample_rate / sound_speed
+        rec[:, 13] = np.floor(tau + 0.5) + (self.delay_filter_length - 1) // 2
+        return rec
+
+    def call(self, x):
+        if x.dim() != 3:
+            raise ValueError('RoomReverb expects a 3-D batch, got shape %s' % (tuple(x.shape),))
+        if not x.is_cuda:
+            raise N.KapreNativeError('RoomReverb needs a CUDA tensor')
+        room, rt60, source, mic = self.draw(x.shape[0])
+        self.last_choice = (room, rt60, source, mic)
+        length = x.shape[2] if self.data_format == _CH_FIRST_STR else x.shape[1]
+        if x.shape[0] == 0 or length == 0:
+            return x.float().clone()
+        with torch.cuda.device(x.device):
+            h = ops.rir_ism(self.records(room, rt60, source, mic), mic[:, None, :], self.rir_length,
+                            self.delay_filter_length, self.sample_rate, 343.0, _CH_FIRST_STR, unit_norm=True,
+                            keep=self._captured)
+            H = ops.convolve_ir_spectrum(h, self.plan, _CH_FIRST_STR)
+        return ops.convolve_spectrum(x, H, self.plan, 0, length, self.data_format)
+
+    def get_config(self):
+        config = super().get_config()
+        config.update({'sample_rate': self.sample_rate, 'room_range': [list(r) for r in self.room_range],
+                       'rt60_range': list(self.rt60_range), 'wall_margin': self.wall_margin,
+                       'min_distance': self.min_distance, 'max_order': self.max_order,
+                       'rir_length': self._rir_length_arg, 'delay_filter_length': self.delay_filter_length,
+                       'seed': self.seed, 'data_format': self.data_format_original})
         return config
 
 

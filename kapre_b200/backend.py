@@ -293,6 +293,22 @@ def sosfilt_zi(sos):
     return sos_steady_state(sos)[0]
 
 
+def inverse_sabine(rt60, room, sound_speed=343.0):
+    """The energy absorption ``alpha = 24 ln(10) V / (c S rt60)`` that gives a shoebox room (``room``: its three
+    sides, metres) the reverberation time ``rt60`` (seconds) by Sabine's formula, with ``V`` its volume and ``S`` its
+    wall area.  Raises ValueError when ``alpha > 1``: no absorption gives so short a reverberation in that room."""
+    Lx, Ly, Lz = (float(v) for v in room)
+    rt60, sound_speed = float(rt60), float(sound_speed)
+    if not (min(Lx, Ly, Lz) > 0 and rt60 > 0 and sound_speed > 0 and np.isfinite([Lx, Ly, Lz, rt60, sound_speed]).all()):
+        raise ValueError('room sides, rt60 and sound_speed must be finite and positive, got %r, %r, %r'
+                         % (room, rt60, sound_speed))
+    V, S = Lx * Ly * Lz, 2.0 * (Lx * Ly + Ly * Lz + Lx * Lz)
+    alpha = 24.0 * np.log(10.0) * V / (sound_speed * S * rt60)
+    if alpha > 1.0:
+        raise ValueError('rt60 %g s is too short for a %g x %g x %g m room: absorption %g > 1' % (rt60, Lx, Ly, Lz, alpha))
+    return alpha
+
+
 def k_weighting_coefficients(sample_rate):
     """The two filters of ITU-R BS.1770's K-weighting as ``torchaudio.functional.loudness`` designs them: ((b, a) of
     ``treble_biquad(sample_rate, 4.0, 1500.0, 1 / sqrt(2))``, (b, a) of ``highpass_biquad(sample_rate, 38.0, 0.5)``),

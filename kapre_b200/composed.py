@@ -18,7 +18,7 @@ import torch
 from . import _native as N
 from . import backend, ops
 from .backend import _CH_DEFAULT_STR, _CH_FIRST_STR, _CH_LAST_STR
-from .augmentation import BackgroundNoise, LoudnessNormalization, RandomBiquad, Reverb, TimeStretch
+from .augmentation import BackgroundNoise, LoudnessNormalization, RandomBiquad, Reverb, RoomReverb, TimeStretch
 from .signal import Biquad, IIRFilter, Resample, SOSFilter, Speed
 from .time_frequency import (CQT, STFT, ApplyFilterbank, GriffinLim, InverseFilterbank, InverseSTFT, Layer, Magnitude,
                              MagnitudeToDecibel, Phase, get_registered_object)
@@ -106,11 +106,11 @@ class Sequential(Layer):
 
     def call(self, x):
         start = 0
-        # Leading waveform layers (Resample, Speed, Reverb, the IIR and SOS filters, LoudnessNormalization and
-        # BackgroundNoise) run first, so that the STFT stack behind them still takes the fused launch.
-        while start < len(self.layers) and type(self.layers[start]) in (Resample, Speed, Reverb, IIRFilter, Biquad,
-                                                                        SOSFilter, RandomBiquad, LoudnessNormalization,
-                                                                        BackgroundNoise):
+        # Leading waveform layers (Resample, Speed, Reverb, RoomReverb, the IIR and SOS filters, LoudnessNormalization
+        # and BackgroundNoise) run first, so that the STFT stack behind them still takes the fused launch.
+        while start < len(self.layers) and type(self.layers[start]) in (Resample, Speed, Reverb, RoomReverb, IIRFilter,
+                                                                        Biquad, SOSFilter, RandomBiquad,
+                                                                        LoudnessNormalization, BackgroundNoise):
             x = self.layers[start].call(x)
             start += 1
         on_device = isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3

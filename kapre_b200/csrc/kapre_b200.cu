@@ -45,6 +45,7 @@
 #include "chroma_core.cuh"
 #include "hpss_core.cuh"
 #include "rhythm_core.cuh"
+#include "rir_core.cuh"
 
 // ------------------------------------------------------------------------------------------
 // error handling
@@ -5087,6 +5088,126 @@ int kapre_beat_track(const float* e_dev, const kapre_frames_desc* e_desc, int ba
     if (!frames) return kb_fail(KAPRE_E_INVALID, "beat_track: no frames");
     if (!e_dev || !tempo_dev || !mask_dev || !workspace_dev) return kb_fail(KAPRE_E_INVALID, "null data pointer");
     return kb_rh_launch(kb_beat_kernel, "beat_track", kb_beat_smem(), p.jobs, p, (cudaStream_t)stream, false);
+}
+
+}  // extern "C"
+
+// ---- image-source room impulse responses (rir_core.cuh) -------------------------------------------------------------
+__global__ void __launch_bounds__(KB_RIR_MAX_NW * 32, 1) kb_rir_kernel(const __grid_constant__ KbRirParams p) {
+    extern __shared__ __align__(16) char kb_smem[];
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    kb_rir_tile(p, kb_smem, (long long)blockIdx.x);
+}
+
+// In place, per (item, mic) row of L samples: h *= 1 / sqrt(sum h^2), the sum in float64 in a fixed order (lane l
+// adds samples l, l + 32, ... in turn; then the 32 lane sums are added in lane order).  One warp per row.
+__global__ void __launch_bounds__(256) kb_rir_norm_kernel(float* out, long long sb, long long sm, long long st, int B,
+                                                          int M, int L) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = (int)(threadIdx.x & 31);
+    if (row >= (long long)B * M) return;
+    float* h = out + (row / M) * sb + (row % M) * sm;
+    double part = 0.0;
+    for (int t = lane; t < L; t += 32) {
+        const double v = (double)h[t * st];
+        part = __dadd_rn(part, __dmul_rn(v, v));
+    }
+    double s = 0.0;
+    for (int i = 0; i < 32; ++i) s = __dadd_rn(s, __shfl_sync(0xffffffffu, part, i));
+    if (!(s > 0.0)) return;
+    const double inv = __ddiv_rn(1.0, __dsqrt_rn(s));
+    for (int t = lane; t < L; t += 32) h[t * st] = (float)__dmul_rn((double)h[t * st], inv);
+}
+
+static bool kb_rir_inside(double v, double L) { return std::isfinite(v) && v > 0.0 && v < L; }
+
+// The analytic bound on one response's image count: the lattice boxes [(2n - 1) L, (2n + 1) L] meeting the ball of
+// radius R around the mic, times 8.  It bounds the kernel's work even with a max_order: the tiles enumerate every
+// candidate in the ball and drop the images of higher order one by one.  Below the cap every axis has at most 2^21
+// boxes, so the row, column and image counts and their prefix sums stay far inside int32.
+static double kb_rir_image_bound(const double* rec, const double* mic, double R) {
+    double boxes = 8.0;
+    for (int d = 0; d < 3; ++d) {
+        const double L = rec[d];
+        boxes *= floor((mic[d] + R + L) / (2.0 * L)) - ceil((mic[d] - R - L) / (2.0 * L)) + 1.0;
+    }
+    return boxes;
+}
+
+extern "C" {
+
+int kapre_rir_ism(const double* records_host, const double* records_dev, int batch, int n_mics, int output_length,
+                  int filter_length, double sample_rate, double sound_speed, int flags, float* out_dev,
+                  int64_t stride_b, int64_t stride_m, int64_t stride_t, void* stream) {
+    const int W = filter_length, L = output_length;
+    if (batch < 0 || n_mics < 1 || L < 1)
+        return kb_fail(KAPRE_E_INVALID, "rir_ism: bad size: batch %d, %d mics, output_length %d", batch, n_mics, L);
+    if (W < 1 || W > KB_RIR_MAX_W || !(W & 1))
+        return kb_fail(KAPRE_E_INVALID, "rir_ism: delay_filter_length must be odd, 1 to %d, got %d", KB_RIR_MAX_W, W);
+    if (!(std::isfinite(sample_rate) && sample_rate > 0) || !(std::isfinite(sound_speed) && sound_speed > 0))
+        return kb_fail(KAPRE_E_INVALID, "rir_ism: sample_rate and sound_speed must be finite and positive");
+    if (flags & ~KAPRE_RIR_UNIT_NORM) return kb_fail(KAPRE_E_INVALID, "rir_ism: unknown flags %d", flags);
+    if (batch == 0) return 0;
+    if (!records_host || !records_dev != !out_dev) return kb_fail(KAPRE_E_INVALID, "null argument");
+    const double* mics = records_host + (size_t)batch * KB_RIR_REC;
+    for (int b = 0; b < batch; ++b) {
+        const double* r = records_host + (size_t)b * KB_RIR_REC;
+        for (int d = 0; d < 3; ++d) {
+            if (!(std::isfinite(r[d]) && r[d] > 0))
+                return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d: room sides must be finite and positive", b);
+            if (!kb_rir_inside(r[3 + d], r[d]))
+                return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d: the source must lie strictly inside the room", b);
+        }
+        for (int w = 0; w < 6; ++w)
+            if (!(r[6 + w] >= 0.0 && r[6 + w] <= 1.0))
+                return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d: reflection coefficients must lie in [0, 1]", b);
+        if (!(r[12] == -1.0 || (r[12] >= 0 && r[12] <= 1e6 && r[12] == floor(r[12]))))
+            return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d: max_order must be -1 or a non-negative integer", b);
+        if (!(r[13] >= 0 && r[13] == floor(r[13]) && r[13] + L <= 2147483647.0))
+            return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d: start must be an integer >= 0 with start + "
+                           "output_length < 2^31", b);
+        const double R = (r[13] + L) * sound_speed / sample_rate;
+        for (int m = 0; m < n_mics; ++m) {
+            const double* q = mics + ((size_t)b * n_mics + m) * 3;
+            for (int d = 0; d < 3; ++d)
+                if (!kb_rir_inside(q[d], r[d]))
+                    return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d mic %d must lie strictly inside the room", b, m);
+            const double dist = sqrt((q[0] - r[3]) * (q[0] - r[3]) + (q[1] - r[4]) * (q[1] - r[4]) +
+                                     (q[2] - r[5]) * (q[2] - r[5]));
+            if (!(dist >= 1e-3))
+                return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d mic %d is closer than 1 mm to the source", b, m);
+            const double n_img = kb_rir_image_bound(r, q, R);
+            if (!(n_img <= (double)KB_RIR_MAX_IMAGES))
+                return kb_fail(KAPRE_E_INVALID, "rir_ism: item %d mic %d: up to %.3g images, above the cap of %lld "
+                               "(a shorter response or a larger room)", b, m, n_img,
+                               (long long)KB_RIR_MAX_IMAGES);
+        }
+    }
+    if (!records_dev) return 0;                             // validation only
+    KbRirParams p{};
+    p.nw = KB_RIR_MAX_NW;
+    p.n_tt = (L + 32 * p.nw - 1) / (32 * p.nw);
+    const long long tiles = (long long)batch * n_mics * p.n_tt;
+    if (tiles > 2147483647LL || (double)batch * n_mics / 8.0 > 2147483647.0)
+        return kb_fail(KAPRE_E_INVALID, "rir_ism: %lld tiles exceed the grid", tiles);
+    p.rec = records_dev;
+    p.mic = records_dev + (size_t)batch * KB_RIR_REC;
+    p.out = out_dev; p.o_sb = stride_b; p.o_sm = stride_m; p.o_st = stride_t;
+    p.B = batch; p.M = n_mics; p.L = L; p.W = W;
+    p.fs = sample_rate; p.c = sound_speed;
+    const int half = (W - 1) / 2;
+    for (int k = 0; k < W; ++k) {
+        const double w = W == 1 ? 1.0 : 0.5 - 0.5 * cos(2.0 * 3.14159265358979323846 * k / (W - 1));
+        p.ws[k] = (float)(((k + 1 - half) & 1) ? -w : w);
+    }
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc = kb_launch(kb_rir_kernel, {.grid = (int)tiles, .block = 32 * p.nw, .smem = kb_rir_smem(32 * p.nw).total,
+                                       .st = st, .pdl = true, .timed = true}, p);
+    if (rc || !(flags & KAPRE_RIR_UNIT_NORM)) return rc;
+    const long long rows = (long long)batch * n_mics;
+    return kb_launch(kb_rir_norm_kernel, {.grid = (int)((rows + 7) / 8), .block = 256, .st = st, .pdl = true}, out_dev,
+                     (long long)stride_b, (long long)stride_m, (long long)stride_t, batch, n_mics, L);
 }
 
 }  // extern "C"

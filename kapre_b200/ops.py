@@ -1014,6 +1014,47 @@ def convolve_spectrum(x: torch.Tensor, H: torch.Tensor, plan: ConvolvePlan, star
     return _crop(y, start, length, data_format)
 
 
+RIR_RECORD = 14                 # float64 per item: room[3], source[3], beta[6], max_order (-1: none), start
+RIR_MAX_IMAGES = 1 << 24        # kapre_rir_ism's cap on a response's image bound (KB_RIR_MAX_IMAGES)
+_rir_captured = []              # pinned records of captures made without a holder: a graph may replay them at any time
+
+
+def rir_ism(records, mics, output_length, filter_length, sample_rate, sound_speed, data_format=_CH_LAST_STR,
+            unit_norm=False, keep=None):
+    """``kapre_rir_ism`` on the current device: ``records`` (B, 14) and ``mics`` (B, M, 3) host float64 arrays, the
+    responses as float32 (B, L, M) channels_last or (B, M, L) channels_first.  Values the kernel cannot take raise
+    ValueError before anything is launched.  The records go up in one host-to-device copy; under CUDA graph capture
+    they are staged in a pinned buffer appended to ``keep`` (a list the caller holds for the graph's life; by default
+    one kept for the process), because the graph's copy node reads it on every replay.  ``unit_norm``: each response scaled to unit L2 norm (a second
+    launch)."""
+    _require_cuda()
+    records = np.ascontiguousarray(records, np.float64)
+    mics = np.ascontiguousarray(mics, np.float64)
+    B, M = mics.shape[0], mics.shape[1]
+    L = int(output_length)
+    host = torch.from_numpy(np.concatenate([records.ravel(), mics.ravel()]))
+    dev = torch.device('cuda', torch.cuda.current_device())
+    if data_format == _CH_LAST_STR:
+        out = torch.empty((B, L, M), dtype=torch.float32, device=dev)
+        sb, st, sm = out.stride()
+    else:
+        out = torch.empty((B, M, L), dtype=torch.float32, device=dev)
+        sb, sm, st = out.stride()
+    lib = N.lib()
+    args = (int(filter_length), float(sample_rate), float(sound_speed), N.RIR_UNIT_NORM if unit_norm else 0)
+    # validation alone (null device pointers), so that a bad value raises before the upload and the launch
+    if lib.kapre_rir_ism(_ptr(host), None, B, M, L, *args, None, sb, sm, st, _stream_ptr()) == -1:
+        raise ValueError(lib.kapre_last_error().decode())
+    if B == 0:
+        return out
+    if torch.cuda.is_current_stream_capturing():
+        host = host.pin_memory()
+        (_rir_captured if keep is None else keep).append(host)
+    rec_dev = host.to(dev, non_blocking=True)
+    N.check(lib.kapre_rir_ism(_ptr(host), _ptr(rec_dev), B, M, L, *args, _ptr(out), sb, sm, st, _stream_ptr()))
+    return out
+
+
 IIR_MAX_ORDER = 8
 
 

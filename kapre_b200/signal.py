@@ -27,7 +27,7 @@ __all__ = ['Frame', 'Energy', 'LogmelToMFCC', 'Resample', 'Speed', 'Convolve', '
            'Biquad', 'sosfilt', 'sosfiltfilt', 'SOSFilter', 'add_noise', 'loudness', 'Loudness', 'loudness_stats', 'true_peak',
            'LoudnessStats', 'kaldi_fbank', 'kaldi_mfcc', 'kaldi_spectrogram', 'yin', 'pyin',
            'YIN', 'PYIN', 'chroma_stft', 'chroma_cqt', 'chroma_cens', 'estimate_tuning', 'hpss', 'harmonic',
-           'percussive', 'onset_strength', 'onset_detect', 'tempogram', 'tempo', 'beat_track']
+           'percussive', 'onset_strength', 'onset_detect', 'tempogram', 'tempo', 'beat_track', 'simulate_rir_ism']
 
 
 def _resolve(fmt):
@@ -1396,3 +1396,68 @@ def beat_track(waveform=None, sample_rate=22050, onset_envelope=None, hop_length
         if bpm is None:
             bpm = ops.tempo(ops.tempogram(e.detach(), plan.W, True, True, fmt), plan, False, fmt)
         return ops.beat_track(e, cfg, bpm, fmt)
+
+
+def _host64(v, name, shapes):
+    """A host value (number, NumPy array or CPU tensor) as float64 whose shape, or shape without its leading batch
+    axis, is one of ``shapes`` (None: any length)."""
+    if isinstance(v, torch.Tensor):
+        if v.is_cuda:
+            raise ValueError('%s must be a host value (geometry is read on the host), got a CUDA tensor' % name)
+        v = v.detach().numpy()
+    a = np.asarray(v, np.float64)
+
+    def fits(shape):
+        return any(len(shape) == len(t) and all(x is None or x == y for x, y in zip(t, shape)) for t in shapes)
+    if not (fits(a.shape) or (a.ndim and fits(a.shape[1:]))):
+        raise ValueError('%s must have shape %s, or a batch of them, got %s' % (name, ' or '.join(map(str, shapes)),
+                                                                              a.shape))
+    return a
+
+
+def simulate_rir_ism(room, source, mic_array, max_order, absorption, output_length, delay_filter_length=81,
+                     sound_speed=343.0, sample_rate=16000.0, data_format='default'):
+    """Room impulse responses of a shoebox room by the image-source method (named and shaped after torchaudio's old
+    prototype ``simulate_rir_ism``; the maths is this library's own, modelled on pyroomacoustics' shoebox ISM and not
+    checked against either, DESIGN.md §RIR).
+
+    ``room`` (sides, metres) and ``source`` are ``(3,)`` or ``(B, 3)``, ``mic_array`` ``(M, 3)`` or ``(B, M, 3)``,
+    ``absorption`` (energy absorption in [0, 1]) a float, ``(6,)`` or ``(B, 6)`` for the walls
+    ``(x=0, x=Lx, y=0, y=Ly, z=0, z=Lz)``: host values (floats, NumPy arrays or CPU tensors).  Each image adds its
+    gain times a Hann-windowed sinc of ``delay_filter_length`` (odd, 1 to 255) taps centred on its delay plus half the
+    filter; ``max_order`` (None or an int >= 0) keeps the images of at most that many reflections.  Returns the first
+    ``output_length`` samples of every response, float32 ``(B, output_length, M)`` / ``(B, M, output_length)`` in
+    waveform layout, so that ``Convolve()(x.expand(...), h)`` gives the array's signals.  One launch, no gradient.
+    Each sample's bits depend on its item's geometry and its index alone.  Out-of-range values raise ValueError
+    before anything is launched."""
+    if max_order is not None and (isinstance(max_order, (bool, np.bool_)) or not isinstance(max_order, (int, np.integer))
+                                  or max_order < 0):
+        raise ValueError('max_order must be None or a non-negative int, got: %r' % (max_order,))
+    if isinstance(output_length, (bool, np.bool_)) or not isinstance(output_length, (int, np.integer)) \
+            or output_length < 1:
+        raise ValueError('output_length must be an int >= 1, got: %r' % (output_length,))
+    if isinstance(delay_filter_length, (bool, np.bool_)) or not isinstance(delay_filter_length, (int, np.integer)):
+        raise ValueError('delay_filter_length must be an odd int from 1 to 255, got: %r' % (delay_filter_length,))
+    backend.validate_data_format_str(data_format)
+    fmt = _resolve(_unwrap_format(data_format))
+    room = _host64(room, 'room', [(3,)])
+    source = _host64(source, 'source', [(3,)])
+    mics = _host64(mic_array, 'mic_array', [(None, 3)])
+    if mics.shape[-2] < 1:
+        raise ValueError('mic_array needs at least one mic, got shape %s' % (mics.shape,))
+    absorption = _host64(absorption, 'absorption', [(), (6,)])
+    B = max(a.shape[0] if a.ndim == nd else 1 for a, nd in ((room, 2), (source, 2), (mics, 3), (absorption, 2)))
+    for a, nd, name in ((room, 2, 'room'), (source, 2, 'source'), (mics, 3, 'mic_array'), (absorption, 2, 'absorption')):
+        if a.ndim == nd and a.shape[0] not in (1, B):
+            raise ValueError('%s has batch %d, expected 1 or %d' % (name, a.shape[0], B))
+    room = np.broadcast_to(room.reshape(-1, 3), (B, 3))
+    source = np.broadcast_to(source.reshape(-1, 3), (B, 3))
+    mics = np.broadcast_to(mics.reshape((-1,) + mics.shape[-2:]), (B,) + mics.shape[-2:])
+    absorption = np.broadcast_to(absorption.reshape(-1, 6) if absorption.ndim else absorption.reshape(1, 1), (B, 6))
+    if not np.all((absorption >= 0) & (absorption <= 1)):
+        raise ValueError('absorption must lie in [0, 1]')
+    records = np.zeros((B, ops.RIR_RECORD), np.float64)
+    records[:, 0:3], records[:, 3:6], records[:, 6:12] = room, source, np.sqrt(1.0 - absorption)
+    records[:, 12] = -1.0 if max_order is None else float(max_order)
+    return ops.rir_ism(records, mics, int(output_length), int(delay_filter_length), float(sample_rate),
+                       float(sound_speed), fmt)
